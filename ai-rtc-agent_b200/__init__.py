@@ -1,4 +1,4 @@
-"""B200-native per-frame img2img path behind the lib/pipeline.py / lib/wrapper.py call surface of
+"""H100-native per-frame img2img path behind the lib/pipeline.py / lib/wrapper.py call surface of
 yondonfu/ai-rtc-agent.  Layout:
 
   csrc/   hand-written sm_100a CUDA (tcgen05 / TMA / TMEM) + the C ABI (include/b200sd.h)

@@ -1,4 +1,4 @@
-// tcgen05 flash attention (see attention.cuh).
+// wgmma flash attention (see attention.cuh).
 #include "attention.cuh"
 
 #include <cudaTypedefs.h>
@@ -8,21 +8,18 @@
 #include "igemm.cuh"  // b2_set_error
 #include "launch.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace b2 {
 
-constexpr int AT_BQ = 128;      // query rows per CTA == UMMA M
-constexpr int AT_STAGES = 2;    // K/V ring depth
-constexpr int AT_THREADS = 320; // warp0 TMA, warp1 MMA (+TMEM alloc), warps 2-9 softmax (two warps per TMEM lane quarter)
-constexpr int AT_SM_THREADS = 256;
-// TMEM: S (one QK^T tile, BKV columns) at column 0, O accumulator (DP columns) right after it; 256 columns per
-// CTA so that two CTAs share an SM (one's softmax overlaps the other's MMAs).
-// Softmax: a query row (TMEM lane) is shared by TWO threads (warps w and w+4 see the same lane quarter), each owning half
-// of the S columns / O columns.  One warp per scheduler was pure latency (tcgen05.ld -> max chain -> ex2 chain): measured
-// on B200, 288 CTAs (two per SM) took exactly as long as 128 (one per SM), so the second warp per scheduler is free.
-// The pair only exchanges its block maximum (fp16, 512 B of shared memory, two 64-thread named barriers per KV block);
-// the row sums stay private until the end.
-constexpr uint32_t AT_TMEM_COLS = 256;
+constexpr int AT_BQ = 128;      // query rows per CTA: two consumer warpgroups of 64 rows (wgmma M)
+constexpr int AT_STAGES = 3;    // K/V ring depth
+constexpr int AT_CONS = 256;    // warps 0-7: consumer warpgroups (MMAs, online softmax, epilogue)
+constexpr int AT_THREADS = AT_CONS + 32;   // + warp 8: TMA producer
+// Each consumer thread holds two query rows of its warpgroup's S = Q K^T fragment and of the O accumulator (registers).  The
+// softmax numerators P are rounded to fp16 and repacked in registers as the A operand of the P.V wgmma: the m64nNk16 D
+// fragment of S columns [16k, 16k+16) is exactly the A fragment of K step k, so P never touches shared memory.  Row maxima and
+// sums are reduced over the 4 lanes that share a row.
 
 __device__ __forceinline__ float ex2_approx(float x) {
     float y;
@@ -30,7 +27,10 @@ __device__ __forceinline__ float ex2_approx(float x) {
     return y;
 }
 
-template <bool V> struct AttnTag { static constexpr bool value = V; };
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+    const __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&h);
+}
 
 struct AttnParams {
     CUtensorMap tmq, tmk, tmv;
@@ -41,44 +41,32 @@ struct AttnParams {
     float scale_log2;
 };
 
-// PTS = true: P (the softmax numerators, fp16) goes to tensor memory and the P.V product reads its A operand from there
-// (tcgen05.mma "TS" form) -- no 32 KB shared-memory round trip of P per KV block.  TMEM columns: S [0,BKV) fp32,
-// O [BKV, BKV+DP) fp32, P [BKV+DP, BKV+DP+BKV/2) packed fp16: 256 for <1,128>, so two CTAs still share an SM.
-template <int DA, int BKV, bool PTS = false>
-__global__ void __launch_bounds__(AT_THREADS, (DA == 1 ? 2 : 1)) attn_kernel(const __grid_constant__ AttnParams p) {
+template <int DA, int BKV>
+__global__ void __launch_bounds__(AT_THREADS, 1) attn_kernel(const __grid_constant__ AttnParams p) {
     constexpr int DP = DA * 64;
-    static_assert(!PTS || BKV + DP + BKV / 2 <= (int)AT_TMEM_COLS, "P does not fit the CTA's tensor memory");
-    constexpr int NST = PTS ? AT_STAGES + 1 : AT_STAGES;   // the 32 KB the P tile no longer needs in shared memory buy a third K/V stage
-    constexpr int KVA = BKV / 64;                       // kv atoms per block (P / V^T tiles)
+    constexpr int NST = AT_STAGES;
+    constexpr int KVA = BKV / 64;                       // kv atoms per block (V^T tiles)
     constexpr uint32_t Q_BYTES = DA * AT_BQ * 128;      // DA atoms of [128 rows][128 B]
     constexpr uint32_t K_BYTES = DA * BKV * 128;        // DA atoms of [BKV rows][128 B]
     constexpr uint32_t V_BYTES = KVA * DP * 128;        // KVA atoms of [DP rows][128 B]
     constexpr uint32_t STAGE_BYTES = K_BYTES + V_BYTES;
-    constexpr uint32_t P_BYTES = KVA * AT_BQ * 128;
 
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* sQ = smem;
     uint8_t* sKV = sQ + Q_BYTES;
-    uint8_t* sP = sKV + NST * STAGE_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sP + (PTS ? 0 : P_BYTES));
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + NST * STAGE_BYTES);
     uint64_t* q_full = bars;
-    uint64_t* k_full = bars + 1;                // [NST]  K and V^T tiles travel through separate rings: a K slot is
-    uint64_t* k_empty = k_full + NST;     // [NST]  free as soon as QK^T(j) retires, one softmax earlier than the
-    uint64_t* v_full = k_empty + NST;     // [NST]  V slot, so K(j+2) is requested ~1.3 KV blocks before its use
-    uint64_t* v_empty = v_full + NST;     // [NST]  (with one shared ring the K latency was exposed every block)
-    uint64_t* s_full = v_empty + NST;
-    uint64_t* s_empty = s_full + 1;
-    uint64_t* p_full = s_empty + 1;
-    uint64_t* o_done = p_full + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_done + 1);
-    float* xch = reinterpret_cast<float*>(bars + 32);          // 512 B pair-exchange scratch: [2][128] 16-bit block maxima / [128] fp32 row sums
+    uint64_t* k_full = bars + 1;          // [NST]  K and V^T tiles travel through separate rings: a K slot is free as soon
+    uint64_t* k_empty = k_full + NST;     // [NST]  as QK^T(j) retires, before the softmax of block j, so K(j+NST) is
+    uint64_t* v_full = k_empty + NST;     // [NST]  requested a softmax earlier than the V slot of the same stage
+    uint64_t* v_empty = v_full + NST;     // [NST]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * AT_BQ;
     const int h = blockIdx.y, b = blockIdx.z;
     const int nblk = (p.skv + BKV - 1) / BKV;
 
-    if (threadIdx.x == 0) {
+    if (threadIdx.x == AT_CONS) {
         if (smem_u32(smem) & 1023u) {
             printf("b2 attn: dynamic smem base not 1024-aligned\n");
             __trap();
@@ -89,28 +77,17 @@ __global__ void __launch_bounds__(AT_THREADS, (DA == 1 ? 2 : 1)) attn_kernel(con
         mbar_init(q_full, 1);
         for (int s = 0; s < NST; ++s) {
             mbar_init(&k_full[s], 1);
-            mbar_init(&k_empty[s], 1);
+            mbar_init(&k_empty[s], AT_CONS / 32);   // one arrival per consumer warp
             mbar_init(&v_full[s], 1);
-            mbar_init(&v_empty[s], 1);
+            mbar_init(&v_empty[s], AT_CONS / 32);
         }
-        mbar_init(s_full, 1);
-        mbar_init(s_empty, AT_SM_THREADS);
-        mbar_init(p_full, AT_SM_THREADS);
-        mbar_init(o_done, 1);
         fence_mbar_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, AT_TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_launch_dependents();   // the next kernel may start its own prologue now
     pdl_wait();                // ... and everything below reads the previous kernel's output
 
-    if (warp == 0) {
+    if (warp == AT_CONS / 32) {
         if (lane == 0) {
             // ===== TMA producer =====
             mbar_expect_tx(q_full, Q_BYTES);
@@ -135,209 +112,120 @@ __global__ void __launch_bounds__(AT_THREADS, (DA == 1 ? 2 : 1)) attn_kernel(con
                 for (int a = 0; a < KVA; ++a)
                     tma_load_2d(sv + a * (DP * 128), &p.tmv, &v_full[st], (int)(b * p.vt_bstride) + j * BKV + a * 64, h * DP);
             };
-            // issue order = the order in which slots become free: K(j+1) [after QK(j-1)] before V(j) [after PV(j-2)]
+            // issue order = the order in which slots become free: K(j+1) [after QK(j+1-NST)] before V(j) [after PV(j-NST)]
             load_k(0);
             for (int j = 0; j < nblk; ++j) {
                 if (j + 1 < nblk) load_k(j + 1);
                 load_v(j);
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: the whole warp walks the loop (uniform control flow => descriptors stay in uniform
-        // registers), one elected lane issues (see igemm.cu) =====
-        const uint32_t idesc_s = make_idesc_f16(AT_BQ, BKV);
-        const uint32_t idesc_o = make_idesc_f16(AT_BQ, DP);
-        const uint32_t sq_addr = smem_u32(sQ), skv_addr = smem_u32(sKV), sp_addr = smem_u32(sP);
-        auto issue_qk = [&](int j) {
-            const int st = j % NST;
-            mbar_wait(&k_full[st], (j / NST) & 1);
-            mbar_wait(s_empty, (j & 1) ^ 1);
-            tc_fence_after();
-            const uint32_t sk = skv_addr + st * STAGE_BYTES;
-            if (elect_one()) {
-#pragma unroll
-                for (int a = 0; a < DA; ++a) {
-                    const uint64_t dq = make_kmajor_sw128_desc(sq_addr + a * (AT_BQ * 128));
-                    const uint64_t dk = make_kmajor_sw128_desc(sk + a * (BKV * 128));
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) umma_f16(tmem_base, dq + 2 * k, dk + 2 * k, idesc_s, (a | k) ? 1u : 0u);
-                }
-                umma_commit(s_full);
-                umma_commit(&k_empty[st]);
-            }
-            __syncwarp();
-        };
-        mbar_wait(q_full, 0);
-        issue_qk(0);
-        for (int j = 0; j < nblk; ++j) {
-            if (j + 1 < nblk) issue_qk(j + 1);  // issues as soon as softmax(j) has drained S; overlaps its P stores
-            const int st = j % NST;
-            mbar_wait(&v_full[st], (j / NST) & 1);
-            mbar_wait(p_full, j & 1);
-            tc_fence_after();
-            const uint32_t sv = skv_addr + st * STAGE_BYTES + K_BYTES;
-            if (elect_one()) {
-#pragma unroll
-                for (int a = 0; a < KVA; ++a) {
-                    const uint64_t dp = make_kmajor_sw128_desc(sp_addr + a * (AT_BQ * 128));
-                    const uint64_t dv = make_kmajor_sw128_desc(sv + a * (DP * 128));
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint32_t acc = (j > 0 || a > 0 || k > 0) ? 1u : 0u;
-                        if constexpr (PTS)   // A = P from tensor memory: K step (a*4 + k) of 16 elements = 8 packed columns
-                            umma_f16_ts(tmem_base + BKV, tmem_base + BKV + DP + (a * 4 + k) * 8, dv + 2 * k, idesc_o, acc);
-                        else
-                            umma_f16(tmem_base + BKV, dp + 2 * k, dv + 2 * k, idesc_o, acc);
-                    }
-                }
-                umma_commit(o_done);
-                umma_commit(&v_empty[st]);
-            }
-            __syncwarp();
-        }
     } else {
-        // ===== softmax / correction / epilogue: threads (hf = 0, 1) of a pair own query row r, columns [hf*HC, hf*HC + HC) =====
-        constexpr int HC = BKV / 2;           // S columns per thread
-        constexpr int HO = DP / 2;            // O columns per thread
-        const int q = warp & 3;               // TMEM lane quarter this warp may access
-        const int hf = (warp - 2) >> 2;
-        const int r = q * 32 + lane;
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-        float m_run = -INFINITY, l_run = 0.f;
-        const uint32_t tS = lane_addr + hf * HC;
-        const uint32_t tO = lane_addr + BKV + hf * HO;
-        uint16_t* xmax = reinterpret_cast<uint16_t*>(xch);
-        auto pair_sync = [&]() { asm volatile("bar.sync %0, 64;" ::"r"(1 + q) : "memory"); };
-        // one KV block; MASKED is a compile-time flag so that interior blocks carry no per-element compare/select at all
-        auto block = [&](int j, auto masked_tag) {
-            constexpr bool MASKED = decltype(masked_tag)::value;
-            const int kv_valid = p.skv - j * BKV;  // columns >= kv_valid are masked
-            mbar_wait(s_full, j & 1);
-            tc_fence_after();
-            // pass 1: maximum of this thread's columns (kept in registers for pass 2), four independent chains
-            uint32_t v[HC];
+        // ===== consumer warpgroup wg: query rows [64 wg, 64 wg + 64) of the tile; this thread: rows rq and rq + 8 =====
+        const int wg = warp >> 2;
+        const int rq = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int q2 = 2 * (lane & 3);
+        const uint32_t sq_addr = smem_u32(sQ) + (uint32_t)wg * (64 * 128), skv_addr = smem_u32(sKV);
+        float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+        float o[DP / 2];
 #pragma unroll
-            for (int c = 0; c < HC; c += 32) tmem_ld32(tS + c, *reinterpret_cast<uint32_t(*)[32]>(&v[c]));
-            tmem_ld_wait();
-            float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-            for (int i = 0; i < HC; ++i) {
-                if (!MASKED || hf * HC + i < kv_valid) mx4[i & 3] = fmaxf(mx4[i & 3], __uint_as_float(v[i]));
-            }
-            // S(j) is in registers: the next QK^T may overwrite it
-            tc_fence_before();
-            mbar_arrive(s_empty);
-            const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-            // Pair exchange of the block maximum as the upper 16 bits of its fp32 pattern, rounded toward +inf (any common
-            // m >= the true maximum is a valid softmax shift; exp2 arguments stay <= 0).  Unlike an fp16 exchange this keeps
-            // the fp32 exponent range: |s| > 65504 cannot become +inf and poison the row.  The lower clamp keeps a fully
-            // masked half finite.
-            const uint32_t mb = __float_as_uint(fmaxf(mx, -3.0e38f));
-            const uint16_t me = (uint16_t)((mb & 0x80000000u) ? (mb >> 16) : ((mb + 0xffffu) >> 16));
-            xmax[hf * AT_BQ + r] = me;
-            pair_sync();
-            const float mpair = fmaxf(__uint_as_float((uint32_t)me << 16), __uint_as_float((uint32_t)xmax[(hf ^ 1) * AT_BQ + r] << 16));
-            pair_sync();   // both halves have read: the single exchange buffer may be rewritten for the next block
-            const float m_new = fmaxf(m_run, mpair * p.scale_log2);
-            const float alpha = ex2_approx(m_run - m_new);
-            if (j > 0) mbar_wait(o_done, (j - 1) & 1);  // PV(j-1) retired: P buffer + O are ours
-            // pass 2: P = exp2(s*scale - m), to smem (fp16, swizzled K-major), row sum
-            float rs4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-            for (int c = 0; c < HC; c += 32) {
-                uint32_t pk[16];
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    float p0 = ex2_approx(__uint_as_float(v[c + i]) * p.scale_log2 - m_new);
-                    float p1 = ex2_approx(__uint_as_float(v[c + i + 1]) * p.scale_log2 - m_new);
-                    if (MASKED) {
-                        if (hf * HC + c + i >= kv_valid) p0 = 0.f;
-                        if (hf * HC + c + i + 1 >= kv_valid) p1 = 0.f;
-                    }
-                    rs4[(i >> 1) & 3] += p0 + p1;
-                    const __half2 hp = __floats2half2_rn(p0, p1);
-                    pk[i >> 1] = *reinterpret_cast<const uint32_t*>(&hp);
-                }
-                const int cabs = hf * HC + c;      // column inside the KV block
-                if constexpr (PTS) {
-                    tmem_st16(lane_addr + BKV + DP + (cabs >> 1), pk);   // 32 fp16 = 16 packed columns of this thread's lane
-                } else {
-                    uint8_t* prow = sP + (cabs >> 6) * (AT_BQ * 128);
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        const uint32_t chunk = ((cabs & 63) >> 3) + u;
-                        *reinterpret_cast<uint4*>(prow + sw128_offset(r, chunk)) =
-                            make_uint4(pk[4 * u], pk[4 * u + 1], pk[4 * u + 2], pk[4 * u + 3]);
-                    }
-                }
-            }
-            // rescale this thread's half of the running O accumulator (TMEM) when any row of the warp moved its max
-            if (j > 0) {
-                const bool need = __any_sync(0xffffffffu, alpha != 1.0f);
-                if (need) {
-#pragma unroll
-                    for (int c = 0; c < HO; c += 32) {
-                        uint32_t o[32];
-                        tmem_ld32(tO + c, o);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-                        tmem_st32(tO + c, o);
-                    }
-                    tmem_st_wait();
-                }
-            }
-            l_run = l_run * alpha + ((rs4[0] + rs4[1]) + (rs4[2] + rs4[3]));
-            m_run = m_new;
-            if constexpr (PTS) tmem_st_wait();   // P (and a rescaled O) have landed in tensor memory
-            else fence_proxy_async_smem();       // P stores -> visible to the UMMA (async proxy)
-            tc_fence_before();
-            mbar_arrive(p_full);
-        };
+        for (int i = 0; i < DP / 2; ++i) o[i] = 0.f;
+        mbar_wait(q_full, 0);
         for (int j = 0; j < nblk; ++j) {
-            if (p.skv - j * BKV >= BKV) block(j, AttnTag<false>{});   // warp-uniform
-            else block(j, AttnTag<true>{});
-        }
-        // row sum of the pair (both halves used the same running maximum, so the partial sums simply add)
-        pair_sync();                       // nobody still reads the fp16 maxima
-        if (hf == 1) xch[r] = l_run;
-        pair_sync();
-        if (hf == 0) { l_run += xch[r]; }
-        pair_sync();
-        if (hf == 0) xch[r] = l_run;
-        pair_sync();
-        l_run = xch[r];
-        // epilogue: O / l -> fp16 -> global (this thread's half of the head dimension)
-        mbar_wait(o_done, (nblk - 1) & 1);
-        tc_fence_after();
-        const float inv_l = 1.0f / l_run;
-        const bool row_ok = (q0 + r) < p.sq;
-        __half* orow = p.out + ((long)b * p.sq + q0 + r) * p.ldo + h * p.d_real;
+            const int st = j % NST;
+            const uint32_t ph = (uint32_t)(j / NST) & 1u;
+            const uint32_t sk = skv_addr + st * STAGE_BYTES;
+            // S = Q K^T
+            float s[BKV / 2];
 #pragma unroll
-        for (int c = 0; c < HO; c += 32) {
-            uint32_t v[32];
-            tmem_ld32(tO + c, v);
-            tmem_ld_wait();
-            if (row_ok) {
+            for (int i = 0; i < BKV / 2; ++i) s[i] = 0.f;
+            mbar_wait(&k_full[st], ph);
+            wgmma_fence_regs(s);
+            wgmma_fence();
 #pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int col = hf * HO + c + 8 * u;
-                    if (col + 8 <= p.d_real) {
-                        uint4 o;
-                        __half2* oh = reinterpret_cast<__half2*>(&o);
+            for (int a = 0; a < DA; ++a) {
+                const uint64_t dq = make_kmajor_sw128_desc(sq_addr + a * (AT_BQ * 128));
+                const uint64_t dk = make_kmajor_sw128_desc(sk + a * (BKV * 128));
 #pragma unroll
-                        for (int i = 0; i < 4; ++i)
-                            oh[i] = __floats2half2_rn(__uint_as_float(v[8 * u + 2 * i]) * inv_l,
-                                                      __uint_as_float(v[8 * u + 2 * i + 1]) * inv_l);
-                        *reinterpret_cast<uint4*>(orow + col) = o;
-                    }
+                for (int k = 0; k < 4; ++k) Wgmma<BKV>::ss(s, dq + 2 * k, dk + 2 * k, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(s);
+            if (lane == 0) mbar_arrive(&k_empty[st]);   // S is in registers: the K slot may be refilled
+            // online softmax: block maximum, P = exp2(s*scale - m) packed as fp16 A fragments, row sums
+            const int kv_valid = p.skv - j * BKV;  // columns >= kv_valid are masked
+            float alpha[2], m_new[2];
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+                float mx = -INFINITY;
+#pragma unroll
+                for (int jj = 0; jj < BKV / 8; ++jj)
+#pragma unroll
+                    for (int u = 0; u < 2; ++u)
+                        if (8 * jj + q2 + u < kv_valid) mx = fmaxf(mx, s[4 * jj + 2 * hr + u]);
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                m_new[hr] = fmaxf(m_run[hr], mx * p.scale_log2);
+                alpha[hr] = ex2_approx(m_run[hr] - m_new[hr]);
+            }
+            uint32_t pa[BKV / 16][4];
+            float rs[2] = {0.f, 0.f};
+#pragma unroll
+            for (int jj = 0; jj < BKV / 8; ++jj)
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr) {
+                    float p0 = ex2_approx(s[4 * jj + 2 * hr] * p.scale_log2 - m_new[hr]);
+                    float p1 = ex2_approx(s[4 * jj + 2 * hr + 1] * p.scale_log2 - m_new[hr]);
+                    if (8 * jj + q2 >= kv_valid) p0 = 0.f;
+                    if (8 * jj + q2 + 1 >= kv_valid) p1 = 0.f;
+                    rs[hr] += p0 + p1;
+                    pa[jj >> 1][(jj & 1) * 2 + hr] = pack_half2(p0, p1);
                 }
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+                l_run[hr] = l_run[hr] * alpha[hr] + rs[hr];
+                m_run[hr] = m_new[hr];
+            }
+#pragma unroll
+            for (int jj = 0; jj < DP / 8; ++jj)
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr) {
+                    o[4 * jj + 2 * hr] *= alpha[hr];
+                    o[4 * jj + 2 * hr + 1] *= alpha[hr];
+                }
+            // O += P V  (B = V^T tile, K-major over the kv index)
+            const uint32_t sv = sk + K_BYTES;
+            mbar_wait(&v_full[st], ph);
+            wgmma_fence_regs(o);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < BKV / 16; ++kk) {
+                const uint64_t dv = make_kmajor_sw128_desc(sv + (kk >> 2) * (DP * 128)) + 2 * (kk & 3);
+                Wgmma<DP>::rs(o, pa[kk], dv, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(o);
+            if (lane == 0) mbar_arrive(&v_empty[st]);
+        }
+        // epilogue: O / l -> fp16 -> global
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            float l = l_run[hr];
+            l += __shfl_xor_sync(0xffffffffu, l, 1);
+            l += __shfl_xor_sync(0xffffffffu, l, 2);
+            const float inv_l = 1.0f / l;
+            const int r = rq + 8 * hr;
+            if (q0 + r >= p.sq) continue;
+            __half* orow = p.out + ((long)b * p.sq + q0 + r) * p.ldo + h * p.d_real;
+#pragma unroll
+            for (int jj = 0; jj < DP / 8; ++jj) {
+                const int col = 8 * jj + q2;
+                if (col < p.d_real)
+                    *reinterpret_cast<uint32_t*>(orow + col) = pack_half2(o[4 * jj + 2 * hr] * inv_l, o[4 * jj + 2 * hr + 1] * inv_l);
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, AT_TMEM_COLS);
 }
 
 // ------------------------------------------------------------------------------------------ host
@@ -369,17 +257,11 @@ static int encode_2d(CUtensorMap* m, const __half* ptr, long cols, long rows, lo
     return 0;
 }
 
-static bool attn_p_in_tmem(int dp) {
-    static const bool off = getenv("B2_NO_ATTN_PTS") != nullptr;   // debug: P through shared memory again (round-1 data path)
-    return dp == 64 && !off;
-}
-static size_t attn_smem_bytes(int da, int bkv, bool pts) {
+static size_t attn_smem_bytes(int da, int bkv) {
     const size_t q = (size_t)da * AT_BQ * 128;
     const size_t k = (size_t)da * bkv * 128;
     const size_t v = (size_t)(bkv / 64) * da * 64 * 128;
-    const size_t pb = (size_t)(bkv / 64) * AT_BQ * 128;
-    // + barriers + pair-exchange scratch (2 CTAs of <1,128> still fit an SM); P in tensor memory: a third K/V stage instead of P
-    return q + (pts ? (AT_STAGES + 1) * (k + v) : AT_STAGES * (k + v) + pb) + 256 + 512;
+    return q + AT_STAGES * (k + v) + 256;   // + barriers
 }
 
 int attn_plan(const AttnDesc& d, AttnPlan* plan) {
@@ -398,7 +280,7 @@ int attn_plan(const AttnDesc& d, AttnPlan* plan) {
     if (encode_2d(&plan->tmk, d.k, (long)d.heads * d.dp, d.k_rows, d.ldk, 64, bkv, "k")) return -1;
     if (encode_2d(&plan->tmv, d.vt, d.vt_cols, (long)d.heads * d.dp, d.ldvt, 64, d.dp, "vt")) return -1;
     plan->grid = dim3((d.sq + AT_BQ - 1) / AT_BQ, d.heads, d.nb);
-    plan->smem = attn_smem_bytes(d.dp / 64, bkv, attn_p_in_tmem(d.dp));
+    plan->smem = attn_smem_bytes(d.dp / 64, bkv);
     return 0;
 }
 
@@ -406,7 +288,6 @@ int attn_init() {
     static bool attr_set = false;
     if (!attr_set) {
         cudaError_t e1 = cudaFuncSetAttribute(attn_kernel<1, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e1 == cudaSuccess) e1 = cudaFuncSetAttribute(attn_kernel<1, 128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         cudaError_t e2 = cudaFuncSetAttribute(attn_kernel<2, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         cudaError_t e3 = cudaFuncSetAttribute(attn_kernel<3, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess) {
@@ -428,8 +309,7 @@ int attn_launch(const AttnPlan& plan, cudaStream_t s) {
     p.k_bstride = d.k_bstride; p.vt_bstride = d.vt_bstride;
     p.scale_log2 = (float)(1.4426950408889634 / sqrt((double)d.d_real));
     cudaError_t e;
-    if (attn_p_in_tmem(d.dp)) e = launch_k(attn_kernel<1, 128, true>, plan.grid, dim3(AT_THREADS), plan.smem, s, 1, p);
-    else if (d.dp == 64) e = launch_k(attn_kernel<1, 128>, plan.grid, dim3(AT_THREADS), plan.smem, s, 1, p);
+    if (d.dp == 64) e = launch_k(attn_kernel<1, 128>, plan.grid, dim3(AT_THREADS), plan.smem, s, 1, p);
     else if (d.dp == 128) e = launch_k(attn_kernel<2, 128>, plan.grid, dim3(AT_THREADS), plan.smem, s, 1, p);
     else e = launch_k(attn_kernel<3, 64>, plan.grid, dim3(AT_THREADS), plan.smem, s, 1, p);
     if (e != cudaSuccess) {

@@ -1,6 +1,6 @@
-// Flash-style attention on tcgen05: S = Q K^T and O += P V as UMMA (accumulators in TMEM), online
-// softmax in registers by 4 warps (one query row per thread == one TMEM lane), P staged through
-// shared memory in the K-major SWIZZLE_128B layout.  Self-attention (seq 64..9216) and
+// Flash-style attention on wgmma: S = Q K^T and O += P V as warpgroup MMAs with the accumulators in
+// registers, online softmax on the S fragment, P kept in registers as the A operand of the P.V MMA.
+// Self-attention (seq 64..9216) and
 // cross-attention against the cached prompt K/V (77 keys) use the same kernel.
 #pragma once
 #include <cuda.h>

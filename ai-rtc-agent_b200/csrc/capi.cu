@@ -84,8 +84,8 @@ int b2sd_igemm_plan_dry(const b2sd_igemm_desc* d, int autotile, int allow_swap, 
     to_igemm_desc(d, g);
     g.dbg_ts = nullptr;
     IgemmPlan plan;
-    if (autotile == 2) {   // the engine's throughput policy (b2sd_set_concurrency >= 4): 100 KB rings, CTA pairs without split-K
-        g.ring_kb = 100; g.max_splits = 4; g.pair_auto = 1; g.pair_splits = 1;
+    if (autotile == 2) {   // the engine's throughput policy (b2sd_set_concurrency >= 4): CTA pairs without split-K
+        g.max_splits = 4; g.pair_auto = 1; g.pair_splits = 1;
     }
     igemm_set_dry_run(true);
     const int rc = autotile ? igemm_autotile(g, allow_swap != 0, &plan) : igemm_plan(g, &plan);

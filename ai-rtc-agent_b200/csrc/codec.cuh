@@ -6,8 +6,8 @@
 //   rgb_u8_to_nv12   u8 NCHW RGB (what b2sd_step writes)                          -> NV12 surface for NVENC
 // BT.709 or BT.601, limited ("video") or full range, 2x2 chroma sub-sampling: the co-sited-left MPEG-2 / H.264 default is
 // approximated by the box average of the four RGB-derived chroma samples (what NPP / CV-CUDA do).
-// b2_codec_probe() dlopen()s libnvcuvid / libnvidia-encode; the GPU boxes of this project ship neither
-// (profiles/r01_gpu_box_probe.txt), so the session wrappers stop at "codec unavailable" and the synthetic feeder is the source.
+// b2_codec_probe() dlopen()s libnvcuvid / libnvidia-encode; where neither is installed the session wrappers stop at
+// "codec unavailable" and the synthetic feeder is the source.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

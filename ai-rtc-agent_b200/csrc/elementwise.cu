@@ -489,7 +489,7 @@ int groupnorm_launch(const GroupNormArgs& a, cudaStream_t s) {
     // single cooperative launch when the whole grid is co-resident and a chunk fits the register cache
     int per_sm = 0;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gn_fused_kernel, threads, smem);
-    const bool fits = (ppc + rpi - 1) / rpi <= GN_CACHE && (long)nchunks * a.nb <= (long)per_sm * 148 && a.nb <= 16;
+    const bool fits = (ppc + rpi - 1) / rpi <= GN_CACHE && (long)nchunks * a.nb <= (long)per_sm * b2_device_sms() && a.nb <= 16;
     if (fits && a.counters) {
         cudaLaunchConfig_t cfg{};
         cfg.gridDim = dim3(nchunks, a.nb);
@@ -512,7 +512,7 @@ int groupnorm_launch(const GroupNormArgs& a, cudaStream_t s) {
     B2_LAUNCHED("gn_stats", launch_k(gn_stats_kernel, dim3(nchunks, a.nb), dim3(threads), smem, s, 1, a, ppc, vc, rpi));
     const long vec_per_batch = (long)a.hw * vc;
     long blocks = (vec_per_batch + 255) / 256;
-    const long cap = (148 * 4 + a.nb - 1) / a.nb;
+    const long cap = (IG_SMS * 4 + a.nb - 1) / a.nb;
     if (blocks > cap) blocks = cap;
     B2_LAUNCHED("gn_apply", launch_k(gn_apply_kernel, dim3((unsigned)blocks, a.nb), dim3(256), 0, s, 1, a, nchunks, vec_per_batch));
     g_gn_last_launches = 2;
@@ -623,7 +623,7 @@ int upsample2x_launch(const __half* x, __half* y, int nb, int h, int w, int c, c
     const long total = (long)nb * 4 * h * w * (c / 8);
     const int threads = 256;
     long blocks = (total + threads - 1) / threads;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > IG_SMS * 16) blocks = IG_SMS * 16;
     B2_LAUNCHED("upsample2x", launch_k(upsample2x_kernel, dim3((unsigned)blocks), dim3(threads), 0, s, 1,
                                        reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), nb, h, w, c / 8));
     return 0;
@@ -744,15 +744,15 @@ int smallconv_launch(const SmallConvArgs& a, cudaStream_t s) {
         return -1;
     }
     const long npix = (long)a.nb * a.h * a.w_;
-    if (npix >= (1l << 31) - 128 * 148 * 32) {
+    if (npix >= (1l << 31) - 128 * IG_SMS * 32) {
         b2_set_error("smallconv: %ld pixels exceed the 32-bit index range", npix);
         return -1;
     }
     long blocks = (npix + 127) / 128;
-    const int G = blocks * (a.cout / 64) < 148 * 4 ? 16 : 64;   // few pixels: narrower channel groups, more CTAs
+    const int G = blocks * (a.cout / 64) < IG_SMS * 4 ? 16 : 64;   // few pixels: narrower channel groups, more CTAs
     const size_t smem = ((size_t)a.cin * 9 * G + G) * sizeof(float);
     const int groups = a.cout / G;
-    const long cap = (148 * 16 + groups - 1) / groups;   // two full waves of 8 CTAs per SM; beyond that, grid-stride
+    const long cap = (IG_SMS * 16 + groups - 1) / groups;   // two full waves of 8 CTAs per SM; beyond that, grid-stride
     if (blocks > cap) blocks = cap;
     static bool attr = false;
     if (!attr) {
@@ -927,7 +927,7 @@ __global__ void cast_f16_f32_kernel(const __half* __restrict__ x, float* __restr
 }
 static unsigned grid_for(long n) {
     long b = (n + 255) / 256;
-    if (b > 148 * 32) b = 148 * 32;
+    if (b > IG_SMS * 32) b = IG_SMS * 32;
     if (b < 1) b = 1;
     return (unsigned)b;
 }

@@ -114,18 +114,16 @@ struct Op {
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
-// Tile / split-K policy of the frame program (batch-1 driven; derived from the cold-weight sweep in
-// profiles/r01_tile_sweep.md, not from a model).  Fills `plan` for the chosen (BN, splits, orientation).
+// Tile / split-K policy of the frame program (batch-1 driven; derived from a cold-weight sweep of the contractions with
+// tools/bench_op.py, not from a model).  Fills `plan` for the chosen (BN, splits, orientation).
 // allow_swap: the caller is a UNet contraction (never TAESD / V^T / GEGLU).  Host-only: works in igemm dry-run mode.
 static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_out);
 
 // Tile policy + CTA pairs.  The single-CTA policy picks orientation, N tile and split-K.  With d.pair_auto (set by the engine
 // when several frames are in flight) a normal-orientation result with >= 2 M tiles and an N tile that is a multiple of 32 is
-// re-planned as CTA pairs (igemm_pair_kernel) with the same N tile and the split-K factor capped at d.pair_splits: under
-// concurrency the GPU is filled by the other frames, so what counts is SM time per contraction, and a pair stages half the
-// weight bytes per SM, has a deeper ring in the same shared memory and needs no cluster reduction (same-box A/B, 6 lanes:
-// 440.6 -> 470.5 frames/s; the same tiles WITHOUT pairing: 433.0; pairs with the latency policy's split-K: 417.6;
-// profiles/ab_r02u.txt, ab_r02x.txt).  Tuning overrides: B2_PAIR=0/1/2, B2_PAIR_SPLITS=n, B2_PAIR_SINGLE=1 (control: re-plan
+// re-planned as CTA pairs (2-CTA clusters) with the same N tile and the split-K factor capped at d.pair_splits: under
+// concurrency the GPU is filled by the other frames, so what counts is SM time per contraction, and a pair fetches half the
+// weight bytes per SM from L2 (multicast) and needs no cluster reduction.  Tuning overrides: B2_PAIR=0/1/2, B2_PAIR_SPLITS=n, B2_PAIR_SINGLE=1 (control: re-plan
 // with the capped split-K but single CTAs).
 int igemm_autotile(IgemmDesc d, bool allow_swap, IgemmPlan* plan_out) {
     TRY(igemm_autotile_single(d, allow_swap, plan_out));
@@ -182,7 +180,7 @@ static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_o
     auto vt_ok = [&](int bn) { return !d.epi.out2 || d.epi.col2 % bn == 0; };   // fused q/k/v: an N tile is all q/k or all v
     if (tuned && !geglu && n_gemm % 160 == 0 && total_kb >= 40 && vt_ok(160)) {
         // K-heavy contractions that cannot fill the GPU with 160-wide tiles alone (batch 1): wide tiles + cluster
-        // split-K beat 64-wide tiles (profiles/r01_tile_sweep.md: -10..-40 % per launch, weights streamed from HBM)
+        // split-K beat 64-wide tiles (weights streamed from HBM)
         d.BN = 160; d.splits = 1; d.partial = nullptr;
         TRY(igemm_plan(d, &plan));
         const int m_tiles = plan.p.tiles_w * plan.p.tiles_h * plan.p.tiles_n;
@@ -214,7 +212,7 @@ static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_o
         if (bn < 64 && n_gemm >= 64) break;  // narrow tiles re-read A too often: prefer split-K below
         d.BN = bn; d.splits = 1; d.partial = nullptr;
         TRY(igemm_plan(d, &plan));
-        if ((long)plan.grid.x * plan.grid.y >= 132) return 0;
+        if (plan.p.acc_bufs == 2 || (long)plan.grid.x * plan.grid.y >= b2_device_sms()) return 0;   // persistent = a full wave
     }
     // not enough tiles for one wave: smallest reasonable tile, then split K
     int bn = valid.back();
@@ -222,7 +220,7 @@ static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_o
     d.BN = bn; d.splits = 1; d.partial = nullptr;
     TRY(igemm_plan(d, &plan));
     const long ctas = (long)plan.grid.x * plan.grid.y;
-    int splits = ctas >= 96 ? 1 : (int)((148 + ctas - 1) / ctas);
+    int splits = ctas >= 96 ? 1 : (int)((IG_SMS + ctas - 1) / ctas);
     if (tuned && ctas >= 64 && total_kb <= 12) splits = 1;   // the cluster reduction (~3 us) costs more than 5 k-blocks
     const int max_by_k = plan.p.total_kb / 4 > 0 ? plan.p.total_kb / 4 : 1;
     if (splits > max_by_k) splits = max_by_k;
@@ -484,14 +482,11 @@ struct b2sd_engine {
         const bool geglu = (d.epi.flags & IG_GEGLU) != 0;
         const int n_gemm = geglu ? 2 * d.epi.n_valid : d.epi.n_valid;
         const bool extras = d.epi.rowstat_out || d.epi.colsum || d.epi.out2;   // not implemented by the swapped-orientation epilogue
-        // several frames in flight: a 100 KB operand ring lets CTAs of different frames share an SM (measured +5.5 % throughput
-        // at 3 lanes; one frame alone prefers the 200 KB ring on launches with <= 1 CTA per SM)
-        if (concurrency > 1 && d.ring_kb == 0) d.ring_kb = 100;
-        // ... and spreading one contraction over fewer K slices costs latency but less SM time (cluster reduction): +1.5 %
+        // several frames in flight: spreading one contraction over fewer K slices costs latency but less SM time (cluster reduction)
         if (concurrency > 1 && d.max_splits == 0) d.max_splits = 4;
         // ... and with the GPU filled by >= 4 frames, CTA pairs without split-K use the least SM time per contraction
-        // (igemm_autotile): +6.8 % at 6 lanes, +11 % at 8.  Two stage-pipelined lanes of ONE stateful stream (T > 1) run mostly
-        // one UNet at a time and keep split-K: pairs there measured -14 % (SD-1.5 4-step 512^2, profiles/ab_sd15_r02z.txt).
+        // (igemm_autotile).  Two stage-pipelined lanes of ONE stateful stream (T > 1) run mostly one UNet at a time and keep
+        // split-K.
         if (concurrency >= 4 && d.pair_auto == 0) { d.pair_auto = 1; d.pair_splits = 1; }
         IgemmPlan plan;
         TRY(igemm_autotile(d, allow_swap && !extras, &plan));
@@ -565,7 +560,7 @@ struct b2sd_engine {
         static const bool no_tconv = getenv("B2_NO_TCONV") != nullptr;
         static const char* tc_min = getenv("B2_TCONV_MIN_TILES");
         const long tiles = (long)y.n * ((y.h + TC_TH - 1) / TC_TH) * ((y.w + TC_TW - 1) / TC_TW);
-        if (!no_tconv && stride == 1 && tconv_eligible(d) && tiles >= (tc_min ? atoi(tc_min) : 2 * 148)) {
+        if (!no_tconv && stride == 1 && tconv_eligible(d) && tiles >= (tc_min ? atoi(tc_min) : 2 * IG_SMS)) {
             TconvPlan tp;
             TRY(tconv_plan(d, &tp));
             char label[256];
@@ -740,9 +735,6 @@ int b2sd_engine::build_transformer(const std::string& p, const Act& x, int heads
     // whose epilogue also accumulates the row statistics (rowstat_out); the consumer GEMM runs on the RAW rows with gamma folded
     // into its weights and applies mean / rstd in its epilogue (IgEpilogue::colsum).  B2_NO_LNFOLD=1 restores the three
     // layernorm launches + separate V^T GEMM (also used when the batch's V^T columns need per-image padding).
-    // Measured (profiles/ab_sd15_r02l.txt, ab_r02l.txt), with the consumer's colsum / bias' vectors staged in shared memory:
-    // SD-Turbo 512x512 4 lanes 380 -> 421 fps, SD-1.5 4-step 512x512 124 -> 133 fps, 768x768 50.1 -> 52.9 fps.  (A first
-    // version that read those vectors from global memory inside the per-chunk loop LOST 5 % at 16384 tokens.)
     static const bool no_fold = getenv("B2_NO_LNFOLD") != nullptr;
     static const char* fold_rows_env = getenv("B2_LNFOLD_MAX_ROWS");   // tuning: disable the fold above this many tokens
     const long fold_max_rows = fold_rows_env ? atol(fold_rows_env) : (1l << 40);
@@ -1193,8 +1185,8 @@ static int create_engine(const b2sd_config* cfg, std::shared_ptr<WeightStore> st
         b2_set_error("b2sd_create: no CUDA device (this library has no CPU path)");
         return -1;
     }
-    if (prop.major != 10) {
-        b2_set_error("b2sd_create: device sm_%d%d is not Blackwell sm_100 (kernels are sm_100a only)", prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        b2_set_error("b2sd_create: device sm_%d%d is not Hopper sm_90 (kernels are sm_90a only)", prop.major, prop.minor);
         return -1;
     }
     if (igemm_init() || attn_init() || tconv_init()) return -1;

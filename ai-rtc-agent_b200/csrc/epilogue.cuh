@@ -1,8 +1,9 @@
-// Epilogue helpers shared by the tcgen05 contraction kernels (igemm.cu, tconv.cu): accumulator row (TMEM lane = thread)
-// -> bias / scale / residual / ReLU / GEGLU -> fp16 NHWC stores.
+// Epilogue helpers shared by the wgmma contraction kernels (igemm.cu, tconv.cu): accumulator fragment (registers) or staged
+// fp32 row -> bias / scale / residual / ReLU / GEGLU -> fp16 NHWC stores.
 #pragma once
 #include "igemm.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace b2 {
 
@@ -124,190 +125,167 @@ __device__ __forceinline__ void epi_store16(const IgEpilogue& e, const T (&acc)[
     store_half16(e.out + orow * e.ldc + col0, v, nv, (e.ldc & 7) == 0);
 }
 
-// GEGLU: val/gate are 16 accumulator columns each; packed-column index of val[0] is pcol0 (bias
-// uses packed indexing), output column index is ocol0.
-__device__ __forceinline__ void epi_store16_geglu(const IgEpilogue& e, const uint32_t (&val)[16],
-                                                  const uint32_t (&gate)[16], long orow, int pcol_val,
-                                                  int pcol_gate, int ocol0, float mu = 0.f, float rstd = 1.f) {
-    float v[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-        float a = __uint_as_float(val[i]), g = __uint_as_float(gate[i]);
-        if (e.colsum) {   // folded LayerNorm (norm3) of the A rows
-            a = rstd * (a - mu * e.colsum[pcol_val + i]);
-            g = rstd * (g - mu * e.colsum[pcol_gate + i]);
-        }
-        if (e.colbias) {
-            a += e.colbias[pcol_val + i];
-            g += e.colbias[pcol_gate + i];
-        }
-        v[i] = a * gelu_erf(g);
+// Output row of the accumulator fragment (see wgmma.cuh): each thread holds two rows of its warpgroup's 64-row slab.
+struct EpiRow {
+    long orow;      // output row (pixel / token)
+    int b;          // batch item (per-item bias)
+    bool ok;        // inside the output
+    float mu, rstd; // folded LayerNorm statistics of the A row (0 / 1 when unused)
+};
+
+__device__ __forceinline__ void store_half2(__half* dst, float x0, float x1, bool two, bool vec_ok) {
+    if (two && vec_ok) {
+        *reinterpret_cast<__half2*>(dst) = __floats2half2_rn(x0, x1);
+    } else {
+        dst[0] = __float2half_rn(x0);
+        if (two) dst[1] = __float2half_rn(x1);
     }
-    store_half16(e.out + orow * e.ldc + ocol0, v, 16, (e.ldc & 7) == 0);
 }
 
-// Fast epilogue of one output row (no split-K / GEGLU; n_valid % 16 == 0, vectorisable pitches): the residual row
-// is prefetched 32 columns ahead -- the first chunk even before the accumulator is ready -- so its global-memory
-// latency hides behind the mainloop instead of being paid once per 16-column chunk.
-__device__ __forceinline__ void epi_row_fast(const IgEpilogue& e, uint32_t taddr, int ncols, int gcol0, int b, long orow,
-                                             bool row_ok, uint64_t* wait_bar, uint32_t wait_parity = 0) {
-    const bool has_res = e.res != nullptr && row_ok;
-    const __half* rp = e.res ? e.res + orow * e.ldr + gcol0 : nullptr;
-    const float* bp = e.colbias ? e.colbias + (long)b * e.colbias_bstride + gcol0 : nullptr;
-    __half* op = e.out + orow * e.ldc + gcol0;
-    uint4 rr[4];
-    float4 bb[8];
-    auto fetch = [&](int c, uint4 (&r4)[4], float4 (&b8)[8]) {   // residual + bias of columns [c, c+32)
+// Sum of this row's per-thread partial statistics over the 4 lanes that share it, then one fixed-point add per row.
+__device__ __forceinline__ void rowstat_quad(const IgEpilogue& e, const EpiRow& rw, float s1, float s2, int lane) {
+    s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
+    s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
+    s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+    s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
+    if ((lane & 3) == 0 && rw.ok) rowstat_add(e, rw.orow, s1, s2);
+}
+
+// Epilogue of one warpgroup accumulator fragment of BN columns, straight from registers (no split-K, normal orientation):
+// acc[4j + 2h + {0,1}] is row rw[h], columns gcol0 + 8j + 2 (lane % 4) + {0,1}.
+//   ln_fma: LayerNorm-folded launch with vectorisable pitches: x = rstd * acc - rstd * mu * colsum + bias'
+//   GEGLU: tile columns [0, BN/2) are values, [BN/2, BN) gates; out = v * gelu_erf(g)
+//   otherwise: bias / scale / residual / ReLU, optional row statistics and transposed V block
+template <int BN>
+__device__ __forceinline__ void epi_frag(const IgEpilogue& e, const float (&acc)[BN / 2], const EpiRow (&rw)[2], int ntile,
+                                         bool ln_fma, int lane) {
+    const int q2 = 2 * (lane & 3);
+    const bool vec_out = (e.ldc & 1) == 0;
+    if (e.flags & IG_GEGLU) {
+        constexpr int HALF = BN / 2;
+        const int pv0 = ntile * BN, oc0 = ntile * HALF;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) r4[i] = make_uint4(0, 0, 0, 0);
+        for (int j = 0; j < HALF / 8; ++j) {
+            const int c = 8 * j + q2;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) b8[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (c >= ncols) return;
-        if (has_res) {
+            for (int h = 0; h < 2; ++h) {
+                if (!rw[h].ok) continue;
+                float v[2];
 #pragma unroll
-            for (int i = 0; i < 4; ++i)
-                if (c + 8 * i < ncols) r4[i] = reinterpret_cast<const uint4*>(rp + c)[i];
-        }
-        if (bp) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-                if (c + 4 * i < ncols) b8[i] = reinterpret_cast<const float4*>(bp + c)[i];
-        }
-    };
-    float st1 = 0.f, st2 = 0.f;
-    fetch(0, rr, bb);
-    if (wait_bar) {
-        mbar_wait(wait_bar, wait_parity);
-        tc_fence_after();
-    }
-    for (int c = 0; c < ncols; c += 32) {
-        const int left = ncols - c;   // >= 16, multiple of 16
-        uint32_t v[32];
-        if (left >= 32) {
-            tmem_ld32(taddr + c, v);
-        } else {
-            uint32_t lo[16];
-            tmem_ld16(taddr + c, lo);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) { v[i] = lo[i]; v[16 + i] = 0; }
-        }
-        uint4 rn[4];
-        float4 bn[8];
-        fetch(c + 32, rn, bn);   // next pass: latency hides behind this pass
-        tmem_ld_wait();
-        if (row_ok) {
-            const float* bias = reinterpret_cast<const float*>(bb);
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {   // 8 columns per 16-byte store
-                if (8 * g < left) {
-                    const __half2* rh = reinterpret_cast<const __half2*>(&rr[g]);
-                    uint4 o;
-                    __half2* oh = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const int i = 8 * g + 2 * j;
-                        float x0 = (__uint_as_float(v[i]) + bias[i]) * e.acc_scale;
-                        float x1 = (__uint_as_float(v[i + 1]) + bias[i + 1]) * e.acc_scale;
-                        if (e.res) {
-                            const float2 f = __half22float2(rh[j]);
-                            x0 += e.res_scale * f.x;
-                            x1 += e.res_scale * f.y;
+                for (int u = 0; u < 2; ++u) {
+                    float a = acc[4 * j + 2 * h + u], g = acc[4 * (j + HALF / 8) + 2 * h + u];
+                    const int pv = pv0 + c + u, pg = pv0 + HALF + c + u;
+                    if (ln_fma) {
+                        const float nmr = -rw[h].mu * rw[h].rstd;
+                        a = fmaf(rw[h].rstd, a, fmaf(nmr, e.colsum[pv], e.colbias ? e.colbias[pv] : 0.f));
+                        g = fmaf(rw[h].rstd, g, fmaf(nmr, e.colsum[pg], e.colbias ? e.colbias[pg] : 0.f));
+                    } else {
+                        if (e.colsum) {
+                            a = rw[h].rstd * (a - rw[h].mu * e.colsum[pv]);
+                            g = rw[h].rstd * (g - rw[h].mu * e.colsum[pg]);
                         }
-                        if (e.flags & IG_RELU) {
-                            x0 = fmaxf(x0, 0.f);
-                            x1 = fmaxf(x1, 0.f);
-                        }
-                        oh[j] = __floats2half2_rn(x0, x1);
-                        if (e.rowstat_out) {   // LayerNorm statistics of the stored (fp16-rounded) row
-                            const float2 f = __half22float2(oh[j]);
-                            st1 += f.x + f.y;
-                            st2 += f.x * f.x + f.y * f.y;
+                        if (e.colbias) {
+                            a += e.colbias[pv];
+                            g += e.colbias[pg];
                         }
                     }
-                    reinterpret_cast<uint4*>(op + c)[g] = o;
+                    v[u] = a * gelu_erf(g);
+                }
+                store_half2(e.out + rw[h].orow * e.ldc + oc0 + c, v[0], v[1], true, vec_out);
+            }
+        }
+        return;
+    }
+    float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+        const int col = ntile * BN + 8 * j + q2;
+        if (col >= e.n_valid) continue;
+        const bool two = col + 1 < e.n_valid;
+        const bool transposed = e.out2 && col >= e.col2;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            if (!rw[h].ok) continue;
+            float x[2] = {acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]};
+            const float* bp = e.colbias ? e.colbias + (long)rw[h].b * e.colbias_bstride + col : nullptr;
+            if (ln_fma) {
+                const float nmr = -rw[h].mu * rw[h].rstd;
+#pragma unroll
+                for (int u = 0; u < 2; ++u)
+                    x[u] = fmaf(rw[h].rstd, x[u], fmaf(nmr, e.colsum[col + u], bp && (u == 0 || two) ? bp[u] : 0.f));
+            } else {
+                if (e.colsum) {
+#pragma unroll
+                    for (int u = 0; u < 2; ++u)
+                        if (u == 0 || two) x[u] = rw[h].rstd * (x[u] - rw[h].mu * e.colsum[col + u]);
+                }
+                if (bp) {
+                    x[0] += bp[0];
+                    if (two) x[1] += bp[1];
+                }
+                if (e.acc_scale != 1.0f) {
+                    x[0] *= e.acc_scale;
+                    x[1] *= e.acc_scale;
+                }
+                if (e.res) {
+                    const __half* rp = e.res + rw[h].orow * e.ldr + col;
+                    if (two && (e.ldr & 1) == 0) {
+                        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(rp));
+                        x[0] += e.res_scale * f.x;
+                        x[1] += e.res_scale * f.y;
+                    } else {
+                        x[0] += e.res_scale * __half2float(rp[0]);
+                        if (two) x[1] += e.res_scale * __half2float(rp[1]);
+                    }
+                }
+                if (e.flags & IG_RELU) {
+                    x[0] = fmaxf(x[0], 0.f);
+                    x[1] = fmaxf(x[1], 0.f);
                 }
             }
+            if (transposed) {   // V block of the fused q/k/v projection -> V^T
+                __half* tp = e.out2 + (long)(col - e.col2) * e.ld2 + rw[h].orow;
+                tp[0] = __float2half_rn(x[0]);
+                if (two) tp[e.ld2] = __float2half_rn(x[1]);
+                continue;
+            }
+            if (e.rowstat_out && !ln_fma) {   // statistics of the values as stored (fp16-rounded)
+                const float r0 = __half2float(__float2half_rn(x[0]));
+                const float r1 = two ? __half2float(__float2half_rn(x[1])) : 0.f;
+                s1[h] += r0 + r1;
+                s2[h] += r0 * r0 + r1 * r1;
+            }
+            store_half2(e.out + rw[h].orow * e.ldc + col, x[0], x[1], two, vec_out);
         }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) rr[i] = rn[i];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) bb[i] = bn[i];
     }
-    if (e.rowstat_out && row_ok && ncols > 0) rowstat_add(e, orow, st1, st2);
+    if (e.rowstat_out && !ln_fma) {
+        rowstat_quad(e, rw[0], s1[0], s2[0], lane);
+        rowstat_quad(e, rw[1], s1[1], s2[1], lane);
+    }
 }
 
-// LayerNorm-folded epilogue of one output row (non-split, see IgEpilogue::colsum): the tile's colsum / bias' vectors were
-// staged in shared memory (`lnv`: [ncols_tile] colsum, then [ncols_tile] bias') while the mainloop ran, so the per-chunk loop
-// has no global-memory loads on its critical path.  c_tile0 = first column of this call inside the staged tile.
-__device__ __forceinline__ void epi_row_ln(const IgEpilogue& e, uint32_t taddr, int ncols, int gcol0, long orow, bool row_ok,
-                                           const float* lnv, int tile_cols, float mu, float rstd) {
-    const float* cs = lnv;
-    const float* bb = lnv + tile_cols;
-    const float nmr = -mu * rstd;
-    for (int c = 0; c < ncols; c += 32) {
-        const int left = ncols - c;
-        uint32_t v[32];
-        if (left >= 32) {
-            tmem_ld32(taddr + c, v);
-        } else {
-            uint32_t lo[16];
-            tmem_ld16(taddr + c, lo);
+// Fragment -> fp32 tile in shared memory laid out [4-column group][128 rows] float4 (split-K partials: conflict-free for the
+// peers' DSMEM reads), or [column][128 rows] when `colmajor` (swapped orientation: rows are output channels, columns pixels).
+// r0 = this thread's first row inside the 128-row tile; only columns [c0, c0 + NC) of the fragment are written, at c - c0.
+template <int BN>
+__device__ __forceinline__ void frag_to_smem(float* dst, const float (&acc)[BN / 2], int r0, int lane, int c0, int nc, bool colmajor) {
+    const int q2 = 2 * (lane & 3);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) { v[i] = lo[i]; v[16 + i] = 0; }
-        }
-        tmem_ld_wait();
-        if (!row_ok) continue;
-        const bool transposed = e.out2 && gcol0 + c >= e.col2;
+    for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + q2 - c0;
+        if (c < 0 || c >= nc) continue;
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-            if (8 * g >= left) break;
-            float x[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const int i = 8 * g + j;
-                x[j] = fmaf(rstd, __uint_as_float(v[i]), fmaf(nmr, cs[c + i], bb[c + i]));   // rstd*acc - rstd*mu*colsum + bias'
-            }
-            if (transposed) {   // V block of the fused q/k/v projection -> V^T (32 lanes = 32 consecutive tokens)
-                __half* tp = e.out2 + (long)(gcol0 + c + 8 * g - e.col2) * e.ld2 + orow;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) tp[(long)j * e.ld2] = __float2half_rn(x[j]);
+        for (int h = 0; h < 2; ++h) {
+            const int r = r0 + 8 * h;
+            if (colmajor) {
+                dst[c * 128 + r] = acc[4 * j + 2 * h];
+                dst[(c + 1) * 128 + r] = acc[4 * j + 2 * h + 1];
             } else {
-                uint4 o;
-                __half2* oh = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) oh[j] = __floats2half2_rn(x[2 * j], x[2 * j + 1]);
-                *reinterpret_cast<uint4*>(e.out + orow * e.ldc + gcol0 + c + 8 * g) = o;
+                *reinterpret_cast<float2*>(dst + (((c >> 2) * 128 + r) << 2) + (c & 3)) =
+                    make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
             }
         }
     }
-}
-
-// GEGLU with the LayerNorm (norm3) folded: value columns [0, half_n), gate columns [half_n, 2*half_n) of the tile
-__device__ __forceinline__ void epi_row_geglu_ln(const IgEpilogue& e, uint32_t taddr, int half_n, int ocol0, long orow, bool row_ok,
-                                                 const float* lnv, int tile_cols, float mu, float rstd) {
-    const float* cs = lnv;
-    const float* bb = lnv + tile_cols;
-    const float nmr = -mu * rstd;
-    for (int c = 0; c < half_n; c += 16) {
-        uint32_t a[16], g[16];
-        tmem_ld16(taddr + c, a);
-        tmem_ld16(taddr + half_n + c, g);
-        tmem_ld_wait();
-        if (!row_ok) continue;
-        float v[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            const float av = fmaf(rstd, __uint_as_float(a[i]), fmaf(nmr, cs[c + i], bb[c + i]));
-            const float gv = fmaf(rstd, __uint_as_float(g[i]), fmaf(nmr, cs[half_n + c + i], bb[half_n + c + i]));
-            v[i] = av * gelu_erf(gv);
-        }
-        store_half16(e.out + orow * e.ldc + ocol0 + c, v, 16, (e.ldc & 7) == 0);
-    }
-}
-
-__device__ __forceinline__ bool epi_fast_ok(const IgEpilogue& e) {
-    return !(e.flags & (IG_SPLITK | IG_GEGLU)) && (e.n_valid & 15) == 0 && (e.ldc & 7) == 0 && (!e.res || (e.ldr & 7) == 0) &&
-           (e.colbias_bstride & 3) == 0 && !e.colsum && !e.out2;
 }
 
 }  // namespace b2

@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM kernel + host-side plan builder. See igemm.cuh for the design.
+// wgmma implicit-GEMM kernel + host-side plan builder. See igemm.cuh for the design.
 #include "igemm.cuh"
 
 #include <cudaTypedefs.h>
@@ -31,21 +31,22 @@ void b2_set_error(const char* fmt, ...) {
     va_end(ap);
 }
 
-// Swapped orientation: an accumulator row (TMEM lane, thread) is an output CHANNEL, its columns are the pixels of the
-// tile, so the NHWC store needs a transpose.  It goes through a small fp32 shared-memory tile T[pixel][128 channels]:
-// thread r parks its channel's values for a chunk of <= 32 pixels (conflict-free 4-byte stores), then the 128 epilogue
-// threads sweep T row-wise: one thread = 8 consecutive channels of one pixel (16-byte residual load, 16-byte store), a
-// warp = two complete 256-byte pixel rows.  Bias, scale, residual and ReLU are applied in that coalesced sweep.
-constexpr int SWAP_CH = 32;   // pixels per transposition chunk (T = 32 x 128 fp32 = 16 KB)
+// Swapped orientation: an accumulator row is an output CHANNEL, its columns are the pixels of the tile, so the NHWC store
+// needs a transpose.  It goes through a small fp32 shared-memory tile T[pixel][128 channels]: the consumer warpgroups park a
+// chunk of <= 32 pixels of their fragments there, then the 256 consumer threads sweep T row-wise: one thread = 8 consecutive
+// channels of one pixel (16-byte residual load, 16-byte store), a warp = two complete 256-byte pixel rows.  Bias, scale,
+// residual and ReLU are applied in that coalesced sweep.
+constexpr int SWAP_CH = 32;                        // pixels per transposition chunk (T = 32 x 128 fp32 = 16 KB)
+constexpr int SWAP_ITEMS = SWAP_CH * 16 / IG_CONS;   // (pixel, 8-channel) items per consumer thread and chunk
 
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+__device__ __forceinline__ void cons_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(IG_CONS) : "memory"); }
 
 // What one thread needs from global memory for its (pixel, 8-channel) items of a chunk: fetched BEFORE the
-// transposition barrier so the latency overlaps the TMEM/DSMEM reads that fill T.
+// transposition barrier so the latency overlaps the fills of T.
 struct SwapPre {
-    uint4 res[SWAP_CH / 8];
-    float4 b0[SWAP_CH / 8], b1[SWAP_CH / 8];
-    long orow[SWAP_CH / 8];      // < 0: nothing to store
+    uint4 res[SWAP_ITEMS];
+    float4 b0[SWAP_ITEMS], b1[SWAP_ITEMS];
+    long orow[SWAP_ITEMS];      // < 0: nothing to store
 };
 
 __device__ __forceinline__ void swap_prefetch(const IgemmParams& p, SwapPre& pre, int npix, int j0, int ntile, int n0, int h0,
@@ -53,8 +54,8 @@ __device__ __forceinline__ void swap_prefetch(const IgemmParams& p, SwapPre& pre
     const IgEpilogue& e = p.epi;
     const int tw = 1 << p.tw_log2, th = 1 << p.th_log2;
 #pragma unroll
-    for (int k = 0; k < SWAP_CH / 8; ++k) {
-        const int item = t + 128 * k;
+    for (int k = 0; k < SWAP_ITEMS; ++k) {
+        const int item = t + IG_CONS * k;
         pre.orow[k] = -1;
         pre.res[k] = make_uint4(0, 0, 0, 0);
         pre.b0[k] = pre.b1[k] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -81,9 +82,9 @@ __device__ __forceinline__ void swap_prefetch(const IgemmParams& p, SwapPre& pre
 __device__ __forceinline__ void swap_store_chunk(const IgemmParams& p, const SwapPre& pre, const float* T, int ntile, int t) {
     const IgEpilogue& e = p.epi;
 #pragma unroll
-    for (int k = 0; k < SWAP_CH / 8; ++k) {
+    for (int k = 0; k < SWAP_ITEMS; ++k) {
         if (pre.orow[k] < 0) continue;
-        const int item = t + 128 * k;
+        const int item = t + IG_CONS * k;
         const int pl = item >> 4, q = item & 15;
         const int cout0 = ntile * IG_BM + q * 8;
         const float4 a0 = *reinterpret_cast<const float4*>(T + pl * IG_BM + q * 8);
@@ -116,7 +117,7 @@ __device__ __forceinline__ void swap_store_chunk(const IgemmParams& p, const Swa
 // Cluster split-K: sum one 16-column (4 x float4) strip of accumulator row `row` over the K slices held in the peers'
 // shared memory.  All loads of up to four slices are in flight together (a dependent chain of DSMEM round trips was
 // the dominant cost of the reduction); the summation order is fixed => bit-reproducible.
-// (pair launches: cluster dims (2,1,splits), the K slice s of this CTA's M half lives in cluster rank 2*s + rank_add)
+// (pair launches: cluster dims (2,1,splits), the K slice s of this CTA's M tile lives in cluster rank 2*s + rank_add)
 template <int SPL>
 __device__ __forceinline__ void splitk_sum16(uint32_t stg_local, int cc, int row, float (&acc)[16], int rank_mul = 1, int rank_add = 0) {
 #pragma unroll
@@ -141,32 +142,32 @@ __device__ __forceinline__ void splitk_sum16(uint32_t stg_local, int cc, int row
 }
 
 // ------------------------------------------------------------------------------------------
-// PAIR: the CTAs (2j, 2j+1) of grid.x form a CTA pair (cluster dims (2,1,splits)) that computes two neighbouring M tiles with
-// ONE tcgen05.mma.cta_group::2 stream of M = 256: each CTA loads its own 128 pixel rows and half of the weight tile, the even
-// CTA issues the MMAs for both, every CTA drains its own 128 accumulator rows.  Barrier plumbing across the pair: the odd
-// CTA's (otherwise idle) MMA warp relays "my operands of this stage have landed" to the leader; ring slots are released in both
-// CTAs by a multicast commit; both epilogues arrive on the leader's accumulator-drained barrier.
-template <bool PAIR>
+// Warp roles: warps 0-3 and 4-7 are the two consumer warpgroups (accumulator rows [0,64) and [64,128) of the tile, wgmma
+// M = 64 each, the fp32 accumulator lives in their registers), warp 8 lane 0 is the TMA producer.  The consumers run the
+// epilogue of a tile straight from their registers, so a persistent CTA's next mainloop starts after that epilogue; the
+// producer meanwhile fills the ring for the next tile.
+//
+// PAIR: the CTAs (2j, 2j+1) of grid.x form a cluster pair (cluster dims (2,1,splits)) that computes two neighbouring M tiles
+// with the same weight tile: each CTA loads its own 128 pixel rows and HALF of the weight rows, multicast into both CTAs'
+// shared memory, so each SM fetches half of the weight bytes from L2.  A ring slot is refilled only when the warps of BOTH
+// CTAs have released it (every consumer warp arrives on its own and on the peer's empty barrier).
+template <int BN, bool PAIR>
 __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                                ~static_cast<uintptr_t>(1023));
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const uint32_t stage_bytes = IG_BM * IG_BK * 2 + (uint32_t)(PAIR ? p.BN / 2 : p.BN) * IG_BK * 2;
+    constexpr uint32_t A_BYTES = IG_BM * IG_BK * 2;
+    constexpr uint32_t stage_bytes = A_BYTES + (uint32_t)BN * IG_BK * 2;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.num_stages * stage_bytes);
     uint64_t* empty_bar = full_bar + IG_MAX_STAGES;
-    uint64_t* tmem_full_bar = empty_bar + IG_MAX_STAGES;   // [2] accumulator ready   (MMA -> epilogue)
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;          // [2] accumulator drained (epilogue -> MMA)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-    uint64_t* peer_full = full_bar + 32;                   // [stages] (pair leader) the peer CTA's operands have landed
-    const int cr = PAIR ? (int)(blockIdx.x & 1) : 0;       // rank inside the CTA pair (0 = leader)
-    const int mt_first = PAIR ? (int)(blockIdx.x & ~1u) + cr : (int)blockIdx.x;   // first M tile of this CTA ...
+    const int cr = PAIR ? (int)(blockIdx.x & 1) : 0;       // rank inside the CTA pair
+    const int mt_first = (int)blockIdx.x;                  // first M tile of this CTA ...
     const int mt_step = (int)gridDim.x;                    // ... and the stride of a persistent launch (even for pairs)
-    const int mt_guard = PAIR ? cr : 0;                    // pairs iterate together: the loop bound looks at the leader's tile
+    const int mt_guard = PAIR ? cr : 0;                    // pairs iterate together: the loop bound looks at the even CTA's tile
 
-    // Persistent over M tiles: CTA x handles tiles x, x + gridDim.x, ... with two TMEM accumulators, so the epilogue of
-    // tile i overlaps the mainloop of tile i+1 and the prologue (barriers, TMEM, descriptors) is paid once per CTA.
+    // Persistent over M tiles: CTA x handles tiles x, x + gridDim.x, ...; the prologue (barriers, descriptors) is paid once.
     const int num_mtiles = p.tiles_w * p.tiles_h * p.tiles_n;
     const int ntile = blockIdx.y;
     const int kb_begin = blockIdx.z * p.kb_per_split;
@@ -174,46 +175,29 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
     [[maybe_unused]] unsigned long long* ts = p.dbg_ts ? p.dbg_ts + ((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 8 : nullptr;
     B2_TS(if (ts && threadIdx.x == 0) ts[0] = globaltimer_ns();)
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == IG_CONS) {
         for (int s = 0; s < p.nseg; ++s) tma_prefetch_desc(&p.tmA[s]);
         tma_prefetch_desc(&p.tmB);
         for (int s = 0; s < p.num_stages; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-            if (PAIR) mbar_init(&peer_full[s], 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(&tmem_full_bar[s], 1);
-            mbar_init(&tmem_empty_bar[s], PAIR ? 256 : 128);
+            mbar_init(&empty_bar[s], (PAIR ? 2 : 1) * (IG_CONS / 32));   // one arrival per consumer warp (of both CTAs)
         }
         fence_mbar_init();
     }
-    if (PAIR) {   // the peer's barriers exist before anything arrives on them; both CTAs are resident (execution barrier only:
-        cluster_arrive_relaxed();   // the release/acquire form costs a MEMBAR.ALL.GPU + L1 invalidate)
+    if (PAIR) {   // the peer's barriers exist before anything arrives on them (execution barrier only: the release/acquire form
+        cluster_arrive_relaxed();   // costs a MEMBAR.ALL.GPU + L1 invalidate)
         cluster_wait();
     }
-    if (warp == 1) {
-        if (PAIR) {
-            tmem_alloc_2cta(tmem_slot, p.tmem_cols);
-            tmem_relinquish_2cta();
-        } else {
-            tmem_alloc(tmem_slot, p.tmem_cols);
-            tmem_relinquish();
-        }
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     pdl_launch_dependents();   // the next kernel may start its own prologue now
     pdl_wait();                // ... and everything below reads the previous kernel's output
     B2_TS(if (ts && threadIdx.x == 0) ts[1] = globaltimer_ns();)
-    const uint32_t acc_stride = p.acc_bufs > 1 ? (uint32_t)p.BN : 0u;   // column offset of the second accumulator
 
-    if (warp == 0) {
+    if (warp == IG_CONS / 32) {
         if (lane == 0) {
             // ===== TMA producer =====
+            [[maybe_unused]] const uint16_t pair_mask = PAIR ? (uint16_t)(3u << (cluster_ctarank() & ~1u)) : (uint16_t)0;
             int stage = 0;
             uint32_t phase = 0;
             for (int mt = mt_first; mt - mt_guard < num_mtiles; mt += mt_step) {
@@ -237,7 +221,7 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
 #endif
                     mbar_expect_tx(&full_bar[stage], p.a_bytes + p.b_bytes);
                     uint8_t* sa = smem + (size_t)stage * stage_bytes;
-                    uint8_t* sb = sa + IG_BM * IG_BK * 2;
+                    uint8_t* sb = sa + A_BYTES;
                     int dy = 0, dx = 0;
                     if (p.seg_ntap[seg] == 9) {
                         dy = tap / 3 - 1;
@@ -246,8 +230,10 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
                     // normal: pixels -> A (M side), weights -> B.  swapped: weights (128 output channels) -> A, pixels -> B
                     tma_load_4d(p.swap ? sb : sa, &p.tmA[seg], &full_bar[stage], p.seg_c0[seg] + cb * IG_BK,
                                 w0 * p.stride + dx, h0 * p.stride + dy, n0);
-                    tma_load_2d(p.swap ? sa : sb, &p.tmB, &full_bar[stage], kb * IG_BK,
-                                ntile * (p.swap ? IG_BM : p.BN) + (PAIR ? cr * (p.BN / 2) : 0));
+                    if (PAIR)
+                        tma_load_2d_mc(sb + cr * (BN / 2) * 128, &p.tmB, &full_bar[stage], kb * IG_BK, ntile * BN + cr * (BN / 2), pair_mask);
+                    else
+                        tma_load_2d(p.swap ? sa : sb, &p.tmB, &full_bar[stage], kb * IG_BK, ntile * (p.swap ? IG_BM : BN));
                     B2_TS(if (ts && mt == (int)blockIdx.x && kb == kb_begin) ts[2] = globaltimer_ns();)
                     if (++cb == p.seg_cblocks[seg]) {
                         cb = 0;
@@ -263,243 +249,123 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
                 }
             }
         }
-    } else if (warp == 1 && PAIR && cr == 1) {
-        // ===== pair follower: relay "operands of this stage have landed in MY shared memory" to the leader =====
-        const uint32_t leader_peer_full = dsmem_map(smem_u32(peer_full), cluster_ctarank() & ~1u);
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int mt = mt_first; mt - mt_guard < num_mtiles; mt += mt_step) {
-            for (int kb = kb_begin; kb < kb_end; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                if (elect_one()) mbar_arrive_remote(leader_peer_full + (uint32_t)stage * 8u);
-                __syncwarp();
-                if (++stage == p.num_stages) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        // The whole warp walks the loop (warp-uniform control flow keeps descriptors in uniform registers, which is
-        // what UTCHMMA consumes); one elected lane issues.  A divergent single-thread loop issues ~2.5x slower
-        // (probe.cu / tools/probe_rowshift.py).
-        const uint32_t idesc = make_idesc_f16(PAIR ? 2 * IG_BM : IG_BM, p.BN);
-        const uint32_t smem_base = smem_u32(smem);
-        [[maybe_unused]] const uint16_t pair_mask = (uint16_t)(3u << (cluster_ctarank() & ~1u));
-        int stage = 0;
-        uint32_t phase = 0;
-        int it = 0;
-        for (int mt = mt_first; mt < num_mtiles; mt += mt_step, ++it) {
-            const int buf = it & 1;
-            // epilogue has drained this accumulator (pairs: both CTAs' epilogues arrive here)
-            mbar_wait(&tmem_empty_bar[buf], ((it >> 1) & 1) ^ 1);
-            tc_fence_after();
-            const uint32_t tacc = tmem_base + (uint32_t)buf * acc_stride;
-            for (int kb = kb_begin; kb < kb_end; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                if (PAIR) mbar_wait(&peer_full[stage], phase);
-                tc_fence_after();
-                B2_TS(if (ts && it == 0 && kb == kb_begin && lane == 0) ts[3] = globaltimer_ns();)
-                const uint32_t sa = smem_base + (uint32_t)stage * stage_bytes;
-                const uint64_t da = make_kmajor_sw128_desc(sa);
-                const uint64_t db = make_kmajor_sw128_desc(sa + IG_BM * IG_BK * 2);
-                const uint32_t acc0 = kb > kb_begin ? 1u : 0u;
-#ifdef B2_BOUND_STUDY
-                if (p.dbg_mode == 2) {
-                    if (elect_one()) umma_commit(&empty_bar[stage]);
-                } else
-#endif
-                if (elect_one()) {
-                    // +32 B per UMMA_K inside the 128 B swizzle row => +2 in the (addr>>4) field
-                    if (PAIR) {
-                        umma_f16_2cta(tacc, da, db, idesc, acc0);
-                        umma_f16_2cta(tacc, da + 2, db + 2, idesc, 1u);
-                        umma_f16_2cta(tacc, da + 4, db + 4, idesc, 1u);
-                        umma_f16_2cta(tacc, da + 6, db + 6, idesc, 1u);
-                        umma_commit_2cta(&empty_bar[stage], pair_mask);  // frees the slot in BOTH CTAs
-                    } else {
-                        umma_f16(tacc, da, db, idesc, acc0);
-                        umma_f16(tacc, da + 2, db + 2, idesc, 1u);
-                        umma_f16(tacc, da + 4, db + 4, idesc, 1u);
-                        umma_f16(tacc, da + 6, db + 6, idesc, 1u);
-                        umma_commit(&empty_bar[stage]);  // frees the smem slot when these MMAs retire
-                    }
-                }
-                __syncwarp();
-                if (++stage == p.num_stages) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-            if (elect_one()) {
-                if (PAIR) umma_commit_2cta(&tmem_full_bar[buf], pair_mask);
-                else umma_commit(&tmem_full_bar[buf]);
-            }
-            __syncwarp();
-            B2_TS(if (ts && it == 0 && lane == 0) ts[4] = globaltimer_ns();)
-        }
     } else {
-        // ===== epilogue: TMEM -> registers -> global =====
-        const int q = warp & 3;  // TMEM lane quarter this warp may access
-        const int r = q * 32 + lane;
-        const int wi = r % p.tw;
-        const int hi = (r / p.tw) % p.th;
-        const int ni = r / (p.tw * p.th);
+        // ===== consumer warpgroups: wgmma mainloop, then the epilogue from registers =====
+        const int wg = warp >> 2;                                   // accumulator rows [64 wg, 64 wg + 64) of the tile
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // this thread's rows: r0 and r0 + 8
+        [[maybe_unused]] const uint32_t peer_empty = PAIR ? dsmem_map(smem_u32(empty_bar), cluster_ctarank() ^ 1u) : 0u;
         const IgEpilogue& e = p.epi;
-        // LayerNorm-folded launches: stage this N tile's colsum / bias' in shared memory while the mainloop runs
-        const bool ln_smem = e.colsum && !p.swap && !(e.flags & IG_SPLITK) && (e.ldc & 7) == 0 && (e.n_valid & 15) == 0;
-        float* lnv = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 512);
-        if (ln_smem) {
-            for (int i = threadIdx.x - 64; i < p.BN; i += 128) {
-                const int gc = ntile * p.BN + i;
-                const bool in = gc < ((e.flags & IG_GEGLU) ? 2 * e.n_valid : e.n_valid);
-                lnv[i] = in ? e.colsum[gc] : 0.f;
-                lnv[p.BN + i] = (in && e.colbias) ? e.colbias[gc] : 0.f;
+        const bool ln_fma = e.colsum && !p.swap && !(e.flags & IG_SPLITK) && (e.ldc & 7) == 0 && (e.n_valid & 15) == 0;
+        const uint32_t smem_base = smem_u32(smem);
+        auto release = [&](int s) {   // this warp's reads of ring slot s have retired
+            if (lane == 0) {
+                mbar_arrive(&empty_bar[s]);
+                if (PAIR) mbar_arrive_remote(peer_empty + (uint32_t)s * 8u);
             }
-            epi_bar_sync();
-        }
-        [[maybe_unused]] const uint32_t leader_tmem_empty = PAIR ? dsmem_map(smem_u32(tmem_empty_bar), cluster_ctarank() & ~1u) : 0u;
+        };
+        int stage = 0;
+        uint32_t phase = 0;
         int it = 0;
         for (int mt = mt_first; mt - mt_guard < num_mtiles; mt += mt_step, ++it) {
-            const int buf = it & 1;
-            const uint32_t par = (it >> 1) & 1;
-            const int w0 = (mt % p.tiles_w) * p.tw, h0 = ((mt / p.tiles_w) % p.tiles_h) * p.th;
-            const int n0 = (mt / (p.tiles_w * p.tiles_h)) * p.tn;
-            const int n = n0 + ni, h = h0 + hi, w = w0 + wi;
-            const bool row_ok = (ni < p.tn) && (n < p.Nb) && (h < p.Ho) && (w < p.Wo);
-            const long orow = ((long)n * p.Ho + h) * p.Wo + w;
-            const uint32_t taddr = tmem_base + (uint32_t)buf * acc_stride + ((uint32_t)(q * 32) << 16);
-            if (p.swap) {
-                mbar_wait(&tmem_full_bar[buf], par);
-                tc_fence_after();
-                if (e.flags & IG_SPLITK) {
-                    float4* stg = reinterpret_cast<float4*>(smem);
-                    for (int c = 0; c < p.BN; c += 16) {
-                        uint32_t v[16];
-                        tmem_ld16(taddr + c, v);
-                        tmem_ld_wait();
+            float acc[BN / 2];
 #pragma unroll
-                        for (int i = 0; i < 4; ++i)
-                            stg[((c >> 2) + i) * IG_BM + r] = make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]),
-                                                                          __uint_as_float(v[4 * i + 2]), __uint_as_float(v[4 * i + 3]));
-                    }
-                } else {
-                    // the operand ring is idle (every MMA has retired): use its head as the transposition tile
-                    float* T = reinterpret_cast<float*>(smem);
-                    for (int c = 0; c < p.BN; c += SWAP_CH) {
-                        SwapPre pre;
-                        swap_prefetch(p, pre, SWAP_CH, c, ntile, n0, h0, w0, r);
-                        uint32_t v[32];
-                        tmem_ld32(taddr + c, v);
-                        tmem_ld_wait();
+            for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+            int prev = -1;
+            for (int kb = kb_begin; kb < kb_end; ++kb) {
+                mbar_wait(&full_bar[stage], phase);
+                B2_TS(if (ts && it == 0 && kb == kb_begin && threadIdx.x == 0) ts[3] = globaltimer_ns();)
+                const uint32_t sa = smem_base + (uint32_t)stage * stage_bytes;
+                const uint64_t da = make_kmajor_sw128_desc(sa + (uint32_t)wg * (64 * 128));
+                const uint64_t db = make_kmajor_sw128_desc(sa + A_BYTES);
+#ifdef B2_BOUND_STUDY
+                if (p.dbg_mode != 2)
+#endif
+                {
+                    wgmma_fence_regs(acc);
+                    wgmma_fence();
+                    // +32 B per K = 16 step inside the 128 B swizzle row => +2 in the (addr >> 4) field
 #pragma unroll
-                        for (int i = 0; i < 32; ++i) T[i * IG_BM + r] = __uint_as_float(v[i]);
-                        epi_bar_sync();
-                        swap_store_chunk(p, pre, T, ntile, r);
-                        epi_bar_sync();
-                    }
+                    for (int k = 0; k < 4; ++k) Wgmma<BN>::ss(acc, da + 2 * k, db + 2 * k, 1u);
+                    wgmma_commit();
+                    wgmma_wait<1>();   // the previous K-block's MMAs have retired: its slot may be refilled
+                    wgmma_fence_regs(acc);
                 }
-            } else if (ln_smem) {
-                float mu, rstd;
-                ln_row_stats(e, orow, row_ok, mu, rstd);     // global loads: in flight while the accumulator completes
-                mbar_wait(&tmem_full_bar[buf], par);
-                tc_fence_after();
-                if (e.flags & IG_GEGLU) {
-                    epi_row_geglu_ln(e, taddr, p.BN / 2, ntile * (p.BN / 2), orow, row_ok, lnv, p.BN, mu, rstd);
-                } else {
-                    int ncols = e.n_valid - ntile * p.BN;
-                    if (ncols > p.BN) ncols = p.BN;
-                    epi_row_ln(e, taddr, ncols, ntile * p.BN, orow, row_ok && ncols > 0, lnv, p.BN, mu, rstd);
-                }
-            } else if (epi_fast_ok(e)) {
-                int ncols = e.n_valid - ntile * p.BN;
-                if (ncols > p.BN) ncols = p.BN;
-                epi_row_fast(e, taddr, ncols, ntile * p.BN, n, orow, row_ok && ncols > 0, &tmem_full_bar[buf], par);
-            } else {
-                mbar_wait(&tmem_full_bar[buf], par);
-                tc_fence_after();
-                if (e.flags & IG_SPLITK) {
-                    // Split-K inside a thread-block cluster (one CTA per K slice, cluster dims (1,1,splits)): every CTA
-                    // parks its fp32 partial tile in its own shared memory, laid out [4-column group][row] so that both
-                    // these stores and the peers' DSMEM reads are conflict-free; the reduction happens after the cluster
-                    // barrier below.
-                    float4* stg = reinterpret_cast<float4*>(smem);
-                    for (int c = 0; c < p.BN; c += 16) {
-                        uint32_t v[16];
-                        tmem_ld16(taddr + c, v);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 4; ++i)
-                            stg[((c >> 2) + i) * IG_BM + r] = make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]),
-                                                                          __uint_as_float(v[4 * i + 2]), __uint_as_float(v[4 * i + 3]));
-                    }
-                } else if (e.flags & IG_GEGLU) {
-                    const int half_n = p.BN / 2;
-                    float mu, rstd;
-                    ln_row_stats(e, orow, row_ok, mu, rstd);
-                    for (int c = 0; c < half_n; c += 16) {
-                        uint32_t a[16], g[16];
-                        tmem_ld16(taddr + c, a);
-                        tmem_ld16(taddr + half_n + c, g);
-                        tmem_ld_wait();
-                        if (row_ok)
-                            epi_store16_geglu(e, a, g, orow, ntile * p.BN + c, ntile * p.BN + half_n + c, ntile * half_n + c, mu, rstd);
-                    }
-                } else {
-                    float mu, rstd;
-                    ln_row_stats(e, orow, row_ok, mu, rstd);
-                    for (int c = 0; c + 32 <= p.BN; c += 32) {
-                        uint32_t v[32];
-                        tmem_ld32(taddr + c, v);
-                        tmem_ld_wait();
-                        if (row_ok) {
-                            epi_store16<0>(e, v, n, orow, ntile * p.BN + c, mu, rstd);
-                            epi_store16<16>(e, v, n, orow, ntile * p.BN + c + 16, mu, rstd);
-                        }
-                    }
-                    if (p.BN & 31) {   // 16-column tail
-                        const int c = p.BN & ~31;
-                        uint32_t v[16];
-                        tmem_ld16(taddr + c, v);
-                        tmem_ld_wait();
-                        if (row_ok) epi_store16<0>(e, v, n, orow, ntile * p.BN + c, mu, rstd);
-                    }
+                if (prev >= 0) release(prev);
+                prev = stage;
+                if (++stage == p.num_stages) {
+                    stage = 0;
+                    phase ^= 1;
                 }
             }
-            // accumulator `buf` is drained: the MMA warp may start the tile after next into it
-            tc_fence_before();
-            if (PAIR && cr == 1) mbar_arrive_remote(leader_tmem_empty + (uint32_t)buf * 8u);
-            else mbar_arrive(&tmem_empty_bar[buf]);
-            B2_TS(if (ts && it == 0 && threadIdx.x == 64) ts[5] = globaltimer_ns();)
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc);
+            if (prev >= 0) release(prev);
+            B2_TS(if (ts && it == 0 && threadIdx.x == 0) ts[4] = globaltimer_ns();)
+
+            const int w0 = (mt % p.tiles_w) * p.tw, h0 = ((mt / p.tiles_w) % p.tiles_h) * p.th;
+            const int n0 = (mt / (p.tiles_w * p.tiles_h)) * p.tn;
+            if (p.swap || (e.flags & IG_SPLITK)) {
+                // one tile per CTA (swapped and split-K plans are never persistent): once both warpgroups have retired their
+                // MMAs the operand ring is idle and its head holds the fp32 tile
+                float* stg = reinterpret_cast<float*>(smem);
+                cons_bar_sync();
+                if (e.flags & IG_SPLITK) {
+                    // Split-K inside a thread-block cluster (one CTA per K slice): every CTA parks its fp32 partial tile in its
+                    // own shared memory, laid out [4-column group][row]; the reduction happens after the cluster barrier below.
+                    frag_to_smem<BN>(stg, acc, r0, lane, 0, BN, false);
+                } else {
+                    for (int c = 0; c < BN; c += SWAP_CH) {
+                        SwapPre pre;
+                        swap_prefetch(p, pre, SWAP_CH, c, ntile, n0, h0, w0, threadIdx.x);
+                        frag_to_smem<BN>(stg, acc, r0, lane, c, SWAP_CH, true);
+                        cons_bar_sync();
+                        swap_store_chunk(p, pre, stg, ntile, threadIdx.x);
+                        cons_bar_sync();
+                    }
+                }
+            } else {
+                EpiRow rw[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = r0 + 8 * h;
+                    const int wi = r % p.tw, hi = (r / p.tw) % p.th, ni = r / (p.tw * p.th);
+                    const int n = n0 + ni, hh = h0 + hi, ww = w0 + wi;
+                    rw[h].ok = (ni < p.tn) && (n < p.Nb) && (hh < p.Ho) && (ww < p.Wo);
+                    rw[h].orow = ((long)n * p.Ho + hh) * p.Wo + ww;
+                    rw[h].b = n;
+                    ln_row_stats(e, rw[h].orow, rw[h].ok, rw[h].mu, rw[h].rstd);
+                }
+                epi_frag<BN>(e, acc, rw, ntile, ln_fma, lane);
+            }
+            B2_TS(if (ts && it == 0 && threadIdx.x == 0) ts[5] = globaltimer_ns();)
         }
     }
-    B2_TS(if (ts && threadIdx.x == 64) ts[6] = globaltimer_ns();)
     if (p.epi.flags & IG_SPLITK) {
-        // ---- cluster-wide deterministic reduction over the K slices through distributed shared memory (one tile per CTA:
-        // split-K launches are never persistent) ----
+        // ---- cluster-wide deterministic reduction over the K slices through distributed shared memory ----
         const int mt = blockIdx.x;
         const int w0 = (mt % p.tiles_w) * p.tw, h0 = ((mt / p.tiles_w) % p.tiles_h) * p.th;
         const int n0 = (mt / (p.tiles_w * p.tiles_h)) * p.tn;
         const int splits = (int)gridDim.z;
-        const int rk_mul = PAIR ? 2 : 1, rk_add = cr;   // cluster rank of K slice s (same M half) = s * rk_mul + rk_add
+        const int rk_mul = PAIR ? 2 : 1, rk_add = cr;   // cluster rank of K slice s (same M tile) = s * rk_mul + rk_add
         cluster_sync_all();  // all partial tiles are in place (release/acquire over the cluster)
-        B2_TS(if (ts && threadIdx.x == 64) ts[6] = globaltimer_ns();)   // split launches: [5] staged, [6] cluster barrier passed, [7] reduced
-        if (warp >= 2 && p.swap) {
-            // swapped orientation: this CTA finalises the pixel columns [rank*cols_per, (rank+1)*cols_per) of the tile
+        B2_TS(if (ts && threadIdx.x == 0) ts[6] = globaltimer_ns();)   // split launches: [6] cluster barrier passed, [7] reduced
+        if (warp < IG_CONS / 32 && p.swap) {
+            // swapped orientation: this CTA finalises the pixel columns [rank*cols_per, (rank+1)*cols_per) of the tile; the two
+            // halves of the consumer threads take alternate 16-pixel strips (8 pixels: one float4 group each) of one channel row
             const int rank = (int)cluster_ctarank();
-            const int cols_per = p.BN / splits;
+            const int cols_per = BN / splits;
             const int ch = cols_per < SWAP_CH ? cols_per : SWAP_CH;
-            const int t = threadIdx.x - 64;               // 0..127 == accumulator row == output channel of the tile
+            const int t = threadIdx.x & (IG_BM - 1);     // accumulator row == output channel of the tile
+            const int half = threadIdx.x >> 7;
             const uint32_t stg_local = smem_u32(smem);
-            float* T = reinterpret_cast<float*>(smem + (size_t)p.BN * IG_BM * 4);   // right after the staging tile
+            float* T = reinterpret_cast<float*>(smem + (size_t)BN * IG_BM * 4);   // right after the staging tile
             for (int c = rank * cols_per; c < (rank + 1) * cols_per; c += ch) {
                 SwapPre pre;
-                swap_prefetch(p, pre, ch, c, ntile, n0, h0, w0, t);
-                for (int g = 0; g < (ch >> 2); g += 4) {     // 16 pixel columns per pass (ch is 8, 16 or 32)
-                    float acc[16];
-                    const int cc = ((c >> 2) + g) >> 2;      // 16-column strip index (c is a multiple of 16 when ch >= 16)
-                    if (ch >= 16) {
+                swap_prefetch(p, pre, ch, c, ntile, n0, h0, w0, threadIdx.x);
+                if (ch >= 16) {
+                    for (int g = 4 * half; g < (ch >> 2); g += 8) {     // 16 pixel columns per pass (ch is 16 or 32)
+                        float acc[16];
+                        const int cc = ((c >> 2) + g) >> 2;      // 16-column strip index
                         switch (splits) {
                             case 2: splitk_sum16<2>(stg_local, cc, t, acc); break;
                             case 4: splitk_sum16<4>(stg_local, cc, t, acc); break;
@@ -507,35 +373,33 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
                         }
 #pragma unroll
                         for (int i = 0; i < 16; ++i) T[(4 * g + i) * IG_BM + t] = acc[i];
-                    } else {
-                        // 8 pixel columns per CTA (BN 64 over 8 slices): two float4 groups
-#pragma unroll
-                        for (int gg = 0; gg < 2; ++gg) {
-                            float4 v[8];
-#pragma unroll
-                            for (int sidx = 0; sidx < 8; ++sidx)
-                                v[sidx] = dsmem_ld_f4(dsmem_map(stg_local, (uint32_t)sidx) + (uint32_t)((((c >> 2) + gg) * IG_BM + t) * 16));
-                            float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-                            for (int sidx = 0; sidx < 8; ++sidx) { a.x += v[sidx].x; a.y += v[sidx].y; a.z += v[sidx].z; a.w += v[sidx].w; }
-                            T[(4 * gg + 0) * IG_BM + t] = a.x;
-                            T[(4 * gg + 1) * IG_BM + t] = a.y;
-                            T[(4 * gg + 2) * IG_BM + t] = a.z;
-                            T[(4 * gg + 3) * IG_BM + t] = a.w;
-                        }
                     }
+                } else {
+                    // 8 pixel columns per CTA (BN 64 over 8 slices): two float4 groups, one per half
+                    const int gg = half;
+                    float4 v[8];
+#pragma unroll
+                    for (int sidx = 0; sidx < 8; ++sidx)
+                        v[sidx] = dsmem_ld_f4(dsmem_map(stg_local, (uint32_t)sidx) + (uint32_t)((((c >> 2) + gg) * IG_BM + t) * 16));
+                    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+                    for (int sidx = 0; sidx < 8; ++sidx) { a.x += v[sidx].x; a.y += v[sidx].y; a.z += v[sidx].z; a.w += v[sidx].w; }
+                    T[(4 * gg + 0) * IG_BM + t] = a.x;
+                    T[(4 * gg + 1) * IG_BM + t] = a.y;
+                    T[(4 * gg + 2) * IG_BM + t] = a.z;
+                    T[(4 * gg + 3) * IG_BM + t] = a.w;
                 }
-                epi_bar_sync();
-                swap_store_chunk(p, pre, T, ntile, t);
-                epi_bar_sync();
+                cons_bar_sync();
+                swap_store_chunk(p, pre, T, ntile, threadIdx.x);
+                cons_bar_sync();
             }
-        } else if (warp >= 2) {
+        } else if (warp < IG_CONS / 32) {
             const int rank = (int)cluster_ctarank() / rk_mul;
             const int rows_per = IG_BM / splits;          // splits in {2,4,8}
-            const int t = threadIdx.x - 64;               // 0..127
-            const int chunks = p.BN >> 4;
+            const int t = threadIdx.x;
+            const int chunks = BN >> 4;
             const uint32_t stg_local = smem_u32(smem);
-            for (int item = t; item < rows_per * chunks; item += 128) {
+            for (int item = t; item < rows_per * chunks; item += IG_CONS) {
                 const int rl = item % rows_per;
                 const int cc = item / rows_per;
                 const int r = rank * rows_per + rl;       // row of the tile this CTA finalises
@@ -552,29 +416,36 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
                     const long orow = ((long)n * p.Ho + h) * p.Wo + w;
                     float mu, rstd;
                     ln_row_stats(p.epi, orow, true, mu, rstd);
-                    epi_store16<0>(p.epi, acc, n, orow, ntile * p.BN + cc * 16, mu, rstd);
+                    epi_store16<0>(p.epi, acc, n, orow, ntile * BN + cc * 16, mu, rstd);
                 }
             }
         }
-        B2_TS(if (ts && threadIdx.x == 64) ts[7] = globaltimer_ns();)
+        B2_TS(if (ts && threadIdx.x == 0) ts[7] = globaltimer_ns();)
         cluster_sync_all();  // nobody may exit while a peer still reads its shared memory
     }
-    tc_fence_before();
-    if (PAIR) {   // both CTAs are done with the pair's tensor memory and with each other's barriers
+    if (PAIR) {   // nobody exits while the peer may still multicast into it or arrive on its barriers
         cluster_arrive_relaxed();
         cluster_wait();
-    } else {
-        __syncthreads();
     }
-    if (warp == 1) {
-        if (PAIR) tmem_dealloc_2cta(tmem_base, p.tmem_cols);
-        else tmem_dealloc(tmem_base, p.tmem_cols);
-    }
-    B2_TS(if (ts && threadIdx.x == 32 && !(p.epi.flags & IG_SPLITK)) ts[7] = globaltimer_ns();)
 }
 
-__global__ void __launch_bounds__(IG_THREADS) igemm_kernel(const __grid_constant__ IgemmParams p) { igemm_body<false>(p); }
-__global__ void __launch_bounds__(IG_THREADS) igemm_pair_kernel(const __grid_constant__ IgemmParams p) { igemm_body<true>(p); }
+template <int BN, bool PAIR>
+__global__ void __launch_bounds__(IG_THREADS, 1) igemm_kernel(const __grid_constant__ IgemmParams p) { igemm_body<BN, PAIR>(p); }
+
+using IgemmFn = void (*)(IgemmParams);
+// every N tile the planner can produce (multiples of 16 up to 256); CTA pairs need BN % 32 == 0.  At 168 registers the widest
+// tiles (BN >= 192: 96+ accumulator registers per thread) spill a few hundred bytes to local memory; the frame program's
+// autotile picks 256 only for the K-heavy split-K launches, its usual tiles are 64 / 128 / 160.
+template <bool PAIR>
+static IgemmFn igemm_fn(int bn) {
+    switch (bn) {
+#define B2_IG_CASE(N) case N: if constexpr (PAIR && (N % 32)) return nullptr; else return igemm_kernel<N, PAIR>;
+        B2_IG_CASE(16) B2_IG_CASE(32) B2_IG_CASE(48) B2_IG_CASE(64) B2_IG_CASE(80) B2_IG_CASE(96) B2_IG_CASE(112) B2_IG_CASE(128)
+        B2_IG_CASE(144) B2_IG_CASE(160) B2_IG_CASE(176) B2_IG_CASE(192) B2_IG_CASE(208) B2_IG_CASE(224) B2_IG_CASE(240) B2_IG_CASE(256)
+#undef B2_IG_CASE
+        default: return nullptr;
+    }
+}
 
 // ------------------------------------------------------------------------------------------
 // host side
@@ -748,6 +619,30 @@ static int plan_swap(const IgemmDesc& d, IgemmPlan* plan) {
     return 0;
 }
 
+int b2_device_sms() {
+    static int sms = 0;
+    if (sms == 0) {
+        int dev = 0, n = 0;
+        if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
+            sms = n;
+        else
+            sms = IG_SMS;
+        cudaGetLastError();   // no device (planning on a CPU-only machine) is not an error of the next call
+    }
+    return sms;
+}
+
+// CTAs of the kernel for this tile that one SM holds at once as far as registers and threads allow (the plan sizes the
+// shared memory).  Dry runs do not touch the device: they assume the one CTA per SM that 288 threads at 168 registers allow.
+static int igemm_ctas_per_sm(int bn, bool pair) {
+    if (g_plan_dry) return 1;
+    IgemmFn fn = pair ? igemm_fn<true>(bn) : igemm_fn<false>(bn);
+    int n = 0;
+    if (fn && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, IG_THREADS, 0) == cudaSuccess && n > 0) return n;
+    cudaGetLastError();
+    return 1;
+}
+
 int igemm_plan(const IgemmDesc& d, IgemmPlan* plan) {
     *plan = IgemmPlan{};
     if (d.swap) return plan_swap(d, plan);
@@ -838,10 +733,10 @@ int igemm_plan(const IgemmDesc& d, IgemmPlan* plan) {
         b2_set_error("igemm: weight ld %d < K %d or misaligned", d.w_ld, total_kb * IG_BK);
         return -1;
     }
-    const int b_rows = pair ? BN / 2 : BN;   // weight rows one CTA stages per K-block
+    const int b_rows = pair ? BN / 2 : BN;   // weight rows one CTA loads per K-block (pairs: multicast to both CTAs)
     if (encode_w_map(&p.tmB, d.w, d.w_rows, d.w_ld, b_rows)) return -1;
     p.a_bytes = (uint32_t)(tw * th * tn) * IG_BK * 2;
-    p.b_bytes = (uint32_t)b_rows * IG_BK * 2;
+    p.b_bytes = (uint32_t)BN * IG_BK * 2;    // weight bytes landing in each CTA per K-block
     // ---- split-K
     int splits = d.splits < 1 ? 1 : d.splits;
     if (splits > total_kb) splits = total_kb;
@@ -869,19 +764,22 @@ int igemm_plan(const IgemmDesc& d, IgemmPlan* plan) {
     // ---- pipeline depth / smem
     // one K-block (64 channels of one tap) per pipeline stage: packing several per stage was measured slower (shallower
     // prefetch, longer MMA issue code)
-    const size_t stage_bytes = (size_t)IG_BM * IG_BK * 2 + (size_t)b_rows * IG_BK * 2;
-    // TMA latency under load is ~1.3 us (tools/timeline.py): throughput per SM = bytes in flight / latency.  With at
-    // most ~1 CTA per SM take the whole shared memory for the ring; with many CTAs keep two co-resident instead.
-    static const char* pc_env = getenv("B2_PERSIST_CTAS");   // tuning: resident CTAs of a persistent launch (default 2 per SM)
-    const int persist_ctas = pc_env ? atoi(pc_env) : 2 * 148;
+    const size_t stage_bytes = (size_t)IG_BM * IG_BK * 2 + (size_t)BN * IG_BK * 2;
+    // The mainloop is TMA-latency bound: throughput per SM = bytes in flight / latency.  When registers admit only one CTA per
+    // SM (the case of this kernel: 288 threads at up to 168 registers) the ring takes (nearly) all the shared memory; only
+    // when two could be resident AND the launch needs them is the ring halved so that they fit.
+    const int per_sm = igemm_ctas_per_sm(BN, pair);
+    const long resident = (long)per_sm * b2_device_sms();   // CTAs the GPU runs at once
+    static const char* pc_env = getenv("B2_PERSIST_CTAS");   // tuning: CTAs of a persistent launch (default: one resident wave)
+    const long persist_ctas = pc_env ? atoi(pc_env) : resident;
     const long all_tiles = (long)p.tiles_w * p.tiles_h * p.tiles_n * n_tiles;
     static const bool no_persist_e = getenv("B2_NO_PERSIST") != nullptr;
-    const bool will_persist = !no_persist_e && splits == 1 && all_tiles > 2 * 148 && 2 * BN <= 512;
+    const bool will_persist = !no_persist_e && splits == 1 && all_tiles > resident && 2 * BN <= 512;
     const long total_ctas = will_persist ? persist_ctas : all_tiles * splits;
     static const char* stage_env = getenv("B2_STAGE_KB");
-    // <= 1 CTA per SM anyway: take (nearly) all the shared memory for the ring, the mainloop is TMA-latency bound
     const size_t ring_budget = stage_env ? (size_t)atoi(stage_env) * 1024
-                                         : (d.ring_kb > 0 ? (size_t)d.ring_kb * 1024 : (size_t)((total_ctas <= 148 ? 200 : 100) * 1024));
+                                         : (d.ring_kb > 0 ? (size_t)d.ring_kb * 1024
+                                                          : (size_t)((per_sm >= 2 && total_ctas > b2_device_sms() ? 100 : 200) * 1024));
     int stages = (int)(ring_budget / stage_bytes);
     if (stages < 2) stages = 2;
     if (stages > IG_MAX_STAGES) stages = IG_MAX_STAGES;
@@ -902,20 +800,19 @@ int igemm_plan(const IgemmDesc& d, IgemmPlan* plan) {
             pipe_bytes = stages * stage_bytes;
         }
     }
-    plan->smem = pipe_bytes + 1024 /*align slack*/ + 512 /*barriers*/ + (d.epi.colsum ? 2 * 256 * sizeof(float) : 0) /*LN vectors*/;
-    // persistent over M tiles when the launch would need more than one co-resident wave (2 CTAs per SM)
+    plan->smem = pipe_bytes + 1024 /*align slack*/ + 512 /*barriers*/;
+    // persistent over M tiles when the launch would need more than one resident wave
     const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-    static const bool no_persist = getenv("B2_NO_PERSIST") != nullptr;
     int grid_x = m_tiles;
     p.acc_bufs = 1;
-    if (!no_persist && splits == 1 && (long)m_tiles * n_tiles > 2 * 148 && 2 * BN <= 512) {
-        grid_x = persist_ctas / n_tiles;
+    if (will_persist) {
+        grid_x = (int)(persist_ctas / n_tiles);
         if (grid_x < 1) grid_x = 1;
         if (grid_x > m_tiles) grid_x = m_tiles;
         p.acc_bufs = 2;
     }
     if (pair) {   // CTAs (2j, 2j+1) of x are a pair: an odd tile count leaves one masked tile; a persistent launch stays within
-        // the co-resident wave (round down)
+        // the resident wave (round down)
         grid_x = (p.acc_bufs == 2 && grid_x > 2) ? (grid_x & ~1) : ((grid_x + 1) & ~1);
     }
     uint32_t cols = 32;
@@ -935,16 +832,16 @@ int igemm_encode_w_map(CUtensorMap* m, const __half* w, int rows, int ld, int bo
 int igemm_init() {
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(igemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             227 * 1024);
-        if (e != cudaSuccess) {
-            b2_set_error("cudaFuncSetAttribute(igemm): %s", cudaGetErrorString(e));
-            return -1;
-        }
-        e = cudaFuncSetAttribute(igemm_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) {
-            b2_set_error("cudaFuncSetAttribute(igemm pair): %s", cudaGetErrorString(e));
-            return -1;
+        for (int bn = 16; bn <= 256; bn += 16) {
+            for (int pair = 0; pair < 2; ++pair) {
+                IgemmFn fn = pair ? igemm_fn<true>(bn) : igemm_fn<false>(bn);
+                if (!fn) continue;
+                cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+                if (e != cudaSuccess) {
+                    b2_set_error("cudaFuncSetAttribute(igemm BN %d%s): %s", bn, pair ? " pair" : "", cudaGetErrorString(e));
+                    return -1;
+                }
+            }
         }
         if (!get_encode()) return -1;
         attr_set = true;
@@ -955,8 +852,13 @@ int igemm_init() {
 int igemm_launch(const IgemmPlan& plan, cudaStream_t stream) {
     if (igemm_init()) return -1;
     const int cz = plan.splits > 1 ? plan.splits : 1;
-    cudaError_t e = plan.pair ? launch_kc(igemm_pair_kernel, plan.grid, dim3(IG_THREADS), plan.smem, stream, 2, cz, plan.p)
-                              : launch_k(igemm_kernel, plan.grid, dim3(IG_THREADS), plan.smem, stream, cz, plan.p);
+    IgemmFn fn = plan.pair ? igemm_fn<true>(plan.p.BN) : igemm_fn<false>(plan.p.BN);
+    if (!fn) {
+        b2_set_error("igemm launch: no kernel for BN %d%s", plan.p.BN, plan.pair ? " (CTA pair)" : "");
+        return -1;
+    }
+    cudaError_t e = plan.pair ? launch_kc(fn, plan.grid, dim3(IG_THREADS), plan.smem, stream, 2, cz, plan.p)
+                              : launch_k(fn, plan.grid, dim3(IG_THREADS), plan.smem, stream, cz, plan.p);
     if (e != cudaSuccess) {
         b2_set_error("igemm launch: %s", cudaGetErrorString(e));
         return -1;

@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution / linear layer on tcgen05 tensor cores (sm_100a).
+// Implicit-GEMM convolution / linear layer on wgmma tensor cores (sm_90a).
 //
 // One kernel covers every contraction of the UNet and TAESD hot path:
 //   conv3x3 (stride 1/2, pad 1), conv1x1, Linear, fused "conv3x3 + 1x1 shortcut" (longer K loop),
@@ -14,11 +14,13 @@
 
 namespace b2 {
 
-constexpr int IG_BM = 128;        // rows (pixels/tokens) per CTA tile == UMMA M
+constexpr int IG_BM = 128;        // rows (pixels/tokens) per CTA tile == two wgmma M = 64 slabs
 constexpr int IG_BK = 64;         // fp16 elements per K-block (128 B = one swizzle row)
 constexpr int IG_MAX_SRC = 3;
 constexpr int IG_MAX_STAGES = 8;
-constexpr int IG_THREADS = 192;   // warp0: TMA, warp1: MMA + TMEM alloc, warps 2-5: epilogue
+constexpr int IG_CONS = 256;      // two consumer warpgroups (MMA + epilogue), warps 0-7
+constexpr int IG_THREADS = IG_CONS + 32;   // + warp 8: TMA producer
+constexpr int IG_SMS = 132;       // H100 SXM streaming multiprocessors (launch-shape policy)
 
 enum : int {
     IG_RELU = 1,    // relu after bias/residual
@@ -69,12 +71,12 @@ struct IgemmParams {
     int tiles_w, tiles_h, tiles_n;
     int Wo, Ho, Nb;
     int stride;                   // input coord = stride * out + tap - 1
-    int BN;                       // UMMA N (multiple of 16, <= 256)
+    int BN;                       // wgmma N (multiple of 16, <= 256)
     int num_stages;
-    int acc_bufs;                 // 1, or 2 when the launch is persistent over M tiles (double-buffered accumulator)
+    int acc_bufs;                 // 1, or 2 when the launch is persistent over M tiles
     uint32_t a_bytes;             // TMA box bytes of one A tile
     uint32_t b_bytes;
-    uint32_t tmem_cols;
+    uint32_t tmem_cols;           // accumulator columns of the tile(s) a CTA holds, rounded up to a power of two (plan info)
     unsigned long long* dbg_ts;   // debug: 8 globaltimer stamps per CTA (null = off)
     int n_pad;
     int swap;                     // 1: weights on the M side (128 output channels per CTA), pixels on the N side
@@ -101,12 +103,12 @@ struct IgemmDesc {
     int BN;           // 0 = auto
     int swap;         // 1 = swapped orientation: D^T = W . X^T, BN pixels (64/128/256) on the N side, transposed store
     int splits;       // 0/1 = none
-    int ring_kb;      // operand ring budget in KB, 0 = auto (200 when the launch has <= 1 CTA per SM, else 100)
+    int ring_kb;      // operand ring budget in KB, 0 = auto (200, or 100 when two CTAs per SM are resident and needed)
     int max_splits;   // cap of the split-K factor chosen by igemm_autotile, 0 = 8
     int pair_auto;    // igemm_autotile only: 0 = single CTAs, 1 = launch every eligible contraction as CTA pairs, 2 = only K >= 1280
     int pair_splits;  // ... and cap the split-K factor of those paired launches (0 = 4); the N tile of the single-CTA policy is kept
-    int pair;         // 1 = CTA pairs (tcgen05.mma.cta_group::2, M = 256 per MMA): neighbouring M tiles share the weight tile,
-                      // each CTA stages half of it.  Normal orientation only, BN % 32 == 0, split-K <= 4.
+    int pair;         // 1 = CTA pairs (2-CTA cluster): neighbouring M tiles share the weight tile, each CTA loads half of it
+                      // and multicasts it to both.  Normal orientation only, BN % 32 == 0, split-K <= 4.
     unsigned long long* dbg_ts;  // optional per-CTA timeline (8 stamps per CTA)
     float* partial;   // unused since split-K moved into a cluster (kept for ABI stability; op-level entry: debug timeline)
     int* tile_counters;  // unused (ABI stability)
@@ -114,13 +116,13 @@ struct IgemmDesc {
 };
 
 struct IgemmPlan {
-    int mode;       // 0 = igemm_kernel, 1 = igemm_pair_kernel (plan-info ABI)
+    int mode;       // 0 = single CTAs, 1 = CTA pairs (plan-info ABI)
     IgemmParams p;
     dim3 grid;
     size_t smem;
     int splits;
     long rows_total;
-    int pair;       // launched as igemm_pair_kernel with cluster dims (2, 1, splits)
+    int pair;       // launched as CTA pairs with cluster dims (2, 1, splits)
 };
 
 // Returns 0 on success; fills plan. Encodes TMA descriptors (host side, no launch).
@@ -132,6 +134,8 @@ int igemm_launch(const IgemmPlan& plan, cudaStream_t stream);
 void igemm_set_dry_run(bool on);
 // one-time function attributes / driver entry points (call outside stream capture)
 int igemm_init();
+// streaming multiprocessors of the current device (IG_SMS when there is none)
+int b2_device_sms();
 // legacy: workspace floats of the former global-memory split-K (no workspace is needed any more)
 size_t igemm_partial_floats(int splits, long rows_total, int n_valid);
 const char* b2_last_error();

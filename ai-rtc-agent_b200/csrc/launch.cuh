@@ -3,7 +3,7 @@
 // Every kernel of the frame program starts with `griddepcontrol.launch_dependents` (the next kernel of the stream /
 // CUDA graph may be scheduled as soon as all CTAs of this one have started) and executes `griddepcontrol.wait`
 // before touching global memory produced by its predecessor.  The successor's launch latency and prologue (barrier
-// init, TMEM allocation, descriptor prefetch) then overlap this kernel's execution instead of sitting on the
+// init, descriptor prefetch) then overlap this kernel's execution instead of sitting on the
 // critical path -- with ~450 launches per frame that is a large fraction of the frame time.
 #pragma once
 #include <cuda_runtime.h>

@@ -1,5 +1,5 @@
-// sm_100a PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM).
-// Hand-written for B200; no CUTLASS/CuTe on the hot path.
+// sm_90a PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), clusters / DSMEM, wgmma.
+// Hand-written for H100; no CUTLASS/CuTe on the hot path.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -17,18 +17,6 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
     uint64_t t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
     return t;
-}
-
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P;\n\t"
-        "elect.sync _|P, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, P;\n\t"
-        "}\n"
-        : "=r"(pred));
-    return pred != 0;
 }
 
 // ---------------------------------------------------------------- mbarrier
@@ -60,7 +48,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     return ok != 0;
 }
 // Bounded wait: a protocol bug traps (sticky error, process keeps control) instead of hanging
-// the GPU box. 4 s is >1000x any legitimate wait in this library.
+// the GPU. 4 s is >1000x any legitimate wait in this library.  No printf here: a call inside a wgmma mainloop makes ptxas
+// serialize the warpgroup MMAs.
 #ifndef B2_WAIT_TIMEOUT_NS
 #define B2_WAIT_TIMEOUT_NS 4000000000ull
 #endif
@@ -72,24 +61,19 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         if ((++spins & 0x3ff) == 0) {
             const uint64_t now = globaltimer_ns();
             if (t0 == 0) t0 = now;
-            else if (now - t0 > B2_WAIT_TIMEOUT_NS) {
-                printf("b2: mbarrier wait timeout (block %d,%d,%d thread %d parity %u)\n", blockIdx.x,
-                       blockIdx.y, blockIdx.z, threadIdx.x, parity);
-                __trap();
-            }
+            else if (now - t0 > B2_WAIT_TIMEOUT_NS) __trap();
         }
     }
 }
 
-// Arrive on a barrier in a peer CTA's shared memory (CTA-pair MMA: operands-landed relay, accumulator-drained).  Default
-// semantics on purpose: what crosses the pair is the ORDER of async-proxy work (TMA landed -> tcgen05.mma may read it; tcgen05.ld
-// retired -> the accumulator may be overwritten), not generic-proxy data, and the .release.cluster / .acquire.cluster forms
-// compile to MEMBAR.ALL.GPU + CCTL.IVALL per use (measured: +6 us per launch).
+// Arrive on a barrier in a peer CTA's shared memory (CTA pairs: "my warpgroups have finished reading this ring slot", so the
+// peer's multicast may overwrite it).  Default semantics on purpose: what crosses the pair is the ORDER of async-proxy work
+// (wgmma reads retired -> TMA may write), not generic-proxy data.
 __device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
     asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 
-// smem writes by normal (generic-proxy) stores -> visible to async proxy (TMA / UMMA reads)
+// smem writes by normal (generic-proxy) stores -> visible to async proxy (TMA / wgmma reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -146,160 +130,41 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
         : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; one thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                         uint32_t idesc, uint32_t accumulate) {
+// Multicast form (CTA pairs): the box lands at the same shared-memory offset in every CTA of `cta_mask` (cluster ranks),
+// and each destination's mbarrier at `bar`'s offset receives the complete_tx of its bytes.
+__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, uint16_t cta_mask) {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// CTA-pair form (cta_group::2): M = 256 over two CTAs of a cluster whose ranks differ in bit 0.  Each CTA holds its own 128 A
-// rows and HALF of the B tile (N/2 rows) at the same shared-memory offsets; the leader (even rank) issues, and the accumulator
-// rows [0,128) / [128,256) land in the leader's / the peer's tensor memory at the same address.  Per MMA the shared-memory
-// operand port of each SM then reads (128 + N/2) rows instead of (128 + N).
-__device__ __forceinline__ void umma_f16_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// ... its completion arrives on the barrier at this CTA-relative offset in every CTA of `cta_mask` (cluster ranks)
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(cta_mask)
-                 : "memory");
-}
-// tensor-memory allocation of a CTA pair: one warp of EACH of the two CTAs issues it (collective)
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2cta() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// Same, with the A operand read from tensor memory ("TS" form): lane i of the A region holds row i, 32-bit column j holds the
-// K elements (2j, 2j+1), so one K = 16 step consumes 8 columns.  Used by the attention kernel's P.V product: P never
-// touches shared memory.
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// mbarrier arrives when all previously issued MMAs of this thread completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                     smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// 32 lanes x 32-bit, 16 consecutive columns: thread t of the warp gets lane (base_lane + t).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
-        "%13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),
-          "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
-        "%13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-        "[%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]),
-          "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]),
-          "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]),
-          "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], "
+        "%5;" ::"r"(smem_u32(smem_dst)),
+        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
         : "memory");
 }
 
-__device__ __forceinline__ void tmem_st_wait() {
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-        "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
-        "%13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]),
-        "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]),
-        "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-        : "memory");
+// ---------------------------------------------------------------- wgmma (warpgroup MMA, accumulators in registers)
+// Every thread of the warpgroup executes these (.sync.aligned).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the compiler must not move accumulator reads/writes across an in-flight wgmma
+template <int N>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // ---------------------------------------------------------------- descriptors
-// K-major operand tile in smem, SWIZZLE_128B: rows of 64 fp16 (128 B), 8-row groups 1024 B apart.
-// Bit layout (cute::UMMA::SmemDescriptor): start[0,14) lbo[16,30) sbo[32,46) version[46,48)=1
-// base_offset[49,52) lbo_mode[52] layout[61,64) (2 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
+// K-major operand tile in smem, SWIZZLE_128B: rows of 64 fp16 (128 B), 8-row groups `sbo` bytes apart (1024 for a dense tile).
+// Bit layout (sm_90 wgmma matrix descriptor): start[0,14) lbo[16,30) sbo[32,46) base_offset[49,52) layout[62,64) (1 = SWIZZLE_128B).
+// The swizzle follows the shared-memory address bits, so tiles start on 1024-byte boundaries except where a caller shifts the
+// start by whole 128-byte rows on purpose (tconv.cu).
+__device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr, uint32_t sbo = 1024) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);
     d |= (uint64_t)1 << 16;            // LBO (unused for swizzled K-major)
-    d |= (uint64_t)(1024 >> 4) << 32;  // SBO: 8 rows * 128 B
-    d |= (uint64_t)1 << 46;            // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;            // SWIZZLE_128B
+    d |= (uint64_t)(sbo >> 4) << 32;   // SBO: 8 rows * 128 B
+    d |= (uint64_t)1 << 62;            // SWIZZLE_128B
     return d;
-}
-// kind::f16 instruction descriptor: D=f32, A=B=f16, both K-major, M x N.
-__host__ __device__ __forceinline__ uint32_t make_idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// byte offset of (row, 16-byte chunk) inside a SWIZZLE_128B K-major tile (base 1024-aligned)
-__device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t chunk16) {
-    return row * 128u + ((chunk16 ^ (row & 7u)) << 4);
 }
 
 }  // namespace b2

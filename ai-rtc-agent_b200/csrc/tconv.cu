@@ -23,34 +23,20 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tconv_kernel(const __grid_const
     uint64_t* w_full = reinterpret_cast<uint64_t*>(sA + (size_t)p.nbuf * p.abuf_bytes);
     uint64_t* a_full = w_full + 1;
     uint64_t* a_empty = a_full + TC_MAX_ABUF;
-    uint64_t* tmem_full_bar = a_empty + TC_MAX_ABUF;   // [2] accumulator ready   (MMA -> epilogue)
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;      // [2] accumulator drained (epilogue -> MMA)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == TC_CONS) {
         tma_prefetch_desc(&p.tmA);
         tma_prefetch_desc(&p.tmB);
         mbar_init(w_full, 1);
         for (int s = 0; s < p.nbuf; ++s) {
             mbar_init(&a_full[s], 1);
-            mbar_init(&a_empty[s], 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(&tmem_full_bar[s], 1);
-            mbar_init(&tmem_empty_bar[s], 128);
+            mbar_init(&a_empty[s], 4);   // the four warps of the warpgroup that consumed the halo
         }
         fence_mbar_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, 2 * TC_C);   // two fp32 accumulators of 64 columns
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     // the weights are constants of the stream: request them before the programmatic-dependency wait
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == TC_CONS) {
         mbar_expect_tx(w_full, 9 * TC_WTILE);
         for (int tap = 0; tap < 9; ++tap) tma_load_2d(sW + tap * TC_WTILE, &p.tmB, w_full, tap * TC_C, 0);
     }
@@ -58,7 +44,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tconv_kernel(const __grid_const
     pdl_wait();
 
     const int tiles_per_img = p.tiles_w * p.tiles_h;
-    if (warp == 0) {
+    if (warp == TC_CONS / 32) {
         if (lane == 0) {
             // ===== halo producer: one (TH+2) x (TW+2) pixel tile per output tile =====
             int slot = 0;
@@ -74,76 +60,65 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tconv_kernel(const __grid_const
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: the whole warp walks the loop, one elected lane issues (see igemm_kernel) =====
-        const uint32_t idesc = make_idesc_f16(IG_BM, TC_C);
+    } else {
+        // ===== consumer warpgroup wg: the CTA's tiles it = wg, wg + 2, ... (all 128 pixels of each, as two M = 64 slabs), so
+        // one warpgroup's epilogue overlaps the other's MMAs =====
+        const int wg = warp >> 2;
         const uint32_t sa_base = smem_u32(sA);
         const uint64_t db0 = make_kmajor_sw128_desc(smem_u32(sW));
         constexpr int pitch = TC_TW + 2;   // pixels per halo row: the 8-row core groups of the A operand are `pitch` pixels apart
+        const int rq = (warp & 3) * 16 + (lane >> 2);   // this thread's first row inside a 64-row slab
+        const IgEpilogue& e = p.epi;
         mbar_wait(w_full, 0);
-        tc_fence_after();
-        int slot = 0;
-        uint32_t phase = 0;
-        int it = 0;
-        for (int mt = blockIdx.x; mt < p.num_tiles; mt += gridDim.x, ++it) {
-            const int buf = it & 1;
-            mbar_wait(&tmem_empty_bar[buf], ((it >> 1) & 1) ^ 1);   // the epilogue has drained this accumulator
-            mbar_wait(&a_full[slot], phase);
-            tc_fence_after();
-            const uint32_t tacc = tmem_base + (uint32_t)buf * TC_C;
-            // A descriptor of tap (0,0): rows r = 8*hi + wi -> halo pixel hi*pitch + wi (+ tap shift).  The swizzle follows the
-            // absolute shared-memory address bits, so the 128-byte-granular tap shifts need no base offset (tools/probe).
-            uint64_t da0 = 0;
-            da0 |= (uint64_t)(((sa_base + (uint32_t)slot * p.abuf_bytes) & 0x3ffff) >> 4);
-            da0 |= (uint64_t)1 << 16;
-            da0 |= (uint64_t)((pitch * 128) >> 4) << 32;
-            da0 |= (uint64_t)1 << 46;
-            da0 |= (uint64_t)2 << 61;
+        for (int it = wg, mt = blockIdx.x + wg * gridDim.x; mt < p.num_tiles; it += 2, mt += 2 * gridDim.x) {
+            const int slot = it % p.nbuf;
+            mbar_wait(&a_full[slot], (uint32_t)(it / p.nbuf) & 1u);
+            float acc[2][TC_C / 2];
+#pragma unroll
+            for (int m = 0; m < 2; ++m)
+#pragma unroll
+                for (int i = 0; i < TC_C / 2; ++i) acc[m][i] = 0.f;
+            wgmma_fence_regs(acc[0]);
+            wgmma_fence_regs(acc[1]);
+            wgmma_fence();
+            // A descriptor of tap (0,0): rows r = 8*hi + wi -> halo pixel hi*pitch + wi (+ tap shift); slab m starts at hi = 8m.
+            // The swizzle follows the absolute shared-memory address bits, so the 128-byte-granular tap shifts need no base offset.
+            const uint32_t a0 = sa_base + (uint32_t)slot * p.abuf_bytes;
 #pragma unroll
             for (int tap = 0; tap < 9; ++tap) {
-                const uint64_t da = da0 + (uint64_t)(((tap / 3) * pitch + (tap % 3)) * 8);   // 128 B per pixel = 8 units of 16 B
                 const uint64_t db = db0 + (uint64_t)(tap * (TC_WTILE >> 4));
-                if (elect_one()) {
-                    umma_f16(tacc, da, db, idesc, tap > 0 ? 1u : 0u);
-                    umma_f16(tacc, da + 2, db + 2, idesc, 1u);
-                    umma_f16(tacc, da + 4, db + 4, idesc, 1u);
-                    umma_f16(tacc, da + 6, db + 6, idesc, 1u);
+#pragma unroll
+                for (int m = 0; m < 2; ++m) {
+                    const uint32_t sa = a0 + (uint32_t)((8 * m + tap / 3) * pitch + tap % 3) * 128u;   // 128 B per pixel
+                    const uint64_t da = make_kmajor_sw128_desc(sa, pitch * 128);
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) Wgmma<TC_C>::ss(acc[m], da + 2 * k, db + 2 * k, 1u);
                 }
-                __syncwarp();
             }
-            if (elect_one()) {
-                umma_commit(&a_empty[slot]);          // the halo buffer may be refilled when these MMAs retire
-                umma_commit(&tmem_full_bar[buf]);
-            }
-            __syncwarp();
-            if (++slot == p.nbuf) {
-                slot = 0;
-                phase ^= 1;
-            }
-        }
-    } else {
-        // ===== epilogue: TMEM -> registers -> bias / residual / ReLU -> fp16 NHWC =====
-        const int q = warp & 3;
-        const int r = q * 32 + lane;
-        const int hi = r >> 3, wl = r & 7;
-        const IgEpilogue& e = p.epi;
-        int it = 0;
-        for (int mt = blockIdx.x; mt < p.num_tiles; mt += gridDim.x, ++it) {
-            const int buf = it & 1;
-            const uint32_t par = (it >> 1) & 1;
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc[0]);
+            wgmma_fence_regs(acc[1]);
+            if (lane == 0) mbar_arrive(&a_empty[slot]);   // the halo buffer may be refilled
+            // ===== epilogue: registers -> bias / residual / ReLU -> fp16 NHWC =====
             const int tiw = mt % p.tiles_w, tih = (mt / p.tiles_w) % p.tiles_h, n0 = mt / tiles_per_img;
-            const int h = tih * TC_TH + hi, w = tiw * TC_TW + wl;
-            const bool row_ok = (h < p.Ho) && (w < p.Wo);
-            const long orow = ((long)n0 * p.Ho + h) * p.Wo + w;
-            const uint32_t taddr = tmem_base + (uint32_t)buf * TC_C + ((uint32_t)(q * 32) << 16);
-            epi_row_fast(e, taddr, TC_C, 0, n0, orow, row_ok, &tmem_full_bar[buf], par);
-            tc_fence_before();
-            mbar_arrive(&tmem_empty_bar[buf]);
+#pragma unroll
+            for (int m = 0; m < 2; ++m) {
+                EpiRow rw[2];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = 64 * m + rq + 8 * h;
+                    const int hh = tih * TC_TH + (r >> 3), ww = tiw * TC_TW + (r & 7);
+                    rw[h].ok = (hh < p.Ho) && (ww < p.Wo);
+                    rw[h].orow = ((long)n0 * p.Ho + hh) * p.Wo + ww;
+                    rw[h].b = n0;
+                    rw[h].mu = 0.f;
+                    rw[h].rstd = 1.f;
+                }
+                epi_frag<TC_C>(e, acc[m], rw, 0, false, lane);
+            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 2 * TC_C);
 }
 
 // ------------------------------------------------------------------------------------------ host side
@@ -175,17 +150,14 @@ int tconv_plan(const IgemmDesc& d, TconvPlan* plan) {
     p.nbuf = nb_env ? atoi(nb_env) : 4;
     if (p.nbuf < 2) p.nbuf = 2;
     if (p.nbuf > TC_MAX_ABUF) p.nbuf = TC_MAX_ABUF;
+    // even depth: the two warpgroups take alternate tiles, so every halo slot then belongs to one warpgroup and its phase
+    // parity wait cannot be satisfied by the other warpgroup's earlier use of the slot
+    p.nbuf &= ~1;
     p.abuf_bytes = (TC_HALO_BYTES + 1023u) & ~1023u;
     p.epi = d.epi;
     if (igemm_encode_act_map(&p.tmA, d.src[0], TC_C, TC_TW + 2, TC_TH + 2, 1, 1)) return -1;
     if (igemm_encode_w_map(&p.tmB, d.w, d.w_rows, d.w_ld, TC_C)) return -1;
-    int sms = 148;
-    {
-        int dev = 0;
-        cudaDeviceProp prop;
-        if (cudaGetDevice(&dev) == cudaSuccess && cudaGetDeviceProperties(&prop, dev) == cudaSuccess && prop.multiProcessorCount > 0)
-            sms = prop.multiProcessorCount;
-    }
+    const int sms = b2_device_sms();
     plan->grid = dim3(p.num_tiles < sms ? p.num_tiles : sms, 1, 1);
     plan->smem = 9 * (size_t)TC_WTILE + (size_t)p.nbuf * p.abuf_bytes + 1024 /*align slack*/ + 512 /*barriers*/;
     plan->rows_total = (long)d.Nb * d.Ho * d.Wo;

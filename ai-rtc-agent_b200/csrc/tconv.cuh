@@ -1,21 +1,22 @@
-// Persistent 3x3 convolution for the TAESD body (64 -> 64 channels, stride 1) on tcgen05 tensor cores.
+// Persistent 3x3 convolution for the TAESD body (64 -> 64 channels, stride 1) on wgmma tensor cores.
 //
 // TAESD (lib/wrapper.py:445-453: the reference's vae_encoder / vae_decoder engines) is 60 such convolutions over up to
 // 512x512 pixels.  With one 64-wide N tile the generic tap-by-tap kernel (igemm.cu) spends its shared-memory port on
 // refilling operands: per output tile it re-fetches the activations nine times (once per filter tap) and the 72 KB weight
 // matrix once.  Here
 //   * the whole weight matrix (9 taps x [64 x 64]) is loaded ONCE per CTA and stays resident in shared memory,
-//   * one TMA load brings an (16+2) x (8+2)-pixel halo tile; the nine taps are nine shifted UMMA descriptors over it,
-//   * CTAs are persistent (one per SM) with a ring of halo buffers and two TMEM accumulators, so loads, MMAs and the
-//     epilogue of neighbouring tiles overlap.
+//   * one TMA load brings an (16+2) x (8+2)-pixel halo tile; the nine taps are nine shifted wgmma descriptors over it,
+//   * CTAs are persistent (one per SM) with a ring of halo buffers and two consumer warpgroups that take alternate tiles
+//     (accumulators in registers), so loads, MMAs and the epilogue of neighbouring tiles overlap.
 // Operand fill drops from 216 KB to 23 KB per 128-pixel tile.
 #pragma once
 #include "igemm.cuh"
 
 namespace b2 {
 
-constexpr int TC_THREADS = 192;        // warp0: TMA producer, warp1: MMA issuer + TMEM, warps 2-5: epilogue
-constexpr int TC_TW = 8, TC_TH = 16;   // output tile: 16 rows x 8 columns = 128 pixels (= UMMA M); 8-pixel rows are the 8-row core groups
+constexpr int TC_CONS = 256;           // warps 0-7: two consumer warpgroups (MMA + epilogue)
+constexpr int TC_THREADS = TC_CONS + 32;   // + warp 8: TMA producer
+constexpr int TC_TW = 8, TC_TH = 16;   // output tile: 16 rows x 8 columns = 128 pixels (= two wgmma M = 64 slabs); 8-pixel rows are the 8-row core groups
 constexpr int TC_C = 64;               // input channels == output channels == one 128-byte swizzle row
 constexpr int TC_MAX_ABUF = 6;
 

@@ -6,9 +6,8 @@ lib/pipeline.py:50-51,83,96.  What exists here:
     engine's frame formats (u8 NHWC RGB in, u8 NCHW RGB out), as CUDA kernels behind the C ABI;
   * codec_libraries(): dlopen probe of libnvcuvid / libnvidia-encode.
 
-What does not: decoder / encoder sessions.  The GPU boxes this was built on ship neither library nor the Video Codec SDK
-headers (profiles/r01_gpu_box_probe.txt), so open_decoder / open_encoder raise CodecUnavailable and the synthetic feeder stays
-the frame source -- stated, not silently faked."""
+What does not: decoder / encoder sessions.  Without those libraries and the Video Codec SDK headers, open_decoder /
+open_encoder raise CodecUnavailable and the synthetic feeder stays the frame source -- stated, not silently faked."""
 from __future__ import annotations
 
 import torch

@@ -80,7 +80,7 @@ class StreamDiffusion:
         if not use_denoising_batch:
             raise NotImplementedError("img2img mode must use denoising batch for now.")
         if torch_dtype != torch.float16:
-            raise NotImplementedError("the sm_100a kernels compute in fp16 (fp32 accumulate) like the reference engines")
+            raise NotImplementedError("the sm_90a kernels compute in fp16 (fp32 accumulate) like the reference engines")
         self.arch = arch
         self.device = torch.device(device)
         self.dtype = torch_dtype
@@ -121,7 +121,7 @@ class StreamDiffusion:
         cfg.do_add_noise = int(do_add_noise)
         cfg.use_cuda_graph = int(use_cuda_graph)
         if not torch.cuda.is_available():
-            raise capi.B2Error("no CUDA device: the B200 pipeline has no CPU fallback")
+            raise capi.B2Error("no CUDA device: the H100 pipeline has no CPU fallback")
         if self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
         torch.cuda.set_device(self.device)

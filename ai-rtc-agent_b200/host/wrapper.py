@@ -1,6 +1,6 @@
 """Drop-in for the reference's `lib/wrapper.py:StreamDiffusionWrapper` (lib/wrapper.py:34-407): same
 constructor keywords and defaults, same validation errors, same methods and externally-read attributes,
-with the TensorRT/diffusers model behind it replaced by the sm_100a engine (host/stream.py).
+with the TensorRT/diffusers model behind it replaced by the sm_90a engine (host/stream.py).
 
 Not carried over (unreachable from lib/pipeline.py:23-42 and listed out-of-scope in SURVEY.md section 8):
 ControlNet, safety checker, similar-image filter, DataParallel, txt2img sampling, xformers/sfast/TensorRT

@@ -8,7 +8,7 @@ loads the diffusers-layout checkpoint from disk (or seeded synthetic weights wit
 LCM-LoRA (non-turbo models) and the given LoRAs into the UNet (lib/wrapper.py:683-697), lets the engine lay the weights out
 in its kernel-native formats and writes `<engine-dir>/engines--<model>/b2sd-<arch>-<hash>.b2pack`.  Every later
 StreamDiffusionWrapper / StreamDiffusionPipeline start with the same model + LoRA recipe loads that blob instead of the
-checkpoint (no safetensors parsing, no LoRA fusing, no repacking, no raw copy in HBM).  Needs a B200 (packing runs on it)."""
+checkpoint (no safetensors parsing, no LoRA fusing, no repacking, no raw copy in HBM).  Needs an H100 (packing runs on it)."""
 from __future__ import annotations
 
 import argparse

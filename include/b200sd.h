@@ -92,7 +92,7 @@ int b2sd_op_igemm(const b2sd_igemm_desc* d, void* stream);
  * given) or the engine's tile policy (autotile = 1: latency policy of a single frame in flight; 2: throughput policy of >= 4
  * frames in flight; allow_swap = the contraction may use the swapped orientation) would launch for this contraction.  Pointers in the descriptor only need plausible alignment.  For tests of the host logic. */
 typedef struct {
-    int mode;          /* 0 = igemm_kernel, 1 = igemm_pair_kernel (CTA pairs); the halo-tile kernel is requested with B2SD_IG_TCONV */
+    int mode;          /* 0 = igemm_kernel on single CTAs, 1 = CTA pairs (2-CTA clusters); the halo-tile kernel is requested with B2SD_IG_TCONV */
     int swap, bn, splits;
     int grid_x, grid_y, grid_z;
     int num_stages;    /* operand ring depth */

@@ -2,7 +2,7 @@
 implementation SURVEY.md 8(c) states the u8 tolerance against.
 
 Three implementations of the same frame (identical seeded fp16 weights, prompt embedding, noise, frames):
-  A. this repo's sm_100a engine, through the C ABI (host/stream.py);
+  A. this repo's sm_90a engine, through the C ABI (host/stream.py);
   B. the oracle's functions executed by torch's GPU library kernels in fp32 (TF32 off) -- oracle/torch_gpu.py;
   C. the same in fp16 with fused SDPA -- what a plain torch/diffusers fp16 deployment of the reference computes.
 B is tied to the CPU oracle at the tiny size (test_gpu_oracle_equals_cpu_oracle), so A-vs-B at 512x512 / 768x768 is parity
@@ -28,7 +28,7 @@ def _weights(turbo, full=True):
 def _engine(arch, usd, vsd, emb, tl, hw, frames_in_flight=1):
     from ai_rtc_agent_b200.host.stream import StreamDiffusion
     sd = StreamDiffusion(arch, usd, vsd, tl, lambda p: emb, width=hw, height=hw, device="cuda")
-    if frames_in_flight > 1:   # throughput launch policy: 100 KB operand rings, CTA pairs (igemm_pair_kernel) without split-K
+    if frames_in_flight > 1:   # throughput launch policy: 100 KB operand rings, CTA pairs without split-K
         sd.set_concurrency(frames_in_flight)
     sd.prepare("p", guidance_scale=0.0)
     return sd
@@ -109,7 +109,7 @@ def test_three_implementations_full_size(cuda, turbo, tl, hw, nframes, in_flight
 @pytest.mark.parametrize("name,tl,hw", [("sd15_T4_512", [18, 26, 35, 45], 512), ("sd15_T4_768", [18, 26, 35, 45], 768)])
 def test_full_size_golden_fixture(cuda, name, tl, hw):
     """Committed CPU-oracle fixtures (tests/golden/make_golden_fullsize.py, generated where the oracle has minutes per
-    frame): eps of every stream-batch slot and an 8x-subsampled u8 image for each frame."""
+    frame): eps of every stream-batch slot (at 768x768 on a 1/2 grid) and an 8x-subsampled u8 image for each frame."""
     import os
     import numpy as np
     from oracle import weights as ow
@@ -121,9 +121,10 @@ def test_full_size_golden_fixture(cuda, name, tl, hw):
     sd = _engine(arch, usd, vsd, emb, tl, hw)
     assert np.array_equal(sd.init_noise.float().numpy(), gold["init_noise"].astype(np.float32))
     st = int(gold["u8_stride"])
+    es = int(gold["eps_stride"]) if "eps_stride" in gold.files else 1
     for i in range(gold["eps"].shape[0]):
         out = sd.step_u8(ow.make_frame(hw, hw, seed=i).cuda()).cpu().numpy()
-        eps = sd.get_tensor("eps").float().permute(0, 3, 1, 2).numpy()
+        eps = sd.get_tensor("eps").float().permute(0, 3, 1, 2).numpy()[..., ::es, ::es]
         ref = gold["eps"][i].astype(np.float32)
         rel = np.abs(eps - ref).max() / np.abs(ref).max()
         d = np.abs(out[:, :, ::st, ::st].astype(np.int32) - gold["u8"][i].astype(np.int32))

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit-GEMM kernel (conv3x3 / 1x1 / Linear / GEGLU / split-K) through
+"""GPU parity of the wgmma implicit-GEMM kernel (conv3x3 / 1x1 / Linear / GEGLU / split-K) through
 the C ABI (b2sd_op_igemm) against plain PyTorch fp32 ops on the same fp16-rounded operands.
 
 Tolerance: operands are exact fp16; accumulation is fp32 in both; the only difference is the final
@@ -211,7 +211,7 @@ def test_linear_swapped_orientation(cuda, m, k, n, bn, splits):
 @pytest.mark.parametrize("nb,h,w,relu,res", [
     (1, 16, 8, False, False),      # exactly one 16x8 tile: descriptor / tap-shift sanity
     (1, 64, 64, True, True),       # TAESD block tail at the latent size: bias + skip + ReLU
-    (1, 256, 256, True, False),    # 512 tiles on 148 persistent CTAs: ring wrap-around, both TMEM accumulators
+    (1, 256, 256, True, False),    # 512 tiles on persistent CTAs: ring wrap-around, several tiles per CTA
     (2, 40, 28, True, True),       # ragged extents (partial tiles in h and w), two images
     (1, 512, 512, True, True),     # the full-size TAESD body convolution of the 512x512 configs
 ])

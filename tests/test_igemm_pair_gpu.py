@@ -1,5 +1,5 @@
-"""GPU parity of the CTA-pair form of the implicit-GEMM kernel (igemm_pair_kernel: tcgen05.mma.cta_group::2, M = 256 per MMA, every
-CTA stages half of the weight tile) through the C ABI, against plain PyTorch fp32 ops on the same fp16-rounded operands and --
+"""GPU parity of the CTA-pair form of the implicit-GEMM kernel (a 2-CTA cluster on neighbouring M tiles: every CTA loads half of the
+weight tile and multicasts it to both) through the C ABI, against plain PyTorch fp32 ops on the same fp16-rounded operands and --
 bit for bit -- against the single-CTA kernel with the same tile / split-K (same fp32 summation order per output element)."""
 import math
 

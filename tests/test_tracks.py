@@ -1,19 +1,17 @@
 """Drop-in proof for the caller of the hot path (SURVEY.md 8 a-1 / f-2), CPU only.
 
-The reference's OWN, UNMODIFIED lib/tracks.py (/root/reference/lib/tracks.py:9-38) is loaded from the read-only reference
-checkout with `aiortc` stubbed (it is not installable offline) and driven by a fake source track.  It must run against this
-repo's pipeline call contract -- `pipeline(frame)` -- through warm-up, frame dropping and steady state, and this repo's
-non-blocking adapter (host/tracks.py) must make the same pipeline calls in the same order and return the same frames.
-/root/reference does not exist on the GPU box: those cases skip there; the adapter's own behaviour is tested everywhere."""
+The reference's own, unmodified lib/tracks.py (lib/tracks.py:9-38), loaded with `aiortc` stubbed and driven by the fake source
+track and recording pipeline below, was run once per DROP_FRAMES setting; what it returned and the pipeline calls it made are
+stored in tests/golden/reference_tracks.json (tests/golden/make_golden_tracks.py records them from a reference checkout).
+This repo's non-blocking adapter (host/tracks.py) must make the same pipeline calls in the same order and return the same
+frames through warm-up, frame dropping and steady state."""
 import asyncio
-import importlib.util
+import json
 import os
-import sys
-import types
 
 import pytest
 
-REF_TRACKS = "/root/reference/lib/tracks.py"
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_tracks.json")
 
 
 class FakeSource:
@@ -58,23 +56,6 @@ class AsyncRecordingPipeline(RecordingPipeline):
         return Ticket(self(frame), polls=3)
 
 
-def _load_reference_tracks(monkeypatch):
-    if not os.path.exists(REF_TRACKS):
-        pytest.skip("reference checkout not present (GPU box)")
-    aiortc = types.ModuleType("aiortc")
-
-    class MediaStreamTrack:
-        def __init__(self):
-            self._ended = False
-
-    aiortc.MediaStreamTrack = MediaStreamTrack
-    monkeypatch.setitem(sys.modules, "aiortc", aiortc)
-    spec = importlib.util.spec_from_file_location("reference_lib_tracks", REF_TRACKS)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)     # executes the reference's file as it is; nothing is copied into this repo
-    return mod
-
-
 def _drive(track, n):
     async def go():
         return [await track.recv() for _ in range(n)]
@@ -85,20 +66,21 @@ def _drive(track, n):
 def test_reference_tracks_py_runs_unchanged_and_adapter_matches_it(monkeypatch, drop):
     monkeypatch.delenv("WARMUP_FRAMES", raising=False)
     monkeypatch.setenv("DROP_FRAMES", str(drop))
-    ref_mod = _load_reference_tracks(monkeypatch)
-    ref_pipe, our_pipe = RecordingPipeline(), AsyncRecordingPipeline()
-    ref_track = ref_mod.VideoStreamTrack(FakeSource(), ref_pipe)
+    with open(GOLDEN) as f:
+        ref = json.load(f)[str(drop)]
+    ref_out = [tuple(o) for o in ref["outputs"]]
+    ref_calls = [tuple(c) for c in ref["calls"]]
+    our_pipe = AsyncRecordingPipeline()
     from ai_rtc_agent_b200.host.tracks import VideoStreamTrack
     our_track = VideoStreamTrack(FakeSource(), our_pipe)
-    ref_out = _drive(ref_track, 5)
     our_out = _drive(our_track, 5)
     # warm-up: 10 frames through the pipeline, discarded (lib/tracks.py:21-25); then `drop` source frames skipped per output
     first = 10 + drop + 1
     assert ref_out[0] == ("processed", first)
-    assert [f[1] for f in ref_pipe.calls[:10]] == list(range(1, 11))
+    assert [c[1] for c in ref_calls[:10]] == list(range(1, 11))
     assert our_out == ref_out
-    assert our_pipe.calls == ref_pipe.calls
-    assert ref_track.warmup_frame_idx == our_track.warmup_frame_idx == 10
+    assert our_pipe.calls == ref_calls
+    assert ref["warmup_frame_idx"] == our_track.warmup_frame_idx == 10
 
 
 def test_reference_tracks_py_imports_this_repos_pipeline_module(monkeypatch):

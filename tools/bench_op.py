@@ -61,7 +61,7 @@ if "gn" in sys.argv:
         print(f"groupnorm {args}: {timeit_graph(lambda: ops.groupnorm(xa, xb, g, b, y), 20):7.2f} us per launch (chain of 20 in a graph)", flush=True)
     sys.exit(0)
 if "pairsweep" in sys.argv:
-    # CTA pairs (tcgen05.mma.cta_group::2) against the single-CTA kernel, same tile / split-K, weights streamed from HBM
+    # CTA pairs (2-CTA clusters, multicast weight tile) against the single-CTA kernel, same tile / split-K, weights streamed from HBM
     print("B2_STAGE_KB =", os.environ.get("B2_STAGE_KB", "default"))
     for (h, cin, cout, taps) in [(64, 320, 320, 9), (64, 640, 320, 9), (64, 960, 320, 9), (64, 320, 320, 1), (64, 320, 1280, 1), (64, 1280, 320, 1),
                                  (32, 640, 640, 9), (32, 1280, 640, 9), (32, 1920, 640, 9), (32, 640, 640, 1), (32, 2560, 640, 1),

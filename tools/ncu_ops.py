@@ -17,7 +17,7 @@ for rep in range(2):
     if "unet64bn160" in which:  # UNet 64^2 320->320 resnet conv as the engine plans it: 160-wide tiles + cluster split-K 4
         x = rnd(1, 64, 64, 320); w = ops.pack_conv_weight(rnd(320, 320, 3, 3, scale=1/54)); b = torch.randn(1, 320, device=dev)
         y = torch.empty_like(x); ops.igemm([(x, 9)], w, y, colbias=b, bn=160, splits=4)
-    if "unet64pair" in which:   # ... and as the throughput policy plans it: CTA pairs (cta_group::2), 160-wide tiles, no split-K
+    if "unet64pair" in which:   # ... and as the throughput policy plans it: CTA pairs (2-CTA clusters), 160-wide tiles, no split-K
         x = rnd(1, 64, 64, 320); w = ops.pack_conv_weight(rnd(320, 320, 3, 3, scale=1/54)); b = torch.randn(1, 320, device=dev)
         y = torch.empty_like(x); ops.igemm([(x, 9)], w, y, colbias=b, bn=160, pair=True)
     if "unet32pair" in which:   # UNet 32^2 1280->640 (up block, K = 11520) on CTA pairs

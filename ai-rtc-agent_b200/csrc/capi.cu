@@ -176,6 +176,8 @@ int b2sd_op_groupnorm(const void* xa, int ca, int lda, const void* xb, int cb, i
     return groupnorm_launch(a, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int b2sd_groupnorm_last_path(void) { return groupnorm_last_path(); }
+
 int b2sd_op_layernorm(const void* x, int ldx, const float* gamma, const float* beta, void* y, int ldy,
                       int64_t rows, int c, float eps, void* stream) {
     return layernorm_launch(reinterpret_cast<const __half*>(x), ldx, gamma, beta, reinterpret_cast<__half*>(y), ldy,

@@ -339,7 +339,9 @@ __global__ void __launch_bounds__(512) gn_fused_kernel(GroupNormArgs a, int ppc,
 }
 
 static thread_local int g_gn_last_launches = 0;
+static thread_local int g_gn_last_path = -1;
 int groupnorm_last_launch_count() { return g_gn_last_launches; }
+int groupnorm_last_path() { return g_gn_last_path; }
 // ---- cluster variant (default when it fits): one thread-block cluster per (batch item, group).  The group's
 // cpg = C/groups channels are a contiguous 2*cpg-byte run per pixel; the pixels are split over the 1/2/4/8 CTAs of the
 // cluster, every thread keeps its <= 32 half2 words in registers, the (sum, sumsq) pairs of the CTAs are pushed into
@@ -464,6 +466,7 @@ int groupnorm_launch(const GroupNormArgs& a, cudaStream_t s) {
         const int ppc = (a.hw + cl - 1) / cl;
         B2_LAUNCHED("gn_cluster", launch_k(gn_cluster_kernel, dim3(a.groups, a.nb, cl), dim3(GNC_THREADS), 0, s, cl, a, ppc));
         g_gn_last_launches = 1;
+        g_gn_last_path = GN_PATH_CLUSTER;
         return 0;
     }
     const int vc = C / 8;
@@ -507,6 +510,7 @@ int groupnorm_launch(const GroupNormArgs& a, cudaStream_t s) {
             return -1;
         }
         g_gn_last_launches = 1;
+        g_gn_last_path = GN_PATH_FUSED;
         return 0;
     }
     B2_LAUNCHED("gn_stats", launch_k(gn_stats_kernel, dim3(nchunks, a.nb), dim3(threads), smem, s, 1, a, ppc, vc, rpi));
@@ -516,6 +520,7 @@ int groupnorm_launch(const GroupNormArgs& a, cudaStream_t s) {
     if (blocks > cap) blocks = cap;
     B2_LAUNCHED("gn_apply", launch_k(gn_apply_kernel, dim3((unsigned)blocks, a.nb), dim3(256), 0, s, 1, a, nchunks, vec_per_batch));
     g_gn_last_launches = 2;
+    g_gn_last_path = GN_PATH_STATS_APPLY;
     return 0;
 }
 

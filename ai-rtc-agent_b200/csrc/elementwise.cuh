@@ -25,7 +25,10 @@ size_t groupnorm_partial_floats(int nb, int groups);
 // host-only: which kernel groupnorm_launch would use.  Returns the cluster size (1/2/4/8) and fills threads per CTA and
 // pixels per CTA for gn_cluster_kernel, or 0 when the whole-grid kernel is used.
 int groupnorm_plan(const GroupNormArgs& a, int* threads, int* pixels_per_cta);
-int groupnorm_last_launch_count();  // 1 (cooperative single launch) or 2, for the most recent call on this thread
+int groupnorm_last_launch_count();  // 1 (cluster or cooperative single launch) or 2, for the most recent call on this thread
+// kernel path of the most recent groupnorm_launch on this thread (-1 before the first)
+enum : int { GN_PATH_CLUSTER = 0, GN_PATH_FUSED = 1, GN_PATH_STATS_APPLY = 2 };
+int groupnorm_last_path();
 
 // LayerNorm over the last dim of [rows][c] fp16 (eps 1e-5, affine), one warp per row.
 int layernorm_launch(const __half* x, int ldx, const float* gamma, const float* beta, __half* y, int ldy,

@@ -96,6 +96,8 @@ def lib() -> C.CDLL:
         vp, ci, cf, i64 = C.c_void_p, C.c_int, C.c_float, C.c_int64
         _lib.b2sd_op_attention.argtypes = [C.POINTER(AttnDesc), vp]
         _lib.b2sd_op_groupnorm.argtypes = [vp, ci, ci, vp, ci, ci, vp, vp, vp, ci, ci, ci, ci, cf, ci, vp]
+        _lib.b2sd_groupnorm_last_path.argtypes = []
+        _lib.b2sd_groupnorm_last_path.restype = C.c_int
         _lib.b2sd_op_layernorm.argtypes = [vp, ci, vp, vp, vp, ci, i64, ci, cf, vp]
         _lib.b2sd_op_upsample2x.argtypes = [vp, vp, ci, ci, ci, ci, vp]
         _lib.b2sd_op_smallconv.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ci, ci, vp]

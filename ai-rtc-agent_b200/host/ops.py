@@ -37,6 +37,26 @@ def igemm(srcs: Sequence[Tuple[torch.Tensor, int]], w: torch.Tensor, out: torch.
           colsum: Optional[torch.Tensor] = None, ln_c: int = 0, ln_eps: float = 1e-5,
           out2: Optional[torch.Tensor] = None, col2: int = 0) -> torch.Tensor:
     """srcs: [(NHWC fp16 tensor, ntap)], w: packed fp16 [rows, K]; out: NHWC fp16 [nb,ho,wo,ldc>=n]."""
+    d = _igemm_desc(srcs, w, out, stride=stride, colbias=colbias, res=res, acc_scale=acc_scale, res_scale=res_scale, relu=relu,
+                    geglu=geglu, bn=bn, splits=splits, n_valid=n_valid, timeline=timeline, swap=swap, tconv=tconv, pair=pair,
+                    rowstat_out=rowstat_out, rowstat_in=rowstat_in, colsum=colsum, ln_c=ln_c, ln_eps=ln_eps, out2=out2, col2=col2)
+    capi.check(capi.lib().b2sd_op_igemm(C.byref(d), capi.current_stream_ptr()), "b2sd_op_igemm")
+    return out
+
+
+def igemm_engine_plan(srcs, w, out, *, autotile: int = 1, allow_swap: bool = True, **kw) -> capi.IgemmPlanInfo:
+    """The tile / split-K / orientation / CTA-pair choice the engine's tile policy makes for this contraction (autotile 1:
+    one frame in flight, 2: >= 4 frames in flight), from the host-only planner; no launch.  Pass its bn, splits, swap and
+    pair (mode == 1) to igemm() to run the contraction the way the frame program does."""
+    d = _igemm_desc(srcs, w, out, **kw)
+    info = capi.IgemmPlanInfo()
+    capi.check(capi.lib().b2sd_igemm_plan_dry(C.byref(d), autotile, int(allow_swap), C.byref(info)), "b2sd_igemm_plan_dry")
+    return info
+
+
+def _igemm_desc(srcs, w, out, *, stride=1, colbias=None, res=None, acc_scale=1.0, res_scale=1.0, relu=False, geglu=False,
+                bn=0, splits=1, n_valid=None, timeline=None, swap=False, tconv=False, pair=False, rowstat_out=None,
+                rowstat_in=None, colsum=None, ln_c=0, ln_eps=1e-5, out2=None, col2=0) -> capi.IgemmDesc:
     d = capi.IgemmDesc()
     d.nseg = len(srcs)
     for i, (t, ntap) in enumerate(srcs):
@@ -72,8 +92,7 @@ def igemm(srcs: Sequence[Tuple[torch.Tensor, int]], w: torch.Tensor, out: torch.
     if out2 is not None:
         assert out2.dtype == torch.float16 and out2.dim() == 2 and out2.stride(1) == 1
         d.out2, d.ld2, d.col2 = out2.data_ptr(), out2.stride(0), col2
-    capi.check(capi.lib().b2sd_op_igemm(C.byref(d), capi.current_stream_ptr()), "b2sd_op_igemm")
-    return out
+    return d
 
 
 def _sp():
@@ -92,14 +111,20 @@ def attention(q, k, vt, out, *, nb, heads, sq, skv, d_real, dp, k_bstride, vt_bs
     return out
 
 
-def groupnorm(xa, xb, gamma, beta, y, *, groups=32, eps=1e-5, silu=True):
-    """xa/xb: NHWC fp16 (xb may be None); y: NHWC fp16 with C = ca + cb."""
+GN_PATHS = {0: "cluster", 1: "fused", 2: "stats+apply"}
+
+
+def groupnorm(xa, xb, gamma, beta, y, *, groups=32, eps=1e-5, silu=True, return_path=False):
+    """xa/xb: NHWC fp16 (xb may be None); y: NHWC fp16 with C = ca + cb.  return_path: also return the kernel path that ran
+    ("cluster", "fused" or "stats+apply", see b2sd_groupnorm_last_path)."""
     nb, h, w, ca = xa.shape
     cb = 0 if xb is None else xb.shape[3]
     capi.check(capi.lib().b2sd_op_groupnorm(
         xa.data_ptr(), ca, xa.stride(2), 0 if xb is None else xb.data_ptr(), cb, 0 if xb is None else xb.stride(2),
         gamma.data_ptr(), beta.data_ptr(), y.data_ptr(), y.stride(2), nb, h * w, groups, eps, int(silu), _sp()),
         "b2sd_op_groupnorm")
+    if return_path:
+        return y, GN_PATHS[capi.lib().b2sd_groupnorm_last_path()]
     return y
 
 

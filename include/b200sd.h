@@ -126,6 +126,9 @@ int b2sd_op_attention(const b2sd_attn_desc* d, void* stream);
 int b2sd_op_groupnorm(const void* xa, int ca, int lda, const void* xb, int cb, int ldb, const float* gamma,
                       const float* beta, void* y, int ldy, int nb, int hw, int groups, float eps, int silu,
                       void* stream);
+/* Kernel path of the most recent GroupNorm launch issued on the calling thread: 0 = one thread-block cluster per
+ * (image, group), 1 = cooperative single-launch kernel, 2 = statistics + apply launches, -1 = none yet. */
+int b2sd_groupnorm_last_path(void);
 int b2sd_op_layernorm(const void* x, int ldx, const float* gamma, const float* beta, void* y, int ldy,
                       int64_t rows, int c, float eps, void* stream);
 int b2sd_op_upsample2x(const void* x, void* y, int nb, int h, int w, int c, void* stream);

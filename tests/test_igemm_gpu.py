@@ -2,14 +2,17 @@
 the C ABI (b2sd_op_igemm) against plain PyTorch fp32 ops on the same fp16-rounded operands.
 
 Tolerance: operands are exact fp16; accumulation is fp32 in both; the only difference is the final
-fp16 rounding of the output (rel 2^-11) plus accumulation-order noise => abs 2e-3*scale + rel 2e-3."""
+fp16 rounding of the output (rel 2^-11) plus accumulation-order noise => abs 2e-3*scale + rel 2e-3.
+
+References of the LayerNorm-folded and prompt-side / ragged-N contractions are float64 on the GPU; the large conv / GEMM
+references stay fp32 with TF32 off (the cuda fixture)."""
 import math
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.util import assert_close
+from tests.util import assert_close, assert_discriminates, guarded, hetero, offset_heavy_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -282,51 +285,100 @@ def test_linear_row_statistics(cuda, m, k, n, splits):
     assert_close(got, want, 2e-3, 1e-5, "row statistics")
 
 
+def _ln_rows(x2d, gamma, beta, neighbour=False):
+    """float64 LayerNorm (eps 1e-5) of the rows of x2d; neighbour=True normalises row r with the statistics of row r-1 (the
+    wrong reference for a row-indexing error of the folded epilogue under split-K, CTA pairs and N tiles)."""
+    xd = x2d.double()
+    mean, var = xd.mean(1, keepdim=True), xd.var(1, unbiased=False, keepdim=True)
+    if neighbour:
+        mean, var = mean.roll(1, 0), var.roll(1, 0)
+    return (xd - mean) * (var + 1e-5).rsqrt() * gamma.double() + beta.double()
+
+
+def _fixed_point_rowstats(x2d):
+    xf = x2d.double()
+    return torch.stack([xf.sum(1), (xf * xf).sum(1)], dim=1).mul(STAT_SCALE).round().to(torch.int64).contiguous()
+
+
 @pytest.mark.parametrize("m,k,n,splits", [(4096, 320, 640, 1), (256, 1280, 2560, 2), (64, 1280, 1280, 4)])
 def test_linear_layernorm_folded(cuda, m, k, n, splits):
-    """y = LayerNorm(x) W^T + b computed as rstd (x W'^T - mean colsum) + bias' from the producer's row statistics."""
+    """y = LayerNorm(x) W^T + b computed as rstd (x W'^T - mean colsum) + bias' from the producer's row statistics.  Every row
+    has its own offset and scale, so a row normalised with another row's statistics is off by O(1)."""
     ops = _ops()
-    x = (_rand((1, 1, m, k), cuda, 1) * 1.5 + 0.3).to(torch.float16)     # non-zero mean
+    x = hetero((1, 1, m, k), (2,), 1, cuda)
     w = _rand((n, k), cuda, 2, 1.0 / math.sqrt(k)).to(torch.float16)
     gamma = (1.0 + 0.1 * _rand((k,), cuda, 3)).float()
     beta = (0.1 * _rand((k,), cuda, 4)).float()
     bias = _rand((n,), cuda, 5).float()
     wp, colsum, bprime = _ln_fold_operands(w, gamma, beta, bias)
-    xf = x.reshape(m, k).double()
-    st = torch.stack([xf.sum(1), (xf * xf).sum(1)], dim=1).mul(STAT_SCALE).round().to(torch.int64).contiguous()
+    st = _fixed_point_rowstats(x.reshape(m, k))
     out = torch.full((1, 1, m, n), float("nan"), dtype=torch.float16, device=cuda)
     ops.igemm([(x, 1)], wp, out, colbias=bprime.reshape(1, n).contiguous(), splits=splits, rowstat_in=st, colsum=colsum, ln_c=k)
-    ln = F.layer_norm(x.reshape(m, k).float(), (k,), gamma, beta, 1e-5)
-    ref = ln @ w.float().t() + bias
-    assert_close(out.reshape(m, n), ref, 6e-3, 4e-3, f"LN-folded linear m={m} k={k} n={n}")
+    ref = _ln_rows(x.reshape(m, k), gamma, beta) @ w.double().t() + bias.double()
+    wrong = _ln_rows(x.reshape(m, k), gamma, beta, neighbour=True) @ w.double().t() + bias.double()
+    assert_discriminates(out.reshape(m, n), ref, wrong, 6e-3, 4e-3, f"LN-folded linear m={m} k={k} n={n}",
+                         "statistics of the neighbouring row")
 
 
-def test_fused_qkv_projection_with_transposed_v(cuda):
-    """One GEMM over [Wq | Wk | Wv] with LayerNorm folded: q/k columns row-major, the V block stored as V^T [C][tokens]
-    (the K-major operand of the attention P.V MMA), replacing a separate swapped-operand GEMM launch."""
+@pytest.mark.parametrize("m,k,n,splits", [(1024, 640, 640, 1), (256, 1280, 1280, 4)])
+def test_linear_layernorm_folded_offset_heavy(cuda, m, k, n, splits):
+    """Rows with |mean|/std of 30..100: the folded epilogue (ln_row_stats) takes the variance as E[x^2] - mean^2 in fp32 from
+    the fixed-point row sums and subtracts mean * colsum from the accumulator; this pins that range as the one in which both
+    hold the usual tolerance.  The error, in units of the tolerance, is printed."""
+    ops = _ops()
+    x = offset_heavy_rows(m, k, cuda).reshape(1, 1, m, k)
+    w = _rand((n, k), cuda, 2, 1.0 / math.sqrt(k)).to(torch.float16)
+    gamma = (1.0 + 0.1 * _rand((k,), cuda, 3)).float()
+    beta = (0.1 * _rand((k,), cuda, 4)).float()
+    bias = _rand((n,), cuda, 5).float()
+    wp, colsum, bprime = _ln_fold_operands(w, gamma, beta, bias)
+    st = _fixed_point_rowstats(x.reshape(m, k))
+    out = torch.full((1, 1, m, n), float("nan"), dtype=torch.float16, device=cuda)
+    ops.igemm([(x, 1)], wp, out, colbias=bprime.reshape(1, n).contiguous(), splits=splits, rowstat_in=st, colsum=colsum, ln_c=k)
+    ref = _ln_rows(x.reshape(m, k), gamma, beta) @ w.double().t() + bias.double()
+    err = ((out.reshape(m, n).double() - ref).abs() / (6e-3 + 4e-3 * ref.abs())).max().item()
+    print(f"LN-folded linear offset-heavy m={m} k={k} n={n} splits={splits}: max error = {err:.3f} x tolerance")
+    wrong = _ln_rows(x.reshape(m, k), gamma, beta, neighbour=True) @ w.double().t() + bias.double()
+    assert_discriminates(out.reshape(m, n), ref, wrong, 6e-3, 4e-3, f"offset-heavy LN-folded linear m={m} k={k} n={n}",
+                         "statistics of the neighbouring row")
+
+
+def fused_qkv_case(cuda, pair):
+    """One GEMM over [Wq | Wk | Wv] with LayerNorm folded, q | k written with the engine's row pitch and V^T [C][tokens] through
+    out2, both into guarded buffers whose pitch is wider than their data (the engine's bump-allocated arena has neighbours on
+    both sides)."""
     ops = _ops()
     m, c = 4096, 320
-    x = (_rand((1, 1, m, c), cuda, 1) + 0.2).to(torch.float16)
+    x = hetero((1, 1, m, c), (2,), 1, cuda)
     wq, wk, wv = (_rand((c, c), cuda, s, 1.0 / math.sqrt(c)).to(torch.float16) for s in (2, 3, 4))
     gamma = (1.0 + 0.1 * _rand((c,), cuda, 5)).float()
     beta = (0.1 * _rand((c,), cuda, 6)).float()
     w = torch.cat([wq, wk, wv]).contiguous()
     wp, colsum, bprime = _ln_fold_operands(w, gamma, beta, None)
-    xf = x.reshape(m, c).double()
-    st = torch.stack([xf.sum(1), (xf * xf).sum(1)], dim=1).mul(STAT_SCALE).round().to(torch.int64).contiguous()
-    qk = torch.full((1, 1, m, 2 * c), float("nan"), dtype=torch.float16, device=cuda)
-    vt = torch.full((c, m), float("nan"), dtype=torch.float16, device=cuda)
-    ops.igemm([(x, 1)], wp, qk, colbias=bprime.reshape(1, -1).contiguous(), n_valid=3 * c, rowstat_in=st, colsum=colsum, ln_c=c,
-              out2=vt, col2=2 * c, bn=160)
-    ln = F.layer_norm(x.reshape(m, c).float(), (c,), gamma, beta, 1e-5)
-    assert_close(qk.reshape(m, 2 * c), ln @ torch.cat([wq, wk]).float().t(), 6e-3, 4e-3, "q | k")
-    assert_close(vt, (ln @ wv.float().t()).t(), 6e-3, 4e-3, "V^T")
+    st = _fixed_point_rowstats(x.reshape(m, c))
+    qk = guarded((m, 2 * c), pitch=2 * c + 64, device=cuda)
+    vt = guarded((c, m), pitch=m + 64, device=cuda)
+    ops.igemm([(x, 1)], wp, qk.view[None, None], colbias=bprime.reshape(1, -1).contiguous(), n_valid=3 * c, rowstat_in=st,
+              colsum=colsum, ln_c=c, out2=vt.view, col2=2 * c, bn=160, pair=pair)
+    qk.assert_untouched("q | k")
+    vt.assert_untouched("V^T")
+    ln, ln_wrong = _ln_rows(x.reshape(m, c), gamma, beta), _ln_rows(x.reshape(m, c), gamma, beta, neighbour=True)
+    wqk = torch.cat([wq, wk]).double().t()
+    bug = "statistics of the neighbouring row"
+    assert_discriminates(qk.view, ln @ wqk, ln_wrong @ wqk, 6e-3, 4e-3, "q | k", bug)
+    assert_discriminates(vt.view, (ln @ wv.double().t()).t(), (ln_wrong @ wv.double().t()).t(), 6e-3, 4e-3, "V^T", bug)
+
+
+def test_fused_qkv_projection_with_transposed_v(cuda):
+    """The V block stored as V^T [C][tokens] (the K-major operand of the attention P.V MMA), replacing a separate
+    swapped-operand GEMM launch."""
+    fused_qkv_case(cuda, pair=False)
 
 
 def test_geglu_layernorm_folded(cuda):
     ops = _ops()
     m, k, inner = 1024, 320, 1280
-    x = (_rand((1, 1, m, k), cuda, 1) + 0.25).to(torch.float16)
+    x = hetero((1, 1, m, k), (2,), 1, cuda)
     w = _rand((2 * inner, k), cuda, 2, 1.0 / math.sqrt(k)).to(torch.float16)
     b = _rand((2 * inner,), cuda, 3).float()
     gamma = (1.0 + 0.1 * _rand((k,), cuda, 4)).float()
@@ -338,11 +390,91 @@ def test_geglu_layernorm_folded(cuda):
         idx += list(range(inner + t * half, inner + (t + 1) * half))
     idx = torch.tensor(idx, device=cuda)
     wp, colsum, bprime = _ln_fold_operands(w[idx].contiguous(), gamma, beta, b[idx])
-    xf = x.reshape(m, k).double()
-    st = torch.stack([xf.sum(1), (xf * xf).sum(1)], dim=1).mul(STAT_SCALE).round().to(torch.int64).contiguous()
+    st = _fixed_point_rowstats(x.reshape(m, k))
     out = torch.empty((1, 1, m, inner), dtype=torch.float16, device=cuda)
     ops.igemm([(x, 1)], wp, out, colbias=bprime.reshape(1, -1).contiguous(), geglu=True, bn=128, n_valid=inner,
               rowstat_in=st, colsum=colsum, ln_c=k)
-    proj = F.layer_norm(x.reshape(m, k).float(), (k,), gamma, beta, 1e-5) @ w.float().t() + b
-    ref = proj[:, :inner] * F.gelu(proj[:, inner:])
-    assert_close(out.reshape(m, inner), ref, 8e-3, 5e-3, "LN-folded GEGLU")
+
+    def geglu_ref(neighbour):
+        proj = _ln_rows(x.reshape(m, k), gamma, beta, neighbour) @ w.double().t() + b.double()
+        return proj[:, :inner] * F.gelu(proj[:, inner:])
+    assert_discriminates(out.reshape(m, inner), geglu_ref(False), geglu_ref(True), 8e-3, 5e-3, "LN-folded GEGLU",
+                         "statistics of the neighbouring row")
+
+
+# ---- prompt-side and ragged-N contractions, run with the tiles the engine's policy picks ----------------------------------------
+def _engine_tiles(ops, srcs, w, out, autotile, allow_swap, **kw):
+    info = ops.igemm_engine_plan(srcs, w, out, autotile=autotile, allow_swap=allow_swap, **kw)
+    return dict(bn=info.bn, splits=info.splits, swap=bool(info.swap), pair=info.mode == 1)
+
+
+def _gemm64(a, b):
+    """float64 a @ b^T on the GPU (the prompt-side GEMMs are small)."""
+    return a.double() @ b.double().t()
+
+
+@pytest.mark.parametrize("autotile", [1, 2])
+@pytest.mark.parametrize("d", [768, 1024])
+@pytest.mark.parametrize("cp", [320, 512, 1024, 1536])
+def test_prompt_vt_projection(cuda, cp, d, autotile):
+    """The cross-attention V^T cache as the engine builds it (engine.cu, prompt program): to_v weights [Cp, D] on the M side,
+    the 77-token context [77, D] on the N side, n_valid = 77 written with a row pitch of 128.  Columns 77..127 and the rows
+    after Cp are guarded.  Catches: a ragged N tile storing past n_valid, V^T columns shifted by one token."""
+    ops = _ops()
+    L, pitch = 77, 128
+    wv = _rand((1, 1, cp, d), cuda, 1, 1.0 / math.sqrt(d)).to(torch.float16)
+    ctx = hetero((L, d), (0,), 2, cuda, offset=1.0, scale=(0.5, 2.0))
+    out = guarded((cp, L), pitch=pitch, device=cuda)
+    o4 = out.view[None, None]
+    tiles = _engine_tiles(ops, [(wv, 1)], ctx, o4, autotile, False, n_valid=L)
+    ops.igemm([(wv, 1)], ctx, o4, n_valid=L, **tiles)
+    out.assert_untouched(f"prompt V^T cp={cp} d={d} {tiles}")
+    ref = _gemm64(wv.reshape(cp, d), ctx)
+    assert_discriminates(out.view, ref, ref.roll(1, 1), 2e-3, 2e-3, f"prompt V^T cp={cp} d={d} {tiles}",
+                         "token columns shifted by one")
+
+
+@pytest.mark.parametrize("autotile", [1, 2])
+@pytest.mark.parametrize("cp", [512, 1024, 1536])
+def test_prompt_k_projection_sd15(cuda, cp, autotile):
+    """K of the SD-1.5 prompt cache: ctx [77, 768] x to_k [Cp, 768]^T, 77 rows (a partial M tile) with the tiles the engine
+    picks; the rows after the 77th are guarded.  Catches: rows of the partial M tile written past the end, a dropped K block."""
+    ops = _ops()
+    L, d = 77, 768
+    ctx = hetero((1, 1, L, d), (2,), 2, cuda, offset=1.0, scale=(0.5, 2.0))
+    wk = _rand((cp, d), cuda, 1, 1.0 / math.sqrt(d)).to(torch.float16)
+    out = guarded((L, cp), device=cuda)
+    o4 = out.view[None, None]
+    tiles = _engine_tiles(ops, [(ctx, 1)], wk, o4, autotile, False)
+    ops.igemm([(ctx, 1)], wk, o4, **tiles)
+    out.assert_untouched(f"prompt K cp={cp} {tiles}")
+    ref = _gemm64(ctx.reshape(L, d), wk)
+    wrong = _gemm64(ctx.reshape(L, d)[:, 64:], wk[:, 64:])
+    assert_discriminates(out.view, ref, wrong, 2e-3, 2e-3, f"prompt K cp={cp} {tiles}", "first K block dropped")
+
+
+@pytest.mark.parametrize("autotile", [1, 2])
+@pytest.mark.parametrize("n", [77, 100, 120])
+@pytest.mark.parametrize("m,k", [(4096, 320), (1024, 640), (256, 1280)])
+def test_ragged_n_linear(cuda, m, k, n, autotile):
+    """N not a multiple of 16, with bias and residual, through the plan the engine's tile policy picks (the swapped orientation
+    where it allows it: n % 8 == 0), into a guarded output with spare columns up to the next multiple of 64.  Catches: stores
+    past n_valid, bias / residual columns misaligned by one."""
+    ops = _ops()
+    x = _rand((1, 1, m, k), cuda, 1).to(torch.float16)
+    w = _rand((n, k), cuda, 2, 1.0 / math.sqrt(k)).to(torch.float16)
+    bias = _rand((1, n), cuda, 3).float().contiguous()
+    pitch = -(-n // 64) * 64 + 64
+    res = hetero((m, pitch), (1,), 4, cuda)[:, :n]     # the residual stream is read through the same kind of pitched view
+    out = guarded((m, n), pitch=pitch, device=cuda)
+    o4 = out.view[None, None]
+    tiles = _engine_tiles(ops, [(x, 1)], w, o4, autotile, True, colbias=bias, res=res[None, None])
+    ops.igemm([(x, 1)], w, o4, colbias=bias, res=res[None, None], **tiles)
+    what = f"ragged linear m={m} k={k} n={n} {tiles}"
+    out.assert_untouched(what)
+    acc = _gemm64(x.reshape(m, k), w)
+    ref = acc + bias.double() + res.double()
+    assert_discriminates(out.view, ref, acc + bias.double() + res.double().roll(1, 1), 4e-3, 3e-3, what,
+                         "residual columns shifted by one")
+    assert_discriminates(out.view, ref, acc + bias.double().roll(1, 1) + res.double(), 4e-3, 3e-3, what,
+                         "bias columns shifted by one")

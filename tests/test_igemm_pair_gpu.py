@@ -7,7 +7,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.test_igemm_gpu import STAT_SCALE, _ln_fold_operands, _nhwc16, _ops, _rand, _ref_conv
+from tests.test_igemm_gpu import STAT_SCALE, _nhwc16, _ops, _rand, _ref_conv, fused_qkv_case
 from tests.util import assert_close
 
 pytestmark = pytest.mark.gpu
@@ -67,23 +67,7 @@ def test_conv3x3_pair(cuda, nb, h, w, cin, cout, stride, bn, splits, relu):
 
 def test_fused_qkv_pair(cuda):
     """LayerNorm-folded fused q/k/v projection with the transposed V store, on CTA pairs."""
-    ops = _ops()
-    m, c = 4096, 320
-    x = (_rand((1, 1, m, c), cuda, 1) + 0.2).to(torch.float16)
-    wq, wk, wv = (_rand((c, c), cuda, s, 1.0 / math.sqrt(c)).to(torch.float16) for s in (2, 3, 4))
-    gamma = (1.0 + 0.1 * _rand((c,), cuda, 5)).float()
-    beta = (0.1 * _rand((c,), cuda, 6)).float()
-    w = torch.cat([wq, wk, wv]).contiguous()
-    wp, colsum, bprime = _ln_fold_operands(w, gamma, beta, None)
-    xf = x.reshape(m, c).double()
-    st = torch.stack([xf.sum(1), (xf * xf).sum(1)], dim=1).mul(STAT_SCALE).round().to(torch.int64).contiguous()
-    qk = torch.full((1, 1, m, 2 * c), float("nan"), dtype=torch.float16, device=cuda)
-    vt = torch.full((c, m), float("nan"), dtype=torch.float16, device=cuda)
-    ops.igemm([(x, 1)], wp, qk, colbias=bprime.reshape(1, -1).contiguous(), n_valid=3 * c, rowstat_in=st, colsum=colsum, ln_c=c,
-              out2=vt, col2=2 * c, bn=160, pair=True)
-    ln = F.layer_norm(x.reshape(m, c).float(), (c,), gamma, beta, 1e-5)
-    assert_close(qk.reshape(m, 2 * c), ln @ torch.cat([wq, wk]).float().t(), 6e-3, 4e-3, "q | k")
-    assert_close(vt, (ln @ wv.float().t()).t(), 6e-3, 4e-3, "V^T")
+    fused_qkv_case(cuda, pair=True)
 
 
 def test_geglu_pair(cuda):

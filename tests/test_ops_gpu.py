@@ -1,14 +1,18 @@
 """GPU parity of the attention and SIMT helper kernels through the C ABI against PyTorch fp32 ops.
 
 Tolerances: fp16 operands, fp32 math; outputs rounded to fp16 once.  Attention additionally rounds
-P to fp16 before P.V (as every fp16 flash-attention does): abs 2e-3 on O(1) outputs."""
+P to fp16 before P.V (as every fp16 flash-attention does): abs 2e-3 on O(1) outputs.
+
+The discriminating tests (hetero inputs, poisoned keys, guarded outputs) compute their references in float64 on the GPU and
+check, with assert_discriminates, that a named plausible bug would land well outside the tolerance."""
+import ctypes
 import math
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.util import assert_close
+from tests.util import assert_close, assert_discriminates, guarded, hetero, offset_heavy_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -78,12 +82,172 @@ def test_cross_attention_shared_kv(cuda, nb, heads, seq, d, dp, skv):
     assert_close(out, ref, 2e-3, 4e-3, f"cross-attn nb={nb} heads={heads} seq={seq}")
 
 
+# ---- attention under poison: masks, batch strides, padded head dims, peaked softmax -----------------------------------------
+ATTN_TOL = (2e-3, 4e-3)
+
+
+def _bkv(dp):
+    return 64 if dp == 192 else 128   # KV block of attn_kernel (the dp = 192 variant halves it)
+
+
+def _attn64(q, k, v, d):
+    """float64 softmax(q k^T / sqrt(d)) v; q [nb,heads,sq,d], k/v [nb or 1,heads,skv,d]; returns [nb*sq, heads*d]."""
+    s = q.double() @ k.double().transpose(-1, -2) / math.sqrt(d)
+    o = torch.softmax(s, dim=-1) @ v.double()
+    return o.permute(0, 2, 1, 3).reshape(q.shape[0] * q.shape[2], -1)
+
+
+def _q_layout(q, dp):
+    """[nb,heads,sq,d] -> the kernel's [nb*sq, heads*dp] (each head zero-padded to dp)."""
+    nb, heads, sq, d = q.shape
+    qp = torch.zeros(nb, sq, heads, dp, dtype=torch.float16, device=q.device)
+    qp[..., :d] = q.permute(0, 2, 1, 3)
+    return qp.reshape(nb * sq, heads * dp)
+
+
+def _vt_layout(v, dp, pitch=None):
+    """[nb,heads,skv,d] -> V^T [heads*dp, nb*skv] (key index contiguous), or, for a single batch item, with row pitch `pitch`."""
+    nb, heads, skv, d = v.shape
+    cols = nb * skv if pitch is None else pitch
+    vt = torch.zeros(heads, dp, cols, dtype=torch.float16, device=v.device)
+    vt[:, :d, :nb * skv] = v.permute(1, 3, 0, 2).reshape(heads, d, nb * skv)
+    return vt.reshape(heads * dp, cols)
+
+
+@pytest.mark.parametrize("seq", [144, 576, 4096 + 64])
+@pytest.mark.parametrize("d,dp", [(64, 64), (80, 128), (160, 192)])
+def test_self_attention_batch_tail_poisoned(cuda, seq, d, dp):
+    """Four batch items packed with k_bstride = vt_bstride = seq, as the engine packs them: the tail KV tile of batch item b
+    reads the leading keys of item b+1.  Those keys carry a component along a direction that only item b's queries share, so
+    their logit for item b's queries is ~+30 (a mask leak moves the output by O(1), not O(1/seq)), while for item b+1 they are
+    ordinary keys; their values are raised by 16.  Values get their own offset per (batch item, head).  Catches: the tail not
+    masked, a mask one column too wide, item 0's values used for every item (V^T batch stride ignored).  The output is written
+    with ldo > heads*d into a guarded buffer."""
+    ops = _ops()
+    nb, heads = 4, 2
+    bkv = _bkv(dp)
+    tail = -(-seq // bkv) * bkv - seq        # keys of item b+1 that item b's last tile reads
+    q = _rand((nb, heads, seq, d), cuda, 1)
+    k = _rand((nb, heads, seq, d), cuda, 2)
+    v = hetero((nb, heads, seq, d), (0, 1), 3, cuda, scale=(0.5, 2.0)).float()
+    q[..., :nb] = 0
+    k[..., :nb] = 0
+    big = 7.5 * math.sqrt(d)                 # logit 4 * big / sqrt(d) = 30
+    for b in range(nb):
+        q[b, :, :, b] = 4.0
+        if b + 1 < nb and tail:
+            k[b + 1, :, :tail, b] = big
+            v[b + 1, :, :tail] += 16.0
+    q, k, v = q.half(), k.half(), v.half()
+    out = guarded((nb * seq, heads * d), pitch=heads * d + 64, device=cuda)
+    ops.attention(_q_layout(q, dp), _q_layout(k, dp), _vt_layout(v, dp), out.view, nb=nb, heads=heads, sq=seq, skv=seq,
+                  d_real=d, dp=dp, k_bstride=seq, vt_bstride=seq)
+    out.assert_untouched(f"self-attn out seq={seq} d={d}/{dp}")
+    ref = _attn64(q, k, v, d)
+    what = f"self-attn nb={nb} seq={seq} d={d}/{dp} (tail reads {tail} keys of the next item)"
+    if tail:
+        # item b sees item b+1's first `extra` keys as well (the last item's tail is out of bounds: zero keys, masked)
+        def leak(extra):
+            kk = torch.cat([k, torch.cat([k[1:, :, :extra], torch.zeros_like(k[:1, :, :extra])])], dim=2)
+            vv = torch.cat([v, torch.cat([v[1:, :, :extra], torch.zeros_like(v[:1, :, :extra])])], dim=2)
+            return _attn64(q, kk, vv, d)
+        assert_discriminates(out.view, ref, leak(tail), *ATTN_TOL, what, "tail tile not masked")
+        assert_discriminates(out.view, ref, leak(1), *ATTN_TOL, what, "kv mask one column too wide")
+    s = q.double() @ k.double().transpose(-1, -2) / math.sqrt(d)
+    wrong_v = (torch.softmax(s, dim=-1) @ v[:1].double()).permute(0, 2, 1, 3).reshape(nb * seq, -1)
+    assert_discriminates(out.view, ref, wrong_v, *ATTN_TOL, what, "batch item 0's values for every item")
+
+
+@pytest.mark.parametrize("nb", [1, 4])
+@pytest.mark.parametrize("d,dp,heads", [(40, 64, 8), (64, 64, 5), (80, 128, 8), (160, 192, 8)])
+@pytest.mark.parametrize("rows", [128, 77])
+def test_cross_attention_prompt_poisoned(cuda, nb, d, dp, heads, rows):
+    """attn2 against the 77-token prompt K / V^T cache shared by every batch item (k_bstride = vt_bstride = 0), V^T with row
+    pitch 128.  rows = 128: K and V^T handed over with 128 rows / columns, of which 77..127 are poison (a logit of ~+30 for every
+    query, values of 64) that only the skv = 77 mask keeps out.  rows = 77: the engine's k_rows = vt_cols = 77, with the same
+    poison sitting in memory just past the tensor-map bounds.  dp = 192 runs KV blocks of 64: the second has 13 valid
+    columns.  Catches: a mask one column too wide, a KV tail not masked, reading past k_rows / vt_cols."""
+    ops = _ops()
+    skv, sq = 77, 576
+    q = _rand((nb, heads, sq, d), cuda, 1) * 1.5
+    q[..., 0] = 4.0
+    k = _rand((1, heads, 128, d), cuda, 2)
+    k[..., 0] = 0.0
+    k[:, :, skv:, 0] = 7.5 * math.sqrt(d)
+    v = hetero((1, heads, 128, d), (1,), 3, cuda, scale=(0.5, 2.0)).float()
+    v[:, :, skv:] = 64.0
+    q, k, v = q.half(), k.half(), v.half()
+    kbuf = _q_layout(k, dp)                       # [128, heads*dp]
+    vtbuf = _vt_layout(v, dp, pitch=128)          # [heads*dp, 128]
+    out = guarded((nb * sq, heads * d), pitch=heads * d + 32, device=cuda)
+    ops.attention(_q_layout(q, dp), kbuf[:rows], vtbuf[:, :rows], out.view, nb=nb, heads=heads, sq=sq, skv=skv, d_real=d, dp=dp,
+                  k_bstride=0, vt_bstride=0)
+    out.assert_untouched(f"cross-attn out d={d}/{dp}")
+    ref = _attn64(q, k[:, :, :skv], v[:, :, :skv], d)
+    what = f"cross-attn nb={nb} heads={heads} d={d}/{dp} rows={rows}"
+    assert_discriminates(out.view, ref, _attn64(q, k[:, :, :skv + 1], v[:, :, :skv + 1], d), *ATTN_TOL, what,
+                         "kv mask one column too wide")
+    nread = -(-skv // _bkv(dp)) * _bkv(dp)
+    assert_discriminates(out.view, ref, _attn64(q, k[:, :, :nread], v[:, :, :nread], d), *ATTN_TOL, what, "KV tail not masked")
+
+
+def _online_no_alpha(q, k, v, d, bkv):
+    """The flash-attention recurrence with the O rescale by alpha = exp(m_old - m_new) left out (l is still rescaled): what a
+    kernel computes if it forgets to rescale its accumulator when the running maximum rises."""
+    s = q.double() @ k.double().transpose(-1, -2) / math.sqrt(d)
+    m = torch.full(s.shape[:-1] + (1,), -math.inf, dtype=torch.float64, device=s.device)
+    l = torch.zeros_like(m)
+    o = torch.zeros(s.shape[:-1] + (d,), dtype=torch.float64, device=s.device)
+    for j in range(0, s.shape[-1], bkv):
+        sj = s[..., j:j + bkv]
+        m_new = torch.maximum(m, sj.amax(-1, keepdim=True))
+        p = torch.exp(sj - m_new)
+        l = l * torch.exp(m - m_new) + p.sum(-1, keepdim=True)
+        o = o + p @ v.double()[..., j:j + bkv, :]
+        m = m_new
+    o = o / l
+    return o.permute(0, 2, 1, 3).reshape(q.shape[0] * q.shape[2], -1)
+
+
+@pytest.mark.parametrize("where", ["first", "middle", "last"])
+@pytest.mark.parametrize("d,dp", [(64, 64), (80, 128), (160, 192)])
+def test_attention_peaked_softmax(cuda, where, d, dp):
+    """Logits with std ~9 plus a +70 bonus on one key, placed in the first, a middle or the last KV block: P is close to one-hot,
+    so the alpha rescale of the running accumulator and the fp16 rounding of P carry the whole result.  Catches: O not
+    rescaled when the running maximum rises, the KV block holding the maximum lost (ring stage / phase error)."""
+    ops = _ops()
+    nb, heads, seq = 1, 2, 576
+    bkv = _bkv(dp)
+    t = {"first": 5, "middle": (seq // bkv // 2) * bkv + 7, "last": seq - 3}[where]
+    q = _rand((nb, heads, seq, d), cuda, 1) * 9.0
+    k = _rand((nb, heads, seq, d), cuda, 2)
+    v = _rand((nb, heads, seq, d), cuda, 3)
+    q[..., 0] = 8.0
+    k[..., 0] = 0.0
+    k[..., t, 0] = 70.0 * math.sqrt(d) / 8.0
+    q, k, v = q.half(), k.half(), v.half()
+    out = guarded((nb * seq, heads * d), device=cuda)
+    ops.attention(_q_layout(q, dp), _q_layout(k, dp), _vt_layout(v, dp), out.view, nb=nb, heads=heads, sq=seq, skv=seq,
+                  d_real=d, dp=dp, k_bstride=seq, vt_bstride=seq)
+    out.assert_untouched("peaked attention out")
+    ref = _attn64(q, k, v, d)
+    what = f"peaked attention d={d}/{dp} max at key {t} ({where} block)"
+    j0 = t // bkv * bkv
+    keep = torch.ones(seq, dtype=torch.bool, device=cuda)
+    keep[j0:j0 + bkv] = False
+    assert_discriminates(out.view, ref, _attn64(q, k[:, :, keep], v[:, :, keep], d), *ATTN_TOL, what,
+                         "KV block holding the maximum lost")
+    if where != "first":
+        assert_discriminates(out.view, ref, _online_no_alpha(q, k, v, d, bkv), *ATTN_TOL, what, "O not rescaled by alpha")
+
+
 @pytest.mark.parametrize("nb,h,w,ca,cb,silu,eps", [
     (1, 64, 64, 320, 0, True, 1e-5), (2, 32, 32, 640, 0, False, 1e-6), (1, 16, 16, 1280, 1280, True, 1e-5),
     (1, 32, 32, 1280, 640, True, 1e-5),   # 1920 channels: groups of 60 straddle the concat boundary
     (4, 8, 8, 1280, 0, True, 1e-5), (1, 24, 24, 640, 320, True, 1e-5),
     (1, 64, 64, 640, 320, True, 1e-5),    # cluster of 8 CTAs per group
-    (1, 8, 8, 1280, 1280, True, 1e-5), (1, 96, 96, 640, 320, True, 1e-5),   # too large for a cluster: whole-grid kernel
+    (1, 8, 8, 1280, 1280, True, 1e-5),    # one-CTA cluster
+    (1, 96, 96, 640, 320, True, 1e-5),    # too large for a cluster and for the register cache: statistics + apply launches
 ])
 def test_groupnorm(cuda, nb, h, w, ca, cb, silu, eps):
     ops = _ops()
@@ -101,16 +265,165 @@ def test_groupnorm(cuda, nb, h, w, ca, cb, silu, eps):
     assert_close(y, ref.permute(0, 2, 3, 1), 3e-3, 2e-3, f"groupnorm {ca}+{cb}")
 
 
+def _gn_stats(x, groups=32):
+    """float64 (mean, biased variance) per (batch item, group) of an NHWC tensor."""
+    nb, h, w, c = x.shape
+    xg = x.double().reshape(nb, h * w, groups, c // groups)
+    return xg.mean(dim=(1, 3)), xg.var(dim=(1, 3), unbiased=False)
+
+
+def _gn_apply(x, mean, var, gamma, beta, eps, silu, chan_group=None, groups=32):
+    """GroupNorm(+SiLU) of NHWC x with the given per-(batch item, group) statistics, in float64; chan_group maps channel ->
+    group (default c // cpg)."""
+    c = x.shape[3]
+    if chan_group is None:
+        chan_group = torch.arange(c, device=x.device) // (c // groups)
+    m = mean[:, chan_group][:, None, None, :]
+    r = (var[:, chan_group] + eps).rsqrt()[:, None, None, :]
+    y = (x.double() - m) * r * gamma.double() + beta.double()
+    return F.silu(y) if silu else y
+
+
+def _gn_case(cuda, nb, h, w, ca, cb, eps, seed=1):
+    """hetero NHWC input (own offset / scale per batch item and channel), split at the concat boundary; group 1 of the last batch
+    item is shrunk to std ~2e-3 so its variance is comparable with eps (a swapped eps moves that group's output by O(1))."""
+    c = ca + cb
+    x = hetero((nb, h, w, c), (0, 3), seed, cuda)
+    cpg = c // 32
+    x[nb - 1, :, :, cpg:2 * cpg] = (_rand((h, w, cpg), cuda, seed + 7) * 2e-3).half()
+    gamma = (1 + 0.2 * _rand((c,), cuda, 3)).float()
+    beta = (0.2 * _rand((c,), cuda, 4)).float()
+    xa = x[..., :ca].contiguous()
+    xb = x[..., ca:].contiguous() if cb else None
+    return x, xa, xb, gamma, beta
+
+
+def _gn_expected_path(ca, cb, hw):
+    cl, th, ppc = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    from ai_rtc_agent_b200.host import capi
+    assert capi.lib().b2sd_groupnorm_plan_dry(ca, cb, 32, hw, ctypes.byref(cl), ctypes.byref(th), ctypes.byref(ppc)) == 0
+    return cl.value
+
+
+# (path, cluster size or None, nb, h, w, ca, cb, eps).  The fused / stats+apply split of the non-cluster shapes is the
+# planner's (elementwise.cu groupnorm_launch): fused when a CTA's chunk fits the GN_CACHE = 12 register iterations
+# (ceil(ppc / rpi)) and the whole grid (128 chunks x nb) is co-resident.  (1,96,96,640): vc 80, rpi 6, ppc 72 -> 12 iterations,
+# 128 chunks; 640+320 at 96x96: rpi 4 -> 18 iterations; 640+320 at 72x72: ppc 41, rpi 4 -> 11 iterations, 127 chunks.
+GN_PATH_CASES = [
+    ("cluster", 1, 1, 16, 16, 1280, 0, 1e-5), ("cluster", 1, 4, 16, 16, 1280, 0, 1e-6),
+    ("cluster", 2, 1, 32, 32, 640, 0, 1e-6), ("cluster", 2, 4, 32, 32, 640, 0, 1e-5),
+    ("cluster", 4, 1, 64, 64, 320, 0, 1e-5), ("cluster", 4, 4, 64, 64, 320, 0, 1e-5),
+    ("cluster", 8, 1, 64, 64, 640, 320, 1e-5), ("cluster", 8, 4, 64, 64, 640, 320, 1e-6),   # groups of 30 straddle the concat
+    ("cluster", 4, 2, 32, 32, 1280, 640, 1e-5),                                              # groups of 60 straddle the concat
+    ("fused", None, 1, 96, 96, 640, 0, 1e-5), ("fused", None, 1, 96, 96, 640, 0, 1e-6),
+    ("fused", None, 1, 72, 72, 640, 320, 1e-5),                                              # fused, straddling groups
+    ("stats+apply", None, 1, 96, 96, 640, 320, 1e-5),                                        # straddling groups
+    ("stats+apply", None, 4, 96, 96, 640, 0, 1e-6),   # 4 x 128 chunks: more CTAs than are co-resident
+]
+GN_OCCUPANCY_DEPENDENT = {("fused", 1, 96, 96, 640, 0), ("fused", 1, 72, 72, 640, 320), ("stats+apply", 4, 96, 96, 640, 0)}
+
+
+@pytest.mark.parametrize("path,cl,nb,h,w,ca,cb,eps", GN_PATH_CASES)
+@pytest.mark.parametrize("silu", [True, False])
+def test_groupnorm_paths_discriminate(cuda, path, cl, nb, h, w, ca, cb, eps, silu):
+    """Every GroupNorm kernel (cluster of 1/2/4/8 CTAs, cooperative fused, statistics + apply) against a float64 reference on
+    inputs whose batch items and groups all have different statistics.  Catches: another batch item's statistics, a
+    neighbouring group's statistics, a channel put into the neighbouring group, eps 1e-5 and 1e-6 confused."""
+    ops = _ops()
+    assert _gn_expected_path(ca, cb, h * w) == (cl or 0), "planner no longer picks this cluster size; re-derive the case"
+    x, xa, xb, gamma, beta = _gn_case(cuda, nb, h, w, ca, cb, eps)
+    c = ca + cb
+    y = torch.full((nb, h, w, c), float("nan"), dtype=torch.float16, device=cuda)
+    _, ran = ops.groupnorm(xa, xb, gamma, beta, y, eps=eps, silu=silu, return_path=True)
+    print(f"groupnorm nb={nb} {h}x{w} {ca}+{cb}: path={ran} (wanted {path})")
+    mean, var = _gn_stats(x)
+    ref = _gn_apply(x, mean, var, gamma, beta, eps, silu)
+    what = f"groupnorm[{ran}] nb={nb} {h}x{w} {ca}+{cb} eps={eps}"
+    tol = (3e-3, 2e-3)
+    cpg = c // 32
+    shifted = ((torch.arange(c, device=cuda) + 1) // cpg).clamp(max=31)
+    assert_discriminates(y, ref, _gn_apply(x, mean.roll(1, 1), var.roll(1, 1), gamma, beta, eps, silu), *tol, what,
+                         "statistics of group g-1")
+    assert_discriminates(y, ref, _gn_apply(x, mean, var, gamma, beta, eps, silu, chan_group=shifted), *tol, what,
+                         "group boundary shifted by one channel")
+    assert_discriminates(y, ref, _gn_apply(x, mean, var, gamma, beta, 1e-6 if eps == 1e-5 else 1e-5, silu), *tol, what,
+                         "eps 1e-5 and 1e-6 swapped")
+    if nb > 1:
+        assert_discriminates(y, ref, _gn_apply(x, mean[:1].expand_as(mean), var[:1].expand_as(var), gamma, beta, eps, silu),
+                             *tol, what, "batch item 0's statistics for every item")
+    if ran != path:
+        assert (path, nb, h, w, ca, cb) in GN_OCCUPANCY_DEPENDENT, f"{what}: ran the {ran} path, the planner's choice is {path}"
+        pytest.skip(f"{what}: this device's occupancy selected the {ran} path, not {path} (the output was verified)")
+
+
+@pytest.mark.parametrize("nb,h,w,ca,cb,path", [
+    (1, 32, 32, 640, 0, "cluster"), (2, 64, 64, 640, 320, "cluster"), (1, 16, 16, 1280, 0, "cluster"),
+    (1, 96, 96, 640, 0, "fused"), (1, 96, 96, 640, 320, "stats+apply"),
+])
+def test_groupnorm_offset_heavy(cuda, nb, h, w, ca, cb, path):
+    """Groups whose mean is 30-100 standard deviations away from zero (within fp16 range).  Every GroupNorm kernel computes the
+    variance as E[x^2] - mean^2 in fp32; this pins |mean|/std <= 100 as the operating range in which that holds the usual
+    tolerance.  The case's error, in units of the tolerance, is printed."""
+    ops = _ops()
+    c = ca + cb
+    g = torch.Generator().manual_seed(11)
+    sign = torch.randint(0, 2, (nb, 1, 1, 32, 1), generator=g).double() * 2 - 1
+    mags = torch.stack([torch.linspace(30, 100, 32, dtype=torch.float64)[torch.randperm(32, generator=g)] for _ in range(nb)])
+    gmean = sign * mags.reshape(nb, 1, 1, 32, 1)
+    coff = 0.5 * (torch.rand((nb, 1, 1, 32, c // 32), generator=g, dtype=torch.float64) * 2 - 1)
+    x = (gmean + coff + torch.randn((nb, h, w, 32, c // 32), generator=g, dtype=torch.float64)).reshape(nb, h, w, c)
+    x = x.half().to(cuda)
+    gamma = (1 + 0.2 * _rand((c,), cuda, 3)).float()
+    beta = (0.2 * _rand((c,), cuda, 4)).float()
+    y = torch.full((nb, h, w, c), float("nan"), dtype=torch.float16, device=cuda)
+    _, ran = ops.groupnorm(x[..., :ca].contiguous(), x[..., ca:].contiguous() if cb else None, gamma, beta, y, eps=1e-5,
+                           silu=True, return_path=True)
+    mean, var = _gn_stats(x)
+    ratio = (mean.abs() / var.sqrt()).min().item(), (mean.abs() / var.sqrt()).max().item()
+    ref = _gn_apply(x, mean, var, gamma, beta, 1e-5, True)
+    err = ((y.double() - ref).abs() / (3e-3 + 2e-3 * ref.abs())).max().item()
+    print(f"groupnorm offset-heavy nb={nb} {h}x{w} {ca}+{cb}: path={ran} |mean|/std in [{ratio[0]:.0f}, {ratio[1]:.0f}], "
+          f"max error = {err:.3f} x tolerance")
+    assert ratio[0] >= 25 and ratio[1] >= 90
+    assert_discriminates(y, ref, _gn_apply(x, mean.roll(1, 1), var.roll(1, 1), gamma, beta, 1e-5, True), 3e-3, 2e-3,
+                         f"offset-heavy groupnorm[{ran}]", "statistics of group g-1")
+    if ran != path:
+        pytest.skip(f"offset-heavy {h}x{w} {ca}+{cb}: ran the {ran} path, not {path} (the output was verified)")
+
+
 @pytest.mark.parametrize("rows,c", [(4096, 320), (1024, 640), (77, 1280), (5, 64)])
 def test_layernorm(cuda, rows, c):
+    """Every row has its own offset and scale: catches a kernel that normalises a row with a neighbouring row's statistics."""
     ops = _ops()
-    x = (_rand((rows, c), cuda, 1) * 2 + 0.5).half()
+    x = hetero((rows, c), (0,), 1, cuda)
     gamma = (1 + 0.1 * _rand((c,), cuda, 2)).float()
     beta = (0.1 * _rand((c,), cuda, 3)).float()
     y = torch.empty_like(x)
     ops.layernorm(x, gamma, beta, y)
-    ref = F.layer_norm(x.float(), (c,), gamma, beta, 1e-5)
-    assert_close(y, ref, 3e-3, 2e-3, f"layernorm {rows}x{c}")
+    xd = x.double()
+    ref = F.layer_norm(xd, (c,), gamma.double(), beta.double(), 1e-5)
+    mean, var = xd.mean(1, keepdim=True), xd.var(1, unbiased=False, keepdim=True)
+    wrong = (xd - mean.roll(1, 0)) * (var.roll(1, 0) + 1e-5).rsqrt() * gamma.double() + beta.double()
+    assert_discriminates(y, ref, wrong, 3e-3, 2e-3, f"layernorm {rows}x{c}", "statistics of the neighbouring row")
+
+
+@pytest.mark.parametrize("rows,c", [(1024, 320), (256, 1280)])
+def test_layernorm_offset_heavy(cuda, rows, c):
+    """Rows with |mean|/std of 30..100: layernorm_kernel computes the variance as E[x^2] - mean^2 in fp32; this pins that
+    range as the one in which it holds the usual tolerance.  The error, in units of the tolerance, is printed."""
+    ops = _ops()
+    x = offset_heavy_rows(rows, c, cuda)
+    gamma = (1 + 0.1 * _rand((c,), cuda, 2)).float()
+    beta = (0.1 * _rand((c,), cuda, 3)).float()
+    y = torch.empty_like(x)
+    ops.layernorm(x, gamma, beta, y)
+    xd = x.double()
+    ref = F.layer_norm(xd, (c,), gamma.double(), beta.double(), 1e-5)
+    err = ((y.double() - ref).abs() / (3e-3 + 2e-3 * ref.abs())).max().item()
+    print(f"layernorm offset-heavy {rows}x{c}: max error = {err:.3f} x tolerance")
+    mean, var = xd.mean(1, keepdim=True), xd.var(1, unbiased=False, keepdim=True)
+    wrong = (xd - mean.roll(1, 0)) * (var.roll(1, 0) + 1e-5).rsqrt() * gamma.double() + beta.double()
+    assert_discriminates(y, ref, wrong, 3e-3, 2e-3, f"offset-heavy layernorm {rows}x{c}", "statistics of the neighbouring row")
 
 
 def test_upsample2x(cuda):

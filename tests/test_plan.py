@@ -209,6 +209,16 @@ def test_bad_descriptors_are_rejected():
     assert capi.lib().b2sd_igemm_plan_dry(C.byref(d), 0, 0, C.byref(info)) != 0
 
 
+def test_groupnorm_last_path_is_per_thread():
+    """b2sd_groupnorm_last_path reports the launch made on the calling thread: -1 on a thread that has launched none."""
+    import threading
+    got = []
+    t = threading.Thread(target=lambda: got.append(capi.lib().b2sd_groupnorm_last_path()))
+    t.start()
+    t.join()
+    assert got == [-1]
+
+
 @pytest.mark.parametrize("ca,cb,hw,expect", [(320, 0, 4096, 4), (640, 320, 4096, 8), (640, 0, 1024, 2), (1280, 640, 1024, 4),
                                              (1280, 0, 256, 1), (1280, 1280, 64, 1), (640, 320, 96 * 96, 0), (100, 0, 64, None)])
 def test_groupnorm_launch_shape(ca, cb, hw, expect):

@@ -1,4 +1,6 @@
 """Shared helpers for the parity tests."""
+import math
+
 import torch
 
 
@@ -33,3 +35,77 @@ def assert_close(got, ref, tol_abs, tol_rel, what=""):
     err = (got - ref).abs()
     ok = bool((err <= tol_abs + tol_rel * ref.abs()).all()) and not bool(torch.isnan(got).any())
     assert ok, what + "\n" + describe_mismatch(got, ref, tol_abs, tol_rel)
+
+
+# ---- discriminating inputs, guard bands and wrong references ------------------------------------------------------------------
+def hetero(shape, dims, seed, device, offset=3.0, scale=(0.1, 4.0), dtype=torch.float16):
+    """randn(shape) in which every index of the dimensions `dims` (e.g. (0, 3) = every (batch item, channel) of an NHWC tensor,
+    (0,) = every row of a token matrix) gets its own offset, uniform in [-offset, offset], and its own scale, log-uniform in
+    `scale`.  Each GroupNorm group, LayerNorm row and batch item then has clearly different statistics, so a kernel that applies
+    the statistics of the wrong one is off by O(1) rather than by sampling noise.  Seeded, drawn on the CPU, rounded to `dtype`."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    pshape = [shape[d] if d in dims else 1 for d in range(len(shape))]
+    off = (torch.rand(pshape, generator=g, dtype=torch.float64) * 2 - 1) * offset
+    lo, hi = math.log(scale[0]), math.log(scale[1])
+    sc = torch.exp(lo + (hi - lo) * torch.rand(pshape, generator=g, dtype=torch.float64))
+    x = torch.randn(shape, generator=g, dtype=torch.float64) * sc + off
+    return x.to(dtype).to(device)
+
+
+def offset_heavy_rows(rows, c, device, seed=12):
+    """fp16 [rows, c] whose row means are 30..100 standard deviations from zero (alternating sign, std ~1)."""
+    g = torch.Generator().manual_seed(seed)
+    mags = torch.linspace(30, 100, rows, dtype=torch.float64)[torch.randperm(rows, generator=g)]
+    sign = torch.ones(rows, dtype=torch.float64)
+    sign[1::2] = -1
+    coff = 0.5 * (torch.rand((1, c), generator=g, dtype=torch.float64) * 2 - 1)
+    x = (sign * mags)[:, None] + coff + torch.randn((rows, c), generator=g, dtype=torch.float64)
+    return x.half().to(device)
+
+
+SENTINEL = 0x7D5A   # an fp16 NaN with a payload no arithmetic produces (kernels write the canonical 0x7E00 / 0x7FFF)
+
+
+class Guarded:
+    """An output allocation [lead + rows + tail, pitch] filled with the SENTINEL bit pattern; `view` is the [rows, cols] window
+    a kernel may write (pitch > cols leaves spare columns, as in the engine's strided buffers).  assert_untouched() checks, bit
+    for bit, the bands of rows before and after the window and the spare columns [cols, pitch) of every row."""
+
+    def __init__(self, rows, cols, pitch=None, device="cuda", lead=8, tail=64):
+        pitch = cols if pitch is None else pitch
+        assert pitch >= cols and pitch % 8 == 0
+        self.rows, self.cols, self.pitch, self.lead = rows, cols, pitch, lead
+        self.buf = torch.empty((lead + rows + tail, pitch), dtype=torch.float16, device=device)
+        self.buf.view(torch.int16).fill_(SENTINEL)
+        self.view = self.buf[lead:lead + rows, :cols]
+
+    def assert_untouched(self, what=""):
+        bits = self.buf.view(torch.int16)
+        mask = torch.ones_like(bits, dtype=torch.bool)
+        mask[self.lead:self.lead + self.rows, :self.cols] = False
+        bad = (bits != SENTINEL) & mask
+        if bad.any():
+            idx = bad.nonzero()
+            idx[:, 0] -= self.lead
+            raise AssertionError(f"{what}: {int(bad.sum())} guard elements written outside the [{self.rows}, {self.cols}] window "
+                                 f"(pitch {self.pitch}); first (row, col) relative to the window: {idx[:8].tolist()}")
+
+
+def guarded(shape, pitch=None, device="cuda", lead=8, tail=64):
+    """Guarded output for a [rows, cols] result (shape may have leading unit dimensions folded into rows)."""
+    rows = math.prod(shape[:-1])
+    return Guarded(rows, shape[-1], pitch, device, lead, tail)
+
+
+def assert_discriminates(got, ref, wrong_ref, tol_abs, tol_rel, what="", bug=""):
+    """got matches ref within tol_abs + tol_rel*|ref|, AND the plausible wrong answer `wrong_ref` (the result a kernel with the
+    named bug would produce, built in plain torch) is off from ref by at least 10x that tolerance somewhere.  The second half
+    proves the test would fail on that bug without planting the bug in a kernel."""
+    got = got.detach().double()
+    ref = ref.detach().double().to(got.device)
+    wrong = wrong_ref.detach().double().to(got.device)
+    assert_close(got, ref, tol_abs, tol_rel, what)
+    margin = ((wrong - ref).abs() / (tol_abs + tol_rel * ref.abs())).nan_to_num(nan=float("inf"))
+    worst = margin.max().item()
+    assert worst >= 10.0, (f"{what}: the wrong reference '{bug}' differs from the reference by at most {worst:.2f}x the "
+                           "tolerance; the test cannot tell that bug apart")

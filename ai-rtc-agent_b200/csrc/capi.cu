@@ -46,7 +46,7 @@ static void to_igemm_desc(const b2sd_igemm_desc* d, IgemmDesc& g) {
     g.epi.ldr = d->ldr;
     g.epi.acc_scale = d->acc_scale;
     g.epi.res_scale = d->res_scale;
-    g.epi.flags = d->flags & (IG_RELU | IG_GEGLU);
+    g.epi.flags = d->flags & (IG_RELU | IG_GEGLU | IG_SILU);
     g.epi.n_valid = d->n_valid;
     g.epi.rowstat_out = static_cast<unsigned long long*>(d->rowstat_out);
     g.epi.rowstat_in = static_cast<const unsigned long long*>(d->rowstat_in);
@@ -191,6 +191,12 @@ int b2sd_op_upsample2x(const void* x, void* y, int nb, int h, int w, int c, void
 
 int b2sd_op_smallconv(const void* x, const void* w_oihw, const float* bias, void* y, int ldy, int nb, int h,
                       int w, int cin, int cout, int in_h, int in_w, int flags, void* stream) {
+    return b2sd_op_smallconv_ex(x, w_oihw, bias, y, ldy, nb, h, w, cin, cout, in_h, in_w, flags, nullptr, 0, 0, nullptr, stream);
+}
+
+int b2sd_op_smallconv_ex(const void* x, const void* w_oihw, const float* bias, void* y, int ldy, int nb, int h, int w,
+                         int cin, int cout, int in_h, int in_w, int flags, const void* res, int ldr, int64_t res_bstride,
+                         const float* in_off, void* stream) {
     SmallConvArgs a{};
     static float* wt = nullptr;  // op-level entry only: re-prepared on every call
     if (!wt && cudaMalloc(&wt, 36 * 1024 * sizeof(float)) != cudaSuccess) {
@@ -202,7 +208,30 @@ int b2sd_op_smallconv(const void* x, const void* w_oihw, const float* bias, void
     a.x = x; a.wt = wt; a.bias = bias;
     a.y = reinterpret_cast<__half*>(y); a.ldy = ldy;
     a.nb = nb; a.h = h; a.w_ = w; a.cin = cin; a.cout = cout; a.in_h = in_h; a.in_w = in_w; a.flags = flags;
+    a.res = reinterpret_cast<const __half*>(res); a.ldr = ldr; a.res_bstride = (long)res_bstride; a.in_off = in_off;
     return smallconv_launch(a, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2sd_op_maxpool2x2(const void* x, void* y, int nb, int h, int w, int c, void* stream) {
+    return maxpool2x2_launch(reinterpret_cast<const __half*>(x), reinterpret_cast<__half*>(y), nb, h, w, c,
+                             reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2sd_op_hed_project(const void* x, int ldx, int c, int64_t npix, const float* w, const float* bias, float* out, void* stream) {
+    return hed_project_launch(reinterpret_cast<const __half*>(x), ldx, c, (long)npix, w, bias, out, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2sd_op_hed_fuse(const float* const* maps, const int* hs, const int* ws, int levels, int h, int w, void* out_u8,
+                     void* edge_f16, void* stream) {
+    HedFuseArgs a{};
+    if (!maps || !hs || !ws || levels < 1 || levels > 5) {
+        b2_set_error("b2sd_op_hed_fuse: 1..5 side outputs required");
+        return -1;
+    }
+    for (int k = 0; k < levels; ++k) { a.maps[k] = maps[k]; a.hs[k] = hs[k]; a.ws[k] = ws[k]; }
+    a.levels = levels; a.h = h; a.w = w;
+    a.out = static_cast<uint8_t*>(out_u8); a.edge_f16 = static_cast<__half*>(edge_f16);
+    return hed_fuse_launch(a, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int b2sd_op_lcm_step(void* x, const void* eps, const void* noise, const float* coef, void* out_latent, int T,

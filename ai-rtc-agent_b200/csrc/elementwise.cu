@@ -651,7 +651,9 @@ int smallconv_prep_launch(const __half* w_oihw, float* wt, int cout, int cin, cu
     return 0;
 }
 
-template <int CIN>
+// EXT: the residual / SiLU epilogue (ControlNet) is compiled in; the other instantiations stay as lean as before (the head's
+// 3-channel kernel sits at 64 registers)
+template <int CIN, bool EXT>
 __global__ void __launch_bounds__(128) smallconv_kernel(SmallConvArgs a, int G) {
     B2_PDL_ENTRY();
     extern __shared__ float ws[];  // [CIN*9][G] weights of this CTA's G-channel output group, then bias[G]
@@ -693,10 +695,12 @@ __global__ void __launch_bounds__(128) smallconv_kernel(SmallConvArgs a, int G) 
                         const long idx = (((long)n * CIN + c) * a.in_h + sy) * a.in_w + sx;
                         v = (a.flags & SC_IN_F32_NCHW) ? reinterpret_cast<const float*>(a.x)[idx]
                                                        : __half2float(reinterpret_cast<const __half*>(a.x)[idx]);
+                        if (EXT && (a.flags & SC_IN_OFFSET)) v = v * 255.0f - a.in_off[c];
                     } else if (a.flags & SC_IN_U8) {
                         // lib/pipeline.py:61 convertto(scale=1/255); the 2x-1 of VaeImageProcessor and the
                         // (x+1)/2 of EncoderTiny cancel
-                        v = (float)reinterpret_cast<const uint8_t*>(a.x)[base + c] * (1.0f / 255.0f);
+                        const float raw = (float)reinterpret_cast<const uint8_t*>(a.x)[base + c];
+                        v = (EXT && (a.flags & SC_IN_OFFSET)) ? raw - a.in_off[c] : raw * (1.0f / 255.0f);
                     } else {
                         v = __half2float(reinterpret_cast<const __half*>(a.x)[base + c]);
                         if (a.flags & SC_IN_TANH3) v = tanhf(v * (1.0f / 3.0f)) * 3.0f;
@@ -731,9 +735,19 @@ __global__ void __launch_bounds__(128) smallconv_kernel(SmallConvArgs a, int G) 
 #pragma unroll
                 for (int o = 0; o < 4; ++o) {
                     float v0 = acc[8 * j + 2 * o], v1 = acc[8 * j + 2 * o + 1];
+                    if (EXT && a.res) {
+                        const float2 r = __half22float2(*reinterpret_cast<const __half2*>(
+                            a.res + n * a.res_bstride + (long)(p - n * a.w_ * a.h) * a.ldr + cg * G + q + 8 * j + 2 * o));
+                        v0 += r.x;
+                        v1 += r.y;
+                    }
                     if (a.flags & SC_OUT_RELU) {
                         v0 = fmaxf(v0, 0.f);
                         v1 = fmaxf(v1, 0.f);
+                    }
+                    if (EXT && (a.flags & SC_OUT_SILU)) {
+                        v0 = v0 / (1.0f + expf(-v0));
+                        v1 = v1 / (1.0f + expf(-v1));
                     }
                     hh[o] = __floats2half2_rn(v0, v1);
                 }
@@ -744,8 +758,19 @@ __global__ void __launch_bounds__(128) smallconv_kernel(SmallConvArgs a, int G) 
 }
 
 int smallconv_launch(const SmallConvArgs& a, cudaStream_t s) {
-    if ((a.cout & 63) || (a.ldy & 7) || (a.cin != 3 && a.cin != 4) || !a.wt) {
-        b2_set_error("smallconv: cin %d cout %d unsupported (cout must be a multiple of 64; prepared weights required)", a.cin, a.cout);
+    if ((a.cout & 15) || a.cout > a.ldy || (a.ldy & 7) || (a.cin != 3 && a.cin != 4) || !a.wt) {
+        b2_set_error("smallconv: cin %d cout %d ldy %d unsupported (cout must be a multiple of 16 and <= ldy; prepared weights "
+                     "required)", a.cin, a.cout, a.ldy);
+        return -1;
+    }
+    // the residual is read as __half2 pairs
+    if (a.res && ((a.ldr & 1) || (a.res_bstride & 1) || (reinterpret_cast<uintptr_t>(a.res) & 3))) {
+        b2_set_error("smallconv: the residual needs an even pitch (%d), an even batch stride (%ld) and 4-byte alignment", a.ldr,
+                     a.res_bstride);
+        return -1;
+    }
+    if ((a.flags & SC_IN_OFFSET) && (!a.in_off || a.cin != 3 || (a.flags & SC_IN_TANH3))) {
+        b2_set_error("smallconv: the offset input mode needs a 3-channel frame and the offsets");
         return -1;
     }
     const long npix = (long)a.nb * a.h * a.w_;
@@ -754,19 +779,29 @@ int smallconv_launch(const SmallConvArgs& a, cudaStream_t s) {
         return -1;
     }
     long blocks = (npix + 127) / 128;
-    const int G = blocks * (a.cout / 64) < IG_SMS * 4 ? 16 : 64;   // few pixels: narrower channel groups, more CTAs
+    // few pixels (or a cout that is not a multiple of 64): narrower channel groups, more CTAs
+    const int G = (a.cout & 63) || blocks * (a.cout / 64) < IG_SMS * 4 ? 16 : 64;
     const size_t smem = ((size_t)a.cin * 9 * G + G) * sizeof(float);
     const int groups = a.cout / G;
     const long cap = (IG_SMS * 16 + groups - 1) / groups;   // two full waves of 8 CTAs per SM; beyond that, grid-stride
     if (blocks > cap) blocks = cap;
     static bool attr = false;
     if (!attr) {
-        cudaFuncSetAttribute(smallconv_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
-        cudaFuncSetAttribute(smallconv_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
+        cudaFuncSetAttribute(smallconv_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
+        cudaFuncSetAttribute(smallconv_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
+        cudaFuncSetAttribute(smallconv_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
+        cudaFuncSetAttribute(smallconv_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
         attr = true;
     }
-    if (a.cin == 3) B2_LAUNCHED("smallconv", launch_k(smallconv_kernel<3>, dim3((unsigned)blocks, groups), dim3(128), smem, s, 1, a, G));
-    else B2_LAUNCHED("smallconv", launch_k(smallconv_kernel<4>, dim3((unsigned)blocks, groups), dim3(128), smem, s, 1, a, G));
+    const dim3 grid((unsigned)blocks, groups);
+    if (a.res || (a.flags & (SC_OUT_SILU | SC_IN_OFFSET))) {
+        if (a.cin == 3) B2_LAUNCHED("smallconv", launch_k(smallconv_kernel<3, true>, grid, dim3(128), smem, s, 1, a, G));
+        else B2_LAUNCHED("smallconv", launch_k(smallconv_kernel<4, true>, grid, dim3(128), smem, s, 1, a, G));
+    } else if (a.cin == 3) {
+        B2_LAUNCHED("smallconv", launch_k(smallconv_kernel<3, false>, grid, dim3(128), smem, s, 1, a, G));
+    } else {
+        B2_LAUNCHED("smallconv", launch_k(smallconv_kernel<4, false>, grid, dim3(128), smem, s, 1, a, G));
+    }
     return 0;
 }
 
@@ -954,7 +989,8 @@ __global__ void pack_conv_weight_kernel(const __half* __restrict__ w, __half* __
         const int c = (int)(e % cn);
         const int tap = (int)((e / cn) % taps);
         const int oo = (int)(e / ((long)cn * taps));
-        dst[(long)oo * dst_ld + koff + tap * cn + c] = w[((long)oo * i + (c0 + c)) * taps + tap];
+        // input channels beyond the tensor's own (a narrow layer run as a 64-channel contraction) get zero weights
+        dst[(long)oo * dst_ld + koff + tap * cn + c] = c0 + c < i ? w[((long)oo * i + (c0 + c)) * taps + tap] : __float2half(0.f);
     }
 }
 int pack_conv_weight_launch(const __half* w_oihw, __half* dst, int dst_ld, int koff, int o, int i, int taps, int c0,
@@ -1017,6 +1053,111 @@ int row_sum_launch(const __half* w, long rows, int k, float* out, cudaStream_t s
 int row_dot_launch(const __half* w, long rows, int k, const float* v, const float* bias, float* out, cudaStream_t s) {
     row_dot_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(w, rows, k, v, bias, out);
     B2_CHECK_LAUNCH("row_dot");
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------ HED edge detector (ControlNet)
+__global__ void maxpool2x2_kernel(const __half2* __restrict__ x, __half2* __restrict__ y, int nb, int h, int w, int c2) {
+    B2_PDL_ENTRY();
+    const int ho = h / 2, wo = w / 2;
+    const long total = (long)nb * ho * wo * c2;
+    for (long e = (long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long)gridDim.x * blockDim.x) {
+        const int cc = (int)(e % c2);
+        long p = e / c2;
+        const int xo = (int)(p % wo);
+        p /= wo;
+        const int yo = (int)(p % ho);
+        const int n = (int)(p / ho);
+        const __half2* src = x + (((long)n * h + 2 * yo) * w + 2 * xo) * c2 + cc;
+        const long row = (long)w * c2;
+        y[e] = __hmax2(__hmax2(src[0], src[c2]), __hmax2(src[row], src[row + c2]));
+    }
+}
+
+int maxpool2x2_launch(const __half* x, __half* y, int nb, int h, int w, int c, cudaStream_t s) {
+    if ((c & 1) || (h & 1) || (w & 1)) {
+        b2_set_error("maxpool2x2: c, h and w must be even (c=%d, %dx%d)", c, h, w);
+        return -1;
+    }
+    const long total = (long)nb * (h / 2) * (w / 2) * (c / 2);
+    long blocks = (total + 255) / 256;
+    if (blocks > IG_SMS * 16) blocks = IG_SMS * 16;
+    B2_LAUNCHED("maxpool2x2", launch_k(maxpool2x2_kernel, dim3((unsigned)blocks), dim3(256), 0, s, 1,
+                                       reinterpret_cast<const __half2*>(x), reinterpret_cast<__half2*>(y), nb, h, w, c / 2));
+    return 0;
+}
+
+// one warp per pixel: out[p] = bias + sum_c x[p][c] * w[c]
+__global__ void hed_project_kernel(const __half* __restrict__ x, int ldx, int c, long npix, const float* __restrict__ w,
+                                   const float* __restrict__ bias, float* __restrict__ out) {
+    B2_PDL_ENTRY();
+    const int lane = threadIdx.x & 31;
+    for (long p = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; p < npix; p += ((long)gridDim.x * blockDim.x) >> 5) {
+        const __half2* xp = reinterpret_cast<const __half2*>(x + p * ldx);
+        float acc = 0.f;
+        for (int k = lane; k < c / 2; k += 32) {
+            const float2 f = __half22float2(xp[k]);
+            acc = fmaf(f.x, w[2 * k], fmaf(f.y, w[2 * k + 1], acc));
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+        if (lane == 0) out[p] = acc + bias[0];
+    }
+}
+
+int hed_project_launch(const __half* x, int ldx, int c, long npix, const float* w, const float* bias, float* out, cudaStream_t s) {
+    if ((c & 1) || (ldx & 1)) {
+        b2_set_error("hed_project: c and ldx must be even");
+        return -1;
+    }
+    long blocks = (npix * 32 + 255) / 256;
+    if (blocks > IG_SMS * 16) blocks = IG_SMS * 16;
+    B2_LAUNCHED("hed_project", launch_k(hed_project_kernel, dim3((unsigned)blocks), dim3(256), 0, s, 1, x, ldx, c, npix, w, bias, out));
+    return 0;
+}
+
+// HEDdetector post-processing: bilinear (half-pixel centres, edge clamp: cv2.INTER_LINEAR) upsampling of every side output to
+// h x w, mean, sigmoid, * 255, clip, truncation to u8, replicated to 3 channels (HWC3); optionally the edge value as fp16
+__global__ void hed_fuse_kernel(HedFuseArgs a) {
+    B2_PDL_ENTRY();
+    const long npix = (long)a.h * a.w;
+    for (long p = (long)blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += (long)gridDim.x * blockDim.x) {
+        const int x = (int)(p % a.w), y = (int)(p / a.w);
+        float sum = 0.f;
+#pragma unroll
+        for (int k = 0; k < 5; ++k) {   // compile-time indices into the argument arrays (no local-memory copy)
+            if (k >= a.levels) break;
+            const int hk = a.hs[k], wk = a.ws[k];
+            float sy = ((float)y + 0.5f) * ((float)hk / (float)a.h) - 0.5f;
+            float sx = ((float)x + 0.5f) * ((float)wk / (float)a.w) - 0.5f;
+            sy = fmaxf(sy, 0.f);
+            sx = fmaxf(sx, 0.f);
+            const int y0 = min((int)sy, hk - 1), x0 = min((int)sx, wk - 1);
+            const int y1 = min(y0 + 1, hk - 1), x1 = min(x0 + 1, wk - 1);
+            const float fy = sy - (float)y0, fx = sx - (float)x0;
+            const float* m = a.maps[k];
+            const float top = m[(long)y0 * wk + x0] * (1.f - fx) + m[(long)y0 * wk + x1] * fx;
+            const float bot = m[(long)y1 * wk + x0] * (1.f - fx) + m[(long)y1 * wk + x1] * fx;
+            sum += top * (1.f - fy) + bot * fy;
+        }
+        const float e = 1.f / (1.f + expf(-sum / (float)a.levels));
+        const uint8_t u = (uint8_t)fminf(fmaxf(e * 255.f, 0.f), 255.f);   // truncation, as numpy's astype(uint8)
+        a.out[3 * p] = u;
+        a.out[3 * p + 1] = u;
+        a.out[3 * p + 2] = u;
+        if (a.edge_f16) a.edge_f16[p] = __float2half_rn((float)u);
+    }
+}
+
+int hed_fuse_launch(const HedFuseArgs& a, cudaStream_t s) {
+    if (a.levels < 1 || a.levels > 5 || !a.out) {
+        b2_set_error("hed_fuse: 1..5 side outputs and an output are required");
+        return -1;
+    }
+    const long npix = (long)a.h * a.w;
+    long blocks = (npix + 255) / 256;
+    if (blocks > IG_SMS * 16) blocks = IG_SMS * 16;
+    B2_LAUNCHED("hed_fuse", launch_k(hed_fuse_kernel, dim3((unsigned)blocks), dim3(256), 0, s, 1, a));
     return 0;
 }
 

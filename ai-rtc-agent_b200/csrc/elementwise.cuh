@@ -39,8 +39,12 @@ int upsample2x_launch(const __half* x, __half* y, int nb, int h, int w, int c, c
 
 // Direct 3x3 conv (pad 1, stride 1) for tiny Cin (<= 4): UNet conv_in (4->320), TAESD encoder head
 // (3->64, reads the u8 NHWC video frame and applies 1/255), TAESD decoder head (4->64, tanh(z/3)*3 in,
-// ReLU out).  w: fp16 [cout][cin][3][3] (PyTorch OIHW), bias fp32 [cout] or null.
-enum : int { SC_IN_U8 = 1, SC_IN_TANH3 = 2, SC_OUT_RELU = 4, SC_IN_F32_NCHW = 8, SC_IN_F16_NCHW = 16 };
+// ReLU out), ControlNet conv_in (4->320, + the conditioning embedding broadcast over the stream batch) and the conditioning
+// embedding's conv_in (3->16, frame / 255 in, SiLU out).  w: fp16 [cout][cin][3][3] (PyTorch OIHW), bias fp32 [cout] or null.
+// cout: a multiple of 64, or of 16 (then 16-channel groups; the caller clears columns cout..ldy-1 of y once).
+// SC_IN_OFFSET (HED's first conv): the frame on the 0..255 scale minus a per-channel offset, zero padding in the shifted domain.
+enum : int { SC_IN_U8 = 1, SC_IN_TANH3 = 2, SC_OUT_RELU = 4, SC_IN_F32_NCHW = 8, SC_IN_F16_NCHW = 16, SC_OUT_SILU = 32,
+             SC_IN_OFFSET = 64 };
 struct SmallConvArgs {
     const void* x;       // fp16 NHWC [nb,h,w,cin] or u8 NHWC when SC_IN_U8
     const float* wt;     // fp32 [cin*9][cout], k = tap*cin + c (smallconv_prep_launch)
@@ -49,10 +53,28 @@ struct SmallConvArgs {
     int nb, h, w_, cin, cout;
     int in_h, in_w;      // source extents (nearest resize when != h,w; VaeImageProcessor.resize)
     int flags;
+    const __half* res;   // optional fp16 NHWC residual added after the bias (before ReLU / SiLU): item n at res + n*res_bstride
+    int ldr;
+    long res_bstride;    // elements between batch items of res; 0 = one residual broadcast to every item
+    const float* in_off; // [3] offsets of SC_IN_OFFSET (device)
 };
 int smallconv_launch(const SmallConvArgs& a, cudaStream_t s);
 // OIHW fp16 -> fp32 [cin*9][cout] (once, at load time)
 int smallconv_prep_launch(const __half* w_oihw, float* wt, int cout, int cin, cudaStream_t s);
+
+// HED edge detector (ControlNet processor "hed"): 2x2/2 max-pool over NHWC fp16 (even h, w, c); the 1x1 C -> 1 side-output
+// projection, fp32 out; the fusion of the side outputs into the u8 edge image (see hed_fuse_kernel).
+int maxpool2x2_launch(const __half* x, __half* y, int nb, int h, int w, int c, cudaStream_t s);
+int hed_project_launch(const __half* x, int ldx, int c, long npix, const float* w, const float* bias, float* out, cudaStream_t s);
+struct HedFuseArgs {
+    const float* maps[5];   // side outputs, fp32 [hs[k]][ws[k]]
+    int hs[5], ws[5];
+    int levels;
+    int h, w;               // output size
+    uint8_t* out;           // u8 [h][w][3]
+    __half* edge_f16;       // optional fp16 [h][w] copy of the u8 value
+};
+int hed_fuse_launch(const HedFuseArgs& a, cudaStream_t s);
 
 // StreamDiffusion scheduler_step_batch + stream-batch buffer update (predict_x0_batch), fused.
 //   x0[i] = c_out[i] * (x[i] - beta[i]*eps[i]) / alpha[i] + c_skip[i] * x[i]
@@ -76,7 +98,7 @@ int timestep_embedding_launch(const float* t, float* out, int nb, int dim, cudaS
 // dtype / layout helpers used when weights are loaded
 int cast_f32_to_f16_launch(const float* x, __half* y, long n, cudaStream_t s);
 int cast_f16_to_f32_launch(const __half* x, float* y, long n, cudaStream_t s);
-// OIHW (fp16) -> packed [O][dst_ld] at column offset koff, K order [tap][c] for channels [c0, c0+cn)
+// OIHW (fp16) -> packed [O][dst_ld] at column offset koff, K order [tap][c] for channels [c0, c0+cn); channels >= i are zero
 int pack_conv_weight_launch(const __half* w_oihw, __half* dst, int dst_ld, int koff, int o, int i, int taps,
                             int c0, int cn, cudaStream_t s);
 // copy rows with a row permutation: dst[r][:] = src[perm[r]][:]

@@ -5,6 +5,7 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math.h>
+#include <stddef.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -134,7 +135,7 @@ int igemm_autotile(IgemmDesc d, bool allow_swap, IgemmPlan* plan_out) {
     const int pair_splits = ps_env ? atoi(ps_env) : (d.pair_splits > 0 ? d.pair_splits : 4);
     const IgemmPlan& pl = *plan_out;
     const int m_tiles = pl.p.tiles_w * pl.p.tiles_h * pl.p.tiles_n;
-    if (pair_mode <= 0 || pl.p.swap || m_tiles < 2 || (pl.p.BN % 32) != 0) return 0;
+    if (pair_mode <= 0 || pl.p.swap || m_tiles < 2 || (pl.p.BN % 32) != 0 || (d.epi.flags & IG_SILU)) return 0;
     if (pair_mode == 2 && pl.p.total_kb < 20) return 0;
     d.swap = 0; d.BN = pl.p.BN; d.splits = pl.splits > pair_splits ? pair_splits : pl.splits; d.partial = nullptr;
     d.pair = pair_single ? 0 : 1;
@@ -147,6 +148,7 @@ int igemm_autotile(IgemmDesc d, bool allow_swap, IgemmPlan* plan_out) {
 static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_out) {
     IgemmPlan& plan = *plan_out;
     const bool geglu = (d.epi.flags & IG_GEGLU) != 0;
+    const bool silu = (d.epi.flags & IG_SILU) != 0;   // SiLU-epilogue kernels exist for N tiles of 16..128 only
     const int n_gemm = geglu ? 2 * d.epi.n_valid : d.epi.n_valid;
     static const bool swap_on = getenv("B2_SWAP") != nullptr, swap_off = getenv("B2_NO_SWAP") != nullptr;
     static const bool tuned = getenv("B2_NO_TUNED_TILES") == nullptr;
@@ -178,7 +180,7 @@ static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_o
     }
     d.swap = 0;
     auto vt_ok = [&](int bn) { return !d.epi.out2 || d.epi.col2 % bn == 0; };   // fused q/k/v: an N tile is all q/k or all v
-    if (tuned && !geglu && n_gemm % 160 == 0 && total_kb >= 40 && vt_ok(160)) {
+    if (tuned && !geglu && !silu && n_gemm % 160 == 0 && total_kb >= 40 && vt_ok(160)) {
         // K-heavy contractions that cannot fill the GPU with 160-wide tiles alone (batch 1): wide tiles + cluster
         // split-K beat 64-wide tiles (weights streamed from HBM)
         d.BN = 160; d.splits = 1; d.partial = nullptr;
@@ -201,6 +203,7 @@ static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_o
     std::vector<int> valid;
     for (int bn : cands) {
         if (geglu && (bn % 32 != 0 || bn < 64)) continue;
+        if (silu && (bn > 128 || bn % 16 || (bn & (bn - 1)))) continue;
         if (n_gemm % bn == 0 && vt_ok(bn)) valid.push_back(bn);
     }
     if (valid.empty()) {  // ragged N: one masked tile size
@@ -276,6 +279,8 @@ struct b2sd_engine {
     float* temb_sin = nullptr; // [B][C0]
     float* temb_h = nullptr;   // [B][4*C0]
     float* temb = nullptr;     // [B][4*C0]
+    float* cn_temb_h = nullptr;   // ControlNet time_embedding (its own weights), [B][4*C0]
+    float* cn_temb = nullptr;
     float* gn_ws = nullptr;    // GroupNorm chunk partials (shared: launches are stream-ordered)
     int* tile_counters = nullptr;
     float coef_host[4][64]{};
@@ -285,6 +290,8 @@ struct b2sd_engine {
     std::vector<Op> prog_frame, prog_prompt, prog_time;
     std::map<std::string, Act> taps;
     SmallConvArgs head{};   // encoder head (reads the caller's frame)
+    SmallConvArgs cn_head{};   // ControlNet conditioning embedding conv_in (reads the caller's frame as the control image)
+    SmallConvArgs hed_head{};  // HED's first conv (reads the caller's frame) when the control image is its edge map
     Act image;              // decoder output, fp16 NHWC (ld 8)
     bool built = false;
     int concurrency = 1;   // frames expected in flight on this GPU (b2sd_set_concurrency): > 1 selects the throughput launch policy
@@ -607,7 +614,10 @@ struct b2sd_engine {
         return add_igemm(dst, d);
     }
 
-    int build_resnet(const std::string& p, const Act& xa, const Act* xb, int cout, Act* out, cudaStream_t s);
+    int build_resnet(const std::string& p, const Act& xa, const Act* xb, int cout, const float* emb, Act* out, cudaStream_t s);
+    int build_cond_embedding(Act* out, cudaStream_t s);
+    int build_hed(const uint8_t** control, cudaStream_t s);
+    int build_controlnet(const Act& cond, std::vector<Act>& skips, Act* mid, cudaStream_t s);
     int build_transformer(const std::string& p, const Act& x, int heads, Act* out, cudaStream_t s);
     int build_taesd_block(const std::string& p, const Act& x, Act* out, cudaStream_t s);
     int build_program(cudaStream_t s);
@@ -643,7 +653,8 @@ struct b2sd_engine {
 
 // ------------------------------------------------------------------------------------------------
 // ResnetBlock2D (diffusers resnet.py): GN+SiLU -> conv1 (+temb) -> GN+SiLU -> conv2, + shortcut(x)
-int b2sd_engine::build_resnet(const std::string& p, const Act& xa, const Act* xb, int cout, Act* out, cudaStream_t s) {
+int b2sd_engine::build_resnet(const std::string& p, const Act& xa, const Act* xb, int cout, const float* emb, Act* out,
+                              cudaStream_t s) {
     cur = p;
     allow_swap = true;
     const int cin = xa.c + (xb ? xb->c : 0);
@@ -661,7 +672,6 @@ int b2sd_engine::build_resnet(const std::string& p, const Act& xa, const Act* xb
         const Raw* wt = get(p + "time_emb_proj.weight");
         if (!colbias || !bsum || !wt) return -1;
         const int tdim = (int)wt->shape[1];
-        const float* emb = temb;
         const __half* wtp = wt->p;
         prog_time.push_back(Op([=](cudaStream_t st) { return small_linear_launch(emb, tdim, wtp, bsum, colbias, cout, B, cout, tdim, 1, st); }, "temb " + p));
         IgemmDesc d{};
@@ -926,6 +936,176 @@ int b2sd_engine::build_taesd_block(const std::string& p, const Act& x, Act* out,
     return add_conv(prog_frame, b, p + ".conv.4.weight", p + ".conv.4.bias", 9, 1, *out, IG_RELU, &x, s);
 }
 
+// ControlNetConditioningEmbedding (diffusers controlnet.py): conv_in 3->16 + SiLU, six 3x3 convs 16->16, 16->32/2, 32->32,
+// 32->96/2, 96->96, 96->256/2 each + SiLU, conv_out 256->C0.  conv_in reads the caller's frame (b2sd_step_ex launches cn_head
+// next to the encoder head); the rest is stage 1 of the frame program (it depends on the frame only).  The 16/32/96-channel
+// activations are stored 64/64/128 wide with zero padding columns, so the following layers run as 64/64/128-channel
+// tensor-core contractions (zero weights on the padding channels, pack_conv_weight_launch).  The epilogues write only the
+// valid columns: the padding is cleared once here, and stays finite (0 * NaN would be NaN).
+int b2sd_engine::build_cond_embedding(Act* out, cudaStream_t s) {
+    const std::string p = "controlnet.controlnet_cond_embedding.";
+    cur = p;
+    allow_swap = false;
+    auto padded = [&](int n, int hh, int ww, int c) {
+        Act a = new_act(n, hh, ww, c, (c + 63) / 64 * 64);
+        if (a.p && a.ld != c && cudaMemsetAsync(a.p, 0, (size_t)a.elems() * 2, s) != cudaSuccess) a.p = nullptr;
+        return a;
+    };
+    Act a = padded(1, cfg.height, cfg.width, 16);
+    if (!a.p) { b2_set_error("controlnet: activation allocation failed"); return -1; }
+    cn_head = SmallConvArgs{};
+    cn_head.wt = small_w(p + "conv_in.weight", s);
+    cn_head.bias = vec({p + "conv_in.bias"});
+    if (!cn_head.wt || !cn_head.bias) return -1;
+    cn_head.y = a.p; cn_head.ldy = a.ld; cn_head.nb = 1; cn_head.h = a.h; cn_head.w_ = a.w; cn_head.cin = 3; cn_head.cout = 16;
+    ++launches;
+    if (cfg.control_processor == B2SD_CONTROL_HED) {   // the control image is HED's edge map, computed in this stage
+        const uint8_t* control = nullptr;
+        TRY(build_hed(&control, s));
+        SmallConvArgs c = cn_head;
+        c.x = control; c.in_h = a.h; c.in_w = a.w; c.flags = SC_IN_U8 | SC_OUT_SILU;
+        prog_frame.push_back(Op([c](cudaStream_t st) { return smallconv_launch(c, st); }, "smallconv controlnet_cond_embedding.conv_in"));
+    }
+    static const int cout[6] = {16, 32, 32, 96, 96, 256}, stride[6] = {1, 2, 1, 2, 1, 2};
+    for (int k = 0; k < 6; ++k) {
+        Act x = a;
+        x.c = x.ld;   // padding channels enter the contraction (zero activations times zero weights)
+        a = padded(1, x.h / stride[k], x.w / stride[k], cout[k]);
+        if (!a.p) { b2_set_error("controlnet: activation allocation failed"); return -1; }
+        const std::string w = p + "blocks." + std::to_string(k);
+        TRY(add_conv(prog_frame, x, w + ".weight", w + ".bias", 9, stride[k], a, IG_SILU, nullptr, s));
+    }
+    *out = new_act(1, lh, lw, cfg.block_out_channels[0]);
+    TRY(add_conv(prog_frame, a, p + "conv_out.weight", p + "conv_out.bias", 9, 1, *out, 0, nullptr, s));
+    taps["cn_cond"] = *out;
+    return 0;
+}
+
+// ControlNetHED_Apache2 (controlnet_aux) + HEDdetector's post-processing, at the engine's resolution: h = frame(0..255) - norm;
+// five blocks of 3x3 convs + ReLU (3->64 x2, 64->128 x2, 128->256 x3, 256->512 x3, 512->512 x3), blocks 2-5 after a 2x2/2
+// max-pool; each block's 1x1 projection to one channel; the five maps upsampled bilinearly, averaged, sigmoid, * 255,
+// truncated to the u8 edge image (3 channels).  The first conv reads the caller's frame (hed_head, launched by b2sd_step_ex).
+int b2sd_engine::build_hed(const uint8_t** control, cudaStream_t s) {
+    const int H = cfg.height, W = cfg.width;
+    static const int ch[5] = {64, 128, 256, 512, 512}, nconv[5] = {2, 2, 3, 3, 3};
+    cur = "hed";
+    allow_swap = false;
+    Act a = new_act(1, H, W, ch[0]);
+    hed_head = SmallConvArgs{};
+    hed_head.wt = small_w("hed.block1.convs.0.weight", s);
+    hed_head.bias = vec({"hed.block1.convs.0.bias"});
+    hed_head.in_off = vec({"hed.norm"});
+    if (!a.p || !hed_head.wt || !hed_head.bias || !hed_head.in_off) return -1;
+    hed_head.y = a.p; hed_head.ldy = a.ld; hed_head.nb = 1; hed_head.h = H; hed_head.w_ = W; hed_head.cin = 3; hed_head.cout = ch[0];
+    ++launches;
+    HedFuseArgs f{};
+    for (int b = 0; b < 5; ++b) {
+        const std::string p = "hed.block" + std::to_string(b + 1) + ".";
+        if (b > 0) {
+            Act o = new_act(1, a.h / 2, a.w / 2, a.c);
+            if (!o.p) return -1;
+            const Act x = a;
+            ++launches;
+            prog_frame.push_back(Op([x, o](cudaStream_t st) { return maxpool2x2_launch(x.p, o.p, 1, x.h, x.w, x.c, st); }, "maxpool2x2 " + p));
+            a = o;
+        }
+        for (int k = b == 0 ? 1 : 0; k < nconv[b]; ++k) {
+            Act o = new_act(1, a.h, a.w, ch[b]);
+            const std::string w = p + "convs." + std::to_string(k);
+            TRY(add_conv(prog_frame, a, w + ".weight", w + ".bias", 9, 1, o, IG_RELU, nullptr, s));
+            a = o;
+        }
+        float* m = static_cast<float*>(prog.alloc((size_t)a.h * a.w * sizeof(float)));
+        const float* pw = vec({p + "projection.weight"});
+        const float* pb = vec({p + "projection.bias"});
+        if (!m || !pw || !pb) return -1;
+        const Act x = a;
+        ++launches;
+        prog_frame.push_back(Op([x, pw, pb, m](cudaStream_t st) { return hed_project_launch(x.p, x.ld, x.c, (long)x.h * x.w, pw, pb, m, st); },
+                                "hed_project " + p));
+        f.maps[b] = m; f.hs[b] = a.h; f.ws[b] = a.w;
+    }
+    f.levels = 5; f.h = H; f.w = W;
+    f.out = static_cast<uint8_t*>(prog.alloc((size_t)H * W * 3));
+    Act edge = new_act(1, H, W, 1);
+    if (!f.out || !edge.p) return -1;
+    f.edge_f16 = edge.p;
+    ++launches;
+    prog_frame.push_back(Op([f](cudaStream_t st) { return hed_fuse_launch(f, st); }, "hed_fuse"));
+    taps["control"] = edge;
+    *control = f.out;
+    return 0;
+}
+
+// ControlNetModel body: conv_in(x) + cond (broadcast to every stream-batch slot), the UNet's down blocks and mid block under the
+// "controlnet." prefix with its own time embedding, then the zero convs: skips[k] <- skips[k] + controlnet_down_blocks.k(f_k),
+// *mid <- *mid + controlnet_mid_block(f_mid), each one 1x1 contraction with the UNet tensor as its epilogue residual, written
+// to a new buffer (conditioning scale 1.0).
+int b2sd_engine::build_controlnet(const Act& cond, std::vector<Act>& skips, Act* mid, cudaStream_t s) {
+    const std::string P = "controlnet.";
+    const int B = cfg.batch, nlev = 4;
+    const int* ch = cfg.block_out_channels;
+    cur = P + "conv_in";
+    allow_swap = true;
+    Act h = new_act(B, lh, lw, ch[0]);
+    {
+        SmallConvArgs a{};
+        a.wt = small_w(P + "conv_in.weight", s);
+        a.bias = vec({P + "conv_in.bias"});
+        if (!a.wt || !a.bias || !h.p) return -1;
+        a.x = x_in.p; a.y = h.p; a.ldy = h.ld; a.nb = B; a.h = lh; a.w_ = lw; a.cin = 4; a.cout = ch[0]; a.in_h = lh; a.in_w = lw;
+        a.res = cond.p; a.ldr = cond.ld; a.res_bstride = 0;
+        ++launches;
+        prog_frame.push_back(Op([a](cudaStream_t st) { return smallconv_launch(a, st); }, "smallconv controlnet.conv_in"));
+    }
+    taps["cn.conv_in"] = h;
+    std::vector<Act> feats{h};
+    for (int i = 0; i < nlev; ++i) {
+        const std::string bp = P + "down_blocks." + std::to_string(i);
+        for (int j = 0; j < cfg.layers_per_block; ++j) {
+            Act o;
+            TRY(build_resnet(bp + ".resnets." + std::to_string(j) + ".", h, nullptr, ch[i], cn_temb, &o, s));
+            h = o;
+            if (cfg.down_attn[i]) {
+                TRY(build_transformer(bp + ".attentions." + std::to_string(j) + ".", h, cfg.heads[i], &o, s));
+                h = o;
+            }
+            feats.push_back(h);
+        }
+        if (i != nlev - 1) {
+            Act o = new_act(B, h.h / 2, h.w / 2, ch[i]);
+            const std::string k = bp + ".downsamplers.0.conv.";
+            TRY(add_conv(prog_frame, h, k + "weight", k + "bias", 9, 2, o, 0, nullptr, s));
+            h = o;
+            feats.push_back(h);
+        }
+    }
+    {
+        Act o;
+        TRY(build_resnet(P + "mid_block.resnets.0.", h, nullptr, ch[nlev - 1], cn_temb, &o, s)); h = o;
+        TRY(build_transformer(P + "mid_block.attentions.0.", h, cfg.heads[nlev - 1], &o, s)); h = o;
+        TRY(build_resnet(P + "mid_block.resnets.1.", h, nullptr, ch[nlev - 1], cn_temb, &o, s)); h = o;
+    }
+    if (feats.size() != skips.size()) {
+        b2_set_error("controlnet: %zu down residuals for %zu UNet skips", feats.size(), skips.size());
+        return -1;
+    }
+    allow_swap = false;
+    for (size_t k = 0; k < feats.size(); ++k) {
+        const std::string w = P + "controlnet_down_blocks." + std::to_string(k);
+        Act o = new_act(skips[k].n, skips[k].h, skips[k].w, skips[k].c);
+        TRY(add_conv(prog_frame, feats[k], w + ".weight", w + ".bias", 1, 1, o, 0, &skips[k], s));
+        skips[k] = o;
+        taps["cn.res." + std::to_string(k)] = o;
+    }
+    Act o = new_act(mid->n, mid->h, mid->w, mid->c);
+    TRY(add_conv(prog_frame, h, P + "controlnet_mid_block.weight", P + "controlnet_mid_block.bias", 1, 1, o, 0, mid, s));
+    *mid = o;
+    taps["cn.mid"] = o;
+    allow_swap = true;
+    return 0;
+}
+
 int b2sd_engine::build_program(cudaStream_t s) {
     prog.reset();
     prog_frame.clear(); prog_prompt.clear(); prog_time.clear();
@@ -941,7 +1121,8 @@ int b2sd_engine::build_program(cudaStream_t s) {
         long words = 0;
         for (int i = 0; i < nlev; ++i) {
             const long tokens_i = (long)B * (lh >> i) * (lw >> i);
-            const int blocks_i = (cfg.down_attn[i] ? cfg.layers_per_block + (cfg.layers_per_block + 1) : 0) + (i == nlev - 1 ? 1 : 0);
+            int blocks_i = (cfg.down_attn[i] ? cfg.layers_per_block + (cfg.layers_per_block + 1) : 0) + (i == nlev - 1 ? 1 : 0);
+            if (cfg.controlnet) blocks_i += (cfg.down_attn[i] ? cfg.layers_per_block : 0) + (i == nlev - 1 ? 1 : 0);
             words += 3 * 2 * tokens_i * blocks_i;
         }
         ln_stats_cap = (size_t)words;
@@ -979,6 +1160,8 @@ int b2sd_engine::build_program(cudaStream_t s) {
             ++li;
         }
     }
+    Act cond;   // ControlNet conditioning embedding of this frame's control image: batch 1, latent resolution, C0 channels
+    if (cfg.controlnet) TRY(build_cond_embedding(&cond, s));
     {
         // latent head + StreamDiffusion.encode_image add-noise: x_t = alpha0 * z + beta0 * init_noise[0]
         Act xt;  // slot 0 of the UNet input batch
@@ -1011,7 +1194,7 @@ int b2sd_engine::build_program(cudaStream_t s) {
         for (int j = 0; j < cfg.layers_per_block; ++j) {
             Act o;
             const std::string bp = "down_blocks." + std::to_string(i);
-            TRY(build_resnet(bp + ".resnets." + std::to_string(j) + ".", h, nullptr, ch[i], &o, s));
+            TRY(build_resnet(bp + ".resnets." + std::to_string(j) + ".", h, nullptr, ch[i], temb, &o, s));
             h = o;
             if (cfg.down_attn[i]) {
                 TRY(build_transformer(bp + ".attentions." + std::to_string(j) + ".", h, cfg.heads[i], &o, s));
@@ -1030,11 +1213,14 @@ int b2sd_engine::build_program(cudaStream_t s) {
     }
     {
         Act o;
-        TRY(build_resnet("mid_block.resnets.0.", h, nullptr, ch[nlev - 1], &o, s)); h = o;
+        TRY(build_resnet("mid_block.resnets.0.", h, nullptr, ch[nlev - 1], temb, &o, s)); h = o;
         TRY(build_transformer("mid_block.attentions.0.", h, cfg.heads[nlev - 1], &o, s)); h = o;
-        TRY(build_resnet("mid_block.resnets.1.", h, nullptr, ch[nlev - 1], &o, s)); h = o;
+        TRY(build_resnet("mid_block.resnets.1.", h, nullptr, ch[nlev - 1], temb, &o, s)); h = o;
         taps["mid"] = h;
     }
+    // ControlNet: its down path + mid block over the same x / timesteps / prompt; the zero convs add its 12 + 1 residuals to the
+    // skips the up path concatenates and to the mid-block output (the UNet's own down path above used them unmodified)
+    if (cfg.controlnet) TRY(build_controlnet(cond, skips, &h, s));
     for (int i = 0; i < nlev; ++i) {
         const int co = ch[nlev - 1 - i];
         const int hd = cfg.heads[nlev - 1 - i];
@@ -1044,7 +1230,7 @@ int b2sd_engine::build_program(cudaStream_t s) {
             skips.pop_back();
             Act o;
             const std::string bp = "up_blocks." + std::to_string(i);
-            TRY(build_resnet(bp + ".resnets." + std::to_string(j) + ".", h, &sk, co, &o, s));
+            TRY(build_resnet(bp + ".resnets." + std::to_string(j) + ".", h, &sk, co, temb, &o, s));
             h = o;
             if (attn) {
                 TRY(build_transformer(bp + ".attentions." + std::to_string(j) + ".", h, hd, &o, s));
@@ -1148,6 +1334,8 @@ int b2sd_create_lane(b2sd_handle parent, const b2sd_config* cfg, b2sd_handle* ou
         return -1;
     }
     b2sd_config c = cfg ? *cfg : parent->cfg;
+    c.controlnet = parent->cfg.controlnet;   // a lane runs the parent's networks
+    c.control_processor = parent->cfg.control_processor;
     for (int i = 0; i < 4; ++i)
         if (c.block_out_channels[i] != parent->cfg.block_out_channels[i] || c.heads[i] != parent->cfg.heads[i] ||
             c.down_attn[i] != parent->cfg.down_attn[i]) {
@@ -1179,6 +1367,14 @@ static int create_engine(const b2sd_config* cfg, std::shared_ptr<WeightStore> st
         b2_set_error("b2sd_create: cross_attention_dim must be a multiple of 64");
         return -1;
     }
+    if (cfg->controlnet != 0 && cfg->controlnet != 1) {
+        b2_set_error("b2sd_create: controlnet must be 0 or 1 (got %d)", cfg->controlnet);
+        return -1;
+    }
+    if (cfg->control_processor != B2SD_CONTROL_FRAME && (cfg->control_processor != B2SD_CONTROL_HED || !cfg->controlnet)) {
+        b2_set_error("b2sd_create: control_processor must be 0 (the frame) or 1 (HED, with a ControlNet) (got %d)", cfg->control_processor);
+        return -1;
+    }
     int dev = 0;
     cudaDeviceProp prop;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess) {
@@ -1204,10 +1400,15 @@ static int create_engine(const b2sd_config* cfg, std::shared_ptr<WeightStore> st
     e->temb_sin = static_cast<float*>(e->state.alloc((size_t)B * C0 * sizeof(float)));
     e->temb_h = static_cast<float*>(e->state.alloc((size_t)B * 4 * C0 * sizeof(float)));
     e->temb = static_cast<float*>(e->state.alloc((size_t)B * 4 * C0 * sizeof(float)));
+    if (cfg->controlnet) {
+        e->cn_temb_h = static_cast<float*>(e->state.alloc((size_t)B * 4 * C0 * sizeof(float)));
+        e->cn_temb = static_cast<float*>(e->state.alloc((size_t)B * 4 * C0 * sizeof(float)));
+    }
     e->gn_ws = static_cast<float*>(e->state.alloc(groupnorm_partial_floats(B, cfg->norm_groups) * sizeof(float)));
     e->tile_counters = static_cast<int*>(e->state.alloc(65536 * sizeof(int)));
     if (e->tile_counters) cudaMemset(e->tile_counters, 0, 65536 * sizeof(int));
-    if (!e->x_in.p || !e->noise || !e->coef || !e->tsteps || !e->ctx || !e->temb || !e->gn_ws) {
+    if (!e->x_in.p || !e->noise || !e->coef || !e->tsteps || !e->ctx || !e->temb || !e->gn_ws ||
+        (cfg->controlnet && (!e->cn_temb_h || !e->cn_temb))) {
         b2_set_error("b2sd_create: cudaMalloc failed");
         delete e;
         return -1;
@@ -1229,6 +1430,7 @@ static bool is_pack_only(const std::string& key, const int64_t* shape, int ndim)
     auto has = [&](const char* t) { return key.find(t) != std::string::npos; };
     if (ndim == 4 && shape[2] == 3) return true;                       // every 3x3 convolution (incl. the Cin <= 4 ones)
     if (ndim == 4 && has("conv_shortcut.weight")) return true;         // packed into the conv2 rows
+    if (ndim == 4 && (has("controlnet_down_blocks.") || has("controlnet_mid_block."))) return true;   // ControlNet zero convs
     if (ndim == 2 && (has(".to_q.weight") || has(".to_k.weight") || has(".to_v.weight"))) return true;   // per-head gather
     if (ndim == 2 && has("ff.net.0.proj.weight")) return true;         // GEGLU value/gate interleave
     return false;
@@ -1279,7 +1481,10 @@ int b2sd_load_tensor(b2sd_handle h, const char* key, const void* ptr, int dtype,
         b2_set_error("b2sd_load_tensor: dtype %d", dtype);
         return -1;
     }
-    if (ndim == 1) {
+    // 1-D parameters get a host copy (fused fp32 vectors); so do HED's [1,3,1,1] offset and [1,C,1,1] projections, read as vectors
+    const std::string k(key);
+    const bool hed_vec = k == "hed.norm" || (k.compare(0, 4, "hed.") == 0 && k.size() > 18 && k.compare(k.size() - 18, 18, ".projection.weight") == 0);
+    if (ndim == 1 || hed_vec) {
         std::vector<__half> hh(n);
         CUDA_OK(cudaMemcpy(hh.data(), r.p, (size_t)n * 2, cudaMemcpyDeviceToHost));
         r.host.resize(n);
@@ -1290,16 +1495,21 @@ int b2sd_load_tensor(b2sd_handle h, const char* key, const void* ptr, int dtype,
     return 0;
 }
 
+// TimestepEmbedding of the UNet (and of the ControlNet, from the same sinusoidal features), then every resnet's projection
 static int refresh_time(b2sd_handle h, cudaStream_t s) {
     const int B = h->cfg.batch, C0 = h->cfg.block_out_channels[0], TD = 4 * C0;
-    const Raw* w1 = h->get("time_embedding.linear_1.weight");
-    const Raw* w2 = h->get("time_embedding.linear_2.weight");
-    const float* b1 = h->vec({"time_embedding.linear_1.bias"});
-    const float* b2v = h->vec({"time_embedding.linear_2.bias"});
-    if (!w1 || !w2 || !b1 || !b2v) return -1;
     TRY(timestep_embedding_launch(h->tsteps, h->temb_sin, B, C0, s));
-    TRY(small_linear_launch(h->temb_sin, C0, w1->p, b1, h->temb_h, TD, B, TD, C0, 0, s));
-    TRY(small_linear_launch(h->temb_h, TD, w2->p, b2v, h->temb, TD, B, TD, TD, 1, s));
+    auto embed = [&](const std::string& p, float* hid, float* out) {
+        const Raw* w1 = h->get(p + "time_embedding.linear_1.weight");
+        const Raw* w2 = h->get(p + "time_embedding.linear_2.weight");
+        const float* b1 = h->vec({p + "time_embedding.linear_1.bias"});
+        const float* b2v = h->vec({p + "time_embedding.linear_2.bias"});
+        if (!w1 || !w2 || !b1 || !b2v) return -1;
+        TRY(small_linear_launch(h->temb_sin, C0, w1->p, b1, hid, TD, B, TD, C0, 0, s));
+        return small_linear_launch(hid, TD, w2->p, b2v, out, TD, B, TD, TD, 1, s);
+    };
+    TRY(embed("", h->temb_h, h->temb));
+    if (h->cfg.controlnet) TRY(embed("controlnet.", h->cn_temb_h, h->cn_temb));
     return h->run(h->prog_time, s);
 }
 
@@ -1382,7 +1592,7 @@ int b2sd_export_packed(b2sd_handle h, const char* path) {
     }
     BlobWriter w{f};
     w.put("B2SDPACK", 8);
-    w.pod((uint32_t)1);
+    w.pod((uint32_t)2);   // 2: b2sd_config carries `controlnet` / `control_processor` (version 1 blobs still load)
     b2sd_config cfg = h->cfg;
     cfg.batch = 0; cfg.height = 0; cfg.width = 0; cfg.use_cuda_graph = 0; cfg.do_add_noise = 0;   // the blob is independent of these
     w.pod(cfg);
@@ -1439,9 +1649,13 @@ int b2sd_import_packed(b2sd_handle h, const char* path) {
     char magic[8];
     rd.get(magic, 8);
     const uint32_t version = rd.pod<uint32_t>();
-    b2sd_config cfg = rd.pod<b2sd_config>();
-    bool same = rd.ok && memcmp(magic, "B2SDPACK", 8) == 0 && version == 1 && cfg.cross_attention_dim == h->cfg.cross_attention_dim &&
-                cfg.layers_per_block == h->cfg.layers_per_block && cfg.norm_groups == h->cfg.norm_groups && cfg.ctx_tokens == h->cfg.ctx_tokens;
+    // version 1 blobs predate the ControlNet fields at the end of b2sd_config: they hold no ControlNet (both fields 0)
+    b2sd_config cfg{};
+    if (version == 1) rd.get(&cfg, offsetof(b2sd_config, controlnet));
+    else cfg = rd.pod<b2sd_config>();
+    bool same = rd.ok && memcmp(magic, "B2SDPACK", 8) == 0 && (version == 1 || version == 2) && cfg.cross_attention_dim == h->cfg.cross_attention_dim &&
+                cfg.layers_per_block == h->cfg.layers_per_block && cfg.norm_groups == h->cfg.norm_groups && cfg.ctx_tokens == h->cfg.ctx_tokens &&
+                cfg.controlnet == h->cfg.controlnet && cfg.control_processor == h->cfg.control_processor;
     for (int i = 0; i < 4 && same; ++i)
         same = cfg.block_out_channels[i] == h->cfg.block_out_channels[i] && cfg.heads[i] == h->cfg.heads[i] && cfg.down_attn[i] == h->cfg.down_attn[i];
     if (!same) {
@@ -1538,6 +1752,14 @@ int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int
     a.x = frame_in; a.in_h = in_h; a.in_w = in_w;
     a.flags = in_kind == B2SD_IN_U8_NHWC ? SC_IN_U8 : (in_kind == B2SD_IN_F32_NCHW ? SC_IN_F32_NCHW : SC_IN_F16_NCHW);
     TRY(smallconv_launch(a, s));
+    if (h->cfg.controlnet) {   // the control image is the frame itself in [0, 1], at the engine's size (same nearest resize)
+        // the control image is the frame itself in [0, 1] at the engine's size (same nearest resize), or HED's edge map, whose
+        // first conv reads the frame here and whose remaining layers run in stage 1
+        const bool hed = h->cfg.control_processor == B2SD_CONTROL_HED;
+        SmallConvArgs c = hed ? h->hed_head : h->cn_head;
+        c.x = frame_in; c.in_h = in_h; c.in_w = in_w; c.flags = a.flags | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
+        TRY(smallconv_launch(c, s));
+    }
     if (h->group) {
         // stage-pipelined lanes of one stateful stream: encoder body | [wait previous frame's UNet stage] last encoder conv,
         // UNet, scheduler step [signal] | decoder.  Lanes run on different streams; only the middle stage is serialised.
@@ -1632,6 +1854,12 @@ int b2sd_profile(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* 
     for (int it = 0; it < iters + 1; ++it) {  // first iteration is a warm-up
         CUDA_OK(cudaEventRecord(ev[0], s));
         TRY(smallconv_launch(a, s));
+        if (h->cfg.controlnet) {
+            const bool hed = h->cfg.control_processor == B2SD_CONTROL_HED;
+            SmallConvArgs c = hed ? h->hed_head : h->cn_head;
+            c.x = frame_in; c.in_h = in_h; c.in_w = in_w; c.flags = SC_IN_U8 | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
+            TRY(smallconv_launch(c, s));
+        }
         CUDA_OK(cudaEventRecord(ev[1], s));
         size_t i = 1;
         for (auto& op : h->prog_frame) {

@@ -11,6 +11,8 @@ __device__ __forceinline__ float gelu_erf(float x) {
     return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));
 }
 
+__device__ __forceinline__ float silu_f(float x) { return x / (1.0f + expf(-x)); }
+
 __device__ __forceinline__ void store_half16(__half* dst, const float* v, int nv, bool vec_ok) {
     if (nv == 16 && vec_ok) {
         uint4 u[2];
@@ -45,7 +47,8 @@ __device__ __forceinline__ void rowstat_add(const IgEpilogue& e, long orow, floa
 
 // 16 accumulator columns [col0, col0+16) of output row `orow` (batch item b); the accumulators are
 // acc[OFF .. OFF+16) of a register array (compile-time indices only: nothing may spill to local memory).
-template <int OFF, int N, typename T>
+// SILU: compile the IG_SILU branch in (kernels that never see the flag leave it out: it costs registers in the wide tiles).
+template <int OFF, int N, typename T, bool SILU = false>
 __device__ __forceinline__ void epi_store16(const IgEpilogue& e, const T (&acc)[N], int b, long orow, int col0, float mu = 0.f,
                                             float rstd = 1.f) {
     int nv = e.n_valid - col0;
@@ -104,6 +107,10 @@ __device__ __forceinline__ void epi_store16(const IgEpilogue& e, const T (&acc)[
 #pragma unroll
         for (int i = 0; i < 16; ++i) v[i] = fmaxf(v[i], 0.0f);
     }
+    if (SILU && (e.flags & IG_SILU)) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) v[i] = silu_f(v[i]);
+    }
     if (e.out2 && col0 >= e.col2) {   // V block of the fused q/k/v projection: transposed store (32 lanes = 32 consecutive tokens)
         __half* tp = e.out2 + (long)(col0 - e.col2) * e.ld2 + orow;
 #pragma unroll
@@ -156,7 +163,7 @@ __device__ __forceinline__ void rowstat_quad(const IgEpilogue& e, const EpiRow& 
 //   ln_fma: LayerNorm-folded launch with vectorisable pitches: x = rstd * acc - rstd * mu * colsum + bias'
 //   GEGLU: tile columns [0, BN/2) are values, [BN/2, BN) gates; out = v * gelu_erf(g)
 //   otherwise: bias / scale / residual / ReLU, optional row statistics and transposed V block
-template <int BN>
+template <int BN, bool SILU = false>
 __device__ __forceinline__ void epi_frag(const IgEpilogue& e, const float (&acc)[BN / 2], const EpiRow (&rw)[2], int ntile,
                                          bool ln_fma, int lane) {
     const int q2 = 2 * (lane & 3);
@@ -241,6 +248,10 @@ __device__ __forceinline__ void epi_frag(const IgEpilogue& e, const float (&acc)
                 if (e.flags & IG_RELU) {
                     x[0] = fmaxf(x[0], 0.f);
                     x[1] = fmaxf(x[1], 0.f);
+                }
+                if (SILU && (e.flags & IG_SILU)) {
+                    x[0] = silu_f(x[0]);
+                    x[1] = silu_f(x[1]);
                 }
             }
             if (transposed) {   // V block of the fused q/k/v projection -> V^T

@@ -79,6 +79,7 @@ __device__ __forceinline__ void swap_prefetch(const IgemmParams& p, SwapPre& pre
     }
 }
 
+template <bool SILU>
 __device__ __forceinline__ void swap_store_chunk(const IgemmParams& p, const SwapPre& pre, const float* T, int ntile, int t) {
     const IgEpilogue& e = p.epi;
 #pragma unroll
@@ -105,6 +106,10 @@ __device__ __forceinline__ void swap_store_chunk(const IgemmParams& p, const Swa
         if (e.flags & IG_RELU) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) v[i] = fmaxf(v[i], 0.f);
+        }
+        if (SILU && (e.flags & IG_SILU)) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v[i] = silu_f(v[i]);
         }
         uint4 o;
         __half2* oh = reinterpret_cast<__half2*>(&o);
@@ -151,7 +156,7 @@ __device__ __forceinline__ void splitk_sum16(uint32_t stg_local, int cc, int row
 // with the same weight tile: each CTA loads its own 128 pixel rows and HALF of the weight rows, multicast into both CTAs'
 // shared memory, so each SM fetches half of the weight bytes from L2.  A ring slot is refilled only when the warps of BOTH
 // CTAs have released it (every consumer warp arrives on its own and on the peer's empty barrier).
-template <int BN, bool PAIR>
+template <int BN, bool PAIR, bool SILU>
 __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -319,7 +324,7 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
                         swap_prefetch(p, pre, SWAP_CH, c, ntile, n0, h0, w0, threadIdx.x);
                         frag_to_smem<BN>(stg, acc, r0, lane, c, SWAP_CH, true);
                         cons_bar_sync();
-                        swap_store_chunk(p, pre, stg, ntile, threadIdx.x);
+                        swap_store_chunk<SILU>(p, pre, stg, ntile, threadIdx.x);
                         cons_bar_sync();
                     }
                 }
@@ -335,7 +340,7 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
                     rw[h].b = n;
                     ln_row_stats(e, rw[h].orow, rw[h].ok, rw[h].mu, rw[h].rstd);
                 }
-                epi_frag<BN>(e, acc, rw, ntile, ln_fma, lane);
+                epi_frag<BN, SILU>(e, acc, rw, ntile, ln_fma, lane);
             }
             B2_TS(if (ts && it == 0 && threadIdx.x == 0) ts[5] = globaltimer_ns();)
         }
@@ -390,7 +395,7 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
                     T[(4 * gg + 3) * IG_BM + t] = a.w;
                 }
                 cons_bar_sync();
-                swap_store_chunk(p, pre, T, ntile, threadIdx.x);
+                swap_store_chunk<SILU>(p, pre, T, ntile, threadIdx.x);
                 cons_bar_sync();
             }
         } else if (warp < IG_CONS / 32) {
@@ -416,7 +421,7 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
                     const long orow = ((long)n * p.Ho + h) * p.Wo + w;
                     float mu, rstd;
                     ln_row_stats(p.epi, orow, true, mu, rstd);
-                    epi_store16<0>(p.epi, acc, n, orow, ntile * BN + cc * 16, mu, rstd);
+                    epi_store16<0, 16, float, SILU>(p.epi, acc, n, orow, ntile * BN + cc * 16, mu, rstd);
                 }
             }
         }
@@ -429,8 +434,8 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
     }
 }
 
-template <int BN, bool PAIR>
-__global__ void __launch_bounds__(IG_THREADS, 1) igemm_kernel(const __grid_constant__ IgemmParams p) { igemm_body<BN, PAIR>(p); }
+template <int BN, bool PAIR, bool SILU = false>
+__global__ void __launch_bounds__(IG_THREADS, 1) igemm_kernel(const __grid_constant__ IgemmParams p) { igemm_body<BN, PAIR, SILU>(p); }
 
 using IgemmFn = void (*)(IgemmParams);
 // every N tile the planner can produce (multiples of 16 up to 256); CTA pairs need BN % 32 == 0.  At 168 registers the widest
@@ -443,6 +448,19 @@ static IgemmFn igemm_fn(int bn) {
         B2_IG_CASE(16) B2_IG_CASE(32) B2_IG_CASE(48) B2_IG_CASE(64) B2_IG_CASE(80) B2_IG_CASE(96) B2_IG_CASE(112) B2_IG_CASE(128)
         B2_IG_CASE(144) B2_IG_CASE(160) B2_IG_CASE(176) B2_IG_CASE(192) B2_IG_CASE(208) B2_IG_CASE(224) B2_IG_CASE(240) B2_IG_CASE(256)
 #undef B2_IG_CASE
+        default: return nullptr;
+    }
+}
+// IG_SILU epilogues (the ControlNet conditioning embedding: N = 16 / 32 / 96 / 256, single CTAs, N tiles <= 128) are separate
+// instantiations, so the SiLU code costs the other kernels no registers (a 256-wide SiLU tile would spill)
+static IgemmFn igemm_select(int bn, bool pair, bool silu) {
+    if (!silu) return pair ? igemm_fn<true>(bn) : igemm_fn<false>(bn);
+    if (pair) return nullptr;
+    switch (bn) {
+        case 16: return igemm_kernel<16, false, true>;
+        case 32: return igemm_kernel<32, false, true>;
+        case 64: return igemm_kernel<64, false, true>;
+        case 128: return igemm_kernel<128, false, true>;
         default: return nullptr;
     }
 }
@@ -634,9 +652,9 @@ int b2_device_sms() {
 
 // CTAs of the kernel for this tile that one SM holds at once as far as registers and threads allow (the plan sizes the
 // shared memory).  Dry runs do not touch the device: they assume the one CTA per SM that 288 threads at 168 registers allow.
-static int igemm_ctas_per_sm(int bn, bool pair) {
+static int igemm_ctas_per_sm(int bn, bool pair, bool silu) {
     if (g_plan_dry) return 1;
-    IgemmFn fn = pair ? igemm_fn<true>(bn) : igemm_fn<false>(bn);
+    IgemmFn fn = igemm_select(bn, pair, silu);
     int n = 0;
     if (fn && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, IG_THREADS, 0) == cudaSuccess && n > 0) return n;
     cudaGetLastError();
@@ -668,6 +686,10 @@ int igemm_plan(const IgemmDesc& d, IgemmPlan* plan) {
         return -1;
     }
     const bool pair = d.pair != 0;
+    if ((d.epi.flags & IG_SILU) && !igemm_select(BN, pair, true)) {
+        b2_set_error("igemm: no SiLU-epilogue kernel for BN %d%s (16/32/64/128, single CTAs)", BN, pair ? " (CTA pair)" : "");
+        return -1;
+    }
     if (pair && BN % 32 != 0) {
         b2_set_error("igemm(pair): BN %d must be a multiple of 32", BN);
         return -1;
@@ -768,7 +790,7 @@ int igemm_plan(const IgemmDesc& d, IgemmPlan* plan) {
     // The mainloop is TMA-latency bound: throughput per SM = bytes in flight / latency.  When registers admit only one CTA per
     // SM (the case of this kernel: 288 threads at up to 168 registers) the ring takes (nearly) all the shared memory; only
     // when two could be resident AND the launch needs them is the ring halved so that they fit.
-    const int per_sm = igemm_ctas_per_sm(BN, pair);
+    const int per_sm = igemm_ctas_per_sm(BN, pair, (d.epi.flags & IG_SILU) != 0);
     const long resident = (long)per_sm * b2_device_sms();   // CTAs the GPU runs at once
     static const char* pc_env = getenv("B2_PERSIST_CTAS");   // tuning: CTAs of a persistent launch (default: one resident wave)
     const long persist_ctas = pc_env ? atoi(pc_env) : resident;
@@ -833,8 +855,8 @@ int igemm_init() {
     static bool attr_set = false;
     if (!attr_set) {
         for (int bn = 16; bn <= 256; bn += 16) {
-            for (int pair = 0; pair < 2; ++pair) {
-                IgemmFn fn = pair ? igemm_fn<true>(bn) : igemm_fn<false>(bn);
+            for (int pair = 0; pair < 3; ++pair) {   // single CTAs, CTA pairs, single CTAs with the SiLU epilogue
+                IgemmFn fn = igemm_select(bn, pair == 1, pair == 2);
                 if (!fn) continue;
                 cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
                 if (e != cudaSuccess) {
@@ -852,9 +874,10 @@ int igemm_init() {
 int igemm_launch(const IgemmPlan& plan, cudaStream_t stream) {
     if (igemm_init()) return -1;
     const int cz = plan.splits > 1 ? plan.splits : 1;
-    IgemmFn fn = plan.pair ? igemm_fn<true>(plan.p.BN) : igemm_fn<false>(plan.p.BN);
+    IgemmFn fn = igemm_select(plan.p.BN, plan.pair, (plan.p.epi.flags & IG_SILU) != 0);
     if (!fn) {
-        b2_set_error("igemm launch: no kernel for BN %d%s", plan.p.BN, plan.pair ? " (CTA pair)" : "");
+        b2_set_error("igemm launch: no kernel for BN %d%s%s", plan.p.BN, plan.pair ? " (CTA pair)" : "",
+                     (plan.p.epi.flags & IG_SILU) ? " with the SiLU epilogue" : "");
         return -1;
     }
     cudaError_t e = plan.pair ? launch_kc(fn, plan.grid, dim3(IG_THREADS), plan.smem, stream, 2, cz, plan.p)

@@ -26,6 +26,7 @@ enum : int {
     IG_RELU = 1,    // relu after bias/residual
     IG_GEGLU = 2,   // tile columns [0,BN/2) = value, [BN/2,BN) = gate; out = v * gelu_erf(g)
     IG_SPLITK = 4,  // set by the planner: K is split over a thread-block cluster, partial tiles are reduced through DSMEM
+    IG_SILU = 8,    // x * sigmoid(x) after bias/residual (ControlNet conditioning embedding)
 };
 
 struct IgEpilogue {

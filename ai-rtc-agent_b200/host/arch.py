@@ -120,6 +120,65 @@ def unet_param_shapes(a: UNetArch) -> Dict[str, Shape]:
     return out
 
 
+CN_EMBED_CHANNELS = (16, 32, 96, 256)   # ControlNetModel conditioning_embedding_out_channels (diffusers default)
+
+
+def controlnet_param_shapes(a: UNetArch) -> Dict[str, Shape]:
+    """diffusers ControlNetModel with the UNet's architecture fields: the conditioning embedding, a copy of the UNet's conv_in /
+    time_embedding / down blocks / mid block, and one zero conv (1x1) per down residual plus the mid-block one."""
+    ch = a.block_out_channels
+    emb = CN_EMBED_CHANNELS
+    out: Dict[str, Shape] = {}
+    p = "controlnet_cond_embedding"
+    out.update(_conv(f"{p}.conv_in", emb[0], 3, 3))
+    for i in range(len(emb) - 1):
+        out.update(_conv(f"{p}.blocks.{2 * i}", emb[i], emb[i], 3))
+        out.update(_conv(f"{p}.blocks.{2 * i + 1}", emb[i + 1], emb[i], 3))
+    out.update(_conv(f"{p}.conv_out", ch[0], emb[-1], 3))
+    unet = unet_param_shapes(a)
+    out.update({k: v for k, v in unet.items() if k.startswith(("conv_in.", "time_embedding.", "down_blocks.", "mid_block."))})
+    skip = [ch[0]]
+    for i, co in enumerate(ch):
+        skip += [co] * (a.layers_per_block + (1 if i < len(ch) - 1 else 0))
+    for k, c in enumerate(skip):
+        out.update(_conv(f"controlnet_down_blocks.{k}", c, c, 1))
+    out.update(_conv("controlnet_mid_block", ch[-1], ch[-1], 1))
+    return out
+
+
+HED_BLOCKS = ((3, 64, 2), (64, 128, 2), (128, 256, 3), (256, 512, 3), (512, 512, 3))   # (in, out, convs)
+
+
+def hed_param_shapes() -> Dict[str, Shape]:
+    """controlnet_aux ControlNetHED_Apache2 (lllyasviel/Annotators ControlNetHED.pth): the input offset `norm` and five
+    DoubleConvBlocks of 3x3 convs with a 1x1 projection to one channel each."""
+    out: Dict[str, Shape] = {"norm": (1, 3, 1, 1)}
+    for b, (ci, co, n) in enumerate(HED_BLOCKS, start=1):
+        for k in range(n):
+            out.update(_conv(f"block{b}.convs.{k}", co, ci if k == 0 else co, 3))
+        out.update(_conv(f"block{b}.projection", 1, co, 1))
+    return out
+
+
+def synthetic_hed(seed: int = 2468) -> Dict[str, torch.Tensor]:
+    """Seeded fp32 HED weights.  Its input is on the 0..255 scale: He gain on the ReLU convs keeps the activations' second
+    moment (~70^2) through block 5, far inside fp16; the projections are scaled so that the side outputs are O(1) and the
+    sigmoid of their mean gives a graded edge map rather than a saturated one."""
+    g = torch.Generator().manual_seed(seed)
+    sd: Dict[str, torch.Tensor] = {}
+    for name, shape in hed_param_shapes().items():
+        if name == "norm":
+            t = 100.0 + 30.0 * torch.rand(shape, generator=g)
+        elif name.endswith("bias"):
+            t = 0.05 * torch.randn(shape, generator=g)
+        elif ".projection." in name:
+            t = torch.randn(shape, generator=g) * (0.03 / math.sqrt(shape[1]))
+        else:
+            t = torch.randn(shape, generator=g) * math.sqrt(2.0 / math.prod(shape[1:]))
+        sd[name] = t
+    return sd
+
+
 def taesd_param_shapes() -> Dict[str, Shape]:
     """madebyollin/taesd AutoencoderTiny: nn.Sequential indices as diffusers builds them."""
     out: Dict[str, Shape] = {}
@@ -153,7 +212,8 @@ def taesd_param_shapes() -> Dict[str, Shape]:
 
 def synthetic_state_dict(shapes: Dict[str, Shape], seed: int, relu_net: bool = False) -> Dict[str, torch.Tensor]:
     """Seeded fp16 weights with fan-in scaling (activations stay O(1) through the whole network); used by
-    bench.py / smoke when no checkpoint exists.  Not a trained model: outputs are noise-like images."""
+    bench.py / smoke when no checkpoint exists.  Not a trained model: outputs are noise-like images.  A ControlNet's zero
+    convs are drawn like any other layer (non-zero), so that its residuals reach the output."""
     g = torch.Generator().manual_seed(seed)
     sd: Dict[str, torch.Tensor] = {}
     for name, shape in shapes.items():

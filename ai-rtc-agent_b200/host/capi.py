@@ -61,7 +61,7 @@ class EngineConfig(C.Structure):
         ("block_out_channels", C.c_int * 4), ("heads", C.c_int * 4), ("down_attn", C.c_int * 4),
         ("cross_attention_dim", C.c_int), ("layers_per_block", C.c_int), ("norm_groups", C.c_int),
         ("ctx_tokens", C.c_int), ("batch", C.c_int), ("height", C.c_int), ("width", C.c_int),
-        ("do_add_noise", C.c_int), ("use_cuda_graph", C.c_int),
+        ("do_add_noise", C.c_int), ("use_cuda_graph", C.c_int), ("controlnet", C.c_int), ("control_processor", C.c_int),
     ]
 
 
@@ -69,6 +69,9 @@ IN_U8_NHWC, IN_F32_NCHW, IN_F16_NCHW = 0, 1, 2
 OUT_U8_NCHW, OUT_F16_NCHW = 0, 1
 IG_RELU = 1
 IG_GEGLU = 2
+IG_SILU = 8
+SC_IN_U8, SC_IN_TANH3, SC_OUT_RELU, SC_OUT_SILU, SC_IN_OFFSET = 1, 2, 4, 32, 64
+CONTROL_FRAME, CONTROL_HED = 0, 1
 IG_TCONV = 64
 IG_PAIR = 128
 
@@ -101,6 +104,10 @@ def lib() -> C.CDLL:
         _lib.b2sd_op_layernorm.argtypes = [vp, ci, vp, vp, vp, ci, i64, ci, cf, vp]
         _lib.b2sd_op_upsample2x.argtypes = [vp, vp, ci, ci, ci, ci, vp]
         _lib.b2sd_op_smallconv.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ci, ci, vp]
+        _lib.b2sd_op_smallconv_ex.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ci, ci, vp, ci, i64, vp, vp]
+        _lib.b2sd_op_maxpool2x2.argtypes = [vp, vp, ci, ci, ci, ci, vp]
+        _lib.b2sd_op_hed_project.argtypes = [vp, ci, ci, i64, vp, vp, vp, vp]
+        _lib.b2sd_op_hed_fuse.argtypes = [C.POINTER(vp), C.POINTER(ci), C.POINTER(ci), ci, ci, ci, vp, vp, vp]
         _lib.b2sd_op_lcm_step.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, vp]
         _lib.b2sd_op_post_u8.argtypes = [vp, ci, vp, ci, ci, ci, vp]
         _lib.b2sd_op_nv12_to_rgb.argtypes = [vp, ci, vp, ci, vp, ci, ci, ci, vp]
@@ -132,7 +139,7 @@ def lib() -> C.CDLL:
         for name in ("create", "create_lane", "destroy", "load_tensor", "prepare", "export_packed", "import_packed", "set_prompt_embeds", "set_timesteps", "step",
                      "step_ex", "get_tensor", "launches_per_step"):
             getattr(_lib, "b2sd_" + name).restype = C.c_int
-        for name in ("attention", "groupnorm", "layernorm", "upsample2x", "smallconv", "lcm_step", "post_u8", "nv12_to_rgb", "rgb_to_nv12"):
+        for name in ("attention", "groupnorm", "layernorm", "upsample2x", "smallconv", "smallconv_ex", "maxpool2x2", "hed_project", "hed_fuse", "lcm_step", "post_u8", "nv12_to_rgb", "rgb_to_nv12"):
             getattr(_lib, "b2sd_op_" + name).restype = C.c_int
     return _lib
 

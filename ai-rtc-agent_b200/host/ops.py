@@ -30,7 +30,7 @@ def _view(t: torch.Tensor) -> capi.ActView:
 
 def igemm(srcs: Sequence[Tuple[torch.Tensor, int]], w: torch.Tensor, out: torch.Tensor, *,
           stride: int = 1, colbias: Optional[torch.Tensor] = None, res: Optional[torch.Tensor] = None,
-          acc_scale: float = 1.0, res_scale: float = 1.0, relu: bool = False, geglu: bool = False,
+          acc_scale: float = 1.0, res_scale: float = 1.0, relu: bool = False, geglu: bool = False, silu: bool = False,
           bn: int = 0, splits: int = 1, n_valid: Optional[int] = None, timeline: Optional[torch.Tensor] = None, swap: bool = False,
           tconv: bool = False, pair: bool = False,
           rowstat_out: Optional[torch.Tensor] = None, rowstat_in: Optional[torch.Tensor] = None,
@@ -38,7 +38,7 @@ def igemm(srcs: Sequence[Tuple[torch.Tensor, int]], w: torch.Tensor, out: torch.
           out2: Optional[torch.Tensor] = None, col2: int = 0) -> torch.Tensor:
     """srcs: [(NHWC fp16 tensor, ntap)], w: packed fp16 [rows, K]; out: NHWC fp16 [nb,ho,wo,ldc>=n]."""
     d = _igemm_desc(srcs, w, out, stride=stride, colbias=colbias, res=res, acc_scale=acc_scale, res_scale=res_scale, relu=relu,
-                    geglu=geglu, bn=bn, splits=splits, n_valid=n_valid, timeline=timeline, swap=swap, tconv=tconv, pair=pair,
+                    geglu=geglu, silu=silu, bn=bn, splits=splits, n_valid=n_valid, timeline=timeline, swap=swap, tconv=tconv, pair=pair,
                     rowstat_out=rowstat_out, rowstat_in=rowstat_in, colsum=colsum, ln_c=ln_c, ln_eps=ln_eps, out2=out2, col2=col2)
     capi.check(capi.lib().b2sd_op_igemm(C.byref(d), capi.current_stream_ptr()), "b2sd_op_igemm")
     return out
@@ -55,7 +55,7 @@ def igemm_engine_plan(srcs, w, out, *, autotile: int = 1, allow_swap: bool = Tru
 
 
 def _igemm_desc(srcs, w, out, *, stride=1, colbias=None, res=None, acc_scale=1.0, res_scale=1.0, relu=False, geglu=False,
-                bn=0, splits=1, n_valid=None, timeline=None, swap=False, tconv=False, pair=False, rowstat_out=None,
+                silu=False, bn=0, splits=1, n_valid=None, timeline=None, swap=False, tconv=False, pair=False, rowstat_out=None,
                 rowstat_in=None, colsum=None, ln_c=0, ln_eps=1e-5, out2=None, col2=0) -> capi.IgemmDesc:
     d = capi.IgemmDesc()
     d.nseg = len(srcs)
@@ -82,7 +82,8 @@ def _igemm_desc(srcs, w, out, *, stride=1, colbias=None, res=None, acc_scale=1.0
         assert res.dtype == torch.float16
         d.res, d.ldr = res.data_ptr(), res.stride(2)
     d.acc_scale, d.res_scale = acc_scale, res_scale
-    d.flags = (capi.IG_RELU if relu else 0) | (capi.IG_GEGLU if geglu else 0) | (capi.IG_TCONV if tconv else 0) | (capi.IG_PAIR if pair else 0)
+    d.flags = (capi.IG_RELU if relu else 0) | (capi.IG_GEGLU if geglu else 0) | (capi.IG_TCONV if tconv else 0) | (capi.IG_PAIR if pair else 0) \
+        | (capi.IG_SILU if silu else 0)
     if rowstat_out is not None:
         assert rowstat_out.dtype == torch.int64 and rowstat_out.is_contiguous()
         d.rowstat_out = rowstat_out.data_ptr()
@@ -149,6 +150,48 @@ def smallconv(x, w_oihw, bias, y, *, flags=0):
                                             y.data_ptr(), y.stride(2), nb, h, w, cin, cout, in_h, in_w, flags, _sp()),
                "b2sd_op_smallconv")
     return y
+
+
+def smallconv_ex(x, w_oihw, bias, y, *, flags=0, res=None, res_bstride=None, in_off=None):
+    """smallconv with SiLU output (flags & 32), cout a multiple of 16 (y may be wider: its extra columns are not written) and an
+    optional fp16 NHWC residual; res_bstride = elements between its batch items (default: its own; 0 broadcasts item 0)."""
+    nb, in_h, in_w, cin = x.shape
+    _, h, w, _ = y.shape
+    cout = w_oihw.shape[0]
+    rp, ldr, bs = 0, 0, 0
+    if res is not None:
+        assert res.dtype == torch.float16 and res.stride(3) == 1
+        rp, ldr = res.data_ptr(), res.stride(2)
+        bs = res.stride(0) if res_bstride is None else res_bstride
+    capi.check(capi.lib().b2sd_op_smallconv_ex(x.data_ptr(), w_oihw.data_ptr(), bias.data_ptr() if bias is not None else None,
+                                               y.data_ptr(), y.stride(2), nb, h, w, cin, cout, in_h, in_w, flags, rp, ldr, bs,
+                                               in_off.data_ptr() if in_off is not None else None, _sp()), "b2sd_op_smallconv_ex")
+    return y
+
+
+def maxpool2x2(x, y):
+    nb, h, w, c = x.shape
+    capi.check(capi.lib().b2sd_op_maxpool2x2(x.data_ptr(), y.data_ptr(), nb, h, w, c, _sp()), "b2sd_op_maxpool2x2")
+    return y
+
+
+def hed_project(x, w, bias, out):
+    """x NHWC fp16 [1,h,w,c] (pitch x.stride(2)); w fp32 [c], bias fp32 [1]; out fp32 [h*w]."""
+    _, h, ww, c = x.shape
+    capi.check(capi.lib().b2sd_op_hed_project(x.data_ptr(), x.stride(2), c, h * ww, w.data_ptr(), bias.data_ptr(), out.data_ptr(),
+                                              _sp()), "b2sd_op_hed_project")
+    return out
+
+
+def hed_fuse(maps, out_u8, edge_f16=None):
+    """maps: fp32 CUDA tensors [hk, wk]; out_u8: u8 [h, w, 3]."""
+    n = len(maps)
+    ptrs = (C.c_void_p * n)(*[m.data_ptr() for m in maps])
+    hs = (C.c_int * n)(*[m.shape[0] for m in maps])
+    ws = (C.c_int * n)(*[m.shape[1] for m in maps])
+    capi.check(capi.lib().b2sd_op_hed_fuse(ptrs, hs, ws, n, out_u8.shape[0], out_u8.shape[1], out_u8.data_ptr(),
+                                           edge_f16.data_ptr() if edge_f16 is not None else None, _sp()), "b2sd_op_hed_fuse")
+    return out_u8
 
 
 def lcm_step(x, eps, noise, coef, out_latent, do_add_noise=True):

@@ -74,7 +74,14 @@ class StreamDiffusion:
                  torch_dtype: torch.dtype = torch.float16, width: int = 512, height: int = 512,
                  do_add_noise: bool = True, use_denoising_batch: bool = True, frame_buffer_size: int = 1,
                  cfg_type: str = "self", device: str = "cuda", use_cuda_graph: bool = True,
-                 packed_blob: Optional[str] = None, parent: Optional["StreamDiffusion"] = None):
+                 packed_blob: Optional[str] = None, parent: Optional["StreamDiffusion"] = None,
+                 controlnet_sd: Optional[Dict[str, torch.Tensor]] = None,
+                 hed_sd: Optional[Dict[str, torch.Tensor]] = None):
+        """controlnet_sd: a diffusers ControlNetModel state dict (empty when the weights come from packed_blob); every
+        stream-batch slot is then conditioned on the current frame's control image: the frame itself, or with hed_sd (a
+        ControlNetHED.pth state dict, empty with packed_blob) its HED edge map.  Lanes inherit their parent's ControlNet."""
+        if hed_sd is not None and controlnet_sd is None:
+            raise ValueError("the HED processor needs a ControlNet")
         if frame_buffer_size != 1:
             raise NotImplementedError("frame_buffer_size > 1 is not on the reference's path (lib/pipeline.py:28)")
         if not use_denoising_batch:
@@ -120,6 +127,8 @@ class StreamDiffusion:
         cfg.height, cfg.width = height, width
         cfg.do_add_noise = int(do_add_noise)
         cfg.use_cuda_graph = int(use_cuda_graph)
+        cfg.controlnet = int(controlnet_sd is not None)
+        cfg.control_processor = capi.CONTROL_HED if hed_sd is not None else capi.CONTROL_FRAME
         if not torch.cuda.is_available():
             raise capi.B2Error("no CUDA device: the H100 pipeline has no CPU fallback")
         if self.device.index is None:
@@ -141,6 +150,8 @@ class StreamDiffusion:
         else:
             self._load("", unet_sd)
             self._load("vae.", vae_sd)
+            self._load("controlnet.", controlnet_sd or {})
+            self._load("hed.", hed_sd or {})
 
     def set_concurrency(self, frames_in_flight: int) -> None:
         """Tell the engine how many frames will be in flight on this GPU (before prepare()): > 1 selects the throughput

@@ -55,6 +55,75 @@ def load_taesd(repo_dir: str) -> Dict[str, torch.Tensor]:
     raise FileNotFoundError(f"no TAESD safetensors under {repo_dir}")
 
 
+def load_controlnet(repo_dir: str, arch: A.UNetArch) -> Dict[str, torch.Tensor]:
+    """A diffusers ControlNetModel directory (config.json + diffusion_pytorch_model{.fp16,}.safetensors), checked against the
+    UNet architecture it will be attached to."""
+    import json
+    cfg_path = os.path.join(repo_dir, "config.json")
+    if os.path.exists(cfg_path):
+        with open(cfg_path) as f:
+            cfg = json.load(f)
+        want = {"block_out_channels": list(arch.block_out_channels), "cross_attention_dim": arch.cross_attention_dim,
+                "layers_per_block": arch.layers_per_block,
+                "conditioning_embedding_out_channels": list(A.CN_EMBED_CHANNELS)}
+        for key, val in want.items():
+            if key in cfg and cfg[key] != val:
+                raise ValueError(f"ControlNet {repo_dir}: {key} = {cfg[key]}, the {arch.name} UNet needs {val}")
+    for name in ("diffusion_pytorch_model.fp16.safetensors", "diffusion_pytorch_model.safetensors"):
+        p = os.path.join(repo_dir, name)
+        if os.path.exists(p):
+            sd = {k: v.to(torch.float16) for k, v in _load_safetensors(p).items()}
+            A.validate_state_dict(sd, A.controlnet_param_shapes(arch), "ControlNet checkpoint")
+            return sd
+    raise FileNotFoundError(f"no ControlNet safetensors under {repo_dir}")
+
+
+def synthetic_controlnet(arch: A.UNetArch, seed: int = 5678, zero_init: bool = False) -> Dict[str, torch.Tensor]:
+    """Seeded ControlNet weights.  zero_init=True: the zero convs and the conditioning embedding's conv_out are zero, as in a
+    ControlNet freshly initialised from a UNet (its residuals are then exactly zero)."""
+    sd = A.synthetic_state_dict(A.controlnet_param_shapes(arch), seed=seed)
+    if zero_init:
+        for k in sd:
+            if k.startswith(("controlnet_down_blocks.", "controlnet_mid_block.", "controlnet_cond_embedding.conv_out.")):
+                sd[k] = torch.zeros_like(sd[k])
+    return sd
+
+
+def resolve_controlnet(controlnet_id_or_path: str, arch: A.UNetArch, synthetic_ok: bool) -> Dict[str, torch.Tensor]:
+    """A ControlNet on disk (directory or HF-cache id), else seeded synthetic weights when those are allowed, else an error."""
+    repo = find_local_repo(controlnet_id_or_path)
+    if repo is not None:
+        return load_controlnet(repo, arch)
+    if synthetic_ok:
+        logger.warning("no ControlNet %s on disk: using seeded synthetic weights", controlnet_id_or_path)
+        return synthetic_controlnet(arch)
+    raise FileNotFoundError(f"ControlNet '{controlnet_id_or_path}' not found on disk; set {ALLOW_SYNTHETIC_ENV}=1 to run with "
+                            "seeded synthetic weights")
+
+
+ANNOTATORS_ID = "lllyasviel/Annotators"
+
+
+def load_hed(path: str) -> Dict[str, torch.Tensor]:
+    """ControlNetHED.pth (a plain state dict, loaded without unpickling code), checked against the HED inventory."""
+    sd = torch.load(path, map_location="cpu", weights_only=True)
+    sd = {k: v.float() for k, v in sd.items()}
+    A.validate_state_dict(sd, A.hed_param_shapes(), "HED checkpoint")
+    return sd
+
+
+def resolve_hed(synthetic_ok: bool) -> Dict[str, torch.Tensor]:
+    """ControlNetHED.pth from a local lllyasviel/Annotators snapshot, else seeded synthetic weights when allowed, else an error."""
+    repo = find_local_repo(ANNOTATORS_ID)
+    if repo is not None and os.path.exists(os.path.join(repo, "ControlNetHED.pth")):
+        return load_hed(os.path.join(repo, "ControlNetHED.pth"))
+    if synthetic_ok:
+        logger.warning("no %s/ControlNetHED.pth on disk: using seeded synthetic HED weights", ANNOTATORS_ID)
+        return A.synthetic_hed()
+    raise FileNotFoundError(f"{ANNOTATORS_ID}/ControlNetHED.pth not found on disk; set {ALLOW_SYNTHETIC_ENV}=1 to run with seeded "
+                            "synthetic weights")
+
+
 def fuse_lora(unet_sd: Dict[str, torch.Tensor], lora_sd: Dict[str, torch.Tensor], scale: float = 1.0, strict: bool = True) -> int:
     """W += scale * (alpha / rank) * up @ down for every UNet module the LoRA names (diffusers/peft key styles
     `...to_q.lora_A.weight` / `lora.down.weight`, and kohya `lora_unet_*`).  Returns the number of fused layers.
@@ -117,10 +186,12 @@ def layout_variant(batch: int, height: int, width: int) -> str:
 
 
 def packed_blob_path(engine_dir, model_id_or_path: str, arch_name: str, use_lcm_lora: bool, lcm_lora_id: Optional[str],
-                     lora_dict: Optional[Dict[str, float]], vae_id: Optional[str], synthetic: bool, variant: str = "") -> str:
+                     lora_dict: Optional[Dict[str, float]], vae_id: Optional[str], synthetic: bool, variant: str = "",
+                     controlnet: Optional[str] = None, control_processor: Optional[str] = None) -> str:
     """Where the packed-weight blob of this model lives: `<engine_dir>/engines--<model>/b2sd-<arch>-<recipe hash>.b2pack`,
     the directory naming of the reference's TensorRT cache (lib/wrapper.py:593, `engines--` + model id with / -> --).
-    The hash covers everything that changes the weight VALUES (LoRAs and their scales, LCM-LoRA, VAE, synthetic seed), not
+    The hash covers everything that changes the weight VALUES (LoRAs and their scales, LCM-LoRA, VAE, ControlNet, synthetic
+    seed), not
     batch / resolution / prompt (the blob does not depend on them, unlike the reference's static-shape engines)."""
     import hashlib
     import json
@@ -130,6 +201,14 @@ def packed_blob_path(engine_dir, model_id_or_path: str, arch_name: str, use_lcm_
         if os.path.exists(path):   # a replaced LoRA file must not hit the old blob
             st = os.stat(path)
             recipe.setdefault("lora_files", []).append((path, st.st_size, int(st.st_mtime)))
+    if controlnet is not None:
+        recipe["controlnet"] = controlnet
+        recipe["control_processor"] = control_processor
+        repo = find_local_repo(controlnet)
+        for name in sorted(os.listdir(repo)) if repo else ():   # replaced ControlNet weights must not hit the old blob
+            if name.endswith((".safetensors", ".json")):
+                st = os.stat(os.path.join(repo, name))
+                recipe.setdefault("controlnet_files", []).append((name, st.st_size, int(st.st_mtime)))
     digest = hashlib.sha256(json.dumps(recipe, sort_keys=True).encode()).hexdigest()[:16]
     name = "engines--" + model_id_or_path.strip("/").replace("/", "--")
     return os.path.join(str(engine_dir), name, f"b2sd-{arch_name}-{digest}.b2pack")

@@ -3,8 +3,10 @@ constructor keywords and defaults, same validation errors, same methods and exte
 with the TensorRT/diffusers model behind it replaced by the sm_90a engine (host/stream.py).
 
 Not carried over (unreachable from lib/pipeline.py:23-42 and listed out-of-scope in SURVEY.md section 8):
-ControlNet, safety checker, similar-image filter, DataParallel, txt2img sampling, xformers/sfast/TensorRT
-acceleration switches.  Their keywords are accepted; asking for one of those features raises."""
+safety checker, similar-image filter, DataParallel, txt2img sampling, xformers/sfast/TensorRT acceleration switches, and
+ControlNet preprocessors other than HED.  Their keywords are accepted; asking for one of those features raises.  A ControlNet
+runs with controlnet_processor_id="hed" (the default: the frame's HED edge map is the control image) or None (the frame
+itself)."""
 from __future__ import annotations
 
 import logging
@@ -93,8 +95,10 @@ class StreamDiffusionWrapper:
         unsupported = []
         if mode == "txt2img":
             unsupported.append("mode='txt2img'")
-        if controlnet_id_or_path is not None:
-            unsupported.append("controlnet")
+        if controlnet_id_or_path is not None and controlnet_processor_id not in (None, "hed"):
+            # the reference prints "ControlNet conditioning not supported." for an unknown id and runs unconditioned; a caller
+            # who asked for a preprocessor should not silently get the raw frame instead
+            unsupported.append(f"controlnet_processor_id={controlnet_processor_id!r} (only 'hed', or None: the frame itself)")
         if use_safety_checker:
             unsupported.append("safety checker")
         if enable_similar_image_filter:
@@ -128,11 +132,12 @@ class StreamDiffusionWrapper:
 
         self.stream: StreamDiffusion = self._load_model(
             model_id_or_path=model_id_or_path, lora_dict=lora_dict, lcm_lora_id=lcm_lora_id, vae_id=vae_id,
-            t_index_list=t_index_list, do_add_noise=do_add_noise, use_lcm_lora=use_lcm_lora, cfg_type=cfg_type)
+            t_index_list=t_index_list, do_add_noise=do_add_noise, use_lcm_lora=use_lcm_lora, cfg_type=cfg_type,
+            controlnet_id_or_path=controlnet_id_or_path, controlnet_processor_id=controlnet_processor_id)
 
     # -- model loading: replaces _load_trt_model/_load_model (lib/wrapper.py:409-944) --------------------
     def _load_model(self, model_id_or_path, lora_dict, lcm_lora_id, vae_id, t_index_list, do_add_noise,
-                    use_lcm_lora, cfg_type) -> StreamDiffusion:
+                    use_lcm_lora, cfg_type, controlnet_id_or_path=None, controlnet_processor_id=None) -> StreamDiffusion:
         """Like the reference (lib/wrapper.py:583-615): first try the cached artefact under `engine_dir` -- there TensorRT engine
         files, here the packed-weight blob -- and on any failure fall through to the full path (load weights, fuse LoRAs),
         after which the blob is written for the next start (lib/wrapper.py:889-910 moves the engines into the cache)."""
@@ -146,6 +151,8 @@ class StreamDiffusionWrapper:
         kw = dict(torch_dtype=self.dtype, width=self.width, height=self.height, do_add_noise=do_add_noise,
                   use_denoising_batch=self.use_denoising_batch, frame_buffer_size=self.frame_buffer_size, cfg_type=cfg_type,
                   device=self.device)
+        cn = controlnet_id_or_path is not None
+        hed = cn and controlnet_processor_id == "hed"
         blob = None
         # blobs are kept for real checkpoints; seeded synthetic weights (benchmarks, tests) only with B200SD_PACK_CACHE=synthetic
         mode = os.getenv("B200SD_PACK_CACHE", "1")
@@ -154,11 +161,13 @@ class StreamDiffusionWrapper:
         if use_cache:
             blob = W.packed_blob_path(self.engine_dir, model_id_or_path, arch.name, use_lcm_lora and not self.sd_turbo, lcm_lora_id,
                                       lora_dict, vae_id, synthetic=not have_ckpt,
-                                      variant=W.layout_variant(self.batch_size, self.height, self.width))
+                                      variant=W.layout_variant(self.batch_size, self.height, self.width),
+                                      controlnet=controlnet_id_or_path, control_processor=controlnet_processor_id)
         encoder = make_prompt_encoder(repo if have_ckpt else None, arch.cross_attention_dim, self.device, allow_synthetic=synthetic_ok)
         if blob is not None and os.path.exists(blob) and (have_ckpt or synthetic_ok):
             try:
-                sd = StreamDiffusion(arch, {}, {}, t_index_list, encoder, packed_blob=blob, **kw)
+                sd = StreamDiffusion(arch, {}, {}, t_index_list, encoder, packed_blob=blob,
+                                     controlnet_sd={} if cn else None, hed_sd={} if hed else None, **kw)
                 logger.info("loaded packed weights from %s", blob)
                 self.packed_blob = blob
                 return sd
@@ -166,8 +175,10 @@ class StreamDiffusionWrapper:
                 logger.warning("packed-weight blob %s unusable (%s); rebuilding from the checkpoint", blob, exc)
         arch, unet_sd, vae_sd, repo = resolve_weights(model_id_or_path, vae_id, lcm_lora_id, use_lcm_lora, lora_dict,
                                                       self.sd_turbo)
+        cn_sd = W.resolve_controlnet(controlnet_id_or_path, arch, synthetic_ok) if cn else None
+        hed_sd = W.resolve_hed(synthetic_ok) if hed else None
         self._blob_to_write = blob
-        return StreamDiffusion(arch, unet_sd, vae_sd, t_index_list, encoder, **kw)
+        return StreamDiffusion(arch, unet_sd, vae_sd, t_index_list, encoder, controlnet_sd=cn_sd, hed_sd=hed_sd, **kw)
 
     def _on_stream(self):
         return torch.cuda.stream(self._ext_stream) if self._ext_stream is not None else _NullCtx()

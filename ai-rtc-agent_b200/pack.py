@@ -31,19 +31,26 @@ def parse_lora(specs):
     return out
 
 
-def main(argv=None) -> int:
+def build_parser() -> argparse.ArgumentParser:
     ap = argparse.ArgumentParser(prog="python -m ai_rtc_agent_b200.pack", description=__doc__.split("\n\n")[0])
     ap.add_argument("--model-id", default="lykon/dreamshaper-8", help="HF id (looked up under $HF_HUB_CACHE) or a local directory (agent.py:443)")
     ap.add_argument("--lora", action="append", metavar="PATH[:SCALE]", help="LoRA safetensors to fuse (repeatable; build.py:23-25)")
     ap.add_argument("--lcm-lora-id", default=None)
     ap.add_argument("--no-lcm-lora", action="store_true")
     ap.add_argument("--vae-id", default=None)
+    ap.add_argument("--controlnet-id", default=None, help="diffusers ControlNetModel (HF id or local directory) packed with the UNet")
+    ap.add_argument("--controlnet-processor-id", default="hed", type=lambda v: None if v.lower() == "none" else v,
+                    help="control-image preprocessor: hed (default, the reference's) or none (the frame itself)")
     ap.add_argument("--engine-dir", default=os.getenv("TRT_ENGINES_CACHE", "./models/engines"), help="cache root (lib/pipeline.py:35)")
     ap.add_argument("--width", type=int, default=512)
     ap.add_argument("--height", type=int, default=512)
     ap.add_argument("--t-index-list", type=int, nargs="+", default=None)
     ap.add_argument("--force", action="store_true", help="rebuild even if the blob exists")
-    args = ap.parse_args(argv)
+    return ap
+
+
+def main(argv=None) -> int:
+    args = build_parser().parse_args(argv)
     logging.basicConfig(level=logging.INFO, format="%(message)s")
 
     from .host import arch as A
@@ -56,7 +63,8 @@ def main(argv=None) -> int:
     have_ckpt = repo is not None and os.path.isdir(os.path.join(repo, "unet"))
     blob = W.packed_blob_path(args.engine_dir, args.model_id, A.arch_for(args.model_id).name, not args.no_lcm_lora and not turbo,
                               args.lcm_lora_id, loras, args.vae_id, synthetic=not have_ckpt,
-                              variant=W.layout_variant(len(t_index_list), args.height, args.width))
+                              variant=W.layout_variant(len(t_index_list), args.height, args.width), controlnet=args.controlnet_id,
+                              control_processor=args.controlnet_processor_id)
     if not have_ckpt:
         if not (os.getenv(W.ALLOW_SYNTHETIC_ENV) or args.model_id.startswith(("tiny", "synthetic"))):
             raise SystemExit(f"pack: no checkpoint for '{args.model_id}' on disk (set {W.ALLOW_SYNTHETIC_ENV}=1 to pack seeded synthetic weights)")
@@ -66,6 +74,7 @@ def main(argv=None) -> int:
     t0 = time.time()
     w = StreamDiffusionWrapper(model_id_or_path=args.model_id, t_index_list=t_index_list, lora_dict=loras or None,
                                lcm_lora_id=args.lcm_lora_id, vae_id=args.vae_id, use_lcm_lora=not args.no_lcm_lora,
+                               controlnet_id_or_path=args.controlnet_id, controlnet_processor_id=args.controlnet_processor_id,
                                width=args.width, height=args.height, output_type="pt", mode="img2img", engine_dir=args.engine_dir)
     reused = w.packed_blob is not None
     w.prepare(prompt="", num_inference_steps=50, guidance_scale=0.0)

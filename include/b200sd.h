@@ -40,6 +40,8 @@ typedef struct {
 enum {
     B2SD_IG_RELU = 1,
     B2SD_IG_GEGLU = 2,
+    B2SD_IG_SILU = 8,        /* x * sigmoid(x) after bias / residual (ControlNet conditioning embedding); single CTAs with
+                                bn 16 / 32 / 64 / 128 only, not with B2SD_IG_TCONV or B2SD_IG_PAIR */
     B2SD_IG_TCONV = 64,      /* run the persistent halo-tile kernel (stride-1 3x3, 64 -> 64 channels: the TAESD body) */
     B2SD_IG_PAIR = 128       /* CTA pairs: tcgen05.mma.cta_group::2 (M = 256 per MMA), each CTA stages half of the weight tile;
                                 normal orientation, bn % 32 == 0, splits <= 4 */
@@ -47,7 +49,7 @@ enum {
 
 /* conv3x3 / conv1x1 / Linear as one implicit GEMM:
  *   out[row][j] = acc_scale * (sum_seg sum_tap sum_c src[seg](row, tap, c) * w[j][k] + colbias[b][j])
- *                 + res_scale * res[row][j]        (then ReLU / GEGLU per flags)
+ *                 + res_scale * res[row][j]        (then ReLU / SiLU / GEGLU per flags)
  * K order of the packed weight rows = segments in sequence, each [tap][c]. */
 typedef struct {
     b2sd_act_view src[3];
@@ -136,6 +138,20 @@ int b2sd_op_upsample2x(const void* x, void* y, int nb, int h, int w, int c, void
  * 2 = tanh(x/3)*3 on the input (DecoderTiny), 4 = ReLU on the output */
 int b2sd_op_smallconv(const void* x, const void* w_oihw, const float* bias, void* y, int ldy, int nb, int h,
                       int w, int cin, int cout, int in_h, int in_w, int flags, void* stream);
+/* Same, plus flag 32 = SiLU on the output, flag 64 = input on the 0..255 scale minus in_off[c] (device fp32 [3]; HED's first
+ * conv, zero padding in the shifted domain), cout a multiple of 16 (columns cout..ldy-1 of y are not written), and an optional
+ * fp16 NHWC residual added after the bias: item n at res + n * res_bstride (0 = one residual for every item), pitch ldr
+ * (res 4-byte aligned, ldr and res_bstride even).  b2sd_op_smallconv is this with res = in_off = NULL. */
+int b2sd_op_smallconv_ex(const void* x, const void* w_oihw, const float* bias, void* y, int ldy, int nb, int h, int w,
+                         int cin, int cout, int in_h, int in_w, int flags, const void* res, int ldr, int64_t res_bstride,
+                         const float* in_off, void* stream);
+/* HED edge detector pieces: 2x2/2 max-pool (NHWC fp16, even h / w / c); per-pixel projection C -> 1 (fp32 weights [c],
+ * bias [1], fp32 out [npix]); fusion of `levels` fp32 side outputs (maps[k] of hs[k] x ws[k]) into the u8 edge image
+ * [h][w][3] (bilinear half-pixel upsampling, mean, sigmoid, * 255, truncation); edge_f16 (optional) gets the value as fp16. */
+int b2sd_op_maxpool2x2(const void* x, void* y, int nb, int h, int w, int c, void* stream);
+int b2sd_op_hed_project(const void* x, int ldx, int c, int64_t npix, const float* w, const float* bias, float* out, void* stream);
+int b2sd_op_hed_fuse(const float* const* maps, const int* hs, const int* ws, int levels, int h, int w, void* out_u8,
+                     void* edge_f16, void* stream);
 /* StreamDiffusion scheduler_step_batch + stream-batch buffer update (see elementwise.cuh) */
 int b2sd_op_lcm_step(void* x, const void* eps, const void* noise, const float* coef, void* out_latent, int T,
                      int hw, int do_add_noise, void* stream);
@@ -170,7 +186,16 @@ typedef struct {
     int height, width;           /* image size, multiples of 64 */
     int do_add_noise;            /* lib/wrapper.py:53 */
     int use_cuda_graph;          /* replay the frame program as one CUDA graph */
+    int controlnet;              /* 1: a ControlNet (weights under "controlnet." + diffusers ControlNetModel keys) conditions
+                                    every stream-batch slot on the current frame (control image = frame / 255 at the engine's
+                                    size); its 12 + 1 residuals are added to the UNet's skips and mid-block output.  0: none.
+                                    A lane inherits its parent's value. */
+    int control_processor;       /* with controlnet = 1: B2SD_CONTROL_FRAME (0) or B2SD_CONTROL_HED (1): the control image is the
+                                    HED edge map of the frame (controlnet_aux HEDdetector at the engine's size; weights under
+                                    "hed." + ControlNetHED.pth keys, e.g. "hed.block1.convs.0.weight", "hed.norm").  Inherited
+                                    by lanes. */
 } b2sd_config;
+enum { B2SD_CONTROL_FRAME = 0, B2SD_CONTROL_HED = 1 };
 
 int b2sd_create(const b2sd_config* cfg, b2sd_handle* out);
 int b2sd_destroy(b2sd_handle h);
@@ -184,7 +209,8 @@ int b2sd_destroy(b2sd_handle h);
 int b2sd_create_lane(b2sd_handle parent, const b2sd_config* cfg, b2sd_handle* out);
 
 /* Weights under diffusers state-dict names: UNet keys as-is ("down_blocks.0.resnets.0.conv1.weight"),
- * TAESD keys prefixed "vae." ("vae.encoder.layers.0.weight").  ptr may be host or device memory.
+ * TAESD keys prefixed "vae." ("vae.encoder.layers.0.weight"), ControlNet keys prefixed "controlnet."
+ * ("controlnet.controlnet_cond_embedding.conv_in.weight").  ptr may be host or device memory.
  * dtype: 0 = fp16, 1 = fp32.  Replaces the ONNX export + TensorRT build of lib/wrapper.py:785-910.
  * After the first b2sd_prepare the raw copies of parameters that only feed the packing kernels are released (set
  * B2_KEEP_RAW=1 to keep them); loading further tensors into such an engine is an error. */
@@ -228,7 +254,10 @@ int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int
                  int out_kind, void* stream);
 
 /* Parity/debug taps: copies a named intermediate of the last step to host memory as fp16 NHWC.
- * Names: "x_t", "unet_in", "eps", "x0", "image", "conv_in", "down.I.J", "mid", "up.I.J".
+ * Names: "x_t", "unet_in", "eps", "x0", "image", "conv_in", "down.I.J", "mid", "up.I.J"; with a ControlNet also "cn_cond"
+ * (conditioning embedding, batch 1), "cn.conv_in" (its conv_in(x) + cn_cond), "cn.res.K" (UNet skip K, in push order 0..11,
+ * plus ControlNet residual K: what the up path reads) and "cn.mid" ("mid" plus the mid-block residual); with HED also
+ * "control" (the u8 edge value as fp16, [1][h][w][1]).
  * Returns the element count via *count (pass dst = NULL to query).  Synchronises `stream`. */
 int b2sd_get_tensor(b2sd_handle h, const char* name, void* dst, int64_t capacity, int64_t* count, int* dims4,
                     void* stream);

@@ -669,7 +669,10 @@ __global__ void __launch_bounds__(128) smallconv_kernel(SmallConvArgs a, int G) 
     for (int i = threadIdx.x; i < G; i += blockDim.x) bs[i] = a.bias ? a.bias[cg * G + i] : 0.f;
     __syncthreads();
     const int npix = a.nb * a.h * a.w_;           // < 2^31 (checked by the launcher)
-    const bool same_size = a.in_h == a.h && a.in_w == a.w_;   // no resize: skip the per-tap integer divisions
+    const bool same_size = a.in_h == a.h && a.in_w == a.w_;   // no resize: skip the per-tap index arithmetic
+    // torch's nearest rule (F.interpolate, mode "nearest", size given): src = min(floor(dst * (in / out)), in - 1) with
+    // the scale rounded to fp32 first. It differs from the exact floor(dst * in / out) wherever out has an odd factor.
+    const float scale_y = (float)a.in_h / (float)a.h, scale_x = (float)a.in_w / (float)a.w_;
     for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += gridDim.x * blockDim.x) {
         const int xw = p % a.w_;
         const int yh = (p / a.w_) % a.h;
@@ -679,11 +682,14 @@ __global__ void __launch_bounds__(128) smallconv_kernel(SmallConvArgs a, int G) 
         for (int tap = 0; tap < 9; ++tap) {
             const int yy = yh + tap / 3 - 1, xx = xw + tap % 3 - 1;
             const bool in = (yy >= 0) && (yy < a.h) && (xx >= 0) && (xx < a.w_);
-            // nearest resize (VaeImageProcessor.resize -> F.interpolate default mode): src = floor(dst*in/out)
+            // nearest resize (VaeImageProcessor.resize -> F.interpolate default mode)
             int sy = 0, sx = 0;
             if (in) {
                 if (same_size) { sy = yy; sx = xx; }
-                else { sy = (int)(((long)yy * a.in_h) / a.h); sx = (int)(((long)xx * a.in_w) / a.w_); }
+                else {
+                    sy = min((int)floorf((float)yy * scale_y), a.in_h - 1);
+                    sx = min((int)floorf((float)xx * scale_x), a.in_w - 1);
+                }
             }
             const long base = (((long)n * a.in_h + sy) * a.in_w + sx) * CIN;
 #pragma unroll

@@ -21,12 +21,13 @@ from . import unet as ounet
 
 def build(cfg: ounet.UNetConfig, unet_sd16: Dict[str, torch.Tensor], vae_sd16: Dict[str, torch.Tensor],
           t_index_list: List[int], hw: int, prompt_embeds: torch.Tensor, init_noise: Optional[torch.Tensor],
-          dtype: torch.dtype = torch.float32, device: str = "cuda") -> ostream.StreamOracle:
-    """StreamOracle on `device` in `dtype`, prepared like the engine (guidance 0.0, the engine's fp16-rounded noise)."""
+          dtype: torch.dtype = torch.float32, device: str = "cuda", width: Optional[int] = None) -> ostream.StreamOracle:
+    """StreamOracle on `device` in `dtype`, prepared like the engine (guidance 0.0, the engine's fp16-rounded noise).
+    The frame is hw x hw, or hw high and `width` wide."""
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False
     orc = ostream.StreamOracle({k: v.float() for k, v in unet_sd16.items()}, cfg, {k: v.float() for k, v in vae_sd16.items()},
-                               t_index_list, hw, hw)
+                               t_index_list, hw if width is None else width, hw)
     orc.prepare(prompt_embeds.float(), guidance_scale=0.0, init_noise=None if init_noise is None else init_noise.float())
     if init_noise is None:
         orc.init_noise = orc.init_noise.half().float()

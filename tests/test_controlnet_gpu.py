@@ -218,6 +218,8 @@ def _hed16():
 
 
 def _engine(turbo, t_index_list, hw, cn16, full=False, graph=True, blob=None, concurrency=1, hed=None):
+    """hw: the engine size, an int for a square engine or (height, width)"""
+    height, width = (hw, hw) if isinstance(hw, int) else hw
     from ai_rtc_agent_b200.host import arch as A
     from ai_rtc_agent_b200.host.stream import StreamDiffusion
     from oracle import unet as ounet
@@ -229,11 +231,11 @@ def _engine(turbo, t_index_list, hw, cn16, full=False, graph=True, blob=None, co
     usd, vsd = ow.make_unet_weights(cfg), ow.make_taesd_weights()
     emb = ow.make_prompt_embeds(cfg.cross_attention_dim)
     if blob is not None:
-        sd = StreamDiffusion(arch, {}, {}, t_index_list, lambda p: emb, width=hw, height=hw, use_cuda_graph=graph,
+        sd = StreamDiffusion(arch, {}, {}, t_index_list, lambda p: emb, width=width, height=height, use_cuda_graph=graph,
                              packed_blob=blob, controlnet_sd={} if cn16 is not None else None,
                              hed_sd={} if hed is not None else None)
     else:
-        sd = StreamDiffusion(arch, usd, vsd, t_index_list, lambda p: emb, width=hw, height=hw, use_cuda_graph=graph,
+        sd = StreamDiffusion(arch, usd, vsd, t_index_list, lambda p: emb, width=width, height=height, use_cuda_graph=graph,
                              controlnet_sd=cn16, hed_sd=hed)
     if concurrency > 1:
         sd.set_concurrency(concurrency)
@@ -244,18 +246,24 @@ def _engine(turbo, t_index_list, hw, cn16, full=False, graph=True, blob=None, co
 def _oracle(cfg, usd, vsd, cn16, emb, t_index_list, hw, init_noise, hed=None):
     from oracle import controlnet as ocn
     from oracle import weights as ow
-    orc = ocn.ControlNetStreamOracle(ow.to_float(usd), cfg, ow.to_float(vsd), ow.to_float(cn16), t_index_list, hw, hw,
+    height, width = (hw, hw) if isinstance(hw, int) else hw
+    orc = ocn.ControlNetStreamOracle(ow.to_float(usd), cfg, ow.to_float(vsd), ow.to_float(cn16), t_index_list, width, height,
                                      hed_sd=hed)
     orc.prepare(emb.float(), guidance_scale=0.0, init_noise=init_noise.float())
     return orc
 
 
 @pytest.mark.parametrize("processor", [None, "hed"])
-@pytest.mark.parametrize("turbo,t_index_list", [(True, [32]), (False, [32]), (True, [18, 26, 35, 45]),
-                                                (False, [18, 26, 35, 45])])
-def test_tiny_controlnet_engine_matches_oracle(cuda, turbo, t_index_list, processor):
+@pytest.mark.parametrize("turbo,t_index_list,hw", [
+    pytest.param(True, [32], 128, id="True-t_index_list0"), pytest.param(False, [32], 128, id="False-t_index_list1"),
+    pytest.param(True, [18, 26, 35, 45], 128, id="True-t_index_list2"),
+    pytest.param(False, [18, 26, 35, 45], 128, id="False-t_index_list3"),
+    pytest.param(True, [32], (192, 128), id="True-T1-192x128"),              # height x width: HED levels 192x128 ... 12x8
+    pytest.param(False, [18, 26, 35, 45], (192, 128), id="False-T4-192x128"),
+])
+def test_tiny_controlnet_engine_matches_oracle(cuda, turbo, t_index_list, hw, processor):
     """Both architectures, T = 1 and 4, 8 frames: every ControlNet tap and every UNet tap on the first and last frame, the u8
-    frames and the x_t_latent_buffer state on every frame."""
+    frames and the x_t_latent_buffer state on every frame; square and non-square engines."""
     from oracle import controlnet as ocn
     from oracle import pipeline as opipe
     from oracle import unet as ounet
@@ -263,11 +271,11 @@ def test_tiny_controlnet_engine_matches_oracle(cuda, turbo, t_index_list, proces
     cfg = ounet.tiny_config(turbo)
     cn16 = ocn.make_weights(cfg)
     hed = _hed16() if processor == "hed" else None
-    sd, cfg, usd, vsd, emb = _engine(turbo, t_index_list, 128, cn16, hed=hed)
-    orc = _oracle(cfg, usd, vsd, cn16, emb, t_index_list, 128, sd.init_noise, hed=hed)
+    sd, cfg, usd, vsd, emb = _engine(turbo, t_index_list, hw, cn16, hed=hed)
+    orc = _oracle(cfg, usd, vsd, cn16, emb, t_index_list, hw, sd.init_noise, hed=hed)
     T = len(t_index_list)
     for i in range(8):
-        frame = ow.make_frame(128, 128, seed=20 + i)
+        frame = ow.make_frame(orc.height, orc.width, seed=20 + i)
         out = sd.step_u8(frame.to(cuda))
         ref = opipe.frame_to_u8(orc, frame)
         _u8_check(out, ref, f"frame {i}")

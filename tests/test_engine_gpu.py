@@ -24,6 +24,8 @@ def _cmp(name, got_nhwc, ref_nchw, rows):
 
 
 def _build(arch_name, turbo, t_index_list, hw, cuda, seed=0):
+    """hw: the engine size, an int for a square engine or (height, width)"""
+    height, width = (hw, hw) if isinstance(hw, int) else hw
     from ai_rtc_agent_b200.host import arch as A
     from ai_rtc_agent_b200.host.stream import StreamDiffusion
     from oracle import stream as ostream
@@ -36,10 +38,10 @@ def _build(arch_name, turbo, t_index_list, hw, cuda, seed=0):
     usd16 = ow.make_unet_weights(cfg)
     vsd16 = ow.make_taesd_weights()
     emb = ow.make_prompt_embeds(cfg.cross_attention_dim)
-    sd = StreamDiffusion(arch, usd16, vsd16, t_index_list, lambda p: emb, width=hw, height=hw, device="cuda",
+    sd = StreamDiffusion(arch, usd16, vsd16, t_index_list, lambda p: emb, width=width, height=height, device="cuda",
                          use_cuda_graph=bool(int(os.getenv("B200SD_TEST_GRAPH", "1"))))
     sd.prepare("p", guidance_scale=0.0)
-    orc = ostream.StreamOracle(ow.to_float(usd16), cfg, ow.to_float(vsd16), t_index_list, hw, hw)
+    orc = ostream.StreamOracle(ow.to_float(usd16), cfg, ow.to_float(vsd16), t_index_list, width, height)
     orc.prepare(emb.float(), guidance_scale=0.0, init_noise=sd.init_noise.float())
     return sd, orc
 
@@ -51,14 +53,23 @@ def _u8_check(got, ref, what):
     return frac, d.max().item()
 
 
-@pytest.mark.parametrize("turbo", [True, False])
-def test_tiny_unet_taps_single_step(cuda, turbo):
+def _hw_id(hw):
+    return "" if hw == 128 else f"-{hw[0]}x{hw[1]}"
+
+
+# non-square tiny engines (height, width): latent levels 16x24 ... 2x3 and 24x16 ... 3x2
+_TINY_NONSQUARE = [(128, 192), (192, 128)]
+
+
+@pytest.mark.parametrize("turbo,hw", [pytest.param(t, hw, id=f"{t}{_hw_id(hw)}")
+                                      for hw in [128] + _TINY_NONSQUARE for t in (True, False)])
+def test_tiny_unet_taps_single_step(cuda, turbo, hw):
     """Layer-by-layer: every UNet block output, eps, x0, decoded image of one frame (T=1)."""
     from oracle import pipeline as opipe
     from oracle import unet as ounet
     from oracle import weights as ow
-    sd, orc = _build("tiny", turbo, [32], 128, cuda)
-    frame = ow.make_frame(128, 128, seed=0)
+    sd, orc = _build("tiny", turbo, [32], hw, cuda)
+    frame = ow.make_frame(orc.height, orc.width, seed=0)
     out = sd.step_u8(frame.to(cuda))
     ref_u8 = opipe.frame_to_u8(orc, frame)
     taps = {}
@@ -80,16 +91,19 @@ def test_tiny_unet_taps_single_step(cuda, turbo):
     _u8_check(out, ref_u8, "tiny u8 frame")
 
 
-@pytest.mark.parametrize("turbo,t_index_list", [(True, [32]), (False, [18, 26, 35, 45])])
-def test_tiny_stream_loop(cuda, turbo, t_index_list):
+@pytest.mark.parametrize("turbo,t_index_list,hw", [
+    pytest.param(True, [32], 128, id="True-t_index_list0"),
+    pytest.param(False, [18, 26, 35, 45], 128, id="False-t_index_list1"),
+] + [pytest.param(False, [18, 26, 35, 45], hw, id=f"False-T4{_hw_id(hw)}") for hw in _TINY_NONSQUARE])
+def test_tiny_stream_loop(cuda, turbo, t_index_list, hw):
     """8 consecutive frames through the stream-batch loop: u8 outputs (incl. the T-1 frame output lag) and the
     x_t_latent_buffer state must track the oracle frame by frame."""
     from oracle import pipeline as opipe
     from oracle import weights as ow
-    sd, orc = _build("tiny", turbo, t_index_list, 128, cuda)
+    sd, orc = _build("tiny", turbo, t_index_list, hw, cuda)
     T = len(t_index_list)
     for i in range(8):
-        frame = ow.make_frame(128, 128, seed=i)
+        frame = ow.make_frame(orc.height, orc.width, seed=i)
         out = sd.step_u8(frame.to(cuda))
         ref = opipe.frame_to_u8(orc, frame)
         _u8_check(out, ref, f"frame {i}")
@@ -155,18 +169,23 @@ def test_tiny_update_prompt_and_t_index(cuda):
 
 
 def test_resize_and_float_entry(cuda):
-    """Non-native frame size -> nearest resize (VaeImageProcessor); float (3,H,W) entry == u8 entry."""
+    """Non-native frame size -> nearest resize (VaeImageProcessor); float (3,H,W) entries (f32 and f16) == u8 entry.  Also a
+    400x300 camera-sized noise frame through a non-square 192x128 (W x H) engine, end to end against the oracle.  (The exact
+    resize index rule is pinned by test_ops_gpu.py's test_smallconv_resize_index_map; this case does not tell the rules apart.)"""
     from oracle import pipeline as opipe
     from oracle import weights as ow
-    sd, orc = _build("tiny", True, [32], 128, cuda)
-    frame = ow.make_frame(96, 160, seed=3)
-    out = sd.step_u8(frame.to(cuda))
-    ref = opipe.frame_to_u8(orc, frame)
-    _u8_check(out, ref, "resized frame")
-    x = (frame.to(cuda).float() / 255.0).permute(0, 3, 1, 2).squeeze(0)
-    img = sd(x)  # (1,3,H,W) fp16 in [-1,1]
-    u8 = ((img / 2 + 0.5).clamp(0, 1)[0] * 255.0).clamp(0, 255).to(torch.uint8)[None]
-    assert torch.equal(u8, out)
+    for hw, (fh, fw), smooth in [(128, (96, 160), True), ((128, 192), (300, 400), False)]:
+        sd, orc = _build("tiny", True, [32], hw, cuda)
+        frame = ow.make_frame(fh, fw, seed=3, smooth=smooth)
+        what = f"{fw}x{fh} frame into a {orc.width}x{orc.height} engine"
+        out = sd.step_u8(frame.to(cuda))
+        ref = opipe.frame_to_u8(orc, frame)
+        _u8_check(out, ref, what)
+        x = (frame.to(cuda).float() / 255.0).permute(0, 3, 1, 2).squeeze(0)
+        for entry in (x, x.half()):
+            img = sd(entry)  # (1,3,H,W) fp16 in [-1,1]
+            u8 = ((img / 2 + 0.5).clamp(0, 1)[0] * 255.0).clamp(0, 255).to(torch.uint8)[None]
+            assert torch.equal(u8, out), f"{what}: {entry.dtype} entry"
 
 
 @pytest.mark.parametrize("turbo,t_index_list,hw,nframes", [

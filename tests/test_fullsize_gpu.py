@@ -25,9 +25,15 @@ def _weights(turbo, full=True):
     return cfg, arch, ow.make_unet_weights(cfg), ow.make_taesd_weights(), ow.make_prompt_embeds(cfg.cross_attention_dim)
 
 
+def _hw(hw):
+    """(height, width) of an engine size given as an int (square) or (height, width)"""
+    return (hw, hw) if isinstance(hw, int) else hw
+
+
 def _engine(arch, usd, vsd, emb, tl, hw, frames_in_flight=1):
     from ai_rtc_agent_b200.host.stream import StreamDiffusion
-    sd = StreamDiffusion(arch, usd, vsd, tl, lambda p: emb, width=hw, height=hw, device="cuda")
+    height, width = _hw(hw)
+    sd = StreamDiffusion(arch, usd, vsd, tl, lambda p: emb, width=width, height=height, device="cuda")
     if frames_in_flight > 1:   # throughput launch policy: 100 KB operand rings, CTA pairs without split-K
         sd.set_concurrency(frames_in_flight)
     sd.prepare("p", guidance_scale=0.0)
@@ -76,17 +82,25 @@ def test_gpu_oracle_equals_cpu_oracle(cuda):
     (False, [18, 26, 35, 45], 512, 5, 2),    # config 3 under the policy of its two stage-pipelined lanes (100 KB rings, split-K <= 4)
     (False, [18, 26, 35, 45], 512, 2, 4),    # ... and with CTA pairs on the SD-1.5 shapes (conv projections, head dims 40/80/160)
     (False, [18, 26, 35, 45], 768, 2, 4),    # odd tile extents (odd M-tile counts: masked second tile of the last pair)
+    # non-square engines (height, width): the 6x8 level of 384x512 runs swapped; 768x448 has a 12x7 level (Wo = 7)
+    pytest.param(True, [32], (384, 512), 2, 1, id="turbo-T1-384x512-1"),
+    pytest.param(True, [32], (384, 512), 2, 8, id="turbo-T1-384x512-8"),
+    pytest.param(True, [32], (448, 768), 2, 1, id="turbo-T1-448x768-1"),
+    pytest.param(True, [32], (448, 768), 2, 8, id="turbo-T1-448x768-8"),
+    pytest.param(False, [18, 26, 35, 45], (768, 448), 4, 1, id="sd15-T4-768x448-1"),
+    pytest.param(False, [18, 26, 35, 45], (768, 448), 2, 4, id="sd15-T4-768x448-4"),
 ])
 def test_three_implementations_full_size(cuda, turbo, tl, hw, nframes, in_flight):
     from oracle import pipeline as opipe
     from oracle import torch_gpu as tg
     from oracle import weights as ow
+    height, width = _hw(hw)
     cfg, arch, usd, vsd, emb = _weights(turbo)
     sd = _engine(arch, usd, vsd, emb, tl, hw, in_flight)
-    ref32 = tg.build(cfg, usd, vsd, tl, hw, emb, sd.init_noise, torch.float32)
-    ref16 = tg.build(cfg, usd, vsd, tl, hw, emb, sd.init_noise, torch.float16)
+    ref32 = tg.build(cfg, usd, vsd, tl, height, emb, sd.init_noise, torch.float32, width=width)
+    ref16 = tg.build(cfg, usd, vsd, tl, height, emb, sd.init_noise, torch.float16, width=width)
     for i in range(nframes):
-        f = ow.make_frame(hw, hw, seed=i).cuda()
+        f = ow.make_frame(height, width, seed=i).cuda()
         out = sd.step_u8(f)
         u32 = opipe.frame_to_u8(ref32, f)
         with tg.fused_attention():
@@ -96,7 +110,7 @@ def test_three_implementations_full_size(cuda, turbo, tl, hw, nframes, in_flight
         f32, m32 = _u8(out, u32)
         f16, m16 = _u8(out, u16)
         l32, lm32 = _u8(u16, u32)
-        print(f"{hw}x{hw} T={len(tl)} frame {i}: eps engine-vs-fp32 rel {rel:.2e} cos {cos:.6f} | torch-fp16-vs-fp32 rel {rel16:.2e} | "
+        print(f"{height}x{width} T={len(tl)} frame {i}: eps engine-vs-fp32 rel {rel:.2e} cos {cos:.6f} | torch-fp16-vs-fp32 rel {rel16:.2e} | "
               f"u8 engine-vs-fp32 {f32:.5f}/{m32}  engine-vs-torch-fp16 {f16:.5f}/{m16}  torch-fp16-vs-fp32 {l32:.5f}/{lm32}")
         assert rel <= 2e-2 and cos >= 0.999, f"frame {i}: eps vs fp32 library run"
         assert f32 >= 0.999 and m32 <= 8, f"frame {i}: u8 vs fp32 library run"
@@ -104,6 +118,40 @@ def test_three_implementations_full_size(cuda, turbo, tl, hw, nframes, in_flight
         if len(tl) > 1:
             rb, cb = _rel_cos(sd.get_tensor("unet_in")[1:], ref32.x_t_latent_buffer)
             assert rb <= 2e-2 and cb >= 0.999, f"frame {i}: x_t_latent_buffer"
+
+
+@pytest.mark.parametrize("turbo,tl,hw", [
+    pytest.param(False, [18, 26, 35, 45], 512, id="sd15-T4-512"),          # the square control
+    pytest.param(True, [32], (384, 512), id="turbo-T1-384x512"),
+    pytest.param(True, [32], (448, 768), id="turbo-T1-448x768"),
+    pytest.param(False, [18, 26, 35, 45], (768, 448), id="sd15-T4-768x448"),
+])
+def test_full_size_unet_taps(cuda, turbo, tl, hw):
+    """Every UNet tap, x_t, eps and x0 of the second frame against the fp32 GPU oracle run layer by layer (unet_forward with
+    taps) on the same UNet input, as the tiny test does against the CPU oracle.  The non-square engines must meet the
+    tolerance the square 512x512 control meets: a mix-up of H and W anywhere in the UNet shows as a tap out of tolerance."""
+    from oracle import pipeline as opipe
+    from oracle import torch_gpu as tg
+    from oracle import unet as ounet
+    from oracle import weights as ow
+    height, width = _hw(hw)
+    cfg, arch, usd, vsd, emb = _weights(turbo)
+    sd = _engine(arch, usd, vsd, emb, tl, hw)
+    ref = tg.build(cfg, usd, vsd, tl, height, emb, sd.init_noise, torch.float32, width=width)
+    with torch.no_grad():
+        for i in range(2):
+            f = ow.make_frame(height, width, seed=i).cuda()
+            sd.step_u8(f)
+            opipe.frame_to_u8(ref, f)
+        taps = {}
+        ounet.unet_forward(ref.unet_sd, ref.cfg, ref.last["unet_in"], ref.sub_timesteps_tensor, ref.prompt_embeds, taps)
+    rows = [(n, *_rel_cos(sd.get_tensor(n), r)) for n, r in taps.items()]
+    rows += [(n, *_rel_cos(sd.get_tensor(n), ref.last[n])) for n in ("x_t", "eps", "x0")]
+    table = "\n".join(f"  {n:12s} relerr={e:.2e} cos={c:.6f}" for n, e, c in rows)
+    print(f"{height}x{width} T={len(tl)}: {len(rows)} taps, worst relerr {max(e for _, e, _ in rows):.2e}, "
+          f"lowest cos {min(c for _, _, c in rows):.6f}\n{table}")
+    for n, e, c in rows:
+        assert e <= 2e-2 and c >= 0.999, f"{height}x{width}: tap {n} relerr {e:.2e} cos {c:.6f}"
 
 
 @pytest.mark.parametrize("name,tl,hw", [("sd15_T4_512", [18, 26, 35, 45], 512), ("sd15_T4_768", [18, 26, 35, 45], 768)])

@@ -108,6 +108,10 @@ def test_geglu(cuda):
     (1, 128, 128, 64, 64, 2, 1, False),   # TAESD encoder stride-2 conv
     (2, 24, 24, 128, 64, 1, 1, True),     # 768-class odd extents (partial tiles)
     (1, 64, 64, 320, 4, 1, 1, False),     # conv_out: Cout=4 padded to N=16
+    (1, 12, 7, 1280, 1280, 1, 4, False),  # 768x448 12x7 level: a 12-row x 7-column tile (84 pixels)
+    (4, 56, 96, 320, 320, 1, 1, False),   # 448x768 top level at batch 4
+    (1, 96, 56, 320, 320, 2, 1, False),   # 768x448 downsample to 48x28
+    (1, 56, 96, 320, 4, 1, 1, False),     # conv_out at 448x768
 ])
 def test_conv3x3(cuda, nb, h, w, cin, cout, stride, splits, relu):
     ops = _ops()
@@ -179,6 +183,10 @@ def test_swapped_operands_vt(cuda):
     (4, 8, 8, 1280, 1280, 1, 256, 8, False),   # four images in one pixel tile
     (1, 64, 64, 320, 320, 2, 256, 1, False),   # stride-2 downsample
     (2, 24, 24, 128, 192, 1, 128, 1, False),   # ragged extents
+    (1, 6, 8, 1280, 1280, 1, 64, 8, False),    # 384x512 SD-Turbo 6x8 level: an 8x8 pixel tile with two masked rows
+    (1, 12, 7, 1280, 1280, 1, 64, 8, True),    # 768x448 12x7 level: one masked column per pixel row
+    (4, 2, 3, 256, 256, 1, 64, 4, False),      # tiny 128x192 2x3 level, four images in one pixel tile
+    (1, 24, 14, 1280, 1280, 2, 128, 4, False), # 768x448 stride-2 downsample to 12x7
 ])
 def test_conv3x3_swapped_orientation(cuda, nb, h, w, cin, cout, stride, bn, splits, res):
     """D^T = W . X^T: output channels on the MMA M side, a tile of bn pixels on the N side, transposed store."""

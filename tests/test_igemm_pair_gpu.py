@@ -46,6 +46,10 @@ def test_linear_pair(cuda, m, k, n, bn, splits):
     (1, 64, 64, 320, 320, 2, 160, 1, False),    # stride 2
     (2, 24, 24, 128, 64, 1, 64, 1, True),       # odd extents (partial tiles)
     (1, 256, 256, 64, 64, 1, 64, 1, True),      # 512 M tiles: persistent pairs, two accumulators
+    (4, 96, 56, 320, 320, 1, 160, 1, False),    # 768x448 top level at batch 4
+    (1, 48, 64, 640, 640, 2, 160, 1, False),    # 384x512: stride 2 to 24x32
+    (4, 12, 7, 1280, 1280, 1, 64, 1, False),    # 12x7 level at batch 4: one 12x7 tile (84 of 128 rows) per image
+    (1, 384, 256, 64, 64, 1, 64, 1, True),      # TAESD body of a 768x512 frame: persistent pairs, non-square
 ])
 def test_conv3x3_pair(cuda, nb, h, w, cin, cout, stride, bn, splits, relu):
     ops = _ops()

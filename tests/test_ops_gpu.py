@@ -474,6 +474,104 @@ def test_smallconv_resize_nearest(cuda):
     assert_close(y, ref, 2e-3, 2e-3, "encoder head with nearest resize")
 
 
+# camera frames into engine sizes; the last pair has an exact 5:4 ratio, where every nearest rule agrees
+_RESIZE_PAIRS = [((600, 800), (576, 768)), ((720, 1280), (448, 768)), ((1080, 1920), (832, 896)), ((300, 400), (128, 192)),
+                 ((150, 200), (576, 768)), ((480, 640), (384, 512))]
+_EXACT_RATIO = ((480, 640), (384, 512))
+
+
+def _pair_id(p):
+    return "x".join(map(str, p))
+
+
+def _nearest_index_map(src, dst, device):
+    """long [2, h, w]: the (row, column) of the source pixel that F.interpolate(size=dst, mode="nearest") reads for each
+    output pixel, found by resizing a tensor of source coordinates on `device`."""
+    yy, xx = torch.meshgrid(torch.arange(src[0], dtype=torch.float32), torch.arange(src[1], dtype=torch.float32), indexing="ij")
+    return F.interpolate(torch.stack([yy, xx])[None].to(device), size=dst, mode="nearest")[0].long().cpu()
+
+
+def _integer_rule_map(src, dst):
+    """The exact-integer rule floor(dst * in / out), for comparison: it differs from torch's wherever out has an odd factor."""
+    ys = torch.arange(dst[0]) * src[0] // dst[0]
+    xs = torch.arange(dst[1]) * src[1] // dst[1]
+    return torch.stack(torch.meshgrid(ys, xs, indexing="ij"))
+
+
+def _coordinate_frame(h, w):
+    """u8 [1, h, w, 3] whose pixel (y, x) encodes its own coordinates: R = x & 255, G = y & 255, B = (x >> 8) | (y >> 8) << 4."""
+    yy, xx = torch.meshgrid(torch.arange(h), torch.arange(w), indexing="ij")
+    return torch.stack([xx & 255, yy & 255, (xx >> 8) | ((yy >> 8) << 4)], -1).to(torch.uint8)[None]
+
+
+@pytest.mark.parametrize("entry", ["u8", "f32", "f16"])
+@pytest.mark.parametrize("src,dst", _RESIZE_PAIRS, ids=[f"{_pair_id(s)}-{_pair_id(d)}" for s, d in _RESIZE_PAIRS])
+def test_smallconv_resize_index_map(cuda, src, dst, entry):
+    """Every output pixel of the frame resize reads the source pixel torch's nearest rule picks (VaeImageProcessor.resize ->
+    F.interpolate(size=...)): min(floor(dst * fp32(in / out)), in - 1).  The frame encodes each pixel's coordinates and the
+    conv copies them through (centre-tap identity weights), so the decoded output is the index map itself.  Catches the
+    exact-integer rule floor(dst * in / out): 800 -> 768 differs from torch on 7 rows / columns, 720 -> 448 on row 308."""
+    ops = _ops()
+    frame = _coordinate_frame(*src)
+    if entry == "u8":
+        x, flags = frame.to(cuda), 1
+    else:   # the (3, H, W) float entries; the wrapper reads (nb, in_h, in_w, cin) from the shape, the data stays NCHW
+        dt, flags = (torch.float32, 8) if entry == "f32" else (torch.float16, 16)
+        x = (frame.permute(0, 3, 1, 2).double() / 255.0).to(dt).contiguous().to(cuda).permute(0, 2, 3, 1)
+    w = torch.zeros((16, 3, 3, 3), dtype=torch.float16, device=cuda)
+    w[[0, 1, 2], [0, 1, 2], 1, 1] = 1.0
+    y = torch.full((1, *dst, 16), float("nan"), dtype=torch.float16, device=cuda)
+    ops.smallconv(x, w, None, y, flags=flags)
+    code = (y[0, ..., :3].double() * 255.0).round().long().cpu()
+    got = torch.stack([code[..., 1] | (code[..., 2] >> 4) << 8, code[..., 0] | (code[..., 2] & 15) << 8])
+    ref = _nearest_index_map(src, dst, "cpu")
+    assert torch.equal(ref, _nearest_index_map(src, dst, cuda)), "torch's CPU and CUDA nearest rules disagree"
+    integer = _integer_rule_map(src, dst)
+    assert torch.equal(integer, ref) == ((src, dst) == _EXACT_RATIO), "the pair cannot tell the integer rule from torch's"
+    bad_rows = (got[0] != ref[0]).any(1).nonzero().flatten().tolist()
+    bad_cols = (got[1] != ref[1]).any(0).nonzero().flatten().tolist()
+    assert torch.equal(got, ref), (f"{entry} {src} -> {dst}: source rows differ at output rows {bad_rows[:16]}, source columns "
+                                   f"at output columns {bad_cols[:16]}")
+
+
+@pytest.mark.parametrize("head", ["silu", "offset"])
+def test_smallconv_ext_heads_resize(cuda, head):
+    """The epilogue instantiations read the frame through the same resize: the ControlNet conditioning embedding's conv_in (u8,
+    SiLU) and HED's first conv (u8 minus per-channel offsets, ReLU), on a 400x300 noise frame into a 192x128 engine, against a
+    float64 conv of the frame resized by torch.  Catches the exact-integer resize rule (3 source columns differ)."""
+    ops = _ops()
+    from oracle import weights as ow
+    src, dst = (300, 400), (128, 192)
+    frame = ow.make_frame(*src, seed=31, smooth=False)
+    g = torch.Generator().manual_seed(32)
+
+    def resized(m):   # float64 NCHW [1, 3, h, w] of the frame read through the index map m
+        return frame[0][m[0], m[1]].permute(2, 0, 1)[None].double().to(cuda)
+    if head == "silu":
+        wt = (torch.randn((16, 3, 3, 3), generator=g) * 0.8).half().to(cuda)
+        bias = (torch.randn(16, generator=g) * 0.5).float().to(cuda)
+        out = torch.full((1, *dst, 16), float("nan"), dtype=torch.float16, device=cuda)
+        ops.smallconv_ex(frame.to(cuda), wt, bias, out, flags=1 | 32)
+        tol = (2e-3, 4e-3)
+
+        def f(m):
+            x = (resized(m) / 255.0).half().double()
+            return F.silu(F.conv2d(x, wt.double(), bias.double(), padding=1)).permute(0, 2, 3, 1)
+    else:
+        off = torch.tensor([117.0, 104.5, 96.25], device=cuda)
+        wt = (torch.randn((64, 3, 3, 3), generator=g) * 0.2).half().to(cuda)
+        bias = (torch.randn(64, generator=g) * 0.5).float().to(cuda)
+        out = torch.full((1, *dst, 64), float("nan"), dtype=torch.float16, device=cuda)
+        ops.smallconv_ex(frame.to(cuda), wt, bias, out, flags=1 | 4 | 64, in_off=off)
+        tol = (5e-2, 4e-3)
+
+        def f(m):
+            x = (resized(m) - off.double().view(1, 3, 1, 1)).half().double()
+            return F.relu(F.conv2d(x, wt.double(), bias.double(), padding=1)).permute(0, 2, 3, 1)
+    ref, wrong = f(_nearest_index_map(src, dst, "cpu")), f(_integer_rule_map(src, dst))
+    assert_discriminates(out, ref, wrong, *tol, f"smallconv {head} head, {src} -> {dst}", bug="exact-integer resize rule")
+
+
 def test_smallconv_taesd_decoder_head(cuda):
     ops = _ops()
     z = (_rand((1, 16, 16, 4), cuda, 1) * 2).half()

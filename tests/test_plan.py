@@ -77,10 +77,11 @@ def _check(info, d, total_kb, geglu=False, pairs_ok=False):
             assert info.grid_x == (info.m_tiles + 1) // 2 * 2 if info.mode == 1 else info.grid_x == info.m_tiles
 
 
-def _unet_shapes(chs, nb, latent=64):
-    """(h, srcs, cout, stride, geglu, allow_swap) of every contraction family of a UNet with block channels `chs`"""
+def _unet_shapes(chs, nb, lh=64, lw=64):
+    """(nb, (h, w), srcs, cout, stride, geglu, allow_swap) of every contraction family of a UNet with block channels `chs` on an
+    lh x lw latent"""
     out = []
-    res = [latent, latent // 2, latent // 4, latent // 8]
+    res = [(lh >> k, lw >> k) for k in range(4)]
     for lvl, (c, r) in enumerate(zip(chs, res)):
         cin_prev = chs[max(lvl - 1, 0)]
         out += [(r, [(cin_prev, 9)], c, 1, False, True), (r, [(c, 9)], c, 1, False, True),          # resnet conv1 / conv2
@@ -95,29 +96,39 @@ def _unet_shapes(chs, nb, latent=64):
     return [(nb,) + s for s in out]
 
 
-@pytest.mark.parametrize("nb,latent", [(1, 64), (4, 64), (4, 96), (1, 32)])
-def test_autotile_invariants_over_the_frame_program(nb, latent):
-    """BASELINE.json configs: 512x512 at stream batch 1 / 4, 768x768 at batch 4, 256x256 at batch 1"""
-    shapes = _unet_shapes([320, 640, 1280, 1280], nb, latent)
-    px = latent * 8
-    shapes += [(1, r, [(64, 9)], 64, 1, False, False) for r in (px, px // 2, px // 4, px // 8)]          # TAESD body (one frame)
-    shapes += [(1, r, [(64, 9)], 64, 2, False, False) for r in (px, px // 2, px // 4)]
-    for (b, r, srcs, cout, stride, geglu, allow_swap) in shapes:
-        d, kb = _desc(b, r, r, srcs, cout, stride=stride, geglu=geglu)
+def _latent_cases(cases):
+    """(nb, lh, lw) parameters; square latents keep their "nb-latent" ids"""
+    return [pytest.param(nb, lh, lw, id=f"{nb}-{lh}" if lh == lw else f"{nb}-{lh}x{lw}") for nb, lh, lw in cases]
+
+
+# non-square engines: 384x512 (SD-Turbo 6x8 level on the swapped path), 448x768, 768x448 (Wo = 7 at the 12x7 level) and the
+# 128x192 tiny size (2x3 level, several images in one M tile)
+_NONSQUARE = [(1, 48, 64), (1, 56, 96), (4, 96, 56), (4, 16, 24)]
+
+
+@pytest.mark.parametrize("nb,lh,lw", _latent_cases([(1, 64, 64), (4, 64, 64), (4, 96, 96), (1, 32, 32)] + _NONSQUARE))
+def test_autotile_invariants_over_the_frame_program(nb, lh, lw):
+    """BASELINE.json configs: 512x512 at stream batch 1 / 4, 768x768 at batch 4, 256x256 at batch 1; and non-square engines"""
+    shapes = _unet_shapes([320, 640, 1280, 1280], nb, lh, lw)
+    shapes += [(1, (lh * 8 >> k, lw * 8 >> k), [(64, 9)], 64, 1, False, False) for k in range(4)]   # TAESD body (one frame)
+    shapes += [(1, (lh * 8 >> k, lw * 8 >> k), [(64, 9)], 64, 2, False, False) for k in range(3)]
+    for (b, (rh, rw), srcs, cout, stride, geglu, allow_swap) in shapes:
+        d, kb = _desc(b, rh, rw, srcs, cout, stride=stride, geglu=geglu)
         info = _plan(d, 1, int(allow_swap))
         _check(info, d, kb, geglu)
         ctas = info.grid_x * info.grid_y * info.grid_z
         if not info.swap:   # one CTA per SM: no launch cuts its operand ring to share an SM, however many CTAs it has
-            assert info.num_stages >= _full_ring_stages(info), f"{ctas} CTAs: ring of {info.num_stages} stages ({srcs}->{cout} @{r})"
+            assert info.num_stages >= _full_ring_stages(info), \
+                f"{ctas} CTAs: ring of {info.num_stages} stages ({srcs}->{cout} @{rh}x{rw})"
 
 
-@pytest.mark.parametrize("nb,latent", [(1, 64), (4, 64), (4, 96)])
-def test_throughput_policy_invariants(nb, latent):
+@pytest.mark.parametrize("nb,lh,lw", _latent_cases([(1, 64, 64), (4, 64, 64), (4, 96, 96)] + _NONSQUARE))
+def test_throughput_policy_invariants(nb, lh, lw):
     """autotile = 2: what the engine plans with >= 4 frames in flight (CTA pairs without split-K, full operand rings)"""
-    shapes = _unet_shapes([320, 640, 1280, 1280], nb, latent)
+    shapes = _unet_shapes([320, 640, 1280, 1280], nb, lh, lw)
     paired = 0
-    for (b, r, srcs, cout, stride, geglu, allow_swap) in shapes:
-        d, kb = _desc(b, r, r, srcs, cout, stride=stride, geglu=geglu)
+    for (b, (rh, rw), srcs, cout, stride, geglu, allow_swap) in shapes:
+        d, kb = _desc(b, rh, rw, srcs, cout, stride=stride, geglu=geglu)
         info = _plan(d, 2, int(allow_swap))
         _check(info, d, kb, geglu, pairs_ok=True)
         single = _plan(d, 1, int(allow_swap))

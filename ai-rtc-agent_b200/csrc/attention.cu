@@ -228,6 +228,198 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_kernel(const __grid_consta
     }
 }
 
+// ------------------------------------------------------------------------------------------ head dim 512
+// Single-head attention of the AutoencoderKL mid blocks (diffusers Attention(heads=1, dim_head=512)).  A 64-row warpgroup cannot
+// hold a 512-wide fp32 O accumulator, so the output columns are split over CTAs: blockIdx.y = head * A5_SLICES + slice, and each
+// CTA computes the full S = Q K^T (32 k16 steps), keeps its own online-softmax statistics and accumulates P V only for its
+// 128-column slice of V^T.  S is recomputed once per slice (4x the Q K^T work, 3 x 17 GFLOP extra at 4096 tokens).  S stays in
+// fp32 registers (upcast softmax); P is rounded to fp16 as the A operand of the P.V MMA, as in attn_kernel.  Warp-level
+// mma.sync m16n8k16 with ldmatrix operands, cp.async double-buffered K / V^T blocks.  Every summation order is fixed, so the
+// output is bit-reproducible.
+constexpr int A5_D = 512;
+constexpr int A5_DS = 128;                 // output columns per CTA
+constexpr int A5_SLICES = A5_D / A5_DS;
+constexpr int A5_BQ = 128;                 // query rows per CTA: 8 warps x 16
+constexpr int A5_BKV = 32;                 // keys per block
+constexpr int A5_THREADS = 256;
+constexpr int A5_QP = A5_D + 8;            // smem row pitches in halves (+16 B: ldmatrix rows fall in different banks)
+constexpr int A5_VP = A5_BKV + 8;
+constexpr size_t A5_Q_ELEMS = (size_t)A5_BQ * A5_QP;
+constexpr size_t A5_K_ELEMS = (size_t)A5_BKV * A5_QP;
+constexpr size_t A5_V_ELEMS = (size_t)A5_DS * A5_VP;
+constexpr size_t A5_SMEM = (A5_Q_ELEMS + 2 * (A5_K_ELEMS + A5_V_ELEMS)) * 2;
+
+struct Attn512Params {
+    const __half* q; const __half* k; const __half* vt;
+    __half* out;
+    int ldq, ldk, ldvt, ldo;
+    int sq, skv;
+    long k_bstride, vt_bstride;
+    float scale_log2;
+};
+
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, int src_bytes) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
+}
+__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+__global__ void __launch_bounds__(A5_THREADS, 1) attn_d512_kernel(const __grid_constant__ Attn512Params p) {
+    extern __shared__ __align__(128) __half sm5[];
+    __half* sQ = sm5;
+    __half* sK = sQ + A5_Q_ELEMS;                 // [2][A5_BKV][A5_QP]
+    __half* sV = sK + 2 * A5_K_ELEMS;             // [2][A5_DS][A5_VP]: V^T rows (output columns) x keys
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int q0 = blockIdx.x * A5_BQ;
+    const int head = blockIdx.y / A5_SLICES, slice = blockIdx.y % A5_SLICES;
+    const int b = blockIdx.z;
+    const int col0 = head * A5_D;
+    const int nblk = (p.skv + A5_BKV - 1) / A5_BKV;
+    const __half* qb = p.q + (long)b * p.sq * p.ldq + col0;
+    const __half* kb = p.k + b * p.k_bstride * p.ldk + col0;
+    const __half* vb = p.vt + (long)(col0 + slice * A5_DS) * p.ldvt + b * p.vt_bstride;
+
+    pdl_launch_dependents();
+    pdl_wait();
+
+    // rows / keys past the end are zero-filled (cp.async src-size 0), so no value outside the operands enters an MMA
+    for (int i = tid; i < A5_BQ * (A5_D / 8); i += A5_THREADS) {
+        const int r = i / (A5_D / 8), c = (i % (A5_D / 8)) * 8;
+        const bool ok = q0 + r < p.sq;
+        cp_async16(smem_u32(sQ + r * A5_QP + c), ok ? qb + (long)(q0 + r) * p.ldq + c : qb, ok ? 16 : 0);
+    }
+    auto load_kv = [&](int j, int buf) {
+        __half* sk = sK + buf * A5_K_ELEMS;
+        __half* sv = sV + buf * A5_V_ELEMS;
+        const int kv0 = j * A5_BKV;
+        for (int i = tid; i < A5_BKV * (A5_D / 8); i += A5_THREADS) {
+            const int r = i / (A5_D / 8), c = (i % (A5_D / 8)) * 8;
+            const bool ok = kv0 + r < p.skv;
+            cp_async16(smem_u32(sk + r * A5_QP + c), ok ? kb + (long)(kv0 + r) * p.ldk + c : kb, ok ? 16 : 0);
+        }
+        for (int i = tid; i < A5_DS * (A5_BKV / 8); i += A5_THREADS) {
+            const int r = i / (A5_BKV / 8), c = (i % (A5_BKV / 8)) * 8;
+            const int valid = p.skv - (kv0 + c);
+            const int bytes = valid >= 8 ? 16 : (valid > 0 ? 2 * valid : 0);
+            cp_async16(smem_u32(sv + r * A5_VP + c), bytes ? vb + (long)r * p.ldvt + kv0 + c : vb, bytes);
+        }
+    };
+    load_kv(0, 0);
+    cp_async_commit();
+
+    const int r_lo = lane >> 2, q2 = 2 * (lane & 3);
+    float o[A5_DS / 8][4];
+#pragma unroll
+    for (int n = 0; n < A5_DS / 8; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    // ldmatrix lane addresses: A (16x16, row-major Q) and B (two n8 tiles x k16 from [n][k] rows: K, V^T)
+    const uint32_t a_base = smem_u32(sQ + (warp * 16 + (lane & 15)) * A5_QP + (lane >> 4) * 8);
+    const int b_row = (lane & 7) + ((lane >> 4) << 3), b_col = ((lane >> 3) & 1) * 8;
+
+    for (int j = 0; j < nblk; ++j) {
+        const int buf = j & 1;
+        if (j + 1 < nblk) {
+            load_kv(j + 1, buf ^ 1);
+            cp_async_commit();
+            cp_async_wait<1>();
+        } else {
+            cp_async_wait<0>();
+        }
+        __syncthreads();
+        // S = Q K^T for this warp's 16 rows x A5_BKV keys
+        float s[A5_BKV / 8][4];
+#pragma unroll
+        for (int n = 0; n < A5_BKV / 8; ++n) s[n][0] = s[n][1] = s[n][2] = s[n][3] = 0.f;
+        const uint32_t k_base = smem_u32(sK + buf * A5_K_ELEMS + b_row * A5_QP + b_col);
+#pragma unroll 4
+        for (int kk = 0; kk < A5_D / 16; ++kk) {
+            uint32_t a[4];
+            ldsm_x4(a_base + kk * 32, a[0], a[1], a[2], a[3]);
+#pragma unroll
+            for (int np = 0; np < A5_BKV / 16; ++np) {
+                uint32_t b0, b1, b2, b3;
+                ldsm_x4(k_base + (np * 16 * A5_QP) * 2 + kk * 32, b0, b1, b2, b3);
+                mma16816(s[2 * np], a, b0, b1);
+                mma16816(s[2 * np + 1], a, b2, b3);
+            }
+        }
+        // online softmax over the valid keys (columns >= kv_valid are masked)
+        const int kv_valid = p.skv - j * A5_BKV;
+        float alpha[2], m_new[2];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            float mx = -INFINITY;
+#pragma unroll
+            for (int n = 0; n < A5_BKV / 8; ++n)
+#pragma unroll
+                for (int u = 0; u < 2; ++u)
+                    if (8 * n + q2 + u < kv_valid) mx = fmaxf(mx, s[n][2 * hr + u]);
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            m_new[hr] = fmaxf(m_run[hr], mx * p.scale_log2);
+            alpha[hr] = ex2_approx(m_run[hr] - m_new[hr]);
+        }
+        uint32_t pa[A5_BKV / 16][4];
+        float rs[2] = {0.f, 0.f};
+#pragma unroll
+        for (int n = 0; n < A5_BKV / 8; ++n)
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+                float p0 = ex2_approx(s[n][2 * hr] * p.scale_log2 - m_new[hr]);
+                float p1 = ex2_approx(s[n][2 * hr + 1] * p.scale_log2 - m_new[hr]);
+                if (8 * n + q2 >= kv_valid) p0 = 0.f;
+                if (8 * n + q2 + 1 >= kv_valid) p1 = 0.f;
+                rs[hr] += p0 + p1;
+                pa[n >> 1][(n & 1) * 2 + hr] = pack_half2(p0, p1);
+            }
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            l_run[hr] = l_run[hr] * alpha[hr] + rs[hr];
+            m_run[hr] = m_new[hr];
+        }
+#pragma unroll
+        for (int n = 0; n < A5_DS / 8; ++n) {
+            o[n][0] *= alpha[0]; o[n][1] *= alpha[0];
+            o[n][2] *= alpha[1]; o[n][3] *= alpha[1];
+        }
+        // O += P V over this CTA's column slice (B = V^T rows, keys contiguous)
+        const uint32_t v_base = smem_u32(sV + buf * A5_V_ELEMS + b_row * A5_VP + b_col);
+#pragma unroll
+        for (int t = 0; t < A5_BKV / 16; ++t)
+#pragma unroll
+            for (int np = 0; np < A5_DS / 16; ++np) {
+                uint32_t b0, b1, b2, b3;
+                ldsm_x4(v_base + (np * 16 * A5_VP) * 2 + t * 32, b0, b1, b2, b3);
+                mma16816(o[2 * np], pa[t], b0, b1);
+                mma16816(o[2 * np + 1], pa[t], b2, b3);
+            }
+        __syncthreads();   // every warp is done with this buffer before the next iteration refills it
+    }
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        float l = l_run[hr];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float inv_l = 1.0f / l;
+        const int r = q0 + warp * 16 + r_lo + 8 * hr;
+        if (r >= p.sq) continue;
+        __half* orow = p.out + ((long)b * p.sq + r) * p.ldo + col0 + slice * A5_DS;
+#pragma unroll
+        for (int n = 0; n < A5_DS / 8; ++n)
+            *reinterpret_cast<uint32_t*>(orow + 8 * n + q2) = pack_half2(o[n][2 * hr] * inv_l, o[n][2 * hr + 1] * inv_l);
+    }
+}
+
 // ------------------------------------------------------------------------------------------ host
 static int encode_2d(CUtensorMap* m, const __half* ptr, long cols, long rows, long ld, int box_cols, int box_rows,
                      const char* what) {
@@ -266,6 +458,20 @@ static size_t attn_smem_bytes(int da, int bkv) {
 
 int attn_plan(const AttnDesc& d, AttnPlan* plan) {
     *plan = AttnPlan{};
+    if (d.dp == A5_D) {   // attn_d512_kernel: plain pointers (cp.async), no tensor maps
+        const auto misaligned = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) != 0; };
+        if (d.d_real != A5_D || (d.ldq & 7) || (d.ldk & 7) || (d.ldvt & 7) || (d.ldo & 7) || (d.vt_bstride & 7) ||
+            misaligned(d.q) || misaligned(d.k) || misaligned(d.vt) || misaligned(d.out) || d.sq < 1 || d.skv < 1) {
+            b2_set_error("attn(d512): needs d_real 512, row pitches and the V^T batch stride multiples of 8, 16-byte aligned "
+                         "pointers (d_real %d ldq %d ldk %d ldvt %d ldo %d vt_bstride %ld)", d.d_real, d.ldq, d.ldk, d.ldvt, d.ldo,
+                         d.vt_bstride);
+            return -1;
+        }
+        plan->d = d;
+        plan->grid = dim3((d.sq + A5_BQ - 1) / A5_BQ, d.heads * A5_SLICES, d.nb);
+        plan->smem = A5_SMEM;
+        return 0;
+    }
     if (d.dp != 64 && d.dp != 128 && d.dp != 192) {
         b2_set_error("attn: padded head dim %d unsupported", d.dp);
         return -1;
@@ -290,7 +496,8 @@ int attn_init() {
         cudaError_t e1 = cudaFuncSetAttribute(attn_kernel<1, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         cudaError_t e2 = cudaFuncSetAttribute(attn_kernel<2, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         cudaError_t e3 = cudaFuncSetAttribute(attn_kernel<3, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess) {
+        cudaError_t e4 = cudaFuncSetAttribute(attn_d512_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)A5_SMEM);
+        if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess || e4 != cudaSuccess) {
             b2_set_error("cudaFuncSetAttribute(attn) failed");
             return -1;
         }
@@ -302,6 +509,19 @@ int attn_init() {
 int attn_launch(const AttnPlan& plan, cudaStream_t s) {
     if (attn_init()) return -1;
     const AttnDesc& d = plan.d;
+    if (d.dp == A5_D) {
+        Attn512Params q5;
+        q5.q = d.q; q5.k = d.k; q5.vt = d.vt; q5.out = d.out;
+        q5.ldq = d.ldq; q5.ldk = d.ldk; q5.ldvt = d.ldvt; q5.ldo = d.ldo;
+        q5.sq = d.sq; q5.skv = d.skv; q5.k_bstride = d.k_bstride; q5.vt_bstride = d.vt_bstride;
+        q5.scale_log2 = (float)(1.4426950408889634 / sqrt((double)d.d_real));
+        const cudaError_t e5 = launch_k(attn_d512_kernel, plan.grid, dim3(A5_THREADS), plan.smem, s, 1, q5);
+        if (e5 != cudaSuccess) {
+            b2_set_error("attn(d512) launch: %s", cudaGetErrorString(e5));
+            return -1;
+        }
+        return 0;
+    }
     AttnParams p;
     p.tmq = plan.tmq; p.tmk = plan.tmk; p.tmv = plan.tmv;
     p.out = d.out; p.ldo = d.ldo;

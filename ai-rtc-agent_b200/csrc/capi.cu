@@ -46,7 +46,7 @@ static void to_igemm_desc(const b2sd_igemm_desc* d, IgemmDesc& g) {
     g.epi.ldr = d->ldr;
     g.epi.acc_scale = d->acc_scale;
     g.epi.res_scale = d->res_scale;
-    g.epi.flags = d->flags & (IG_RELU | IG_GEGLU | IG_SILU);
+    g.epi.flags = d->flags & (IG_RELU | IG_GEGLU | IG_SILU | IG_PAD0);
     g.epi.n_valid = d->n_valid;
     g.epi.rowstat_out = static_cast<unsigned long long*>(d->rowstat_out);
     g.epi.rowstat_in = static_cast<const unsigned long long*>(d->rowstat_in);
@@ -66,6 +66,10 @@ int b2sd_op_igemm(const b2sd_igemm_desc* d, void* stream) {
     IgemmDesc g{};
     to_igemm_desc(d, g);
     if (d->flags & B2SD_IG_TCONV) {   // the persistent halo-tile kernel (64 -> 64 channel 3x3 convolutions)
+        if (d->flags & B2SD_IG_PAD0) {
+            b2_set_error("b2sd_op_igemm: the halo-tile kernel has no tap-origin-0 variant");
+            return -1;
+        }
         TconvPlan tp;
         if (tconv_plan(g, &tp)) return -1;
         return tconv_launch(tp, reinterpret_cast<cudaStream_t>(stream));

@@ -1,4 +1,4 @@
-// Per-frame engine: TAESD encoder -> stream-batched UNet -> LCM step -> TAESD decoder, assembled once
+// Per-frame engine: VAE encoder (TAESD, or the model's AutoencoderKL) -> stream-batched UNet -> LCM step -> VAE decoder, assembled once
 // (at b2sd_prepare) as a static list of kernel launches over preallocated HBM buffers and replayed as
 // a CUDA graph.  Mirrors what the reference reaches through StreamDiffusion.__call__
 // (lib/wrapper.py:330) and its three TensorRT engines (lib/wrapper.py:445-466).
@@ -51,6 +51,7 @@ struct Act {
 struct Raw {  // a loaded parameter, fp16 on device (+ host fp32 copy for 1-D tensors)
     __half* p = nullptr;      // null once released (pack-only parameters after the first successful prepare)
     bool pack_only = false;   // only ever read by the packing kernels (3x3 / shortcut convs, q/k/v, GEGLU, Cin<=4 convs)
+    bool derived = false;     // computed by the engine from loaded parameters (exact weight foldings): dropped on any reload
     std::vector<int64_t> shape;
     std::vector<float> host;
     long numel() const {
@@ -135,7 +136,7 @@ int igemm_autotile(IgemmDesc d, bool allow_swap, IgemmPlan* plan_out) {
     const int pair_splits = ps_env ? atoi(ps_env) : (d.pair_splits > 0 ? d.pair_splits : 4);
     const IgemmPlan& pl = *plan_out;
     const int m_tiles = pl.p.tiles_w * pl.p.tiles_h * pl.p.tiles_n;
-    if (pair_mode <= 0 || pl.p.swap || m_tiles < 2 || (pl.p.BN % 32) != 0 || (d.epi.flags & IG_SILU)) return 0;
+    if (pair_mode <= 0 || pl.p.swap || m_tiles < 2 || (pl.p.BN % 32) != 0 || (d.epi.flags & (IG_SILU | IG_PAD0))) return 0;
     if (pair_mode == 2 && pl.p.total_kb < 20) return 0;
     d.swap = 0; d.BN = pl.p.BN; d.splits = pl.splits > pair_splits ? pair_splits : pl.splits; d.partial = nullptr;
     d.pair = pair_single ? 0 : 1;
@@ -149,6 +150,7 @@ static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_o
     IgemmPlan& plan = *plan_out;
     const bool geglu = (d.epi.flags & IG_GEGLU) != 0;
     const bool silu = (d.epi.flags & IG_SILU) != 0;   // SiLU-epilogue kernels exist for N tiles of 16..128 only
+    const bool pad0 = (d.epi.flags & IG_PAD0) != 0;   // tap-origin-0 kernels: N tiles of 64 / 128 / 256, normal orientation
     const int n_gemm = geglu ? 2 * d.epi.n_valid : d.epi.n_valid;
     static const bool swap_on = getenv("B2_SWAP") != nullptr, swap_off = getenv("B2_NO_SWAP") != nullptr;
     static const bool tuned = getenv("B2_NO_TUNED_TILES") == nullptr;
@@ -159,7 +161,7 @@ static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_o
     const long rows_all = (long)d.Nb * d.Ho * d.Wo;
     // Swapped orientation by default only where it measured faster (tools/bench_op.py, cold weights): the 8x8 level,
     // where a 128-pixel M tile would be half empty.  B2_SWAP=1 forces it for every eligible UNet contraction.
-    const bool swap_here = allow_swap && !geglu && d.epi.n_valid >= 128 && (d.epi.n_valid & 7) == 0 &&
+    const bool swap_here = allow_swap && !geglu && !pad0 && d.epi.n_valid >= 128 && (d.epi.n_valid & 7) == 0 &&
                            (swap_on || (!swap_off && tuned && rows_all <= 64 && total_kb >= 90));
     if (swap_here) {
         d.swap = 1;
@@ -180,7 +182,7 @@ static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_o
     }
     d.swap = 0;
     auto vt_ok = [&](int bn) { return !d.epi.out2 || d.epi.col2 % bn == 0; };   // fused q/k/v: an N tile is all q/k or all v
-    if (tuned && !geglu && !silu && n_gemm % 160 == 0 && total_kb >= 40 && vt_ok(160)) {
+    if (tuned && !geglu && !silu && !pad0 && n_gemm % 160 == 0 && total_kb >= 40 && vt_ok(160)) {
         // K-heavy contractions that cannot fill the GPU with 160-wide tiles alone (batch 1): wide tiles + cluster
         // split-K beat 64-wide tiles (weights streamed from HBM)
         d.BN = 160; d.splits = 1; d.partial = nullptr;
@@ -204,6 +206,7 @@ static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_o
     for (int bn : cands) {
         if (geglu && (bn % 32 != 0 || bn < 64)) continue;
         if (silu && (bn > 128 || bn % 16 || (bn & (bn - 1)))) continue;
+        if (pad0 && bn != 64 && bn != 128 && bn != 256) continue;
         if (n_gemm % bn == 0 && vt_ok(bn)) valid.push_back(bn);
     }
     if (valid.empty()) {  // ragged N: one masked tile size
@@ -614,7 +617,14 @@ struct b2sd_engine {
         return add_igemm(dst, d);
     }
 
-    int build_resnet(const std::string& p, const Act& xa, const Act* xb, int cout, const float* emb, Act* out, cudaStream_t s);
+    int build_resnet(const std::string& p, const Act& xa, const Act* xb, int cout, const float* emb, Act* out, cudaStream_t s,
+                     float eps = 1e-5f);
+    int build_vae_attention(const std::string& p, const Act& x, Act* out, cudaStream_t s);
+    int build_kl_encoder(Act* out, std::string* latent_conv, cudaStream_t s);
+    int build_kl_decoder(const Act& x0, cudaStream_t s);
+    std::vector<float> host_copy(const std::string& key);
+    int derive(const std::string& name, const std::vector<int64_t>& shape, const std::vector<float>& v);
+    const float* const_vec(const std::string& name, const std::vector<float>& v);
     int build_cond_embedding(Act* out, cudaStream_t s);
     int build_hed(const uint8_t** control, cudaStream_t s);
     int build_controlnet(const Act& cond, std::vector<Act>& skips, Act* mid, cudaStream_t s);
@@ -652,39 +662,47 @@ struct b2sd_engine {
 };
 
 // ------------------------------------------------------------------------------------------------
-// ResnetBlock2D (diffusers resnet.py): GN+SiLU -> conv1 (+temb) -> GN+SiLU -> conv2, + shortcut(x)
+// ResnetBlock2D (diffusers resnet.py): GN+SiLU -> conv1 (+temb) -> GN+SiLU -> conv2, + shortcut(x).  emb = nullptr: no time
+// embedding (the AutoencoderKL's resnets, temb_channels=None).
 int b2sd_engine::build_resnet(const std::string& p, const Act& xa, const Act* xb, int cout, const float* emb, Act* out,
-                              cudaStream_t s) {
+                              cudaStream_t s, float eps) {
     cur = p;
     allow_swap = true;
     const int cin = xa.c + (xb ? xb->c : 0);
     const int B = xa.n;
     Act n1 = new_act(B, xa.h, xa.w, cin);
-    TRY(add_groupnorm(xa, xb, p + "norm1", n1, 1e-5f, 1));
+    TRY(add_groupnorm(xa, xb, p + "norm1", n1, eps, 1));
     // conv1 with per-sample column bias = conv1.bias + time_emb_proj(silu(emb))
     Act h1 = new_act(B, xa.h, xa.w, cout);
     {
         int K = 0;
         __half* wp = pack_conv(p + "conv1.weight", {{p + "conv1.weight", 0, cin, 9}}, cout, &K, s);
         if (!wp) return -1;
-        float* colbias = static_cast<float*>(prog.alloc((size_t)B * cout * sizeof(float)));
-        const float* bsum = vec({p + "conv1.bias", p + "time_emb_proj.bias"});
-        const Raw* wt = get(p + "time_emb_proj.weight");
-        if (!colbias || !bsum || !wt) return -1;
-        const int tdim = (int)wt->shape[1];
-        const __half* wtp = wt->p;
-        prog_time.push_back(Op([=](cudaStream_t st) { return small_linear_launch(emb, tdim, wtp, bsum, colbias, cout, B, cout, tdim, 1, st); }, "temb " + p));
+        const float* colbias = nullptr;
+        if (emb) {
+            float* cb = static_cast<float*>(prog.alloc((size_t)B * cout * sizeof(float)));
+            const float* bsum = vec({p + "conv1.bias", p + "time_emb_proj.bias"});
+            const Raw* wt = get(p + "time_emb_proj.weight");
+            if (!cb || !bsum || !wt) return -1;
+            const int tdim = (int)wt->shape[1];
+            const __half* wtp = wt->p;
+            prog_time.push_back(Op([=](cudaStream_t st) { return small_linear_launch(emb, tdim, wtp, bsum, cb, cout, B, cout, tdim, 1, st); }, "temb " + p));
+            colbias = cb;
+        } else {
+            colbias = vec({p + "conv1.bias"}, nullptr, 16);
+            if (!colbias) return -1;
+        }
         IgemmDesc d{};
         d.nseg = 1; d.src[0] = view(n1); d.ntap[0] = 9;
         d.w = wp; d.w_rows = cout; d.w_ld = K; d.stride = 1;
         d.Nb = B; d.Ho = xa.h; d.Wo = xa.w;
         d.epi.out = h1.p; d.epi.ldc = h1.ld;
-        d.epi.colbias = colbias; d.epi.colbias_bstride = cout;
+        d.epi.colbias = colbias; d.epi.colbias_bstride = emb ? cout : 0;
         d.epi.acc_scale = 1.f; d.epi.res_scale = 1.f; d.epi.n_valid = cout;
         TRY(add_igemm(prog_frame, d));
     }
     Act n2 = new_act(B, xa.h, xa.w, cout);
-    TRY(add_groupnorm(h1, nullptr, p + "norm2", n2, 1e-5f, 1));
+    TRY(add_groupnorm(h1, nullptr, p + "norm2", n2, eps, 1));
     *out = new_act(B, xa.h, xa.w, cout);
     IgemmDesc d{};
     d.stride = 1; d.Nb = B; d.Ho = xa.h; d.Wo = xa.w;
@@ -1106,6 +1124,300 @@ int b2sd_engine::build_controlnet(const Act& cond, std::vector<Act>& skips, Act*
     return 0;
 }
 
+// ---- AutoencoderKL (diffusers autoencoder_kl.py / vae.py Encoder, Decoder; cfg.vae == B2SD_VAE_KL) -------------------------------
+// A parameter as fp32 on the host (exact weight foldings at build time; read before the pack-only raw copies are released).
+std::vector<float> b2sd_engine::host_copy(const std::string& key) {
+    const Raw* r = get(key);
+    if (!r || !r->p) {
+        if (r) b2_set_error("parameter '%s' was released before the weight folding that needs it", key.c_str());
+        return {};
+    }
+    std::vector<__half> h((size_t)r->numel());
+    if (cudaMemcpy(h.data(), r->p, h.size() * 2, cudaMemcpyDeviceToHost) != cudaSuccess) {
+        b2_set_error("host copy of '%s' failed", key.c_str());
+        return {};
+    }
+    std::vector<float> f(h.size());
+    for (size_t i = 0; i < h.size(); ++i) f[i] = __half2float(h[i]);
+    return f;
+}
+
+// A parameter the engine computes from loaded ones, stored like a loaded parameter (fp16; packed / exported like the others).
+int b2sd_engine::derive(const std::string& name, const std::vector<int64_t>& shape, const std::vector<float>& v) {
+    Raw r;
+    r.shape = shape;
+    r.derived = true;
+    r.pack_only = shape.size() == 4 && shape[2] == 3;
+    if ((size_t)r.numel() != v.size()) {
+        b2_set_error("derived parameter '%s': %zu values for %ld elements", name.c_str(), v.size(), r.numel());
+        return -1;
+    }
+    std::vector<__half> h(v.size());
+    for (size_t i = 0; i < v.size(); ++i) h[i] = __float2half_rn(v[i]);
+    r.p = static_cast<__half*>((r.pack_only ? raw_only : weights).alloc(h.size() * 2));
+    if (!r.p || cudaMemcpy(r.p, h.data(), h.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) {
+        b2_set_error("derived parameter '%s': upload failed", name.c_str());
+        return -1;
+    }
+    if (shape.size() == 1)
+        for (auto x : h) r.host.push_back(__half2float(x));
+    raw[name] = std::move(r);
+    return 0;
+}
+
+// fp32 device constant vector (cached with the other fp32 vectors)
+const float* b2sd_engine::const_vec(const std::string& name, const std::vector<float>& v) {
+    auto it = fvec.find(name);
+    if (it != fvec.end()) return it->second;
+    float* d = static_cast<float*>(weights.alloc(v.size() * sizeof(float)));
+    if (!d || cudaMemcpy(d, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
+    fvec[name] = d;
+    fvec_bytes[name] = v.size() * sizeof(float);
+    return d;
+}
+
+// Mid-block Attention(heads=1, dim_head=C, residual_connection=True, bias=True, upcast_softmax=True): GroupNorm (eps 1e-6, no
+// SiLU) -> one [q | k | v] GEMM with bias, V stored transposed -> single-head attention (attn_d512_kernel) -> to_out.0 + x.
+int b2sd_engine::build_vae_attention(const std::string& p, const Act& x, Act* out, cudaStream_t s) {
+    cur = p;
+    allow_swap = false;
+    const int C = x.c, M = x.n * x.h * x.w;
+    if (x.n != 1 || C != 512) {
+        b2_set_error("vae attention %s: single image with 512 channels expected (got %d x %d)", p.c_str(), x.n, C);
+        return -1;
+    }
+    Act n = new_act(1, x.h, x.w, C);
+    TRY(add_groupnorm(x, nullptr, p + "group_norm", n, 1e-6f, 0));
+    std::vector<int> id(C);
+    for (int i = 0; i < C; ++i) id[i] = i;
+    __half* w = pack_rows(p + "qkv", {{p + "to_q.weight", id}, {p + "to_k.weight", id}, {p + "to_v.weight", id}}, C, s);
+    if (!w) return -1;
+    const float* bias = fvec.count(p + "qkv.bias") ? fvec[p + "qkv.bias"] : nullptr;
+    if (!bias) {
+        std::vector<float> b;
+        for (const char* t : {"to_q.bias", "to_k.bias", "to_v.bias"}) {
+            const Raw* r = get(p + t);
+            if (!r) return -1;
+            b.insert(b.end(), r->host.begin(), r->host.end());
+        }
+        bias = const_vec(p + "qkv.bias", b);
+        if (!bias) return -1;
+    }
+    Act qk = new_act(1, 1, M, 2 * C);
+    const long vt_ld = (M + 7) / 8 * 8;
+    __half* vt = static_cast<__half*>(prog.alloc((size_t)C * vt_ld * 2));
+    if (!vt || !qk.p) return -1;
+    cudaMemsetAsync(vt, 0, (size_t)C * vt_ld * 2, s);   // pad columns must stay finite
+    LinExtra ex; ex.out2 = vt; ex.ld2 = (int)vt_ld; ex.col2 = 2 * C;
+    TRY(add_linear(prog_frame, tokens(n), w, 3 * C, C, bias, qk.p, 2 * C, nullptr, 0, 0, -1, &ex));
+    Act ao = new_act(1, x.h, x.w, C);
+    AttnDesc a{};
+    a.q = qk.p; a.ldq = 2 * C;
+    a.k = qk.p + C; a.ldk = 2 * C; a.k_bstride = 0; a.k_rows = M;
+    a.vt = vt; a.ldvt = (int)vt_ld; a.vt_bstride = 0; a.vt_cols = M;
+    a.out = ao.p; a.ldo = C;
+    a.nb = 1; a.heads = 1; a.sq = M; a.skv = M; a.d_real = C; a.dp = C;
+    AttnPlan plan;
+    TRY(attn_plan(a, &plan));
+    ++launches;
+    prog_frame.push_back(Op([plan](cudaStream_t st) { return attn_launch(plan, st); }, "attn " + p, 4.0 * (double)M * M * C));
+    const Raw* wo = get(p + "to_out.0.weight");
+    if (!wo) return -1;
+    *out = new_act(1, x.h, x.w, C);
+    return add_linear(prog_frame, tokens(ao), wo->p, C, C, vec({p + "to_out.0.bias"}), out->p, C, x.p, x.ld);
+}
+
+// Encoder: conv_in (reads the caller's frame: `head`), 4 DownEncoderBlock2D (2 resnets, Downsample2D(padding=0) after levels
+// 0-2), mid block, GroupNorm + SiLU.  Returns that last activation and the key of the latent conv that follows it:
+// conv_out composed with rows 0-3 of quant_conv (the distribution's mean), an exact folding (a 1x1 conv after a conv).
+// The image normalisation 2x - 1 = (2/255)(u8 - 127.5) is the smallconv offset input mode with 2/255 folded into the
+// weights: zero padding then applies to 2x - 1, as in the model (a folded bias would be wrong on the border pixels).
+int b2sd_engine::build_kl_encoder(Act* out, std::string* latent_conv, cudaStream_t s) {
+    const std::string P = "vae.encoder.";
+    const int H = cfg.height, W = cfg.width;
+    allow_swap = false;
+    cur = P + "conv_in";
+    const std::string win = P + "conv_in.weight*2/255";
+    if (!has(win)) {
+        const Raw* r = get(P + "conv_in.weight");
+        if (!r) return -1;
+        std::vector<float> v = host_copy(P + "conv_in.weight");
+        if (v.empty()) return -1;
+        for (auto& x : v) x *= 2.0f / 255.0f;
+        TRY(derive(win, r->shape, v));
+    }
+    const Raw* rin = get(win);
+    if (!rin) return -1;
+    const int c0 = (int)rin->shape[0];
+    Act e = new_act(1, H, W, c0);
+    head = SmallConvArgs{};
+    head.wt = small_w(win, s);
+    head.bias = vec({P + "conv_in.bias"});
+    head.in_off = const_vec("vae:in_off", {127.5f, 127.5f, 127.5f});
+    if (!head.wt || !head.bias || !head.in_off || !e.p) return -1;
+    head.y = e.p; head.ldy = e.ld; head.nb = 1; head.h = H; head.w_ = W; head.cin = 3; head.cout = c0;
+    head.flags = SC_IN_U8 | SC_IN_OFFSET;
+    ++launches;
+    for (int i = 0; i < 4; ++i) {
+        const std::string bp = P + "down_blocks." + std::to_string(i);
+        for (int j = 0; j < 2; ++j) {
+            const Raw* w1 = get(bp + ".resnets." + std::to_string(j) + ".conv1.weight");
+            if (!w1) return -1;
+            Act o;
+            TRY(build_resnet(bp + ".resnets." + std::to_string(j) + ".", e, nullptr, (int)w1->shape[0], nullptr, &o, s, 1e-6f));
+            e = o;
+        }
+        if (i < 3) {
+            Act o = new_act(1, e.h / 2, e.w / 2, e.c);
+            TRY(add_conv(prog_frame, e, bp + ".downsamplers.0.conv.weight", bp + ".downsamplers.0.conv.bias", 9, 2, o, IG_PAD0,
+                         nullptr, s));
+            e = o;
+        }
+        taps["vae.enc.down." + std::to_string(i)] = e;
+    }
+    {
+        Act o;
+        TRY(build_resnet(P + "mid_block.resnets.0.", e, nullptr, e.c, nullptr, &o, s, 1e-6f)); e = o;
+        TRY(build_vae_attention(P + "mid_block.attentions.0.", e, &o, s)); e = o;
+        TRY(build_resnet(P + "mid_block.resnets.1.", e, nullptr, e.c, nullptr, &o, s, 1e-6f)); e = o;
+        taps["vae.enc.mid"] = e;
+    }
+    *out = new_act(1, e.h, e.w, e.c);
+    TRY(add_groupnorm(e, nullptr, P + "conv_norm_out", *out, 1e-6f, 1));
+    *latent_conv = P + "conv_out+quant_conv";
+    if (!has(*latent_conv + ".weight")) {
+        const Raw* wc = get(P + "conv_out.weight");
+        const Raw* wq = get("vae.quant_conv.weight");
+        if (!wc || !wq) return -1;
+        const int co = (int)wc->shape[0], ci = (int)wc->shape[1];
+        if (co != 8 || wq->numel() != 64) {
+            b2_set_error("vae: conv_out has %d channels and quant_conv %ld weights (8 and 8x8 expected)", co, wq->numel());
+            return -1;
+        }
+        std::vector<float> w = host_copy(P + "conv_out.weight"), b = host_copy(P + "conv_out.bias"), q = host_copy("vae.quant_conv.weight"),
+                           qb = host_copy("vae.quant_conv.bias");
+        if (w.empty() || b.empty() || q.empty() || qb.empty()) return -1;
+        const size_t per = (size_t)ci * 9;
+        std::vector<float> wf(4 * per, 0.f), bf(4, 0.f);
+        for (int o = 0; o < 4; ++o) {
+            double bo = qb[o];
+            for (int j = 0; j < 8; ++j) {
+                const float qv = q[o * 8 + j];
+                for (size_t k = 0; k < per; ++k) wf[o * per + k] += qv * w[j * per + k];
+                bo += (double)qv * b[j];
+            }
+            bf[o] = (float)bo;
+        }
+        TRY(derive(*latent_conv + ".weight", {4, ci, 3, 3}, wf));
+        TRY(derive(*latent_conv + ".bias", {4}, bf));
+    }
+    return 0;
+}
+
+// Decoder on x0: post_quant_conv and 1/scaling_factor folded into conv_in's weights (exact: 1x1 before a conv).  post_quant_conv's
+// bias is NOT folded into conv_in's bias -- conv_in zero-pads post_quant_conv's output, so its contribution differs on the
+// border: it is computed once per program as conv_in(constant bias image) + conv_in.bias (same kernel, same zero padding) and
+// added as the residual of the frame's conv_in.  Then the mid block, 4 UpDecoderBlock2D (3 resnets, nearest 2x + conv after
+// levels 0-2), GroupNorm + SiLU, conv_out.  `image` holds the decoded image on the [0, 1] scale, (y + 1) / 2 (conv_out's epilogue:
+// 0.5 * (acc + bias + 1)), which is what the TAESD decoder's last conv produces: the tails (post_u8 / post_f16) are shared.
+int b2sd_engine::build_kl_decoder(const Act& x0, cudaStream_t s) {
+    const std::string P = "vae.decoder.";
+    allow_swap = false;
+    cur = P + "conv_in";
+    const float sf = cfg.vae_scaling_factor > 0.f ? cfg.vae_scaling_factor : 0.18215f;
+    const std::string wkey = P + "conv_in+post_quant_conv.weight";
+    if (!has(wkey)) {
+        const Raw* wc = get(P + "conv_in.weight");
+        const Raw* wq = get("vae.post_quant_conv.weight");
+        if (!wc || !wq) return -1;
+        const int co = (int)wc->shape[0];
+        if (wc->shape[1] != 4 || wq->numel() != 16) {
+            b2_set_error("vae: decoder conv_in takes %ld channels and post_quant_conv has %ld weights (4 and 4x4 expected)",
+                         (long)wc->shape[1], wq->numel());
+            return -1;
+        }
+        std::vector<float> w = host_copy(P + "conv_in.weight"), q = host_copy("vae.post_quant_conv.weight");
+        if (w.empty() || q.empty()) return -1;
+        std::vector<float> wf((size_t)co * 4 * 9, 0.f);
+        for (int o = 0; o < co; ++o)
+            for (int j = 0; j < 4; ++j)
+                for (int t = 0; t < 9; ++t) {
+                    double acc = 0.0;
+                    for (int i = 0; i < 4; ++i) acc += (double)w[((size_t)o * 4 + i) * 9 + t] * q[i * 4 + j];
+                    wf[((size_t)o * 4 + j) * 9 + t] = (float)(acc / sf);
+                }
+        TRY(derive(wkey, {co, 4, 3, 3}, wf));
+    }
+    const Raw* rw = get(wkey);
+    const Raw* pqb = get("vae.post_quant_conv.bias");
+    if (!rw || !pqb || pqb->host.size() != 4) {
+        if (rw && pqb) b2_set_error("vae: post_quant_conv.bias must have 4 elements");
+        return -1;
+    }
+    const int cm = (int)rw->shape[0];
+    Act bmap = new_act(1, lh, lw, cm), cst = new_act(1, lh, lw, 4), h = new_act(1, lh, lw, cm);
+    if (!bmap.p || !cst.p || !h.p) return -1;
+    {
+        std::vector<__half> c((size_t)lh * lw * 4);
+        for (size_t i = 0; i < c.size(); ++i) c[i] = __float2half_rn(pqb->host[i % 4]);
+        CUDA_OK(cudaMemcpyAsync(cst.p, c.data(), c.size() * 2, cudaMemcpyHostToDevice, s));
+        SmallConvArgs m{};
+        m.x = cst.p; m.wt = small_w(P + "conv_in.weight", s); m.bias = vec({P + "conv_in.bias"});
+        if (!m.wt || !m.bias) return -1;
+        m.y = bmap.p; m.ldy = cm; m.nb = 1; m.h = lh; m.w_ = lw; m.cin = 4; m.cout = cm; m.in_h = lh; m.in_w = lw;
+        TRY(smallconv_launch(m, s));
+        CUDA_OK(cudaStreamSynchronize(s));   // the host constant image dies with this scope
+    }
+    {
+        SmallConvArgs a{};
+        a.x = x0.p; a.wt = small_w(wkey, s); a.bias = nullptr;
+        if (!a.wt) return -1;
+        a.y = h.p; a.ldy = h.ld; a.nb = 1; a.h = lh; a.w_ = lw; a.cin = 4; a.cout = cm; a.in_h = lh; a.in_w = lw;
+        a.res = bmap.p; a.ldr = bmap.ld; a.res_bstride = 0;
+        ++launches;
+        prog_frame.push_back(Op([a](cudaStream_t st) { return smallconv_launch(a, st); }, "smallconv vae.decoder.conv_in"));
+    }
+    {
+        Act o;
+        TRY(build_resnet(P + "mid_block.resnets.0.", h, nullptr, h.c, nullptr, &o, s, 1e-6f)); h = o;
+        TRY(build_vae_attention(P + "mid_block.attentions.0.", h, &o, s)); h = o;
+        TRY(build_resnet(P + "mid_block.resnets.1.", h, nullptr, h.c, nullptr, &o, s, 1e-6f)); h = o;
+        taps["vae.dec.mid"] = h;
+    }
+    for (int i = 0; i < 4; ++i) {
+        const std::string bp = P + "up_blocks." + std::to_string(i);
+        for (int j = 0; j < 3; ++j) {
+            const Raw* w1 = get(bp + ".resnets." + std::to_string(j) + ".conv1.weight");
+            if (!w1) return -1;
+            Act o;
+            TRY(build_resnet(bp + ".resnets." + std::to_string(j) + ".", h, nullptr, (int)w1->shape[0], nullptr, &o, s, 1e-6f));
+            h = o;
+        }
+        if (i < 3) {
+            Act up = new_act(1, h.h * 2, h.w * 2, h.c);
+            const Act hin = h;
+            ++launches;
+            prog_frame.push_back(Op([hin, up](cudaStream_t st) { return upsample2x_launch(hin.p, up.p, hin.n, hin.h, hin.w, hin.c, st); }, "upsample2x"));
+            Act o = new_act(1, up.h, up.w, h.c);
+            TRY(add_conv(prog_frame, up, bp + ".upsamplers.0.conv.weight", bp + ".upsamplers.0.conv.bias", 9, 1, o, 0, nullptr, s));
+            h = o;
+        }
+        taps["vae.dec.up." + std::to_string(i)] = h;
+    }
+    Act nout = new_act(1, h.h, h.w, h.c);
+    TRY(add_groupnorm(h, nullptr, P + "conv_norm_out", nout, 1e-6f, 1));
+    const std::string bkey = P + "conv_out.bias+1";
+    if (!has(bkey)) {
+        const Raw* b = get(P + "conv_out.bias");
+        if (!b) return -1;
+        std::vector<float> v(b->host);
+        for (auto& x : v) x += 1.f;
+        TRY(derive(bkey, b->shape, v));
+    }
+    image = new_act(1, cfg.height, cfg.width, 3, 8);
+    return add_conv(prog_frame, nout, P + "conv_out.weight", bkey, 9, 1, image, 0, nullptr, s, 0.5f);
+}
+
 int b2sd_engine::build_program(cudaStream_t s) {
     prog.reset();
     prog_frame.clear(); prog_prompt.clear(); prog_time.clear();
@@ -1132,8 +1444,15 @@ int b2sd_engine::build_program(cudaStream_t s) {
     }
 
     allow_swap = false;
+    const bool kl = cfg.vae == B2SD_VAE_KL;
+    Act e;
+    std::string latent_conv;   // the encoder's last conv (its epilogue adds the noise)
+    int li = 1;
+    if (kl) {
+        TRY(build_kl_encoder(&e, &latent_conv, s));
+    } else {
     // ================= TAESD encoder (EncoderTiny) =================
-    Act e = new_act(1, H, W, 64);
+    e = new_act(1, H, W, 64);
     {
         head = SmallConvArgs{};
         head.wt = small_w("vae.encoder.layers.0.weight", s);
@@ -1144,7 +1463,6 @@ int b2sd_engine::build_program(cudaStream_t s) {
         if (!head.bias) return -1;
         ++launches;
     }
-    int li = 1;
     const int enc_blocks[4] = {1, 3, 3, 3};
     for (int st = 0; st < 4; ++st) {
         if (st > 0) {
@@ -1160,17 +1478,21 @@ int b2sd_engine::build_program(cudaStream_t s) {
             ++li;
         }
     }
+    latent_conv = "vae.encoder.layers." + std::to_string(li);
+    }
     Act cond;   // ControlNet conditioning embedding of this frame's control image: batch 1, latent resolution, C0 channels
     if (cfg.controlnet) TRY(build_cond_embedding(&cond, s));
     {
         // latent head + StreamDiffusion.encode_image add-noise: x_t = alpha0 * z + beta0 * init_noise[0]
+        // (AutoencoderKL: z = scaling_factor * mean, the scale applied with alpha0 in the epilogue)
         Act xt;  // slot 0 of the UNet input batch
         xt.p = x_in.p; xt.n = 1; xt.h = lh; xt.w = lw; xt.c = 4; xt.ld = 4;
         Act nz = xt;
         nz.p = noise;
-        const std::string k = "vae.encoder.layers." + std::to_string(li);
+        const float zscale = kl ? (cfg.vae_scaling_factor > 0.f ? cfg.vae_scaling_factor : 0.18215f) : 1.f;
         idx_enc_end = prog_frame.size();   // everything before this conv only touches this engine's own activations
-        TRY(add_conv(prog_frame, e, k + ".weight", k + ".bias", 9, 1, xt, 0, &nz, s, coef_host[0][0], coef_host[1][0]));
+        TRY(add_conv(prog_frame, e, latent_conv + ".weight", latent_conv + ".bias", 9, 1, xt, 0, &nz, s, coef_host[0][0] * zscale,
+                     coef_host[1][0]));
         taps["x_t"] = xt;
     }
     taps["unet_in"] = x_in;
@@ -1265,6 +1587,9 @@ int b2sd_engine::build_program(cudaStream_t s) {
     }
     taps["x0"] = x0;
     allow_swap = false;
+    if (kl) {
+        TRY(build_kl_decoder(x0, s));
+    } else {
     // ================= TAESD decoder (DecoderTiny) =================
     Act dcur = new_act(1, lh, lw, 64);
     {
@@ -1303,6 +1628,7 @@ int b2sd_engine::build_program(cudaStream_t s) {
             TRY(add_conv(prog_frame, dcur, k + ".weight", k + ".bias", 9, 1, image, 0, nullptr, s));
         }
     }
+    }
     taps["image"] = image;
     ++launches;  // post_u8 tail
     if (ln_stats_used) {
@@ -1336,6 +1662,8 @@ int b2sd_create_lane(b2sd_handle parent, const b2sd_config* cfg, b2sd_handle* ou
     b2sd_config c = cfg ? *cfg : parent->cfg;
     c.controlnet = parent->cfg.controlnet;   // a lane runs the parent's networks
     c.control_processor = parent->cfg.control_processor;
+    c.vae = parent->cfg.vae;
+    c.vae_scaling_factor = parent->cfg.vae_scaling_factor;
     for (int i = 0; i < 4; ++i)
         if (c.block_out_channels[i] != parent->cfg.block_out_channels[i] || c.heads[i] != parent->cfg.heads[i] ||
             c.down_attn[i] != parent->cfg.down_attn[i]) {
@@ -1373,6 +1701,14 @@ static int create_engine(const b2sd_config* cfg, std::shared_ptr<WeightStore> st
     }
     if (cfg->control_processor != B2SD_CONTROL_FRAME && (cfg->control_processor != B2SD_CONTROL_HED || !cfg->controlnet)) {
         b2_set_error("b2sd_create: control_processor must be 0 (the frame) or 1 (HED, with a ControlNet) (got %d)", cfg->control_processor);
+        return -1;
+    }
+    if (cfg->vae != B2SD_VAE_TINY && cfg->vae != B2SD_VAE_KL) {
+        b2_set_error("b2sd_create: vae must be 0 (TAESD) or 1 (AutoencoderKL) (got %d)", cfg->vae);
+        return -1;
+    }
+    if (!(cfg->vae_scaling_factor >= 0.f)) {
+        b2_set_error("b2sd_create: vae_scaling_factor must be >= 0 (0 = 0.18215)");
         return -1;
     }
     int dev = 0;
@@ -1458,6 +1794,7 @@ int b2sd_load_tensor(b2sd_handle h, const char* key, const void* ptr, int dtype,
         h->packed.clear(); h->packed_bytes.clear();
         h->fvec.clear(); h->fvec_bytes.clear();
         if (old->second.shape == r.shape) r.p = old->second.p;
+        for (auto it = h->raw.begin(); it != h->raw.end();) it = it->second.derived ? h->raw.erase(it) : std::next(it);
     }
     if (!r.p) r.p = static_cast<__half*>((r.pack_only ? h->raw_only : h->weights).alloc((size_t)n * 2));
     if (!r.p) {
@@ -1592,7 +1929,7 @@ int b2sd_export_packed(b2sd_handle h, const char* path) {
     }
     BlobWriter w{f};
     w.put("B2SDPACK", 8);
-    w.pod((uint32_t)2);   // 2: b2sd_config carries `controlnet` / `control_processor` (version 1 blobs still load)
+    w.pod((uint32_t)3);   // 3: b2sd_config carries `vae` / `vae_scaling_factor` (2: up to `control_processor`; 1 and 2 still load)
     b2sd_config cfg = h->cfg;
     cfg.batch = 0; cfg.height = 0; cfg.width = 0; cfg.use_cuda_graph = 0; cfg.do_add_noise = 0;   // the blob is independent of these
     w.pod(cfg);
@@ -1649,13 +1986,16 @@ int b2sd_import_packed(b2sd_handle h, const char* path) {
     char magic[8];
     rd.get(magic, 8);
     const uint32_t version = rd.pod<uint32_t>();
-    // version 1 blobs predate the ControlNet fields at the end of b2sd_config: they hold no ControlNet (both fields 0)
+    // version 1 blobs predate the ControlNet fields at the end of b2sd_config: they hold no ControlNet (both fields 0);
+    // version 2 blobs end b2sd_config before `vae`: they hold TAESD (vae = 0)
     b2sd_config cfg{};
     if (version == 1) rd.get(&cfg, offsetof(b2sd_config, controlnet));
+    else if (version == 2) rd.get(&cfg, offsetof(b2sd_config, vae));
     else cfg = rd.pod<b2sd_config>();
-    bool same = rd.ok && memcmp(magic, "B2SDPACK", 8) == 0 && (version == 1 || version == 2) && cfg.cross_attention_dim == h->cfg.cross_attention_dim &&
+    bool same = rd.ok && memcmp(magic, "B2SDPACK", 8) == 0 && version >= 1 && version <= 3 && cfg.cross_attention_dim == h->cfg.cross_attention_dim &&
                 cfg.layers_per_block == h->cfg.layers_per_block && cfg.norm_groups == h->cfg.norm_groups && cfg.ctx_tokens == h->cfg.ctx_tokens &&
-                cfg.controlnet == h->cfg.controlnet && cfg.control_processor == h->cfg.control_processor;
+                cfg.controlnet == h->cfg.controlnet && cfg.control_processor == h->cfg.control_processor && cfg.vae == h->cfg.vae &&
+                (cfg.vae != B2SD_VAE_KL || cfg.vae_scaling_factor == h->cfg.vae_scaling_factor);
     for (int i = 0; i < 4 && same; ++i)
         same = cfg.block_out_channels[i] == h->cfg.block_out_channels[i] && cfg.heads[i] == h->cfg.heads[i] && cfg.down_attn[i] == h->cfg.down_attn[i];
     if (!same) {
@@ -1750,14 +2090,15 @@ int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     SmallConvArgs a = h->head;
     a.x = frame_in; a.in_h = in_h; a.in_w = in_w;
-    a.flags = in_kind == B2SD_IN_U8_NHWC ? SC_IN_U8 : (in_kind == B2SD_IN_F32_NCHW ? SC_IN_F32_NCHW : SC_IN_F16_NCHW);
+    const int in_flags = in_kind == B2SD_IN_U8_NHWC ? SC_IN_U8 : (in_kind == B2SD_IN_F32_NCHW ? SC_IN_F32_NCHW : SC_IN_F16_NCHW);
+    a.flags = in_flags | (h->head.flags & SC_IN_OFFSET);   // AutoencoderKL: 2x - 1 as the offset input mode
     TRY(smallconv_launch(a, s));
     if (h->cfg.controlnet) {   // the control image is the frame itself in [0, 1], at the engine's size (same nearest resize)
         // the control image is the frame itself in [0, 1] at the engine's size (same nearest resize), or HED's edge map, whose
         // first conv reads the frame here and whose remaining layers run in stage 1
         const bool hed = h->cfg.control_processor == B2SD_CONTROL_HED;
         SmallConvArgs c = hed ? h->hed_head : h->cn_head;
-        c.x = frame_in; c.in_h = in_h; c.in_w = in_w; c.flags = a.flags | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
+        c.x = frame_in; c.in_h = in_h; c.in_w = in_w; c.flags = in_flags | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
         TRY(smallconv_launch(c, s));
     }
     if (h->group) {
@@ -1850,7 +2191,7 @@ int b2sd_profile(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* 
     for (auto& e : ev) CUDA_OK(cudaEventCreate(&e));
     std::vector<double> acc(nops, 0.0);
     SmallConvArgs a = h->head;
-    a.x = frame_in; a.in_h = in_h; a.in_w = in_w; a.flags = SC_IN_U8;
+    a.x = frame_in; a.in_h = in_h; a.in_w = in_w; a.flags = SC_IN_U8 | (h->head.flags & SC_IN_OFFSET);
     for (int it = 0; it < iters + 1; ++it) {  // first iteration is a warm-up
         CUDA_OK(cudaEventRecord(ev[0], s));
         TRY(smallconv_launch(a, s));
@@ -1881,7 +2222,7 @@ int b2sd_profile(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* 
     std::string js = "[";
     char tmp[512];
     for (size_t k = 0; k < nops; ++k) {
-        const char* nm = k == 0 ? "smallconv head (u8 frame -> 64ch)" : (k == nops - 1 ? "post_u8 tail" : h->prog_frame[k - 1].name.c_str());
+        const char* nm = k == 0 ? "smallconv head (u8 frame -> encoder conv_in)" : (k == nops - 1 ? "post_u8 tail" : h->prog_frame[k - 1].name.c_str());
         const double fl = (k == 0 || k == nops - 1) ? 0.0 : h->prog_frame[k - 1].flops;
         snprintf(tmp, sizeof(tmp), "%s{\"name\": \"%s\", \"ms\": %.6f, \"flops\": %.0f}", k ? ", " : "", nm, acc[k] / iters, fl);
         js += tmp;

@@ -156,7 +156,7 @@ __device__ __forceinline__ void splitk_sum16(uint32_t stg_local, int cc, int row
 // with the same weight tile: each CTA loads its own 128 pixel rows and HALF of the weight rows, multicast into both CTAs'
 // shared memory, so each SM fetches half of the weight bytes from L2.  A ring slot is refilled only when the warps of BOTH
 // CTAs have released it (every consumer warp arrives on its own and on the peer's empty barrier).
-template <int BN, bool PAIR, bool SILU>
+template <int BN, bool PAIR, bool SILU, bool PAD0 = false>
 __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -228,9 +228,9 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
                     uint8_t* sa = smem + (size_t)stage * stage_bytes;
                     uint8_t* sb = sa + A_BYTES;
                     int dy = 0, dx = 0;
-                    if (p.seg_ntap[seg] == 9) {
-                        dy = tap / 3 - 1;
-                        dx = tap % 3 - 1;
+                    if (p.seg_ntap[seg] == 9) {   // PAD0: tap origin 0 (input coord = stride * out + tap)
+                        dy = tap / 3 - (PAD0 ? 0 : 1);
+                        dx = tap % 3 - (PAD0 ? 0 : 1);
                     }
                     // normal: pixels -> A (M side), weights -> B.  swapped: weights (128 output channels) -> A, pixels -> B
                     tma_load_4d(p.swap ? sb : sa, &p.tmA[seg], &full_bar[stage], p.seg_c0[seg] + cb * IG_BK,
@@ -436,6 +436,10 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
 
 template <int BN, bool PAIR, bool SILU = false>
 __global__ void __launch_bounds__(IG_THREADS, 1) igemm_kernel(const __grid_constant__ IgemmParams p) { igemm_body<BN, PAIR, SILU>(p); }
+// IG_PAD0: 3x3 taps read input (stride * out + tap), i.e. F.pad(x, (0, 1, 0, 1)) before an unpadded conv -- the AutoencoderKL
+// Downsample2D(padding=0).  Its own instantiations (single CTAs, N tiles 64 / 128 / 256), so every other kernel is unchanged.
+template <int BN>
+__global__ void __launch_bounds__(IG_THREADS, 1) igemm_pad0_kernel(const __grid_constant__ IgemmParams p) { igemm_body<BN, false, false, true>(p); }
 
 using IgemmFn = void (*)(IgemmParams);
 // every N tile the planner can produce (multiples of 16 up to 256); CTA pairs need BN % 32 == 0.  At 168 registers the widest
@@ -453,7 +457,16 @@ static IgemmFn igemm_fn(int bn) {
 }
 // IG_SILU epilogues (the ControlNet conditioning embedding: N = 16 / 32 / 96 / 256, single CTAs, N tiles <= 128) are separate
 // instantiations, so the SiLU code costs the other kernels no registers (a 256-wide SiLU tile would spill)
-static IgemmFn igemm_select(int bn, bool pair, bool silu) {
+static IgemmFn igemm_select(int bn, bool pair, bool silu, bool pad0 = false) {
+    if (pad0) {
+        if (pair || silu) return nullptr;
+        switch (bn) {
+            case 64: return igemm_pad0_kernel<64>;
+            case 128: return igemm_pad0_kernel<128>;
+            case 256: return igemm_pad0_kernel<256>;
+            default: return nullptr;
+        }
+    }
     if (!silu) return pair ? igemm_fn<true>(bn) : igemm_fn<false>(bn);
     if (pair) return nullptr;
     switch (bn) {
@@ -536,8 +549,8 @@ size_t igemm_partial_floats(int splits, long rows_total, int n_valid) {
 // Swapped orientation plan: output channels on the M side (128 per CTA), a tile of BN pixels on the N side.
 static int plan_swap(const IgemmDesc& d, IgemmPlan* plan) {
     IgemmParams& p = plan->p;
-    if ((d.epi.flags & IG_GEGLU) || d.nseg < 1 || d.nseg > IG_MAX_SRC || d.epi.rowstat_out || d.epi.colsum || d.epi.out2) {
-        b2_set_error("igemm(swap): unsupported (GEGLU / LayerNorm fold / row statistics / transposed V / nseg %d)", d.nseg);
+    if ((d.epi.flags & (IG_GEGLU | IG_PAD0)) || d.nseg < 1 || d.nseg > IG_MAX_SRC || d.epi.rowstat_out || d.epi.colsum || d.epi.out2) {
+        b2_set_error("igemm(swap): unsupported (GEGLU / tap origin 0 / LayerNorm fold / row statistics / transposed V / nseg %d)", d.nseg);
         return -1;
     }
     int BN = d.BN;
@@ -652,9 +665,9 @@ int b2_device_sms() {
 
 // CTAs of the kernel for this tile that one SM holds at once as far as registers and threads allow (the plan sizes the
 // shared memory).  Dry runs do not touch the device: they assume the one CTA per SM that 288 threads at 168 registers allow.
-static int igemm_ctas_per_sm(int bn, bool pair, bool silu) {
+static int igemm_ctas_per_sm(int bn, bool pair, bool silu, bool pad0) {
     if (g_plan_dry) return 1;
-    IgemmFn fn = igemm_select(bn, pair, silu);
+    IgemmFn fn = igemm_select(bn, pair, silu, pad0);
     int n = 0;
     if (fn && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, IG_THREADS, 0) == cudaSuccess && n > 0) return n;
     cudaGetLastError();
@@ -688,6 +701,10 @@ int igemm_plan(const IgemmDesc& d, IgemmPlan* plan) {
     const bool pair = d.pair != 0;
     if ((d.epi.flags & IG_SILU) && !igemm_select(BN, pair, true)) {
         b2_set_error("igemm: no SiLU-epilogue kernel for BN %d%s (16/32/64/128, single CTAs)", BN, pair ? " (CTA pair)" : "");
+        return -1;
+    }
+    if ((d.epi.flags & IG_PAD0) && !igemm_select(BN, pair, (d.epi.flags & IG_SILU) != 0, true)) {
+        b2_set_error("igemm: no tap-origin-0 kernel for BN %d%s (64/128/256, single CTAs, no SiLU)", BN, pair ? " (CTA pair)" : "");
         return -1;
     }
     if (pair && BN % 32 != 0) {
@@ -790,7 +807,7 @@ int igemm_plan(const IgemmDesc& d, IgemmPlan* plan) {
     // The mainloop is TMA-latency bound: throughput per SM = bytes in flight / latency.  When registers admit only one CTA per
     // SM (the case of this kernel: 288 threads at up to 168 registers) the ring takes (nearly) all the shared memory; only
     // when two could be resident AND the launch needs them is the ring halved so that they fit.
-    const int per_sm = igemm_ctas_per_sm(BN, pair, (d.epi.flags & IG_SILU) != 0);
+    const int per_sm = igemm_ctas_per_sm(BN, pair, (d.epi.flags & IG_SILU) != 0, (d.epi.flags & IG_PAD0) != 0);
     const long resident = (long)per_sm * b2_device_sms();   // CTAs the GPU runs at once
     static const char* pc_env = getenv("B2_PERSIST_CTAS");   // tuning: CTAs of a persistent launch (default: one resident wave)
     const long persist_ctas = pc_env ? atoi(pc_env) : resident;
@@ -855,8 +872,8 @@ int igemm_init() {
     static bool attr_set = false;
     if (!attr_set) {
         for (int bn = 16; bn <= 256; bn += 16) {
-            for (int pair = 0; pair < 3; ++pair) {   // single CTAs, CTA pairs, single CTAs with the SiLU epilogue
-                IgemmFn fn = igemm_select(bn, pair == 1, pair == 2);
+            for (int pair = 0; pair < 4; ++pair) {   // single CTAs, CTA pairs, single CTAs with the SiLU epilogue, tap origin 0
+                IgemmFn fn = igemm_select(bn, pair == 1, pair == 2, pair == 3);
                 if (!fn) continue;
                 cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
                 if (e != cudaSuccess) {
@@ -874,10 +891,10 @@ int igemm_init() {
 int igemm_launch(const IgemmPlan& plan, cudaStream_t stream) {
     if (igemm_init()) return -1;
     const int cz = plan.splits > 1 ? plan.splits : 1;
-    IgemmFn fn = igemm_select(plan.p.BN, plan.pair, (plan.p.epi.flags & IG_SILU) != 0);
+    IgemmFn fn = igemm_select(plan.p.BN, plan.pair, (plan.p.epi.flags & IG_SILU) != 0, (plan.p.epi.flags & IG_PAD0) != 0);
     if (!fn) {
-        b2_set_error("igemm launch: no kernel for BN %d%s%s", plan.p.BN, plan.pair ? " (CTA pair)" : "",
-                     (plan.p.epi.flags & IG_SILU) ? " with the SiLU epilogue" : "");
+        b2_set_error("igemm launch: no kernel for BN %d%s%s%s", plan.p.BN, plan.pair ? " (CTA pair)" : "",
+                     (plan.p.epi.flags & IG_SILU) ? " with the SiLU epilogue" : "", (plan.p.epi.flags & IG_PAD0) ? " with tap origin 0" : "");
         return -1;
     }
     cudaError_t e = plan.pair ? launch_kc(fn, plan.grid, dim3(IG_THREADS), plan.smem, stream, 2, cz, plan.p)

@@ -27,6 +27,7 @@ enum : int {
     IG_GEGLU = 2,   // tile columns [0,BN/2) = value, [BN/2,BN) = gate; out = v * gelu_erf(g)
     IG_SPLITK = 4,  // set by the planner: K is split over a thread-block cluster, partial tiles are reduced through DSMEM
     IG_SILU = 8,    // x * sigmoid(x) after bias/residual (ControlNet conditioning embedding)
+    IG_PAD0 = 16,   // 3x3 taps start at the output pixel (input coord = stride * out + tap; zero row/column only at the far edge)
 };
 
 struct IgEpilogue {
@@ -71,7 +72,7 @@ struct IgemmParams {
     int tw, th, tn;               // output tile = tn images x th rows x tw cols  (<= 128 pixels)
     int tiles_w, tiles_h, tiles_n;
     int Wo, Ho, Nb;
-    int stride;                   // input coord = stride * out + tap - 1
+    int stride;                   // input coord = stride * out + tap - 1 (IG_PAD0: + tap)
     int BN;                       // wgmma N (multiple of 16, <= 256)
     int num_stages;
     int acc_bufs;                 // 1, or 2 when the launch is persistent over M tiles

@@ -210,6 +210,125 @@ def taesd_param_shapes() -> Dict[str, Shape]:
     return out
 
 
+@dataclass(frozen=True)
+class VaeArch:
+    """diffusers AutoencoderKL (vae/config.json): DownEncoderBlock2D / UpDecoderBlock2D, SiLU, GroupNorm eps 1e-6."""
+    name: str
+    block_out_channels: Tuple[int, int, int, int]
+    layers_per_block: int = 2
+    latent_channels: int = 4
+    norm_groups: int = 32
+
+
+AUTOENCODER_KL = VaeArch("autoencoder-kl", (128, 256, 512, 512))          # SD-1.5, SD-2.1, SD-Turbo
+# a narrower variant for tests; its last level stays 512 wide, the width of the engine's single-head attention
+TINY_AUTOENCODER_KL = VaeArch("tiny-autoencoder-kl", (64, 128, 128, 512))
+
+
+def vae_arch_for(model_id: str) -> VaeArch:
+    return TINY_AUTOENCODER_KL if model_id.rstrip("/").rsplit("/", 1)[-1].startswith("tiny") else AUTOENCODER_KL
+
+
+def _vae_resnet(prefix: str, ci: int, co: int) -> Iterator[Tuple[str, Shape]]:
+    yield from _norm(prefix + ".norm1", ci)
+    yield from _conv(prefix + ".conv1", co, ci, 3)
+    yield from _norm(prefix + ".norm2", co)
+    yield from _conv(prefix + ".conv2", co, co, 3)
+    if ci != co:
+        yield from _conv(prefix + ".conv_shortcut", co, ci, 1)
+
+
+def _vae_mid(prefix: str, c: int) -> Iterator[Tuple[str, Shape]]:
+    yield from _vae_resnet(prefix + ".resnets.0", c, c)
+    yield from _norm(prefix + ".attentions.0.group_norm", c)
+    for proj in ("to_q", "to_k", "to_v", "to_out.0"):
+        yield from _linear(f"{prefix}.attentions.0.{proj}", c, c)
+    yield from _vae_resnet(prefix + ".resnets.1", c, c)
+
+
+def autoencoder_kl_param_shapes(v: VaeArch = AUTOENCODER_KL) -> Dict[str, Shape]:
+    """State-dict inventory of a diffusers AutoencoderKL with the current attention names (to_q / to_k / to_v / to_out.0)."""
+    ch, lat, n = v.block_out_channels, v.latent_channels, len(v.block_out_channels)
+    out: Dict[str, Shape] = {}
+    out.update(_conv("encoder.conv_in", ch[0], 3, 3))
+    cur = ch[0]
+    for i, co in enumerate(ch):
+        for j in range(v.layers_per_block):
+            out.update(_vae_resnet(f"encoder.down_blocks.{i}.resnets.{j}", cur, co))
+            cur = co
+        if i < n - 1:
+            out.update(_conv(f"encoder.down_blocks.{i}.downsamplers.0.conv", co, co, 3))
+    out.update(_vae_mid("encoder.mid_block", cur))
+    out.update(_norm("encoder.conv_norm_out", cur))
+    out.update(_conv("encoder.conv_out", 2 * lat, cur, 3))
+    out.update(_conv("quant_conv", 2 * lat, 2 * lat, 1))
+    out.update(_conv("post_quant_conv", lat, lat, 1))
+    out.update(_conv("decoder.conv_in", ch[-1], lat, 3))
+    out.update(_vae_mid("decoder.mid_block", ch[-1]))
+    cur = ch[-1]
+    for i, co in enumerate(reversed(ch)):
+        for j in range(v.layers_per_block + 1):
+            out.update(_vae_resnet(f"decoder.up_blocks.{i}.resnets.{j}", cur, co))
+            cur = co
+        if i < n - 1:
+            out.update(_conv(f"decoder.up_blocks.{i}.upsamplers.0.conv", co, co, 3))
+    out.update(_norm("decoder.conv_norm_out", cur))
+    out.update(_conv("decoder.conv_out", 3, cur, 3))
+    return out
+
+
+_LEGACY_VAE_ATTN = {"query": "to_q", "key": "to_k", "value": "to_v", "proj_attn": "to_out.0"}
+
+
+def normalize_autoencoder_kl(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+    """Current diffusers names for a state dict saved with the legacy attention names (query / key / value / proj_attn), and the
+    mid-block q / k / v / out projections as [C, C] matrices however they were stored ([C, C, 1, 1] in older checkpoints), as
+    diffusers' loader does."""
+    out: Dict[str, torch.Tensor] = {}
+    for k, t in sd.items():
+        parts = k.split(".")
+        if ".attentions." in k and len(parts) >= 2 and parts[-2] in _LEGACY_VAE_ATTN:
+            k = ".".join(parts[:-2] + [_LEGACY_VAE_ATTN[parts[-2]], parts[-1]])
+        if ".attentions." in k and k.endswith(".weight") and t.dim() == 4 and t.shape[2:] == (1, 1):
+            t = t.reshape(t.shape[0], t.shape[1])
+        out[k] = t
+    return out
+
+
+def validate_exact(sd: Dict[str, torch.Tensor], shapes: Dict[str, Shape], what: str) -> None:
+    """Every tensor of the inventory present with exactly its shape, and nothing else."""
+    missing = [k for k in shapes if k not in sd]
+    if missing:
+        raise ValueError(f"{what}: {len(missing)} missing tensors, e.g. {missing[:4]}")
+    extra = [k for k in sd if k not in shapes]
+    if extra:
+        raise ValueError(f"{what}: {len(extra)} unexpected tensors, e.g. {extra[:4]}")
+    for k, shp in shapes.items():
+        if tuple(sd[k].shape) != tuple(shp):
+            raise ValueError(f"{what}: {k} has shape {tuple(sd[k].shape)}, expected {shp}")
+
+
+def synthetic_autoencoder_kl(v: VaeArch = AUTOENCODER_KL, seed: int = 8765) -> Dict[str, torch.Tensor]:
+    """Seeded fp16 AutoencoderKL weights: fan-in scaled convs (residual branches' last layers at half gain), GroupNorm affine
+    near identity, nonzero biases everywhere (quant_conv / post_quant_conv included, so that a bias folded across a zero-padded
+    conv shows up on the border pixels), and a decoder conv_out that keeps the image mostly inside [-1, 1]."""
+    g = torch.Generator().manual_seed(seed)
+    sd: Dict[str, torch.Tensor] = {}
+    for name, shape in autoencoder_kl_param_shapes(v).items():
+        leaf = name.rsplit(".", 1)[-1]
+        if "norm" in name.rsplit(".", 2)[-2]:
+            t = 1.0 + 0.1 * torch.randn(shape, generator=g) if leaf == "weight" else 0.1 * torch.randn(shape, generator=g)
+        elif leaf == "bias":
+            t = 0.05 * torch.randn(shape, generator=g)
+        else:
+            gain = 0.5 if name.endswith(("conv2.weight", "to_out.0.weight")) else 1.0
+            if name == "decoder.conv_out.weight":
+                gain = 0.35
+            t = torch.randn(shape, generator=g) * (gain / math.sqrt(math.prod(shape[1:])))
+        sd[name] = t.to(torch.float16)
+    return sd
+
+
 def synthetic_state_dict(shapes: Dict[str, Shape], seed: int, relu_net: bool = False) -> Dict[str, torch.Tensor]:
     """Seeded fp16 weights with fan-in scaling (activations stay O(1) through the whole network); used by
     bench.py / smoke when no checkpoint exists.  Not a trained model: outputs are noise-like images.  A ControlNet's zero

@@ -62,6 +62,7 @@ class EngineConfig(C.Structure):
         ("cross_attention_dim", C.c_int), ("layers_per_block", C.c_int), ("norm_groups", C.c_int),
         ("ctx_tokens", C.c_int), ("batch", C.c_int), ("height", C.c_int), ("width", C.c_int),
         ("do_add_noise", C.c_int), ("use_cuda_graph", C.c_int), ("controlnet", C.c_int), ("control_processor", C.c_int),
+        ("vae", C.c_int), ("vae_scaling_factor", C.c_float),
     ]
 
 
@@ -70,8 +71,10 @@ OUT_U8_NCHW, OUT_F16_NCHW = 0, 1
 IG_RELU = 1
 IG_GEGLU = 2
 IG_SILU = 8
+IG_PAD0 = 16
 SC_IN_U8, SC_IN_TANH3, SC_OUT_RELU, SC_OUT_SILU, SC_IN_OFFSET = 1, 2, 4, 32, 64
 CONTROL_FRAME, CONTROL_HED = 0, 1
+VAE_TINY, VAE_KL = 0, 1
 IG_TCONV = 64
 IG_PAIR = 128
 

@@ -32,13 +32,15 @@ def igemm(srcs: Sequence[Tuple[torch.Tensor, int]], w: torch.Tensor, out: torch.
           stride: int = 1, colbias: Optional[torch.Tensor] = None, res: Optional[torch.Tensor] = None,
           acc_scale: float = 1.0, res_scale: float = 1.0, relu: bool = False, geglu: bool = False, silu: bool = False,
           bn: int = 0, splits: int = 1, n_valid: Optional[int] = None, timeline: Optional[torch.Tensor] = None, swap: bool = False,
-          tconv: bool = False, pair: bool = False,
+          tconv: bool = False, pair: bool = False, pad0: bool = False,
           rowstat_out: Optional[torch.Tensor] = None, rowstat_in: Optional[torch.Tensor] = None,
           colsum: Optional[torch.Tensor] = None, ln_c: int = 0, ln_eps: float = 1e-5,
           out2: Optional[torch.Tensor] = None, col2: int = 0) -> torch.Tensor:
-    """srcs: [(NHWC fp16 tensor, ntap)], w: packed fp16 [rows, K]; out: NHWC fp16 [nb,ho,wo,ldc>=n]."""
+    """srcs: [(NHWC fp16 tensor, ntap)], w: packed fp16 [rows, K]; out: NHWC fp16 [nb,ho,wo,ldc>=n].  pad0: 3x3 taps read input
+    (stride*out + tap), the zero padding only after the last row / column (AutoencoderKL's Downsample2D)."""
     d = _igemm_desc(srcs, w, out, stride=stride, colbias=colbias, res=res, acc_scale=acc_scale, res_scale=res_scale, relu=relu,
                     geglu=geglu, silu=silu, bn=bn, splits=splits, n_valid=n_valid, timeline=timeline, swap=swap, tconv=tconv, pair=pair,
+                    pad0=pad0,
                     rowstat_out=rowstat_out, rowstat_in=rowstat_in, colsum=colsum, ln_c=ln_c, ln_eps=ln_eps, out2=out2, col2=col2)
     capi.check(capi.lib().b2sd_op_igemm(C.byref(d), capi.current_stream_ptr()), "b2sd_op_igemm")
     return out
@@ -55,7 +57,7 @@ def igemm_engine_plan(srcs, w, out, *, autotile: int = 1, allow_swap: bool = Tru
 
 
 def _igemm_desc(srcs, w, out, *, stride=1, colbias=None, res=None, acc_scale=1.0, res_scale=1.0, relu=False, geglu=False,
-                silu=False, bn=0, splits=1, n_valid=None, timeline=None, swap=False, tconv=False, pair=False, rowstat_out=None,
+                silu=False, bn=0, splits=1, n_valid=None, timeline=None, swap=False, tconv=False, pair=False, pad0=False, rowstat_out=None,
                 rowstat_in=None, colsum=None, ln_c=0, ln_eps=1e-5, out2=None, col2=0) -> capi.IgemmDesc:
     d = capi.IgemmDesc()
     d.nseg = len(srcs)
@@ -83,7 +85,7 @@ def _igemm_desc(srcs, w, out, *, stride=1, colbias=None, res=None, acc_scale=1.0
         d.res, d.ldr = res.data_ptr(), res.stride(2)
     d.acc_scale, d.res_scale = acc_scale, res_scale
     d.flags = (capi.IG_RELU if relu else 0) | (capi.IG_GEGLU if geglu else 0) | (capi.IG_TCONV if tconv else 0) | (capi.IG_PAIR if pair else 0) \
-        | (capi.IG_SILU if silu else 0)
+        | (capi.IG_SILU if silu else 0) | (capi.IG_PAD0 if pad0 else 0)
     if rowstat_out is not None:
         assert rowstat_out.dtype == torch.int64 and rowstat_out.is_contiguous()
         d.rowstat_out = rowstat_out.data_ptr()

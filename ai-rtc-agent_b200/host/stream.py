@@ -76,8 +76,11 @@ class StreamDiffusion:
                  cfg_type: str = "self", device: str = "cuda", use_cuda_graph: bool = True,
                  packed_blob: Optional[str] = None, parent: Optional["StreamDiffusion"] = None,
                  controlnet_sd: Optional[Dict[str, torch.Tensor]] = None,
-                 hed_sd: Optional[Dict[str, torch.Tensor]] = None):
-        """controlnet_sd: a diffusers ControlNetModel state dict (empty when the weights come from packed_blob); every
+                 hed_sd: Optional[Dict[str, torch.Tensor]] = None, use_tiny_vae: bool = True,
+                 vae_scaling_factor: float = 0.18215):
+        """vae_sd: TAESD (use_tiny_vae=True) or the model's own AutoencoderKL (use_tiny_vae=False: latents = vae_scaling_factor
+        times the mean of the encoder's distribution, decoded from x0 / vae_scaling_factor).
+        controlnet_sd: a diffusers ControlNetModel state dict (empty when the weights come from packed_blob); every
         stream-batch slot is then conditioned on the current frame's control image: the frame itself, or with hed_sd (a
         ControlNetHED.pth state dict, empty with packed_blob) its HED edge map.  Lanes inherit their parent's ControlNet."""
         if hed_sd is not None and controlnet_sd is None:
@@ -129,6 +132,8 @@ class StreamDiffusion:
         cfg.use_cuda_graph = int(use_cuda_graph)
         cfg.controlnet = int(controlnet_sd is not None)
         cfg.control_processor = capi.CONTROL_HED if hed_sd is not None else capi.CONTROL_FRAME
+        cfg.vae = capi.VAE_TINY if use_tiny_vae else capi.VAE_KL
+        cfg.vae_scaling_factor = 0.0 if use_tiny_vae else float(vae_scaling_factor)
         if not torch.cuda.is_available():
             raise capi.B2Error("no CUDA device: the H100 pipeline has no CPU fallback")
         if self.device.index is None:
@@ -136,7 +141,8 @@ class StreamDiffusion:
         torch.cuda.set_device(self.device)
         self._ctor = dict(torch_dtype=torch_dtype, width=width, height=height, do_add_noise=do_add_noise,
                           use_denoising_batch=use_denoising_batch, frame_buffer_size=frame_buffer_size, cfg_type=cfg_type,
-                          device=device, use_cuda_graph=use_cuda_graph)
+                          device=device, use_cuda_graph=use_cuda_graph, use_tiny_vae=use_tiny_vae,
+                          vae_scaling_factor=vae_scaling_factor)
         self.lanes: List["StreamDiffusion"] = []     # extra engines over this one's weights (add_lane)
         self._parent = parent
         if parent is not None:

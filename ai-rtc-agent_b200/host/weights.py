@@ -55,6 +55,21 @@ def load_taesd(repo_dir: str) -> Dict[str, torch.Tensor]:
     raise FileNotFoundError(f"no TAESD safetensors under {repo_dir}")
 
 
+DEFAULT_VAE_SCALING_FACTOR = 0.18215
+
+
+def load_autoencoder_kl(repo_dir: str, v: A.VaeArch = A.AUTOENCODER_KL) -> Dict[str, torch.Tensor]:
+    """The model's own VAE: `<repo>/vae/diffusion_pytorch_model{.fp16,}.safetensors`, legacy attention names accepted, checked
+    key by key against the AutoencoderKL inventory (its scaling factor: resolve_vae_scaling_factor)."""
+    for name in ("diffusion_pytorch_model.fp16.safetensors", "diffusion_pytorch_model.safetensors"):
+        p = os.path.join(repo_dir, "vae", name)
+        if os.path.exists(p):
+            sd = A.normalize_autoencoder_kl({k: v.to(torch.float16) for k, v in _load_safetensors(p).items()})
+            A.validate_exact(sd, A.autoencoder_kl_param_shapes(v), "AutoencoderKL checkpoint")
+            return sd
+    raise FileNotFoundError(f"no AutoencoderKL safetensors under {repo_dir}/vae")
+
+
 def load_controlnet(repo_dir: str, arch: A.UNetArch) -> Dict[str, torch.Tensor]:
     """A diffusers ControlNetModel directory (config.json + diffusion_pytorch_model{.fp16,}.safetensors), checked against the
     UNet architecture it will be attached to."""
@@ -187,12 +202,13 @@ def layout_variant(batch: int, height: int, width: int) -> str:
 
 def packed_blob_path(engine_dir, model_id_or_path: str, arch_name: str, use_lcm_lora: bool, lcm_lora_id: Optional[str],
                      lora_dict: Optional[Dict[str, float]], vae_id: Optional[str], synthetic: bool, variant: str = "",
-                     controlnet: Optional[str] = None, control_processor: Optional[str] = None) -> str:
+                     controlnet: Optional[str] = None, control_processor: Optional[str] = None, full_vae: bool = False) -> str:
     """Where the packed-weight blob of this model lives: `<engine_dir>/engines--<model>/b2sd-<arch>-<recipe hash>.b2pack`,
     the directory naming of the reference's TensorRT cache (lib/wrapper.py:593, `engines--` + model id with / -> --).
     The hash covers everything that changes the weight VALUES (LoRAs and their scales, LCM-LoRA, VAE, ControlNet, synthetic
     seed), not
-    batch / resolution / prompt (the blob does not depend on them, unlike the reference's static-shape engines)."""
+    batch / resolution / prompt (the blob does not depend on them, unlike the reference's static-shape engines).
+    full_vae (use_tiny_vae=False) enters the recipe only when set, so the names of TAESD blobs do not change."""
     import hashlib
     import json
     recipe = {"lcm": bool(use_lcm_lora), "lcm_id": lcm_lora_id, "vae": vae_id, "synthetic": bool(synthetic), "layout": variant,
@@ -201,6 +217,8 @@ def packed_blob_path(engine_dir, model_id_or_path: str, arch_name: str, use_lcm_
         if os.path.exists(path):   # a replaced LoRA file must not hit the old blob
             st = os.stat(path)
             recipe.setdefault("lora_files", []).append((path, st.st_size, int(st.st_mtime)))
+    if full_vae:
+        recipe["vae_kind"] = "autoencoder_kl"
     if controlnet is not None:
         recipe["controlnet"] = controlnet
         recipe["control_processor"] = control_processor
@@ -214,22 +232,40 @@ def packed_blob_path(engine_dir, model_id_or_path: str, arch_name: str, use_lcm_
     return os.path.join(str(engine_dir), name, f"b2sd-{arch_name}-{digest}.b2pack")
 
 
+def resolve_vae_scaling_factor(repo_dir: Optional[str]) -> float:
+    """AutoencoderKL scaling_factor of a checkpoint directory (vae/config.json), 0.18215 without one."""
+    import json
+    p = os.path.join(repo_dir, "vae", "config.json") if repo_dir else None
+    if p and os.path.exists(p):
+        with open(p) as f:
+            return float(json.load(f).get("scaling_factor", DEFAULT_VAE_SCALING_FACTOR))
+    return DEFAULT_VAE_SCALING_FACTOR
+
+
 def resolve_weights(model_id_or_path: str, vae_id: Optional[str], lcm_lora_id: Optional[str], use_lcm_lora: bool,
-                    lora_dict: Optional[Dict[str, float]], sd_turbo: bool
+                    lora_dict: Optional[Dict[str, float]], sd_turbo: bool, use_tiny_vae: bool = True
                     ) -> Tuple[A.UNetArch, Dict[str, torch.Tensor], Dict[str, torch.Tensor], Optional[str]]:
     """Returns (arch, unet_sd, vae_sd, repo_dir or None).  Order: real checkpoint on disk -> synthetic weights if
-    $B200SD_SYNTHETIC_WEIGHTS is set (or the id starts with "tiny"/"synthetic") -> error."""
+    $B200SD_SYNTHETIC_WEIGHTS is set (or the id starts with "tiny"/"synthetic") -> error.  use_tiny_vae=False: vae_sd is the
+    model's own AutoencoderKL (scaling factor: resolve_vae_scaling_factor); vae_id applies to TAESD only, as in the reference."""
+    if not use_tiny_vae and vae_id is not None:
+        logger.warning("vae_id=%s is ignored with use_tiny_vae=False: the model's own AutoencoderKL is used", vae_id)
     if model_id_or_path in _PRELOADED:
+        if not use_tiny_vae:
+            raise NotImplementedError("preloaded weights carry TAESD only; use_tiny_vae=False loads the AutoencoderKL from disk")
         arch, unet_sd, vae_sd = _PRELOADED[model_id_or_path]
         return arch, unet_sd, vae_sd, find_local_repo(model_id_or_path)
     arch = A.arch_for(model_id_or_path)
     repo = find_local_repo(model_id_or_path)
     if repo is not None and os.path.isdir(os.path.join(repo, "unet")):
         unet_sd = load_unet(repo)
-        vae_repo = find_local_repo(vae_id or "madebyollin/taesd")
-        if vae_repo is None:
-            raise FileNotFoundError("TAESD weights (madebyollin/taesd) not found locally; run download.py where network exists")
-        vae_sd = load_taesd(vae_repo)
+        if use_tiny_vae:
+            vae_repo = find_local_repo(vae_id or "madebyollin/taesd")
+            if vae_repo is None:
+                raise FileNotFoundError("TAESD weights (madebyollin/taesd) not found locally; run download.py where network exists")
+            vae_sd = load_taesd(vae_repo)
+        else:
+            vae_sd = load_autoencoder_kl(repo, A.vae_arch_for(model_id_or_path))
         if use_lcm_lora and not sd_turbo:
             lrepo = find_local_repo(lcm_lora_id or "latent-consistency/lcm-lora-sdv1-5")
             if lrepo is None:
@@ -240,12 +276,16 @@ def resolve_weights(model_id_or_path: str, vae_id: Optional[str], lcm_lora_id: O
             n = fuse_lora(unet_sd, _load_safetensors(path), scale)
             logger.info("fused %d layers of %s (scale %s)", n, path, scale)
         A.validate_state_dict(unet_sd, A.unet_param_shapes(arch), "UNet checkpoint")
-        A.validate_state_dict(vae_sd, A.taesd_param_shapes(), "TAESD checkpoint")
+        if use_tiny_vae:
+            A.validate_state_dict(vae_sd, A.taesd_param_shapes(), "TAESD checkpoint")
         return arch, unet_sd, vae_sd, repo
     if os.getenv(ALLOW_SYNTHETIC_ENV) or model_id_or_path.startswith(("tiny", "synthetic")):
         logger.warning("no checkpoint for %s on disk: using seeded synthetic weights (%s)", model_id_or_path, arch.name)
         unet_sd = A.synthetic_state_dict(A.unet_param_shapes(arch), seed=1234)
-        vae_sd = A.synthetic_state_dict(A.taesd_param_shapes(), seed=4321, relu_net=True)
+        if use_tiny_vae:
+            vae_sd = A.synthetic_state_dict(A.taesd_param_shapes(), seed=4321, relu_net=True)
+        else:
+            vae_sd = A.synthetic_autoencoder_kl(A.vae_arch_for(model_id_or_path))
         return arch, unet_sd, vae_sd, None
     raise FileNotFoundError(
         f"model '{model_id_or_path}' not found on disk (no network for download.py); set {ALLOW_SYNTHETIC_ENV}=1 to run "

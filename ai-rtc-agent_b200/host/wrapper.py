@@ -6,7 +6,8 @@ Not carried over (unreachable from lib/pipeline.py:23-42 and listed out-of-scope
 safety checker, similar-image filter, DataParallel, txt2img sampling, xformers/sfast/TensorRT acceleration switches, and
 ControlNet preprocessors other than HED.  Their keywords are accepted; asking for one of those features raises.  A ControlNet
 runs with controlnet_processor_id="hed" (the default: the frame's HED edge map is the control image) or None (the frame
-itself)."""
+itself).  use_tiny_vae=False encodes and decodes with the model's own AutoencoderKL instead of TAESD (slower, the model's
+image quality); the latent is the mean of the encoder's distribution, not a sample of it."""
 from __future__ import annotations
 
 import logging
@@ -105,8 +106,6 @@ class StreamDiffusionWrapper:
             unsupported.append("similar-image filter")
         if device_ids is not None:
             unsupported.append("DataParallel device_ids (shard streams across GPUs instead, see host/dist.py)")
-        if not use_tiny_vae:
-            unsupported.append("full AutoencoderKL (only TAESD is on the reference's path)")
         if cfg_type in ("full", "initialize"):
             unsupported.append(f"cfg_type='{cfg_type}'")
         if device != "cuda":
@@ -124,6 +123,7 @@ class StreamDiffusionWrapper:
         self.batch_size = len(t_index_list) * frame_buffer_size if use_denoising_batch else frame_buffer_size
         self.use_denoising_batch = use_denoising_batch
         self.use_safety_checker = use_safety_checker
+        self.use_tiny_vae = use_tiny_vae
         self.engine_dir = engine_dir
         self.packed_blob = None
         self._blob_to_write = None
@@ -148,9 +148,14 @@ class StreamDiffusionWrapper:
         repo = W.find_local_repo(model_id_or_path)
         have_ckpt = repo is not None and os.path.isdir(os.path.join(repo, "unet"))
         arch = A.arch_for(model_id_or_path)
+        tiny_vae = self.use_tiny_vae
+        if not tiny_vae and vae_id is not None:   # as in the reference, vae_id names a TAESD
+            logger.warning("vae_id=%s is ignored with use_tiny_vae=False: the model's own AutoencoderKL is used", vae_id)
+            vae_id = None
         kw = dict(torch_dtype=self.dtype, width=self.width, height=self.height, do_add_noise=do_add_noise,
                   use_denoising_batch=self.use_denoising_batch, frame_buffer_size=self.frame_buffer_size, cfg_type=cfg_type,
-                  device=self.device)
+                  device=self.device, use_tiny_vae=tiny_vae,
+                  vae_scaling_factor=W.resolve_vae_scaling_factor(repo if have_ckpt else None))
         cn = controlnet_id_or_path is not None
         hed = cn and controlnet_processor_id == "hed"
         blob = None
@@ -162,7 +167,8 @@ class StreamDiffusionWrapper:
             blob = W.packed_blob_path(self.engine_dir, model_id_or_path, arch.name, use_lcm_lora and not self.sd_turbo, lcm_lora_id,
                                       lora_dict, vae_id, synthetic=not have_ckpt,
                                       variant=W.layout_variant(self.batch_size, self.height, self.width),
-                                      controlnet=controlnet_id_or_path, control_processor=controlnet_processor_id)
+                                      controlnet=controlnet_id_or_path, control_processor=controlnet_processor_id,
+                                      full_vae=not tiny_vae)
         encoder = make_prompt_encoder(repo if have_ckpt else None, arch.cross_attention_dim, self.device, allow_synthetic=synthetic_ok)
         if blob is not None and os.path.exists(blob) and (have_ckpt or synthetic_ok):
             try:
@@ -174,7 +180,7 @@ class StreamDiffusionWrapper:
             except Exception as exc:   # noqa: BLE001 - same policy as lib/wrapper.py:611-615
                 logger.warning("packed-weight blob %s unusable (%s); rebuilding from the checkpoint", blob, exc)
         arch, unet_sd, vae_sd, repo = resolve_weights(model_id_or_path, vae_id, lcm_lora_id, use_lcm_lora, lora_dict,
-                                                      self.sd_turbo)
+                                                      self.sd_turbo, use_tiny_vae=tiny_vae)
         cn_sd = W.resolve_controlnet(controlnet_id_or_path, arch, synthetic_ok) if cn else None
         hed_sd = W.resolve_hed(synthetic_ok) if hed else None
         self._blob_to_write = blob

@@ -37,7 +37,8 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--lora", action="append", metavar="PATH[:SCALE]", help="LoRA safetensors to fuse (repeatable; build.py:23-25)")
     ap.add_argument("--lcm-lora-id", default=None)
     ap.add_argument("--no-lcm-lora", action="store_true")
-    ap.add_argument("--vae-id", default=None)
+    ap.add_argument("--vae-id", default=None, help="TAESD to pack (ignored with --full-vae)")
+    ap.add_argument("--full-vae", action="store_true", help="pack the model's own AutoencoderKL instead of TAESD (use_tiny_vae=False)")
     ap.add_argument("--controlnet-id", default=None, help="diffusers ControlNetModel (HF id or local directory) packed with the UNet")
     ap.add_argument("--controlnet-processor-id", default="hed", type=lambda v: None if v.lower() == "none" else v,
                     help="control-image preprocessor: hed (default, the reference's) or none (the frame itself)")
@@ -64,7 +65,7 @@ def main(argv=None) -> int:
     blob = W.packed_blob_path(args.engine_dir, args.model_id, A.arch_for(args.model_id).name, not args.no_lcm_lora and not turbo,
                               args.lcm_lora_id, loras, args.vae_id, synthetic=not have_ckpt,
                               variant=W.layout_variant(len(t_index_list), args.height, args.width), controlnet=args.controlnet_id,
-                              control_processor=args.controlnet_processor_id)
+                              control_processor=args.controlnet_processor_id, full_vae=args.full_vae)
     if not have_ckpt:
         if not (os.getenv(W.ALLOW_SYNTHETIC_ENV) or args.model_id.startswith(("tiny", "synthetic"))):
             raise SystemExit(f"pack: no checkpoint for '{args.model_id}' on disk (set {W.ALLOW_SYNTHETIC_ENV}=1 to pack seeded synthetic weights)")
@@ -73,7 +74,8 @@ def main(argv=None) -> int:
         os.remove(blob)
     t0 = time.time()
     w = StreamDiffusionWrapper(model_id_or_path=args.model_id, t_index_list=t_index_list, lora_dict=loras or None,
-                               lcm_lora_id=args.lcm_lora_id, vae_id=args.vae_id, use_lcm_lora=not args.no_lcm_lora,
+                               lcm_lora_id=args.lcm_lora_id, vae_id=None if args.full_vae else args.vae_id,
+                               use_lcm_lora=not args.no_lcm_lora, use_tiny_vae=not args.full_vae,
                                controlnet_id_or_path=args.controlnet_id, controlnet_processor_id=args.controlnet_processor_id,
                                width=args.width, height=args.height, output_type="pt", mode="img2img", engine_dir=args.engine_dir)
     reused = w.packed_blob is not None

@@ -42,6 +42,9 @@ enum {
     B2SD_IG_GEGLU = 2,
     B2SD_IG_SILU = 8,        /* x * sigmoid(x) after bias / residual (ControlNet conditioning embedding); single CTAs with
                                 bn 16 / 32 / 64 / 128 only, not with B2SD_IG_TCONV or B2SD_IG_PAIR */
+    B2SD_IG_PAD0 = 16,       /* 3x3 taps at input (stride*out + tap) instead of (stride*out + tap - 1): F.pad(x, (0,1,0,1)) then
+                                an unpadded conv, the AutoencoderKL encoder's Downsample2D; single CTAs, bn 64 / 128 / 256, not
+                                with B2SD_IG_TCONV, B2SD_IG_PAIR, B2SD_IG_SILU or swap */
     B2SD_IG_TCONV = 64,      /* run the persistent halo-tile kernel (stride-1 3x3, 64 -> 64 channels: the TAESD body) */
     B2SD_IG_PAIR = 128       /* CTA pairs: tcgen05.mma.cta_group::2 (M = 256 per MMA), each CTA stages half of the weight tile;
                                 normal orientation, bn % 32 == 0, splits <= 4 */
@@ -111,7 +114,8 @@ int b2sd_igemm_plan_dry(const b2sd_igemm_desc* d, int autotile, int allow_swap, 
 int b2sd_groupnorm_plan_dry(int ca, int cb, int groups, int hw, int* cluster, int* threads, int* pixels_per_cta);
 uint64_t b2sd_igemm_partial_floats(int splits, int64_t rows_total, int n_valid);   /* legacy sizing helper, unused by the cluster split-K */
 
-/* Flash attention (self / cross) of BasicTransformerBlock.attn1 / attn2 (inside unet.engine).
+/* Flash attention (self / cross) of BasicTransformerBlock.attn1 / attn2 (inside unet.engine), and with dp = d_real = 512 the
+ * single-head attention of the AutoencoderKL mid blocks (pitches, V^T batch stride multiples of 8, 16-byte aligned pointers).
  * q: [nb*sq][ldq], head h at columns [h*dp, (h+1)*dp); k likewise (batch b at row b*k_bstride, 0 = shared);
  * vt = V^T: [heads*dp][ldvt] with the key index contiguous (batch b at column b*vt_bstride);
  * out: [nb*sq][ldo], head h at columns [h*d_real, (h+1)*d_real). softmax scale = d_real^-0.5. */
@@ -120,7 +124,7 @@ typedef struct {
     const void* k; int ldk; int64_t k_bstride; int64_t k_rows;
     const void* vt; int ldvt; int64_t vt_bstride; int64_t vt_cols;
     void* out; int ldo;
-    int nb, heads, sq, skv, d_real, dp;
+    int nb, heads, sq, skv, d_real, dp;   /* dp: 64, 128, 192 (zero-padded heads) or 512 (d_real 512) */
 } b2sd_attn_desc;
 int b2sd_op_attention(const b2sd_attn_desc* d, void* stream);
 
@@ -194,8 +198,15 @@ typedef struct {
                                     HED edge map of the frame (controlnet_aux HEDdetector at the engine's size; weights under
                                     "hed." + ControlNetHED.pth keys, e.g. "hed.block1.convs.0.weight", "hed.norm").  Inherited
                                     by lanes. */
+    int vae;                     /* B2SD_VAE_TINY (0): TAESD (weights "vae." + AutoencoderTiny keys).  B2SD_VAE_KL (1): the model's
+                                    own AutoencoderKL (weights "vae." + diffusers AutoencoderKL keys, e.g.
+                                    "vae.encoder.down_blocks.0.resnets.0.conv1.weight", "vae.quant_conv.weight"; mid-block attention
+                                    as to_q / to_k / to_v / to_out.0 with q/k/v as [512][512]); the latent is scaling_factor times the
+                                    mean of the encoder's distribution (not a sample).  Inherited by lanes. */
+    float vae_scaling_factor;    /* with vae = B2SD_VAE_KL: vae/config.json scaling_factor; 0 = 0.18215 */
 } b2sd_config;
 enum { B2SD_CONTROL_FRAME = 0, B2SD_CONTROL_HED = 1 };
+enum { B2SD_VAE_TINY = 0, B2SD_VAE_KL = 1 };
 
 int b2sd_create(const b2sd_config* cfg, b2sd_handle* out);
 int b2sd_destroy(b2sd_handle h);
@@ -254,7 +265,8 @@ int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int
                  int out_kind, void* stream);
 
 /* Parity/debug taps: copies a named intermediate of the last step to host memory as fp16 NHWC.
- * Names: "x_t", "unet_in", "eps", "x0", "image", "conv_in", "down.I.J", "mid", "up.I.J"; with a ControlNet also "cn_cond"
+ * Names: "x_t", "unet_in", "eps", "x0", "image", "conv_in", "down.I.J", "mid", "up.I.J"; with the AutoencoderKL also
+ * "vae.enc.down.I", "vae.enc.mid", "vae.dec.mid", "vae.dec.up.I" (block outputs); with a ControlNet also "cn_cond"
  * (conditioning embedding, batch 1), "cn.conv_in" (its conv_in(x) + cn_cond), "cn.res.K" (UNet skip K, in push order 0..11,
  * plus ControlNet residual K: what the up path reads) and "cn.mid" ("mid" plus the mid-block residual); with HED also
  * "control" (the u8 edge value as fp16, [1][h][w][1]).

@@ -58,6 +58,84 @@ static void to_igemm_desc(const b2sd_igemm_desc* d, IgemmDesc& g) {
     g.epi.col2 = d->col2;
 }
 
+static b2sd_act_view from_view(const ActView& a) {
+    b2sd_act_view v;
+    v.ptr = a.ptr;
+    v.n = a.N; v.h = a.H; v.w = a.W; v.c = a.C; v.ld = a.ld;
+    return v;
+}
+
+static void fill_plan_info(const IgemmPlan& plan, b2sd_igemm_plan_info* out) {
+    out->mode = plan.mode;
+    out->swap = plan.p.swap;
+    out->bn = plan.p.BN;
+    out->splits = plan.splits;
+    out->grid_x = (int)plan.grid.x; out->grid_y = (int)plan.grid.y; out->grid_z = (int)plan.grid.z;
+    out->num_stages = plan.p.num_stages;
+    out->acc_bufs = plan.p.acc_bufs;
+    out->total_kb = plan.p.total_kb;
+    out->kb_per_split = plan.p.kb_per_split;
+    out->tmem_cols = (int)plan.p.tmem_cols;
+    out->m_tiles = plan.p.tiles_w * plan.p.tiles_h * plan.p.tiles_n;
+    out->smem_bytes = (int64_t)plan.smem;
+    out->rows_total = plan.rows_total;
+}
+
+}  // extern "C"
+
+namespace b2 {
+// The inverse of to_igemm_desc: the contraction `g` as planned by `plan` (or, with plan = NULL, as the halo-tile kernel runs
+// it) in the C ABI's terms -- the launch record of the frame program's audit (b2sd_audit_step).
+void igemm_record(const IgemmDesc& g, const IgemmPlan* plan, b2sd_igemm_desc* d, b2sd_igemm_plan_info* info) {
+    *d = b2sd_igemm_desc{};
+    *info = b2sd_igemm_plan_info{};
+    d->nseg = g.nseg;
+    for (int s = 0; s < g.nseg && s < IG_MAX_SRC; ++s) {
+        d->src[s] = from_view(g.src[s]);
+        d->ntap[s] = g.ntap[s];
+    }
+    d->w = g.w;
+    d->w_rows = g.w_rows;
+    d->w_ld = g.w_ld;
+    d->stride = g.stride < 1 ? 1 : g.stride;
+    d->nb = g.Nb; d->ho = g.Ho; d->wo = g.Wo;
+    d->out = g.epi.out;
+    d->ldc = g.epi.ldc;
+    d->colbias = g.epi.colbias;
+    d->colbias_bstride = g.epi.colbias_bstride;
+    d->res = g.epi.res;
+    d->ldr = g.epi.ldr;
+    d->acc_scale = g.epi.acc_scale;
+    d->res_scale = g.epi.res_scale;
+    d->flags = g.epi.flags & (IG_RELU | IG_GEGLU | IG_SILU | IG_PAD0);
+    d->n_valid = g.epi.n_valid;
+    d->rowstat_out = g.epi.rowstat_out;
+    d->rowstat_in = g.epi.rowstat_in;
+    d->colsum = g.epi.colsum;
+    d->ln_c = g.epi.ln_inv_c > 0.f ? (int)lrintf(1.f / g.epi.ln_inv_c) : 0;
+    d->ln_eps = g.epi.ln_eps;
+    d->out2 = g.epi.out2;
+    d->ld2 = g.epi.ld2;
+    d->col2 = g.epi.col2;
+    if (plan) {
+        d->bn = plan->p.BN;
+        d->splits = plan->splits;
+        d->swap = plan->p.swap;
+        if (plan->pair) d->flags |= B2SD_IG_PAIR;
+        fill_plan_info(*plan, info);
+    } else {
+        d->bn = TC_C;
+        d->splits = 1;
+        d->flags |= B2SD_IG_TCONV;
+        info->bn = TC_C;
+        info->splits = 1;
+        info->rows_total = (int64_t)g.Nb * g.Ho * g.Wo;
+    }
+}
+}  // namespace b2
+
+extern "C" {
+
 int b2sd_op_igemm(const b2sd_igemm_desc* d, void* stream) {
     if (!d) {
         b2_set_error("b2sd_op_igemm: null desc");
@@ -95,19 +173,7 @@ int b2sd_igemm_plan_dry(const b2sd_igemm_desc* d, int autotile, int allow_swap, 
     const int rc = autotile ? igemm_autotile(g, allow_swap != 0, &plan) : igemm_plan(g, &plan);
     igemm_set_dry_run(false);
     if (rc) return -1;
-    out->mode = plan.mode;
-    out->swap = plan.p.swap;
-    out->bn = plan.p.BN;
-    out->splits = plan.splits;
-    out->grid_x = (int)plan.grid.x; out->grid_y = (int)plan.grid.y; out->grid_z = (int)plan.grid.z;
-    out->num_stages = plan.p.num_stages;
-    out->acc_bufs = plan.p.acc_bufs;
-    out->total_kb = plan.p.total_kb;
-    out->kb_per_split = plan.p.kb_per_split;
-    out->tmem_cols = (int)plan.p.tmem_cols;
-    out->m_tiles = plan.p.tiles_w * plan.p.tiles_h * plan.p.tiles_n;
-    out->smem_bytes = (int64_t)plan.smem;
-    out->rows_total = plan.rows_total;
+    fill_plan_info(plan, out);
     return 0;
 }
 

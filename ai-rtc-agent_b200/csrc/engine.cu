@@ -27,6 +27,11 @@
 
 using namespace b2;
 
+namespace b2 {
+// capi.cu: a contraction as launched, in the C ABI's terms (plan = NULL: the halo-tile kernel)
+void igemm_record(const IgemmDesc& g, const IgemmPlan* plan, b2sd_igemm_desc* d, b2sd_igemm_plan_info* info);
+}
+
 #define CUDA_OK(expr)                                                                       \
     do {                                                                                    \
         cudaError_t e__ = (expr);                                                           \
@@ -75,7 +80,11 @@ class Arena {
             if (next >= (int)slabs_.size()) {
                 size_t sz = bytes > slab_ ? bytes : slab_;
                 void* p = nullptr;
-                if (cudaMalloc(&p, sz) != cudaSuccess) return nullptr;
+                const cudaError_t e = cudaMalloc(&p, sz);
+                if (e != cudaSuccess) {   // callers only see nullptr: say why, or the caller reports a stale message
+                    b2_set_error("device allocation of %zu bytes failed: %s", sz, cudaGetErrorString(e));
+                    return nullptr;
+                }
                 slabs_.push_back(p);
                 sizes_.push_back(sz);
                 next = (int)slabs_.size() - 1;
@@ -108,6 +117,7 @@ struct Op {
     std::function<int(cudaStream_t)> fn;
     std::string name;
     double flops = 0.0;  // algorithmic 2*MAC count of the launch (0 for non-contraction kernels)
+    b2sd_launch_record rec{};   // what the launch computes (b2sd_audit_step); kind B2SD_LAUNCH_OTHER unless set where it is pushed
     template <class F>
     Op(F f, std::string n = "", double fl = 0.0) : fn(std::move(f)), name(std::move(n)), flops(fl) {}
     int operator()(cudaStream_t s) const { return fn(s); }
@@ -482,9 +492,22 @@ struct b2sd_engine {
 
     // choose N tile / split-K for a good grid (igemm_autotile), plan, and append the launch
     // append a planned contraction
-    void push_igemm(std::vector<Op>& dst, const IgemmPlan& plan, const std::string& label, double flops) {
+    void push_igemm(std::vector<Op>& dst, const IgemmDesc& d, const IgemmPlan& plan, const std::string& label, double flops) {
         if (&dst == &prog_frame) launches += 1;
         dst.push_back(Op([plan](cudaStream_t s) { return igemm_launch(plan, s); }, label, flops));
+        dst.back().rec.kind = B2SD_LAUNCH_IGEMM;
+        igemm_record(d, &plan, &dst.back().rec.igemm, &dst.back().rec.plan);
+    }
+
+    void push_attn(const AttnPlan& plan, const std::string& label) {
+        const AttnDesc& a = plan.d;
+        launches += 1;
+        prog_frame.push_back(Op([plan](cudaStream_t st) { return attn_launch(plan, st); }, label,
+                                4.0 * a.nb * a.heads * (double)a.sq * a.skv * a.d_real));
+        b2sd_launch_record& r = prog_frame.back().rec;
+        r.kind = B2SD_LAUNCH_ATTN;
+        r.attn = b2sd_attn_desc{a.q, a.ldq, a.k, a.ldk, (int64_t)a.k_bstride, (int64_t)a.k_rows, a.vt, a.ldvt, (int64_t)a.vt_bstride,
+                                (int64_t)a.vt_cols, a.out, a.ldo, a.nb, a.heads, a.sq, a.skv, a.d_real, a.dp};
     }
 
     // choose N tile / split-K for a good grid (igemm_autotile), plan, and append the launch
@@ -508,7 +531,7 @@ struct b2sd_engine {
         snprintf(label, sizeof(label), "igemm %s rows=%ld n=%d kb=%d bn=%d splits=%d grid=%u,%u,%u %s", cur.c_str(),
                  plan.rows_total, d.epi.n_valid, plan.p.total_kb, plan.p.BN, plan.splits, plan.grid.x, plan.grid.y,
                  plan.grid.z, plan.p.swap ? "swapped" : (plan.pair ? "pairs" : "taps"));
-        push_igemm(dst, plan, label, 2.0 * (double)plan.rows_total * n_gemm * plan.p.total_kb * IG_BK);
+        push_igemm(dst, d, plan, label, 2.0 * (double)plan.rows_total * n_gemm * plan.p.total_kb * IG_BK);
         return 0;
     }
 
@@ -525,6 +548,10 @@ struct b2sd_engine {
         a.counters = tile_counters;   // zero-initialised, self re-arming
         launches += 1;
         prog_frame.push_back(Op([a](cudaStream_t s) { return groupnorm_launch(a, s); }, "groupnorm " + prefix));
+        b2sd_launch_record& r = prog_frame.back().rec;
+        r.kind = B2SD_LAUNCH_GROUPNORM;
+        r.groupnorm = b2sd_groupnorm_args{a.xa, a.ca, a.lda, a.xb, a.cb, a.ldb, a.gamma, a.beta, a.y, a.ldy, a.nb, a.hw, a.groups,
+                                          a.eps, a.silu};
         return 0;
     }
 
@@ -537,6 +564,9 @@ struct b2sd_engine {
         const int ldx = x.ld, ldy = y.ld, c = x.c;
         ++launches;
         prog_frame.push_back(Op([=](cudaStream_t s) { return layernorm_launch(xp, ldx, g, b, yp, ldy, rows, c, 1e-5f, s); }, "layernorm " + prefix));
+        b2sd_launch_record& r = prog_frame.back().rec;
+        r.kind = B2SD_LAUNCH_LAYERNORM;
+        r.layernorm = b2sd_layernorm_args{xp, ldx, g, b, yp, ldy, (int64_t)rows, c, 1e-5f};
         return 0;
     }
 
@@ -578,6 +608,8 @@ struct b2sd_engine {
                      tp.grid.x, tp.p.nbuf);
             if (&dst == &prog_frame) launches += 1;
             dst.push_back(Op([tp](cudaStream_t st) { return tconv_launch(tp, st); }, label, 2.0 * (double)tp.rows_total * cout * K));
+            dst.back().rec.kind = B2SD_LAUNCH_TCONV;
+            igemm_record(d, nullptr, &dst.back().rec.igemm, &dst.back().rec.plan);
             return 0;
         }
         return add_igemm(dst, d);
@@ -839,9 +871,7 @@ int b2sd_engine::build_transformer(const std::string& p, const Act& x, int heads
         a.nb = B; a.heads = heads; a.sq = HW; a.skv = HW; a.d_real = d_real; a.dp = dp;
         AttnPlan plan;
         TRY(attn_plan(a, &plan));
-        ++launches;
-        prog_frame.push_back(Op([plan](cudaStream_t st) { return attn_launch(plan, st); }, "attn " + p,
-                               4.0 * a.nb * a.heads * (double)a.sq * a.skv * a.d_real));
+        push_attn(plan, "attn " + p);
     }
     const Raw* wo1 = get(t + "attn1.to_out.0.weight");
     if (!wo1) return -1;
@@ -893,9 +923,7 @@ int b2sd_engine::build_transformer(const std::string& p, const Act& x, int heads
         a.nb = B; a.heads = heads; a.sq = HW; a.skv = L; a.d_real = d_real; a.dp = dp;
         AttnPlan plan;
         TRY(attn_plan(a, &plan));
-        ++launches;
-        prog_frame.push_back(Op([plan](cudaStream_t st) { return attn_launch(plan, st); }, "attn " + p,
-                               4.0 * a.nb * a.heads * (double)a.sq * a.skv * a.d_real));
+        push_attn(plan, "attn " + p);
     }
     const Raw* wo2 = get(t + "attn2.to_out.0.weight");
     if (!wo2) return -1;
@@ -930,7 +958,7 @@ int b2sd_engine::build_transformer(const std::string& p, const Act& x, int heads
         }
         IgemmPlan plan;
         TRY(igemm_plan(d, &plan));
-        push_igemm(prog_frame, plan, "igemm geglu " + p, 2.0 * (double)M * (2.0 * inner) * C);
+        push_igemm(prog_frame, d, plan, "igemm geglu " + p, 2.0 * (double)M * (2.0 * inner) * C);
     }
     const Raw* wff2 = get(t + "ff.net.2.weight");
     if (!wff2) return -1;
@@ -1219,8 +1247,7 @@ int b2sd_engine::build_vae_attention(const std::string& p, const Act& x, Act* ou
     a.nb = 1; a.heads = 1; a.sq = M; a.skv = M; a.d_real = C; a.dp = C;
     AttnPlan plan;
     TRY(attn_plan(a, &plan));
-    ++launches;
-    prog_frame.push_back(Op([plan](cudaStream_t st) { return attn_launch(plan, st); }, "attn " + p, 4.0 * (double)M * M * C));
+    push_attn(plan, "attn " + p);
     const Raw* wo = get(p + "to_out.0.weight");
     if (!wo) return -1;
     *out = new_act(1, x.h, x.w, C);
@@ -2233,6 +2260,63 @@ int b2sd_profile(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* 
         return -1;
     }
     memcpy(json_buf, js.c_str(), js.size() + 1);
+    return 0;
+}
+
+// b2sd_step with the frame program run eagerly and the caller's check around every kernel launch (see b2sd.h).  Test aid: the
+// stream is synchronised twice per launch.
+int b2sd_audit_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* frame_out, b2sd_audit_fn fn, void* user,
+                    void* stream) {
+    if (!h || !h->built || !fn || !frame_in || !frame_out || in_h < 1 || in_w < 1) {
+        b2_set_error("b2sd_audit_step: bad arguments (or b2sd_prepare not called)");
+        return -1;
+    }
+    if (h->group) {
+        b2_set_error("b2sd_audit_step: stage-pipelined lanes (b2sd_share_stream_state) are not supported");
+        return -1;
+    }
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    int index = 0;
+    auto audited = [&](b2sd_launch_record rec, const char* label, const std::function<int()>& launch) -> int {
+        rec.label = label;
+        CUDA_OK(cudaStreamSynchronize(s));
+        if (fn(user, index, 0, &rec)) {
+            b2_set_error("b2sd_audit_step: launch %d '%s' rejected before it ran", index, label);
+            return -1;
+        }
+        TRY(launch());
+        CUDA_OK(cudaStreamSynchronize(s));
+        if (fn(user, index, 1, &rec)) {
+            b2_set_error("b2sd_audit_step: launch %d '%s' failed its check", index, label);
+            return -1;
+        }
+        ++index;
+        return 0;
+    };
+    const b2sd_launch_record other{};
+    SmallConvArgs a = h->head;
+    a.x = frame_in; a.in_h = in_h; a.in_w = in_w; a.flags = SC_IN_U8 | (h->head.flags & SC_IN_OFFSET);
+    TRY(audited(other, "smallconv head", [&] { return smallconv_launch(a, s); }));
+    if (h->cfg.controlnet) {
+        const bool hed = h->cfg.control_processor == B2SD_CONTROL_HED;
+        SmallConvArgs c = hed ? h->hed_head : h->cn_head;
+        c.x = frame_in; c.in_h = in_h; c.in_w = in_w; c.flags = SC_IN_U8 | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
+        TRY(audited(other, hed ? "smallconv hed head" : "smallconv controlnet head", [&] { return smallconv_launch(c, s); }));
+    }
+    for (auto& op : h->prog_frame) {
+        if (op.name.compare(0, 7, "memset ") == 0) {   // a memset node, not a kernel launch
+            TRY(op(s));
+            continue;
+        }
+        TRY(audited(op.rec, op.name.c_str(), [&] { return op(s); }));
+    }
+    TRY(audited(other, "post_u8", [&] {
+        return post_u8_launch(h->image.p, h->image.ld, static_cast<uint8_t*>(frame_out), 1, h->cfg.height, h->cfg.width, s);
+    }));
+    if (index != h->launches) {
+        b2_set_error("b2sd_audit_step: %d launches audited, %d expected", index, h->launches);
+        return -1;
+    }
     return 0;
 }
 

@@ -56,6 +56,37 @@ class AttnDesc(C.Structure):
     ]
 
 
+class GroupNormArgs(C.Structure):
+    _fields_ = [
+        ("xa", C.c_void_p), ("ca", C.c_int), ("lda", C.c_int), ("xb", C.c_void_p), ("cb", C.c_int), ("ldb", C.c_int),
+        ("gamma", C.c_void_p), ("beta", C.c_void_p), ("y", C.c_void_p), ("ldy", C.c_int),
+        ("nb", C.c_int), ("hw", C.c_int), ("groups", C.c_int), ("eps", C.c_float), ("silu", C.c_int),
+    ]
+
+
+class LayerNormArgs(C.Structure):
+    _fields_ = [
+        ("x", C.c_void_p), ("ldx", C.c_int), ("gamma", C.c_void_p), ("beta", C.c_void_p), ("y", C.c_void_p), ("ldy", C.c_int),
+        ("rows", C.c_int64), ("c", C.c_int), ("eps", C.c_float),
+    ]
+
+
+LAUNCH_OTHER, LAUNCH_IGEMM, LAUNCH_TCONV, LAUNCH_ATTN, LAUNCH_GROUPNORM, LAUNCH_LAYERNORM = range(6)
+LAUNCH_KINDS = {LAUNCH_OTHER: "other", LAUNCH_IGEMM: "igemm", LAUNCH_TCONV: "tconv", LAUNCH_ATTN: "attn",
+                LAUNCH_GROUPNORM: "groupnorm", LAUNCH_LAYERNORM: "layernorm"}
+
+
+class LaunchRecord(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int), ("label", C.c_char_p),
+        ("igemm", IgemmDesc), ("plan", IgemmPlanInfo), ("attn", AttnDesc),
+        ("groupnorm", GroupNormArgs), ("layernorm", LayerNormArgs),
+    ]
+
+
+AUDIT_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_int, C.POINTER(LaunchRecord))
+
+
 class EngineConfig(C.Structure):
     _fields_ = [
         ("block_out_channels", C.c_int * 4), ("heads", C.c_int * 4), ("down_attn", C.c_int * 4),
@@ -139,6 +170,8 @@ def lib() -> C.CDLL:
         _lib.b2sd_profile_kind.restype = C.c_int
         _lib.b2sd_profile_gate.argtypes = [ci]
         _lib.b2sd_profile_gate.restype = C.c_int
+        _lib.b2sd_audit_step.argtypes = [vp, vp, ci, ci, vp, AUDIT_FN, vp, vp]
+        _lib.b2sd_audit_step.restype = C.c_int
         for name in ("create", "create_lane", "destroy", "load_tensor", "prepare", "export_packed", "import_packed", "set_prompt_embeds", "set_timesteps", "step",
                      "step_ex", "get_tensor", "launches_per_step"):
             getattr(_lib, "b2sd_" + name).restype = C.c_int

@@ -396,6 +396,32 @@ class StreamDiffusion:
                                                self._stream()), "b2sd_profile_kind")
         return {"ms": ms.value, "launches": n.value, "flops": fl.value}
 
+    @torch.no_grad()
+    def audit_step(self, frame_nhwc: torch.Tensor, fn: Callable[[int, bool, "capi.LaunchRecord"], None]) -> torch.Tensor:
+        """step_u8 with the frame program run eagerly and fn(index, after, record) called before and after every kernel launch,
+        with the stream synchronised (b2sd_audit_step): record describes the launch as the engine issues it.  An exception
+        raised by fn aborts the step and is re-raised here.  Returns the u8 frame, as step_u8 does.  Test aid."""
+        self._check()
+        frame_nhwc = frame_nhwc.contiguous()
+        out = torch.empty((1, 3, self.height, self.width), dtype=torch.uint8, device=self.device)
+        failure = []
+
+        def cb(_user, index, after, rec):
+            try:
+                fn(index, bool(after), rec.contents)
+                return 0
+            except BaseException as e:   # an exception cannot cross the C frames: keep it and abort the step
+                failure.append(e)
+                return 1
+
+        cfn = capi.AUDIT_FN(cb)
+        rc = self._lib.b2sd_audit_step(self._handle, frame_nhwc.data_ptr(), frame_nhwc.shape[1], frame_nhwc.shape[2],
+                                       out.data_ptr(), cfn, None, self._stream())
+        if failure:
+            raise failure[0]
+        capi.check(rc, "b2sd_audit_step")
+        return out
+
     @property
     def launches_per_step(self) -> int:
         return self._lib.b2sd_launches_per_step(self._handle)

@@ -287,6 +287,47 @@ int b2sd_profile_kind(b2sd_handle h, const char* kind, int iters, double* ms_per
  * wait for each other between their warm-up and their timed replays, so the timed regions overlap.  0 / 1 switches it off. */
 int b2sd_profile_gate(int participants);
 int b2sd_launches_per_step(b2sd_handle h);
+
+/* Launch audit (test aid, like b2sd_profile): what each launch of the frame program computes, as it is launched.
+ * kind B2SD_LAUNCH_IGEMM / _TCONV: `igemm` is the contraction with the plan's bn / splits / swap and B2SD_IG_PAIR /
+ * B2SD_IG_TCONV in flags (partial = NULL), `plan` the plan (for the halo-tile kernel only bn 64, splits 1 and rows_total);
+ * _ATTN: `attn`; _GROUPNORM / _LAYERNORM: the normalisation's arguments; _OTHER: only `label` (the profiling label). */
+enum { B2SD_LAUNCH_OTHER = 0, B2SD_LAUNCH_IGEMM = 1, B2SD_LAUNCH_TCONV = 2, B2SD_LAUNCH_ATTN = 3, B2SD_LAUNCH_GROUPNORM = 4,
+       B2SD_LAUNCH_LAYERNORM = 5 };
+typedef struct {
+    const void* xa; int ca, lda;
+    const void* xb; int cb, ldb;   /* xb NULL: no second source */
+    const float* gamma; const float* beta;
+    void* y; int ldy;
+    int nb, hw, groups;
+    float eps;
+    int silu;
+} b2sd_groupnorm_args;
+typedef struct {
+    const void* x; int ldx;
+    const float* gamma; const float* beta;
+    void* y; int ldy;
+    int64_t rows; int c;
+    float eps;
+} b2sd_layernorm_args;
+typedef struct {
+    int kind;
+    const char* label;
+    b2sd_igemm_desc igemm;
+    b2sd_igemm_plan_info plan;
+    b2sd_attn_desc attn;
+    b2sd_groupnorm_args groupnorm;
+    b2sd_layernorm_args layernorm;
+} b2sd_launch_record;
+/* One b2sd_step with the frame program run eagerly (no CUDA graph) and `fn` called around every kernel launch: `stream` is
+ * synchronised, fn(user, index, 0, rec) runs, the launch is enqueued, `stream` is synchronised, fn(user, index, 1, rec) runs.
+ * index counts kernel launches (0 .. b2sd_launches_per_step - 1, in launch order; the frame's input heads and the u8 tail are
+ * kind OTHER); the frame program's memset of the LayerNorm statistics is not a kernel launch and gets no call.  A non-zero
+ * return from fn aborts the step with an error.  The output equals b2sd_step's. */
+typedef int (*b2sd_audit_fn)(void* user, int index, int after, const b2sd_launch_record* rec);
+int b2sd_audit_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* frame_out, b2sd_audit_fn fn, void* user,
+                    void* stream);
+
 /* Stage pipelining of ONE stateful stream (stream batch T > 1, where frame n+1 needs frame n's latent buffer and lanes cannot
  * simply alternate): `lane` shares `owner`'s stream-batch state; the frame program of each is cut into TAESD encoder body |
  * last encoder conv + UNet + scheduler step | TAESD decoder, and only the middle stage is serialised between the lanes (one

@@ -89,6 +89,8 @@ def test_gpu_oracle_equals_cpu_oracle(cuda):
     pytest.param(True, [32], (448, 768), 2, 8, id="turbo-T1-448x768-8"),
     pytest.param(False, [18, 26, 35, 45], (768, 448), 4, 1, id="sd15-T4-768x448-1"),
     pytest.param(False, [18, 26, 35, 45], (768, 448), 2, 4, id="sd15-T4-768x448-4"),
+    # 14x14 level: the unfolded transformer program (V^T per image, padded column ranges) at a full attention level
+    pytest.param(False, [18, 26, 35, 45], 448, 3, 1, id="sd15-T4-448x448-1"),
 ])
 def test_three_implementations_full_size(cuda, turbo, tl, hw, nframes, in_flight):
     from oracle import pipeline as opipe

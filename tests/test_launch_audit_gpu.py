@@ -1,0 +1,369 @@
+"""Launch audit of the frame program: every contraction, attention, GroupNorm and LayerNorm launch of a real frame, checked in
+place against a float64 recomputation of its own inputs.
+
+StreamDiffusion.audit_step runs one frame eagerly and calls back before and after every kernel launch with the launch's record
+(descriptor and plan as launched).  Before: the callback snapshots everything the launch reads (sources, weights, bias,
+residual, LayerNorm statistics, Q / K / V^T, normalisation inputs) and the spare pitch columns of its outputs.  After: the
+output is compared with the descriptor-driven reference of tests/launch_ref.py (tolerance atol * rms(ref) + rtol * |ref| per
+class), every check is shown to be discriminating by a named wrong reference that lands >= 10x the tolerance away, the spare
+columns must be bit-identical, and a LayerNorm-statistics producer's fixed-point sums must match its stored fp16 rows.
+
+The audited frame's u8 output must equal, bit for bit, a CUDA-graph step of a lane prepared identically: the audit observes
+the real program.  Device memory is only ever read, never past the last row of a buffer: the spare columns of an output's last
+row are not checked (the pitch can reach past the allocation when an output is a column range of a wider buffer)."""
+from __future__ import annotations
+
+import collections
+import gc
+import time
+
+import pytest
+import torch
+
+from tests import launch_ref as R
+
+pytestmark = pytest.mark.gpu
+
+_T4 = [18, 26, 35, 45]
+
+
+class _Dev:
+    def __init__(self, ptr, shape, strides, typestr):
+        self.__cuda_array_interface__ = {"shape": shape, "strides": strides, "typestr": typestr, "data": (ptr, False),
+                                         "version": 3}
+
+
+_TYPES = {torch.float16: ("<f2", 2), torch.float32: ("<f4", 4), torch.int64: ("<i8", 8)}
+
+
+def _dev(ptr, rows, cols, ld, dtype=torch.float16):
+    """A [rows, cols] device view with row pitch ld (elements) at ptr; never touches memory outside those elements.  (torch
+    takes no read-only views: the audit only ever reads or copies them.)"""
+    ts, es = _TYPES[dtype]
+    return torch.as_tensor(_Dev(int(ptr), (int(rows), int(cols)), (int(ld) * es, es), ts), device="cuda")
+
+
+def _snap(ptr, rows, cols, ld, dtype=torch.float16):
+    if not ptr or rows <= 0 or cols <= 0:
+        return None
+    return _dev(ptr, rows, cols, ld, dtype).clone(memory_format=torch.contiguous_format)
+
+
+def _vec(ptr, n, dtype=torch.float32):
+    return _snap(ptr, 1, n, n, dtype).flatten() if ptr else None
+
+
+def _spare(ptr, rows, c0, ld):
+    """bits of the spare columns [c0, ld) of rows 0 .. rows-2"""
+    if not ptr or rows < 2 or c0 >= ld:
+        return None
+    return _snap(ptr, rows - 1, ld, ld)[:, c0:].view(torch.int16)
+
+
+def _src_view(v):
+    rows = v["n"] * v["h"] * v["w"]
+    return _snap(v["ptr"], rows, v["c"], v["ld"]).reshape(v["n"], v["h"], v["w"], v["c"])
+
+
+def _kind_class(kind, d=None):
+    if kind in ("igemm", "tconv"):
+        if d["flags"] & R.IG_GEGLU:
+            return "geglu+ln" if d["colsum"] else "geglu"
+        return "contraction+ln" if d["colsum"] else "contraction"
+    return "attention" if kind == "attn" else "norm"
+
+
+class Auditor:
+    def __init__(self):
+        self.calls = 0
+        self.launches = collections.Counter()     # per class
+        self.checked = collections.Counter()
+        self.worst = collections.defaultdict(float)
+        self.worst_label = {}
+        self.wrong = collections.defaultdict(collections.Counter)
+        self.other = collections.Counter()
+        self.lnstat = 0.0
+        self.pending = None
+
+    def __call__(self, index, after, rec):
+        from ai_rtc_agent_b200.host import capi
+        kind = capi.LAUNCH_KINDS[rec.kind]
+        label = rec.label.decode()
+        if kind == "other":
+            if not after:
+                self.calls += 1
+                self.other[label.split(" ")[0]] += 1
+            return
+        if not after:
+            self.calls += 1
+            self.pending = (index, getattr(self, "_before_" + ("igemm" if kind == "tconv" else kind))(rec))
+        else:
+            assert self.pending and self.pending[0] == index
+            getattr(self, "_after_" + ("igemm" if kind == "tconv" else kind))(rec, kind, label, self.pending[1])
+            self.pending = None
+        torch.cuda.synchronize()
+
+    def _record(self, cls, label, units, wrongs):
+        self.launches[cls] += 1
+        atol, rtol = R.TOL[cls]
+        assert units <= 1.0, f"{label}: error {units:.3g}x the {cls} tolerance ({atol} rms + {rtol} |ref|)"
+        best = max(wrongs.values()) if wrongs else 0.0
+        assert wrongs and best >= 10.0, f"{label}: no wrong reference lands >= 10x the tolerance away ({wrongs})"
+        for name, m in wrongs.items():
+            if m >= 10.0:
+                self.wrong[cls][name] += 1
+        self.checked[cls] += 1
+        if units >= self.worst[cls]:
+            self.worst[cls], self.worst_label[cls] = units, label
+
+    # ---- contractions (igemm, tconv) ------------------------------------------------------------------------------------
+    def _before_igemm(self, rec):
+        d = R.as_dict(rec.igemm)
+        rows, ng = R.rows_of(d), R.n_gemm(d)
+        s = {"src": [_src_view(d["src"][i]) for i in range(d["nseg"])],
+             "w": _snap(d["w"], d["w_rows"], d["w_ld"], d["w_ld"]),
+             "colbias": _vec(d["colbias"], (d["nb"] - 1) * d["colbias_bstride"] + ng if d["colbias_bstride"] else ng),
+             "res": _snap(d["res"], rows, d["n_valid"], d["ldr"]),
+             "rowstat_in": _snap(d["rowstat_in"], rows, 2, 2, torch.int64),
+             "colsum": _vec(d["colsum"], ng),
+             "rowstat_out": _snap(d["rowstat_out"], rows, 2, 2, torch.int64)}
+        c_out = d["col2"] if d["out2"] else d["n_valid"]
+        s["spare"] = _spare(d["out"], rows, c_out, d["ldc"])
+        if d["out2"]:
+            s["spare2"] = _spare(d["out2"], d["n_valid"] - d["col2"], rows, d["ld2"])
+        return s
+
+    def _after_igemm(self, rec, kind, label, s):
+        d = R.as_dict(rec.igemm)
+        pl = R.as_dict(rec.plan)
+        cls = _kind_class(kind, d)
+        atol, rtol = R.TOL[cls]
+        rows, ng = R.rows_of(d), R.n_gemm(d)
+        k = sum(nt * c for _, _, nt, c in R.k_segments(d))
+        dtype = torch.float32 if 2.0 * rows * ng * k > R.BIG_FLOP else torch.float64
+        acc = R.contraction_acc(d, s["src"], s["w"], None, dtype)
+        def epi(a, dd=d, cb=s["colbias"], res=s["res"], rs=s["rowstat_in"]):
+            return R.epilogue(dd, a, cb, res, rs, s["colsum"])
+
+        ref = epi(acc)
+        main, tr = R.split_out2(d, ref)
+        got = _dev(d["out"], rows, main.shape[1], d["ldc"])
+        units = R.tol_units(got, main, atol, rtol)
+        if tr is not None:
+            got2 = _dev(d["out2"], tr.shape[0], rows, d["ld2"])
+            units = max(units, R.tol_units(got2, tr, atol, rtol))
+        wrongs = {}
+
+        def margin(name, wrong):
+            wm, wt = R.split_out2(d, wrong)
+            m = R.tol_units(wm, main, atol, rtol)
+            if wt is not None:
+                m = max(m, R.tol_units(wt, tr, atol, rtol))
+            wrongs[name] = m
+
+        if d["splits"] > 1:
+            km = R.split_k_lost_mask(d, pl["total_kb"], pl["kb_per_split"], acc.device)
+            margin("last split-K rank lost", epi(R.contraction_acc(d, s["src"], s["w"], km, dtype)))
+        else:
+            km = R.last_block_mask(d, s["w"])
+            margin("last non-zero K block dropped", epi(R.contraction_acc(d, s["src"], s["w"], km, dtype)))
+        if s["colbias"] is not None and d["colbias_bstride"] and d["nb"] > 1:
+            margin("image 0's bias for every image", epi(acc, dd=dict(d, colbias_bstride=0), cb=s["colbias"][:ng]))
+        if s["colsum"] is not None:
+            margin("neighbouring row's LayerNorm statistics", epi(acc, rs=torch.roll(s["rowstat_in"], 1, dims=0)))
+        if s["res"] is not None and d["res_scale"] != 0:
+            margin("residual omitted", epi(acc, res=None))
+        if s["rowstat_out"] is not None:   # the producer's fixed-point statistics of its stored fp16 rows
+            delta = (_dev(d["rowstat_out"], rows, 2, 2, torch.int64) - s["rowstat_out"]).double() / R.STAT_SCALE
+            want = R.rowstat_sums(got)
+            x = got.double()
+            bound = torch.stack([x.abs().sum(1), (x * x).sum(1)], dim=1) * 1e-4 + 1e-3
+            u = ((delta - want).abs() / bound).max().item()
+            self.lnstat = max(self.lnstat, u)
+            assert u <= 1.0, f"{label}: LayerNorm row statistics off by {u:.3g}x their bound"
+        if s["spare"] is not None:
+            c_out = d["col2"] if d["out2"] else d["n_valid"]
+            now = _dev(d["out"], rows - 1, d["ldc"], d["ldc"])[:, c_out:].view(torch.int16)
+            assert torch.equal(now, s["spare"]), f"{label}: stray write into the spare columns [{c_out}, {d['ldc']})"
+        if s.get("spare2") is not None:
+            now = _dev(d["out2"], d["n_valid"] - d["col2"] - 1, d["ld2"], d["ld2"])[:, rows:].view(torch.int16)
+            assert torch.equal(now, s["spare2"]), f"{label}: stray write into the V^T pad columns [{rows}, {d['ld2']})"
+        self._record(cls, label, units, wrongs)
+
+    # ---- attention ------------------------------------------------------------------------------------------------------
+    def _before_attn(self, rec):
+        a = R.as_dict(rec.attn)
+        w = a["heads"] * a["dp"]
+        return {"q": _snap(a["q"], a["nb"] * a["sq"], w, a["ldq"]), "k": _snap(a["k"], a["k_rows"], w, a["ldk"]),
+                "vt": _snap(a["vt"], w, a["vt_cols"], a["ldvt"]),
+                "spare": _spare(a["out"], a["nb"] * a["sq"], a["heads"] * a["d_real"], a["ldo"])}
+
+    def _after_attn(self, rec, kind, label, s):
+        a = R.as_dict(rec.attn)
+        atol, rtol = R.TOL["attention"]
+        ref = R.attention_ref(a, s["q"], s["k"], s["vt"])
+        got = _dev(a["out"], a["nb"] * a["sq"], a["heads"] * a["d_real"], a["ldo"])
+        units = R.tol_units(got, ref, atol, rtol)
+        bkv = 128 if a["dp"] in (64, 128) else 64
+        wrongs = {}
+        if a["skv"] > bkv:
+            wrongs["last KV block dropped"] = R.tol_units(R.attention_ref(a, s["q"], s["k"], s["vt"], drop_last_block=bkv), ref, atol, rtol)
+        else:
+            wrongs["last key dropped"] = R.tol_units(R.attention_ref(a, s["q"], s["k"], s["vt"], drop_last_block=1), ref, atol, rtol)
+        if a["nb"] > 1 and a["k_bstride"] > 0:
+            wrongs["image 0's K/V for every image"] = R.tol_units(R.attention_ref(a, s["q"], s["k"], s["vt"], kv_item0=True), ref, atol, rtol)
+        if a["dp"] != a["d_real"]:
+            wrongs["dp^-0.5 softmax scale"] = R.tol_units(R.attention_ref(a, s["q"], s["k"], s["vt"], dp_scale=True), ref, atol, rtol)
+        if s["spare"] is not None:
+            now = _dev(a["out"], a["nb"] * a["sq"] - 1, a["ldo"], a["ldo"])[:, a["heads"] * a["d_real"]:].view(torch.int16)
+            assert torch.equal(now, s["spare"]), f"{label}: stray write into the spare output columns"
+        self._record("attention", label, units, wrongs)
+
+    # ---- GroupNorm / LayerNorm ------------------------------------------------------------------------------------------
+    def _before_groupnorm(self, rec):
+        g = R.as_dict(rec.groupnorm)
+        rows, c = g["nb"] * g["hw"], g["ca"] + g["cb"]
+        return {"xa": _snap(g["xa"], rows, g["ca"], g["lda"]), "xb": _snap(g["xb"], rows, g["cb"], g["ldb"]) if g["xb"] else None,
+                "gamma": _vec(g["gamma"], c), "beta": _vec(g["beta"], c), "spare": _spare(g["y"], rows, c, g["ldy"])}
+
+    def _after_groupnorm(self, rec, kind, label, s):
+        g = R.as_dict(rec.groupnorm)
+        atol, rtol = R.TOL["norm"]
+        rows, c = g["nb"] * g["hw"], g["ca"] + g["cb"]
+        ref = R.groupnorm_ref(g, s["xa"], s["xb"], s["gamma"], s["beta"])
+        got = _dev(g["y"], rows, c, g["ldy"])
+        wrongs = {"neighbouring group's statistics":
+                  R.tol_units(R.groupnorm_ref(g, s["xa"], s["xb"], s["gamma"], s["beta"], shift_groups=True), ref, atol, rtol)}
+        if s["spare"] is not None:
+            assert torch.equal(_dev(g["y"], rows - 1, g["ldy"], g["ldy"])[:, c:].view(torch.int16), s["spare"]), \
+                f"{label}: stray write into the spare columns"
+        self._record("norm", label, R.tol_units(got, ref, atol, rtol), wrongs)
+
+    def _before_layernorm(self, rec):
+        l = R.as_dict(rec.layernorm)
+        return {"x": _snap(l["x"], l["rows"], l["c"], l["ldx"]), "gamma": _vec(l["gamma"], l["c"]),
+                "beta": _vec(l["beta"], l["c"]), "spare": _spare(l["y"], l["rows"], l["c"], l["ldy"])}
+
+    def _after_layernorm(self, rec, kind, label, s):
+        l = R.as_dict(rec.layernorm)
+        atol, rtol = R.TOL["norm"]
+        ref = R.layernorm_ref(l, s["x"], s["gamma"], s["beta"])
+        got = _dev(l["y"], l["rows"], l["c"], l["ldy"])
+        wrongs = {"neighbouring row's statistics":
+                  R.tol_units(R.layernorm_ref(l, s["x"], s["gamma"], s["beta"], shift_rows=True), ref, atol, rtol)}
+        if s["spare"] is not None:
+            assert torch.equal(_dev(l["y"], l["rows"] - 1, l["ldy"], l["ldy"])[:, l["c"]:].view(torch.int16), s["spare"]), \
+                f"{label}: stray write into the spare columns"
+        self._record("norm", label, R.tol_units(got, ref, atol, rtol), wrongs)
+
+    def table(self, name):
+        lines = [f"launch audit {name}: {self.calls} launches",
+                 f"  {'class':16s} {'launches':>8s} {'checked':>8s} {'worst/tol':>9s}  wrong references applied (worst launch)"]
+        for cls in sorted(self.launches):
+            wr = ", ".join(f"{k}: {v}" for k, v in sorted(self.wrong[cls].items()))
+            lines.append(f"  {cls:16s} {self.launches[cls]:8d} {self.checked[cls]:8d} {self.worst[cls]:9.3f}  {wr}  "
+                         f"({self.worst_label.get(cls, '')})")
+        lines.append("  other launches by label: " + ", ".join(f"{k}: {v}" for k, v in sorted(self.other.items())))
+        lines.append(f"  LayerNorm statistics producers: worst {self.lnstat:.3g}x their bound")
+        return "\n".join(lines)
+
+
+def _engine(turbo, tl, hw, full=False, concurrency=1, cn=False, hed=False, kl=False):
+    from ai_rtc_agent_b200.host import arch as A
+    from ai_rtc_agent_b200.host.stream import StreamDiffusion
+    from oracle import controlnet as ocn
+    from oracle import unet as ounet
+    from oracle import weights as ow
+    height, width = (hw, hw) if isinstance(hw, int) else hw
+    if full:
+        cfg, arch = (ounet.SD_TURBO, A.SD_TURBO) if turbo else (ounet.SD15, A.SD15)
+        varch = A.AUTOENCODER_KL
+    else:
+        cfg, arch, varch = ounet.tiny_config(turbo), (A.TINY_TURBO if turbo else A.TINY_SD15), A.TINY_AUTOENCODER_KL
+    usd = ow.make_unet_weights(cfg)
+    vsd = A.synthetic_autoencoder_kl(varch) if kl else ow.make_taesd_weights()
+    emb = ow.make_prompt_embeds(cfg.cross_attention_dim)
+    cn16 = ocn.make_weights(cfg) if cn else None
+    hed16 = {k: v.half().float() for k, v in A.synthetic_hed().items()} if hed else None
+    sd = StreamDiffusion(arch, usd, vsd, tl, lambda p: emb, width=width, height=height, device="cuda", use_tiny_vae=not kl,
+                         controlnet_sd=cn16, hed_sd=hed16)
+    if concurrency > 1:
+        sd.set_concurrency(concurrency)
+    sd.prepare("p", guidance_scale=0.0)
+    lane = sd.add_lane()
+    # a lane defaults to the launch policy of >= 2 frames in flight (other split-K factors, other summation order): give it
+    # the audited engine's policy, so that the two compute bit-identical frames
+    lane.set_concurrency(concurrency)
+    lane._prepare_like(sd)
+    return sd, lane
+
+
+_TINY = [
+    pytest.param(dict(turbo=True, tl=[32], hw=128), id="tiny-turbo-T1-128"),
+    pytest.param(dict(turbo=False, tl=_T4, hw=(128, 192)), id="tiny-sd15-T4-128x192"),
+    pytest.param(dict(turbo=False, tl=_T4, hw=192), id="tiny-sd15-T4-192"),             # unfolded transformer program: 36 / 9 tokens
+    pytest.param(dict(turbo=True, tl=[32], hw=192, cn=True, hed=True), id="tiny-turbo-T1-192-cn-hed"),
+    pytest.param(dict(turbo=False, tl=_T4, hw=128, kl=True), id="tiny-sd15-T4-128-kl"),
+]
+_FULL = [
+    pytest.param(dict(turbo=True, tl=[32], hw=512, concurrency=1), id="turbo-T1-512-c1"),
+    pytest.param(dict(turbo=True, tl=[32], hw=512, concurrency=8), id="turbo-T1-512-c8"),
+    pytest.param(dict(turbo=False, tl=_T4, hw=512, concurrency=1), id="sd15-T4-512-c1"),
+    pytest.param(dict(turbo=False, tl=_T4, hw=512, concurrency=4), id="sd15-T4-512-c4"),
+    pytest.param(dict(turbo=False, tl=_T4, hw=448, concurrency=1), id="sd15-T4-448-c1"),   # unfolded program at 14x14 (level 2)
+    pytest.param(dict(turbo=True, tl=[32], hw=512, cn=True, hed=True), id="turbo-T1-512-cn-hed"),
+    pytest.param(dict(turbo=True, tl=[32], hw=512, kl=True), id="turbo-T1-512-kl"),
+]
+
+
+def _release_device_memory():
+    """Engines allocate with cudaMalloc, outside torch's caching allocator: hand torch's cached blocks (earlier tests' references
+    and snapshots) back to the driver, and collect engines that only a reference cycle keeps alive (a parent and its lanes
+    refer to each other), so that each configuration starts with the HBM that it alone needs."""
+    gc.collect()
+    torch.cuda.empty_cache()
+
+
+def _audit(cuda, name, cfg, full):
+    from oracle import weights as ow
+    prev = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
+    sd = lane = None
+    _release_device_memory()
+    free0 = torch.cuda.mem_get_info()[0]
+    try:
+        t0 = time.time()
+        sd, lane = _engine(full=full, **cfg)
+        height, width = sd.height, sd.width
+        nframes = 2 if len(cfg["tl"]) > 1 else 1      # T = 4: the second frame runs on a non-zero latent buffer
+        frames = [ow.make_frame(height, width, seed=300 + i).cuda() for i in range(nframes)]
+        for f in frames[:-1]:
+            sd.step_u8(f)
+            lane.step_u8(f)
+        aud = Auditor()
+        got = sd.audit_step(frames[-1], aud).clone()
+        want = lane.step_u8(frames[-1])
+        torch.cuda.synchronize()
+        print("\n" + aud.table(name) + f"\n  wall time {time.time() - t0:.1f} s, "
+              f"free HBM at the start {free0 / 2**30:.1f} GiB")
+        assert aud.calls == sd.launches_per_step, (aud.calls, sd.launches_per_step)
+        for cls in aud.launches:
+            assert aud.checked[cls] == aud.launches[cls], cls
+        assert {"contraction", "attention", "norm"} <= set(aud.checked), dict(aud.checked)
+        assert torch.equal(got, want), "the audited frame differs from a graph step of an identical lane"
+    finally:
+        torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = prev
+        if sd is not None:
+            sd.lanes.clear()   # break the parent <-> lane cycle: both engines are destroyed here, not at some later collection
+        sd = lane = None
+        _release_device_memory()
+
+
+@pytest.mark.parametrize("cfg", _TINY)
+def test_launch_audit_tiny(cuda, request, cfg):
+    _audit(cuda, request.node.callspec.id, cfg, full=False)
+
+
+@pytest.mark.parametrize("cfg", _FULL)
+def test_launch_audit_full_size(cuda, request, cfg):
+    _audit(cuda, request.node.callspec.id, cfg, full=True)

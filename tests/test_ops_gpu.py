@@ -158,6 +158,54 @@ def test_self_attention_batch_tail_poisoned(cuda, seq, d, dp):
     assert_discriminates(out.view, ref, wrong_v, *ATTN_TOL, what, "batch item 0's values for every item")
 
 
+@pytest.mark.parametrize("seq", [36, 196])
+@pytest.mark.parametrize("d,dp", [(40, 64), (80, 128), (160, 192)])
+def test_self_attention_padded_vt_batch_stride(cuda, seq, d, dp):
+    """The transformer program for token counts that are not a multiple of 8 with several images (SD-1.5 at 192x192: 36 and 9
+    tokens; at 448x448: 196 and 49): K rows of image b start at b * seq, but V^T columns at b * seqp, seqp = seq rounded up to
+    8, because each image's V^T is its own GEMM into a column range whose origin the TMA unit needs 16-byte aligned.  The V^T
+    pad columns [b * seqp + seq, (b + 1) * seqp) hold poison (64) that only the skv mask keeps out of P.V, and the batch-tail
+    poison of test_self_attention_batch_tail_poisoned makes the keys item b's tail tile reads from item b+1 dominate its
+    softmax if unmasked.  Catches: V^T addressed with k_bstride, K addressed with vt_bstride, the pad columns or the tail
+    keys leaking in."""
+    ops = _ops()
+    from tests import launch_ref as R
+    nb, heads = 4, 2
+    seqp = -(-seq // 8) * 8
+    bkv = _bkv(dp)
+    tail = -(-seq // bkv) * bkv - seq
+    q = _rand((nb, heads, seq, d), cuda, 1)
+    k = _rand((nb, heads, seq, d), cuda, 2)
+    v = hetero((nb, heads, seq, d), (0, 1), 3, cuda, scale=(0.5, 2.0)).float()
+    q[..., :nb] = 0
+    k[..., :nb] = 0
+    big = 7.5 * math.sqrt(d)
+    for b in range(nb):
+        q[b, :, :, b] = 4.0
+        if b + 1 < nb:
+            k[b + 1, :, :min(tail, seq), b] = big
+            v[b + 1, :, :min(tail, seq)] += 16.0
+    q, k, v = q.half(), k.half(), v.half()
+    vt = torch.zeros(heads, dp, nb, seqp, dtype=torch.float16, device=cuda)
+    vt[:, :, :, seq:] = 64.0                             # pad columns of every image
+    vt[:, :d, :, :seq] = v.permute(1, 3, 0, 2)
+    vt = vt.reshape(heads * dp, nb * seqp)
+    qb, kb = _q_layout(q, dp), _q_layout(k, dp)
+    out = guarded((nb * seq, heads * d), pitch=heads * d + 64, device=cuda)
+    ops.attention(qb, kb, vt, out.view, nb=nb, heads=heads, sq=seq, skv=seq, d_real=d, dp=dp, k_bstride=seq, vt_bstride=seqp)
+    out.assert_untouched(f"self-attn out seq={seq} d={d}/{dp}")
+    a = {"nb": nb, "heads": heads, "sq": seq, "skv": seq, "d_real": d, "dp": dp, "k_bstride": seq, "vt_bstride": seqp}
+    ref = _attn64(q, k, v, d)
+    assert torch.allclose(R.attention_ref(a, qb, kb, vt), ref, rtol=1e-9, atol=1e-9)   # the layout above is what `a` describes
+    what = f"self-attn nb={nb} seq={seq} (V^T stride {seqp}) d={d}/{dp}"
+    assert_discriminates(out.view, ref, R.attention_ref(dict(a, vt_bstride=seq), qb, kb, vt), *ATTN_TOL, what,
+                         "V^T addressed with the K batch stride")
+    assert_discriminates(out.view, ref, R.attention_ref(dict(a, k_bstride=seqp), qb, torch.cat([kb, torch.zeros_like(kb)]), vt),
+                         *ATTN_TOL, what, "K addressed with the V^T batch stride")
+    assert_discriminates(out.view, ref, R.attention_ref(dict(a, skv=seqp), qb, torch.cat([kb, torch.zeros_like(kb[:8])]), vt),
+                         *ATTN_TOL, what, "V^T pad columns (and the keys past seq) not masked")
+
+
 @pytest.mark.parametrize("nb", [1, 4])
 @pytest.mark.parametrize("d,dp,heads", [(40, 64, 8), (64, 64, 5), (80, 128, 8), (160, 192, 8)])
 @pytest.mark.parametrize("rows", [128, 77])

@@ -117,11 +117,41 @@ struct Op {
     std::function<int(cudaStream_t)> fn;
     std::string name;
     double flops = 0.0;  // algorithmic 2*MAC count of the launch (0 for non-contraction kernels)
-    b2sd_launch_record rec{};   // what the launch computes (b2sd_audit_step); kind B2SD_LAUNCH_OTHER unless set where it is pushed
+    b2sd_launch_record rec{};   // what the launch computes (b2sd_audit_step / _refresh); set where it is pushed
     template <class F>
     Op(F f, std::string n = "", double fl = 0.0) : fn(std::move(f)), name(std::move(n)), flops(fl) {}
+    template <class F>
+    Op(F f, std::string n, const b2sd_launch_record& r) : fn(std::move(f)), name(std::move(n)), rec(r) {}
     int operator()(cudaStream_t s) const { return fn(s); }
 };
+
+// Launch records of the elementwise kernels: the launcher's arguments in the C ABI's terms
+b2sd_launch_record smallconv_record(const SmallConvArgs& a) {
+    b2sd_launch_record r{};
+    r.kind = B2SD_LAUNCH_SMALLCONV;
+    r.smallconv = b2sd_smallconv_args{a.x, a.wt, a.bias, a.y, a.ldy, a.nb, a.h, a.w_, a.cin, a.cout, a.in_h, a.in_w, a.flags,
+                                      a.res, a.ldr, (int64_t)a.res_bstride, a.in_off};
+    return r;
+}
+b2sd_launch_record upsample2x_record(const void* x, void* y, int nb, int h, int w, int c) {
+    b2sd_launch_record r{};
+    r.kind = B2SD_LAUNCH_UPSAMPLE2X;
+    r.upsample2x = b2sd_upsample2x_args{x, y, nb, h, w, c};
+    return r;
+}
+b2sd_launch_record post_u8_record(const void* y, int ldy, void* out, int nb, int h, int w) {
+    b2sd_launch_record r{};
+    r.kind = B2SD_LAUNCH_POST_U8;
+    r.post_u8 = b2sd_post_u8_args{y, ldy, out, nb, h, w};
+    return r;
+}
+b2sd_launch_record small_linear_record(const float* in, int in_ld, const void* w, const float* bias, float* out, int out_ld,
+                                       int nb, int n, int k, int silu_in) {
+    b2sd_launch_record r{};
+    r.kind = B2SD_LAUNCH_SMALL_LINEAR;
+    r.small_linear = b2sd_small_linear_args{in, in_ld, w, bias, out, out_ld, nb, n, k, silu_in};
+    return r;
+}
 
 }  // namespace
 
@@ -718,7 +748,8 @@ int b2sd_engine::build_resnet(const std::string& p, const Act& xa, const Act* xb
             if (!cb || !bsum || !wt) return -1;
             const int tdim = (int)wt->shape[1];
             const __half* wtp = wt->p;
-            prog_time.push_back(Op([=](cudaStream_t st) { return small_linear_launch(emb, tdim, wtp, bsum, cb, cout, B, cout, tdim, 1, st); }, "temb " + p));
+            prog_time.push_back(Op([=](cudaStream_t st) { return small_linear_launch(emb, tdim, wtp, bsum, cb, cout, B, cout, tdim, 1, st); }, "temb " + p,
+                                   small_linear_record(emb, tdim, wtp, bsum, cb, cout, B, cout, tdim, 1)));
             colbias = cb;
         } else {
             colbias = vec({p + "conv1.bias"}, nullptr, 16);
@@ -1010,7 +1041,8 @@ int b2sd_engine::build_cond_embedding(Act* out, cudaStream_t s) {
         TRY(build_hed(&control, s));
         SmallConvArgs c = cn_head;
         c.x = control; c.in_h = a.h; c.in_w = a.w; c.flags = SC_IN_U8 | SC_OUT_SILU;
-        prog_frame.push_back(Op([c](cudaStream_t st) { return smallconv_launch(c, st); }, "smallconv controlnet_cond_embedding.conv_in"));
+        prog_frame.push_back(Op([c](cudaStream_t st) { return smallconv_launch(c, st); }, "smallconv controlnet_cond_embedding.conv_in",
+                                smallconv_record(c)));
     }
     static const int cout[6] = {16, 32, 32, 96, 96, 256}, stride[6] = {1, 2, 1, 2, 1, 2};
     for (int k = 0; k < 6; ++k) {
@@ -1052,7 +1084,10 @@ int b2sd_engine::build_hed(const uint8_t** control, cudaStream_t s) {
             if (!o.p) return -1;
             const Act x = a;
             ++launches;
-            prog_frame.push_back(Op([x, o](cudaStream_t st) { return maxpool2x2_launch(x.p, o.p, 1, x.h, x.w, x.c, st); }, "maxpool2x2 " + p));
+            b2sd_launch_record r{};
+            r.kind = B2SD_LAUNCH_MAXPOOL2X2;
+            r.maxpool2x2 = b2sd_maxpool2x2_args{x.p, o.p, 1, x.h, x.w, x.c};
+            prog_frame.push_back(Op([x, o](cudaStream_t st) { return maxpool2x2_launch(x.p, o.p, 1, x.h, x.w, x.c, st); }, "maxpool2x2 " + p, r));
             a = o;
         }
         for (int k = b == 0 ? 1 : 0; k < nconv[b]; ++k) {
@@ -1067,8 +1102,11 @@ int b2sd_engine::build_hed(const uint8_t** control, cudaStream_t s) {
         if (!m || !pw || !pb) return -1;
         const Act x = a;
         ++launches;
+        b2sd_launch_record r{};
+        r.kind = B2SD_LAUNCH_HED_PROJECT;
+        r.hed_project = b2sd_hed_project_args{x.p, x.ld, x.c, (int64_t)x.h * x.w, pw, pb, m};
         prog_frame.push_back(Op([x, pw, pb, m](cudaStream_t st) { return hed_project_launch(x.p, x.ld, x.c, (long)x.h * x.w, pw, pb, m, st); },
-                                "hed_project " + p));
+                                "hed_project " + p, r));
         f.maps[b] = m; f.hs[b] = a.h; f.ws[b] = a.w;
     }
     f.levels = 5; f.h = H; f.w = W;
@@ -1077,7 +1115,11 @@ int b2sd_engine::build_hed(const uint8_t** control, cudaStream_t s) {
     if (!f.out || !edge.p) return -1;
     f.edge_f16 = edge.p;
     ++launches;
-    prog_frame.push_back(Op([f](cudaStream_t st) { return hed_fuse_launch(f, st); }, "hed_fuse"));
+    b2sd_launch_record r{};
+    r.kind = B2SD_LAUNCH_HED_FUSE;
+    for (int k = 0; k < 5; ++k) { r.hed_fuse.maps[k] = f.maps[k]; r.hed_fuse.hs[k] = f.hs[k]; r.hed_fuse.ws[k] = f.ws[k]; }
+    r.hed_fuse.levels = f.levels; r.hed_fuse.h = f.h; r.hed_fuse.w = f.w; r.hed_fuse.out = f.out; r.hed_fuse.edge_f16 = f.edge_f16;
+    prog_frame.push_back(Op([f](cudaStream_t st) { return hed_fuse_launch(f, st); }, "hed_fuse", r));
     taps["control"] = edge;
     *control = f.out;
     return 0;
@@ -1102,7 +1144,7 @@ int b2sd_engine::build_controlnet(const Act& cond, std::vector<Act>& skips, Act*
         a.x = x_in.p; a.y = h.p; a.ldy = h.ld; a.nb = B; a.h = lh; a.w_ = lw; a.cin = 4; a.cout = ch[0]; a.in_h = lh; a.in_w = lw;
         a.res = cond.p; a.ldr = cond.ld; a.res_bstride = 0;
         ++launches;
-        prog_frame.push_back(Op([a](cudaStream_t st) { return smallconv_launch(a, st); }, "smallconv controlnet.conv_in"));
+        prog_frame.push_back(Op([a](cudaStream_t st) { return smallconv_launch(a, st); }, "smallconv controlnet.conv_in", smallconv_record(a)));
     }
     taps["cn.conv_in"] = h;
     std::vector<Act> feats{h};
@@ -1402,7 +1444,7 @@ int b2sd_engine::build_kl_decoder(const Act& x0, cudaStream_t s) {
         a.y = h.p; a.ldy = h.ld; a.nb = 1; a.h = lh; a.w_ = lw; a.cin = 4; a.cout = cm; a.in_h = lh; a.in_w = lw;
         a.res = bmap.p; a.ldr = bmap.ld; a.res_bstride = 0;
         ++launches;
-        prog_frame.push_back(Op([a](cudaStream_t st) { return smallconv_launch(a, st); }, "smallconv vae.decoder.conv_in"));
+        prog_frame.push_back(Op([a](cudaStream_t st) { return smallconv_launch(a, st); }, "smallconv vae.decoder.conv_in", smallconv_record(a)));
     }
     {
         Act o;
@@ -1424,7 +1466,8 @@ int b2sd_engine::build_kl_decoder(const Act& x0, cudaStream_t s) {
             Act up = new_act(1, h.h * 2, h.w * 2, h.c);
             const Act hin = h;
             ++launches;
-            prog_frame.push_back(Op([hin, up](cudaStream_t st) { return upsample2x_launch(hin.p, up.p, hin.n, hin.h, hin.w, hin.c, st); }, "upsample2x"));
+            prog_frame.push_back(Op([hin, up](cudaStream_t st) { return upsample2x_launch(hin.p, up.p, hin.n, hin.h, hin.w, hin.c, st); }, "upsample2x",
+                                    upsample2x_record(hin.p, up.p, hin.n, hin.h, hin.w, hin.c)));
             Act o = new_act(1, up.h, up.w, h.c);
             TRY(add_conv(prog_frame, up, bp + ".upsamplers.0.conv.weight", bp + ".upsamplers.0.conv.bias", 9, 1, o, 0, nullptr, s));
             h = o;
@@ -1535,7 +1578,7 @@ int b2sd_engine::build_program(cudaStream_t s) {
         a.y = h.p; a.ldy = h.ld; a.nb = B; a.h = lh; a.w_ = lw; a.cin = 4; a.cout = ch[0]; a.in_h = lh; a.in_w = lw;
         if (!a.bias) return -1;
         ++launches;
-        prog_frame.push_back(Op([a](cudaStream_t st) { return smallconv_launch(a, st); }, "smallconv"));
+        prog_frame.push_back(Op([a](cudaStream_t st) { return smallconv_launch(a, st); }, "smallconv", smallconv_record(a)));
     }
     taps["conv_in"] = h;
     std::vector<Act> skips{h};
@@ -1591,7 +1634,8 @@ int b2sd_engine::build_program(cudaStream_t s) {
             Act up = new_act(B, h.h * 2, h.w * 2, co);
             const Act hin = h;
             ++launches;
-            prog_frame.push_back(Op([hin, up](cudaStream_t st) { return upsample2x_launch(hin.p, up.p, hin.n, hin.h, hin.w, hin.c, st); }, "upsample2x"));
+            prog_frame.push_back(Op([hin, up](cudaStream_t st) { return upsample2x_launch(hin.p, up.p, hin.n, hin.h, hin.w, hin.c, st); }, "upsample2x",
+                                    upsample2x_record(hin.p, up.p, hin.n, hin.h, hin.w, hin.c)));
             Act o = new_act(B, up.h, up.w, co);
             const std::string k = "up_blocks." + std::to_string(i) + ".upsamplers.0.conv.";
             TRY(add_conv(prog_frame, up, k + "weight", k + "bias", 9, 1, o, 0, nullptr, s));
@@ -1609,7 +1653,10 @@ int b2sd_engine::build_program(cudaStream_t s) {
         __half* xp = x_in.p; const __half* ep = eps.p; const __half* np_ = noise; const float* cf = coef; __half* op = x0.p;
         const int T = B, hw = lh * lw, dan = cfg.do_add_noise;
         ++launches;
-        prog_frame.push_back(Op([=](cudaStream_t st) { return lcm_step_launch(xp, ep, np_, cf, op, T, hw, dan, st); }, "lcm_step"));
+        b2sd_launch_record r{};
+        r.kind = B2SD_LAUNCH_LCM_STEP;
+        r.lcm_step = b2sd_lcm_step_args{xp, ep, np_, cf, op, T, hw, dan};
+        prog_frame.push_back(Op([=](cudaStream_t st) { return lcm_step_launch(xp, ep, np_, cf, op, T, hw, dan, st); }, "lcm_step", r));
         idx_unet_end = prog_frame.size();
     }
     taps["x0"] = x0;
@@ -1628,7 +1675,7 @@ int b2sd_engine::build_program(cudaStream_t s) {
         a.flags = SC_IN_TANH3 | SC_OUT_RELU;
         if (!a.bias) return -1;
         ++launches;
-        prog_frame.push_back(Op([a](cudaStream_t st) { return smallconv_launch(a, st); }, "smallconv"));
+        prog_frame.push_back(Op([a](cudaStream_t st) { return smallconv_launch(a, st); }, "smallconv", smallconv_record(a)));
     }
     li = 2;
     const int dec_blocks[4] = {3, 3, 3, 1};
@@ -1643,7 +1690,8 @@ int b2sd_engine::build_program(cudaStream_t s) {
             Act up = new_act(1, dcur.h * 2, dcur.w * 2, 64);
             const Act hin = dcur;
             ++launches;
-            prog_frame.push_back(Op([hin, up](cudaStream_t s2) { return upsample2x_launch(hin.p, up.p, hin.n, hin.h, hin.w, hin.c, s2); }, "upsample2x"));
+            prog_frame.push_back(Op([hin, up](cudaStream_t s2) { return upsample2x_launch(hin.p, up.p, hin.n, hin.h, hin.w, hin.c, s2); }, "upsample2x",
+                                    upsample2x_record(hin.p, up.p, hin.n, hin.h, hin.w, hin.c)));
             ++li;  // nn.Upsample
             Act o = new_act(1, up.h, up.w, 64);
             TRY(add_conv(prog_frame, up, "vae.decoder.layers." + std::to_string(li) + ".weight", "", 9, 1, o, 0, nullptr, s));
@@ -1859,21 +1907,39 @@ int b2sd_load_tensor(b2sd_handle h, const char* key, const void* ptr, int dtype,
     return 0;
 }
 
-// TimestepEmbedding of the UNet (and of the ControlNet, from the same sinusoidal features), then every resnet's projection
-static int refresh_time(b2sd_handle h, cudaStream_t s) {
+// TimestepEmbedding of the UNet (and of the ControlNet, from the same sinusoidal features): the launches that precede prog_time,
+// with their launch records
+static int time_embedding_ops(b2sd_handle h, std::vector<Op>* ops) {
     const int B = h->cfg.batch, C0 = h->cfg.block_out_channels[0], TD = 4 * C0;
-    TRY(timestep_embedding_launch(h->tsteps, h->temb_sin, B, C0, s));
+    const float* t = h->tsteps;
+    float* sin_ = h->temb_sin;
+    b2sd_launch_record r{};
+    r.kind = B2SD_LAUNCH_TIMESTEP_EMBEDDING;
+    r.timestep_embedding = b2sd_timestep_embedding_args{t, sin_, B, C0};
+    ops->push_back(Op([=](cudaStream_t st) { return timestep_embedding_launch(t, sin_, B, C0, st); }, "timestep_embedding", r));
     auto embed = [&](const std::string& p, float* hid, float* out) {
         const Raw* w1 = h->get(p + "time_embedding.linear_1.weight");
         const Raw* w2 = h->get(p + "time_embedding.linear_2.weight");
         const float* b1 = h->vec({p + "time_embedding.linear_1.bias"});
         const float* b2v = h->vec({p + "time_embedding.linear_2.bias"});
         if (!w1 || !w2 || !b1 || !b2v) return -1;
-        TRY(small_linear_launch(h->temb_sin, C0, w1->p, b1, hid, TD, B, TD, C0, 0, s));
-        return small_linear_launch(hid, TD, w2->p, b2v, out, TD, B, TD, TD, 1, s);
+        const __half *w1p = w1->p, *w2p = w2->p;
+        ops->push_back(Op([=](cudaStream_t st) { return small_linear_launch(sin_, C0, w1p, b1, hid, TD, B, TD, C0, 0, st); },
+                          p + "time_embedding.linear_1", small_linear_record(sin_, C0, w1p, b1, hid, TD, B, TD, C0, 0)));
+        ops->push_back(Op([=](cudaStream_t st) { return small_linear_launch(hid, TD, w2p, b2v, out, TD, B, TD, TD, 1, st); },
+                          p + "time_embedding.linear_2", small_linear_record(hid, TD, w2p, b2v, out, TD, B, TD, TD, 1)));
+        return 0;
     };
     TRY(embed("", h->temb_h, h->temb));
     if (h->cfg.controlnet) TRY(embed("controlnet.", h->cn_temb_h, h->cn_temb));
+    return 0;
+}
+
+// the time embeddings, then every resnet's projection
+static int refresh_time(b2sd_handle h, cudaStream_t s) {
+    std::vector<Op> ops;
+    TRY(time_embedding_ops(h, &ops));
+    TRY(h->run_range(ops, 0, ops.size(), s));
     return h->run(h->prog_time, s);
 }
 
@@ -2263,8 +2329,43 @@ int b2sd_profile(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* 
     return 0;
 }
 
-// b2sd_step with the frame program run eagerly and the caller's check around every kernel launch (see b2sd.h).  Test aid: the
-// stream is synchronised twice per launch.
+// The caller's check around every kernel launch of b2sd_audit_step / b2sd_audit_refresh (see b2sd.h).  Test aid: the stream is
+// synchronised twice per launch.
+struct Audited {
+    const char* entry;
+    b2sd_audit_fn fn;
+    void* user;
+    cudaStream_t s;
+    int index = 0;
+    int launch(b2sd_launch_record rec, const char* label, const std::function<int()>& run) {
+        rec.label = label;
+        CUDA_OK(cudaStreamSynchronize(s));
+        if (fn(user, index, 0, &rec)) {
+            b2_set_error("%s: launch %d '%s' rejected before it ran", entry, index, label);
+            return -1;
+        }
+        TRY(run());
+        CUDA_OK(cudaStreamSynchronize(s));
+        if (fn(user, index, 1, &rec)) {
+            b2_set_error("%s: launch %d '%s' failed its check", entry, index, label);
+            return -1;
+        }
+        ++index;
+        return 0;
+    }
+    int program(std::vector<Op>& ops) {
+        for (auto& op : ops) {
+            if (op.name.compare(0, 7, "memset ") == 0) {   // a memset node, not a kernel launch
+                TRY(op(s));
+                continue;
+            }
+            TRY(launch(op.rec, op.name.c_str(), [&] { return op(s); }));
+        }
+        return 0;
+    }
+};
+
+// b2sd_step with the frame program run eagerly
 int b2sd_audit_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* frame_out, b2sd_audit_fn fn, void* user,
                     void* stream) {
     if (!h || !h->built || !fn || !frame_in || !frame_out || in_h < 1 || in_w < 1) {
@@ -2276,48 +2377,41 @@ int b2sd_audit_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, voi
         return -1;
     }
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    int index = 0;
-    auto audited = [&](b2sd_launch_record rec, const char* label, const std::function<int()>& launch) -> int {
-        rec.label = label;
-        CUDA_OK(cudaStreamSynchronize(s));
-        if (fn(user, index, 0, &rec)) {
-            b2_set_error("b2sd_audit_step: launch %d '%s' rejected before it ran", index, label);
-            return -1;
-        }
-        TRY(launch());
-        CUDA_OK(cudaStreamSynchronize(s));
-        if (fn(user, index, 1, &rec)) {
-            b2_set_error("b2sd_audit_step: launch %d '%s' failed its check", index, label);
-            return -1;
-        }
-        ++index;
-        return 0;
-    };
-    const b2sd_launch_record other{};
+    Audited au{"b2sd_audit_step", fn, user, s};
+    // the input heads and the tail as b2sd_step_ex launches them for a u8 frame, with the caller's frame and size
     SmallConvArgs a = h->head;
     a.x = frame_in; a.in_h = in_h; a.in_w = in_w; a.flags = SC_IN_U8 | (h->head.flags & SC_IN_OFFSET);
-    TRY(audited(other, "smallconv head", [&] { return smallconv_launch(a, s); }));
+    TRY(au.launch(smallconv_record(a), "smallconv head", [&] { return smallconv_launch(a, s); }));
     if (h->cfg.controlnet) {
         const bool hed = h->cfg.control_processor == B2SD_CONTROL_HED;
         SmallConvArgs c = hed ? h->hed_head : h->cn_head;
         c.x = frame_in; c.in_h = in_h; c.in_w = in_w; c.flags = SC_IN_U8 | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
-        TRY(audited(other, hed ? "smallconv hed head" : "smallconv controlnet head", [&] { return smallconv_launch(c, s); }));
+        TRY(au.launch(smallconv_record(c), hed ? "smallconv hed head" : "smallconv controlnet head",
+                      [&] { return smallconv_launch(c, s); }));
     }
-    for (auto& op : h->prog_frame) {
-        if (op.name.compare(0, 7, "memset ") == 0) {   // a memset node, not a kernel launch
-            TRY(op(s));
-            continue;
-        }
-        TRY(audited(op.rec, op.name.c_str(), [&] { return op(s); }));
-    }
-    TRY(audited(other, "post_u8", [&] {
-        return post_u8_launch(h->image.p, h->image.ld, static_cast<uint8_t*>(frame_out), 1, h->cfg.height, h->cfg.width, s);
-    }));
-    if (index != h->launches) {
-        b2_set_error("b2sd_audit_step: %d launches audited, %d expected", index, h->launches);
+    TRY(au.program(h->prog_frame));
+    uint8_t* out = static_cast<uint8_t*>(frame_out);
+    TRY(au.launch(post_u8_record(h->image.p, h->image.ld, out, 1, h->cfg.height, h->cfg.width), "post_u8",
+                  [&] { return post_u8_launch(h->image.p, h->image.ld, out, 1, h->cfg.height, h->cfg.width, s); }));
+    if (au.index != h->launches) {
+        b2_set_error("b2sd_audit_step: %d launches audited, %d expected", au.index, h->launches);
         return -1;
     }
     return 0;
+}
+
+// b2sd_prepare's refresh (prompt program, then refresh_time) run eagerly
+int b2sd_audit_refresh(b2sd_handle h, b2sd_audit_fn fn, void* user, void* stream) {
+    if (!h || !h->built || !fn) {
+        b2_set_error("b2sd_audit_refresh: bad arguments (or b2sd_prepare not called)");
+        return -1;
+    }
+    Audited au{"b2sd_audit_refresh", fn, user, reinterpret_cast<cudaStream_t>(stream)};
+    std::vector<Op> time_ops;
+    TRY(time_embedding_ops(h, &time_ops));
+    TRY(au.program(h->prog_prompt));
+    TRY(au.program(time_ops));
+    return au.program(h->prog_time);
 }
 
 // Start gate for concurrent b2sd_profile_kind calls (one host thread per lane): every call finishes its capture / instantiation /

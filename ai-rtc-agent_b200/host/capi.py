@@ -71,16 +71,70 @@ class LayerNormArgs(C.Structure):
     ]
 
 
-LAUNCH_OTHER, LAUNCH_IGEMM, LAUNCH_TCONV, LAUNCH_ATTN, LAUNCH_GROUPNORM, LAUNCH_LAYERNORM = range(6)
+class SmallConvArgs(C.Structure):
+    _fields_ = [
+        ("x", C.c_void_p), ("wt", C.c_void_p), ("bias", C.c_void_p), ("y", C.c_void_p), ("ldy", C.c_int),
+        ("nb", C.c_int), ("h", C.c_int), ("w", C.c_int), ("cin", C.c_int), ("cout", C.c_int), ("in_h", C.c_int),
+        ("in_w", C.c_int), ("flags", C.c_int), ("res", C.c_void_p), ("ldr", C.c_int), ("res_bstride", C.c_int64),
+        ("in_off", C.c_void_p),
+    ]
+
+
+class Upsample2xArgs(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("y", C.c_void_p), ("nb", C.c_int), ("h", C.c_int), ("w", C.c_int), ("c", C.c_int)]
+
+
+class MaxPool2x2Args(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("y", C.c_void_p), ("nb", C.c_int), ("h", C.c_int), ("w", C.c_int), ("c", C.c_int)]
+
+
+class HedProjectArgs(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("ldx", C.c_int), ("c", C.c_int), ("npix", C.c_int64), ("w", C.c_void_p),
+                ("bias", C.c_void_p), ("out", C.c_void_p)]
+
+
+class HedFuseArgs(C.Structure):
+    _fields_ = [("maps", C.c_void_p * 5), ("hs", C.c_int * 5), ("ws", C.c_int * 5), ("levels", C.c_int), ("h", C.c_int),
+                ("w", C.c_int), ("out", C.c_void_p), ("edge_f16", C.c_void_p)]
+
+
+class LcmStepArgs(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("eps", C.c_void_p), ("noise", C.c_void_p), ("coef", C.c_void_p),
+                ("out_latent", C.c_void_p), ("T", C.c_int), ("hw", C.c_int), ("do_add_noise", C.c_int)]
+
+
+class PostU8Args(C.Structure):
+    _fields_ = [("y", C.c_void_p), ("ldy", C.c_int), ("out", C.c_void_p), ("nb", C.c_int), ("h", C.c_int), ("w", C.c_int)]
+
+
+class SmallLinearArgs(C.Structure):
+    _fields_ = [("in", C.c_void_p), ("in_ld", C.c_int), ("w", C.c_void_p), ("bias", C.c_void_p), ("out", C.c_void_p),
+                ("out_ld", C.c_int), ("nb", C.c_int), ("n", C.c_int), ("k", C.c_int), ("silu_in", C.c_int)]
+
+
+class TimestepEmbeddingArgs(C.Structure):
+    _fields_ = [("t", C.c_void_p), ("out", C.c_void_p), ("nb", C.c_int), ("dim", C.c_int)]
+
+
+(LAUNCH_OTHER, LAUNCH_IGEMM, LAUNCH_TCONV, LAUNCH_ATTN, LAUNCH_GROUPNORM, LAUNCH_LAYERNORM, LAUNCH_SMALLCONV, LAUNCH_UPSAMPLE2X,
+ LAUNCH_MAXPOOL2X2, LAUNCH_HED_PROJECT, LAUNCH_HED_FUSE, LAUNCH_LCM_STEP, LAUNCH_POST_U8, LAUNCH_SMALL_LINEAR,
+ LAUNCH_TIMESTEP_EMBEDDING) = range(15)
 LAUNCH_KINDS = {LAUNCH_OTHER: "other", LAUNCH_IGEMM: "igemm", LAUNCH_TCONV: "tconv", LAUNCH_ATTN: "attn",
-                LAUNCH_GROUPNORM: "groupnorm", LAUNCH_LAYERNORM: "layernorm"}
+                LAUNCH_GROUPNORM: "groupnorm", LAUNCH_LAYERNORM: "layernorm", LAUNCH_SMALLCONV: "smallconv",
+                LAUNCH_UPSAMPLE2X: "upsample2x", LAUNCH_MAXPOOL2X2: "maxpool2x2", LAUNCH_HED_PROJECT: "hed_project",
+                LAUNCH_HED_FUSE: "hed_fuse", LAUNCH_LCM_STEP: "lcm_step", LAUNCH_POST_U8: "post_u8",
+                LAUNCH_SMALL_LINEAR: "small_linear", LAUNCH_TIMESTEP_EMBEDDING: "timestep_embedding"}
 
 
 class LaunchRecord(C.Structure):
+    """b2sd_launch_record: the member named like the kind (LAUNCH_KINDS) holds the launch's arguments"""
     _fields_ = [
         ("kind", C.c_int), ("label", C.c_char_p),
         ("igemm", IgemmDesc), ("plan", IgemmPlanInfo), ("attn", AttnDesc),
         ("groupnorm", GroupNormArgs), ("layernorm", LayerNormArgs),
+        ("smallconv", SmallConvArgs), ("upsample2x", Upsample2xArgs), ("maxpool2x2", MaxPool2x2Args),
+        ("hed_project", HedProjectArgs), ("hed_fuse", HedFuseArgs), ("lcm_step", LcmStepArgs), ("post_u8", PostU8Args),
+        ("small_linear", SmallLinearArgs), ("timestep_embedding", TimestepEmbeddingArgs),
     ]
 
 
@@ -172,6 +226,8 @@ def lib() -> C.CDLL:
         _lib.b2sd_profile_gate.restype = C.c_int
         _lib.b2sd_audit_step.argtypes = [vp, vp, ci, ci, vp, AUDIT_FN, vp, vp]
         _lib.b2sd_audit_step.restype = C.c_int
+        _lib.b2sd_audit_refresh.argtypes = [vp, AUDIT_FN, vp, vp]
+        _lib.b2sd_audit_refresh.restype = C.c_int
         for name in ("create", "create_lane", "destroy", "load_tensor", "prepare", "export_packed", "import_packed", "set_prompt_embeds", "set_timesteps", "step",
                      "step_ex", "get_tensor", "launches_per_step"):
             getattr(_lib, "b2sd_" + name).restype = C.c_int

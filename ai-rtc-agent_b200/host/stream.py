@@ -422,6 +422,27 @@ class StreamDiffusion:
         capi.check(rc, "b2sd_audit_step")
         return out
 
+    @torch.no_grad()
+    def audit_refresh(self, fn: Callable[[int, bool, "capi.LaunchRecord"], None]) -> None:
+        """The prompt / timestep refresh of prepare (cross-attention K / V^T of the prompt, time embeddings, every resnet's
+        per-slot time bias) run eagerly, with fn called around every kernel launch as in audit_step (b2sd_audit_refresh).
+        It recomputes what prepare computed.  Test aid."""
+        self._check()
+        failure = []
+
+        def cb(_user, index, after, rec):
+            try:
+                fn(index, bool(after), rec.contents)
+                return 0
+            except BaseException as e:   # an exception cannot cross the C frames: keep it and abort the refresh
+                failure.append(e)
+                return 1
+
+        rc = self._lib.b2sd_audit_refresh(self._handle, capi.AUDIT_FN(cb), None, self._stream())
+        if failure:
+            raise failure[0]
+        capi.check(rc, "b2sd_audit_refresh")
+
     @property
     def launches_per_step(self) -> int:
         return self._lib.b2sd_launches_per_step(self._handle)

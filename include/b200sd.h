@@ -291,9 +291,13 @@ int b2sd_launches_per_step(b2sd_handle h);
 /* Launch audit (test aid, like b2sd_profile): what each launch of the frame program computes, as it is launched.
  * kind B2SD_LAUNCH_IGEMM / _TCONV: `igemm` is the contraction with the plan's bn / splits / swap and B2SD_IG_PAIR /
  * B2SD_IG_TCONV in flags (partial = NULL), `plan` the plan (for the halo-tile kernel only bn 64, splits 1 and rows_total);
- * _ATTN: `attn`; _GROUPNORM / _LAYERNORM: the normalisation's arguments; _OTHER: only `label` (the profiling label). */
+ * _ATTN: `attn`; _GROUPNORM / _LAYERNORM: the normalisation's arguments; every other kind: its launcher's arguments in the
+ * member of the same name (smallconv, upsample2x, ...).  _OTHER: only `label` (the profiling label), the kind of a record that
+ * nobody filled: both audit entry points fill every launch they issue. */
 enum { B2SD_LAUNCH_OTHER = 0, B2SD_LAUNCH_IGEMM = 1, B2SD_LAUNCH_TCONV = 2, B2SD_LAUNCH_ATTN = 3, B2SD_LAUNCH_GROUPNORM = 4,
-       B2SD_LAUNCH_LAYERNORM = 5 };
+       B2SD_LAUNCH_LAYERNORM = 5, B2SD_LAUNCH_SMALLCONV = 6, B2SD_LAUNCH_UPSAMPLE2X = 7, B2SD_LAUNCH_MAXPOOL2X2 = 8,
+       B2SD_LAUNCH_HED_PROJECT = 9, B2SD_LAUNCH_HED_FUSE = 10, B2SD_LAUNCH_LCM_STEP = 11, B2SD_LAUNCH_POST_U8 = 12,
+       B2SD_LAUNCH_SMALL_LINEAR = 13, B2SD_LAUNCH_TIMESTEP_EMBEDDING = 14 };
 typedef struct {
     const void* xa; int ca, lda;
     const void* xb; int cb, ldb;   /* xb NULL: no second source */
@@ -310,6 +314,45 @@ typedef struct {
     int64_t rows; int c;
     float eps;
 } b2sd_layernorm_args;
+/* direct 3x3 conv (b2sd_op_smallconv_ex): x read per flags (1 u8 NHWC / 255, 8 fp32 NCHW, 16 fp16 NCHW, else fp16 NHWC; 2 =
+ * tanh(x/3)*3; 64 = u8 or NCHW value on the 0..255 scale minus in_off[c]), nearest-resized from in_h x in_w to h x w, rounded to
+ * fp16, convolved with wt = fp32 [cin*9][cout] (k = tap*cin + c, pad 1), + bias, + res (item n at res + n*res_bstride, pitch
+ * ldr), then 4 = ReLU / 32 = SiLU; fp16 out, columns [cout, ldy) untouched */
+typedef struct {
+    const void* x; const float* wt; const float* bias;
+    void* y; int ldy;
+    int nb, h, w, cin, cout, in_h, in_w, flags;
+    const void* res; int ldr; int64_t res_bstride;
+    const float* in_off;
+} b2sd_smallconv_args;
+/* nearest x2 upsampling, NHWC fp16 [nb][h][w][c] -> [nb][2h][2w][c] (both dense) */
+typedef struct { const void* x; void* y; int nb, h, w, c; } b2sd_upsample2x_args;
+/* 2x2 / 2 max-pool, NHWC fp16 [nb][h][w][c] -> [nb][h/2][w/2][c] (both dense) */
+typedef struct { const void* x; void* y; int nb, h, w, c; } b2sd_maxpool2x2_args;
+/* out[p] = bias[0] + sum_c x[p*ldx + c] * w[c], fp32 out [npix] */
+typedef struct { const void* x; int ldx, c; int64_t npix; const float* w; const float* bias; float* out; } b2sd_hed_project_args;
+/* see b2sd_op_hed_fuse */
+typedef struct {
+    const float* maps[5]; int hs[5], ws[5];
+    int levels, h, w;
+    void* out; void* edge_f16;
+} b2sd_hed_fuse_args;
+/* see b2sd_op_lcm_step: x (rewritten in place: slots 1..T-1) and eps fp16 [T][hw][4], coef fp32 [4][T] */
+typedef struct {
+    void* x; const void* eps; const void* noise; const float* coef; void* out_latent;
+    int T, hw, do_add_noise;
+} b2sd_lcm_step_args;
+/* see b2sd_op_post_u8 */
+typedef struct { const void* y; int ldy; void* out; int nb, h, w; } b2sd_post_u8_args;
+/* out[b*out_ld + j] = bias[j] + sum_i act(in[b*in_ld + i]) * w[j*k + i] (w fp16 [n][k], act = SiLU when silu_in), b < nb */
+typedef struct {
+    const float* in; int in_ld;
+    const void* w; const float* bias;
+    float* out; int out_ld;
+    int nb, n, k, silu_in;
+} b2sd_small_linear_args;
+/* out[b] = [cos | sin](t[b] * exp(-ln(10000) * j / (dim/2))), j < dim/2: fp32 [nb][dim] */
+typedef struct { const float* t; float* out; int nb, dim; } b2sd_timestep_embedding_args;
 typedef struct {
     int kind;
     const char* label;
@@ -318,15 +361,28 @@ typedef struct {
     b2sd_attn_desc attn;
     b2sd_groupnorm_args groupnorm;
     b2sd_layernorm_args layernorm;
+    b2sd_smallconv_args smallconv;
+    b2sd_upsample2x_args upsample2x;
+    b2sd_maxpool2x2_args maxpool2x2;
+    b2sd_hed_project_args hed_project;
+    b2sd_hed_fuse_args hed_fuse;
+    b2sd_lcm_step_args lcm_step;
+    b2sd_post_u8_args post_u8;
+    b2sd_small_linear_args small_linear;
+    b2sd_timestep_embedding_args timestep_embedding;
 } b2sd_launch_record;
 /* One b2sd_step with the frame program run eagerly (no CUDA graph) and `fn` called around every kernel launch: `stream` is
  * synchronised, fn(user, index, 0, rec) runs, the launch is enqueued, `stream` is synchronised, fn(user, index, 1, rec) runs.
- * index counts kernel launches (0 .. b2sd_launches_per_step - 1, in launch order; the frame's input heads and the u8 tail are
- * kind OTHER); the frame program's memset of the LayerNorm statistics is not a kernel launch and gets no call.  A non-zero
+ * index counts kernel launches (0 .. b2sd_launches_per_step - 1, in launch order, the frame's input heads first and the u8
+ * tail last); the frame program's memset of the LayerNorm statistics is not a kernel launch and gets no call.  A non-zero
  * return from fn aborts the step with an error.  The output equals b2sd_step's. */
 typedef int (*b2sd_audit_fn)(void* user, int index, int after, const b2sd_launch_record* rec);
 int b2sd_audit_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* frame_out, b2sd_audit_fn fn, void* user,
                     void* stream);
+/* The prompt / timestep refresh of b2sd_prepare (the cross-attention K / V^T projections of the current prompt, then the
+ * timestep embedding, the time MLPs and every resnet's per-slot time bias) run eagerly with the same callback protocol as
+ * b2sd_audit_step; index counts the refresh's kernel launches.  It recomputes what b2sd_prepare computed from the same inputs. */
+int b2sd_audit_refresh(b2sd_handle h, b2sd_audit_fn fn, void* user, void* stream);
 
 /* Stage pipelining of ONE stateful stream (stream batch T > 1, where frame n+1 needs frame n's latent buffer and lanes cannot
  * simply alternate): `lane` shares `owner`'s stream-batch state; the frame program of each is cut into TAESD encoder body |

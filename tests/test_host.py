@@ -23,18 +23,43 @@ def test_shared_library_exports_every_declared_symbol():
     assert isinstance(lib.b2sd_last_error(), (bytes, type(None)))
 
 
-def test_ctypes_struct_layout_matches_the_c_header(tmp_path):
-    """Compile include/b200sd.h with gcc (plain C: the header must stay C-clean) and compare sizeof()."""
-    import subprocess
+def _ctypes_mirrors():
+    """C struct name -> its ctypes mirror in host/capi.py"""
     from ai_rtc_agent_b200.host import capi
-    src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include "b200sd.h"\nint main(void){printf("%zu %zu %zu %zu\\n", sizeof(b2sd_act_view), '
-                   'sizeof(b2sd_igemm_desc), sizeof(b2sd_attn_desc), sizeof(b2sd_config)); return 0;}\n')
-    exe = tmp_path / "sz"
+    return {"b2sd_act_view": capi.ActView, "b2sd_igemm_desc": capi.IgemmDesc, "b2sd_igemm_plan_info": capi.IgemmPlanInfo,
+            "b2sd_attn_desc": capi.AttnDesc, "b2sd_config": capi.EngineConfig, "b2sd_groupnorm_args": capi.GroupNormArgs,
+            "b2sd_layernorm_args": capi.LayerNormArgs, "b2sd_smallconv_args": capi.SmallConvArgs,
+            "b2sd_upsample2x_args": capi.Upsample2xArgs, "b2sd_maxpool2x2_args": capi.MaxPool2x2Args,
+            "b2sd_hed_project_args": capi.HedProjectArgs, "b2sd_hed_fuse_args": capi.HedFuseArgs,
+            "b2sd_lcm_step_args": capi.LcmStepArgs, "b2sd_post_u8_args": capi.PostU8Args,
+            "b2sd_small_linear_args": capi.SmallLinearArgs, "b2sd_timestep_embedding_args": capi.TimestepEmbeddingArgs,
+            "b2sd_launch_record": capi.LaunchRecord}
+
+
+def test_ctypes_struct_layout_matches_the_c_header(tmp_path):
+    """Compile include/b200sd.h with gcc (plain C: the header must stay C-clean) and compare, for every struct it declares,
+    sizeof() and the offsetof() of every field with the ctypes mirror: a mismatch makes the host read garbage descriptors."""
+    import subprocess
+    header = open(os.path.join(ROOT, "include", "b200sd.h")).read()
+    declared = re.findall(r"^typedef struct\s*\{.*?\}\s*(b2sd_[a-z0-9_]+)\s*;", header, re.M | re.S)
+    mirrors = _ctypes_mirrors()
+    assert len(declared) >= 17 and sorted(declared) == sorted(mirrors), "every struct of b200sd.h needs a ctypes mirror"
+    lines, want = [], []
+    for name, cls in mirrors.items():
+        lines.append(f'printf("%zu\\n", sizeof({name}));')
+        want.append((name, "sizeof", ctypes.sizeof(cls)))
+        for field, _ in cls._fields_:
+            lines.append(f'printf("%zu\\n", offsetof({name}, {field}));')
+            want.append((name, field, getattr(cls, field).offset))
+    src = tmp_path / "layout.c"
+    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "b200sd.h"\nint main(void){\n' + "\n".join(lines) +
+                   "\nreturn 0;}\n")
+    exe = tmp_path / "layout"
     subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
-    sizes = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
-    assert sizes == [ctypes.sizeof(capi.ActView), ctypes.sizeof(capi.IgemmDesc), ctypes.sizeof(capi.AttnDesc),
-                     ctypes.sizeof(capi.EngineConfig)]
+    got = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
+    assert len(got) == len(want)
+    bad = [(n, f, c, g) for (n, f, c), g in zip(want, got) if c != g]
+    assert not bad, "(struct, field, ctypes, C): " + repr(bad)
 
 
 def test_no_cpu_fallback():

@@ -1,12 +1,17 @@
-"""Launch audit of the frame program: every contraction, attention, GroupNorm and LayerNorm launch of a real frame, checked in
-place against a float64 recomputation of its own inputs.
+"""Launch audit of the frame program and of the prompt / timestep refresh: every kernel launch of a real frame (contractions,
+attention, GroupNorm, LayerNorm, the input heads and other small convs, upsampling, HED, the scheduler step, the u8 tail) and of
+the refresh (prompt K / V^T projections, timestep embedding, time MLPs, every resnet's time bias), checked in place against a
+float64 recomputation of its own inputs.  No launch is exempt: a launch without a record (kind "other") fails the audit.
 
 StreamDiffusion.audit_step runs one frame eagerly and calls back before and after every kernel launch with the launch's record
-(descriptor and plan as launched).  Before: the callback snapshots everything the launch reads (sources, weights, bias,
-residual, LayerNorm statistics, Q / K / V^T, normalisation inputs) and the spare pitch columns of its outputs.  After: the
+(descriptor and plan as launched); audit_refresh does the same for the refresh.  Before: the callback snapshots everything the
+launch reads (sources, weights, bias, residual, LayerNorm statistics, Q / K / V^T, normalisation inputs, the caller's u8 frame,
+the whole stream-batch buffer the scheduler step rewrites in place) and the spare pitch columns of its outputs.  After: the
 output is compared with the descriptor-driven reference of tests/launch_ref.py (tolerance atol * rms(ref) + rtol * |ref| per
-class), every check is shown to be discriminating by a named wrong reference that lands >= 10x the tolerance away, the spare
-columns must be bit-identical, and a LayerNorm-statistics producer's fixed-point sums must match its stored fp16 rows.
+class, bit for bit for upsample2x / maxpool2x2 / post_u8, the u8 edge map up to +-1 at float64 values within 1e-3 of an
+integer), every check is shown to be discriminating by a named wrong reference that lands >= 10x the tolerance away (bit-exact
+classes: differs on >= 1 % of the outputs), the spare columns must be bit-identical, and a LayerNorm-statistics producer's
+fixed-point sums must match its stored fp16 rows.
 
 The audited frame's u8 output must equal, bit for bit, a CUDA-graph step of a lane prepared identically: the audit observes
 the real program.  Device memory is only ever read, never past the last row of a buffer: the spare columns of an output's last
@@ -33,7 +38,7 @@ class _Dev:
                                          "version": 3}
 
 
-_TYPES = {torch.float16: ("<f2", 2), torch.float32: ("<f4", 4), torch.int64: ("<i8", 8)}
+_TYPES = {torch.float16: ("<f2", 2), torch.float32: ("<f4", 4), torch.int64: ("<i8", 8), torch.uint8: ("|u1", 1)}
 
 
 def _dev(ptr, rows, cols, ld, dtype=torch.float16):
@@ -70,7 +75,15 @@ def _kind_class(kind, d=None):
         if d["flags"] & R.IG_GEGLU:
             return "geglu+ln" if d["colsum"] else "geglu"
         return "contraction+ln" if d["colsum"] else "contraction"
-    return "attention" if kind == "attn" else "norm"
+    return {"attn": "attention", "groupnorm": "norm", "layernorm": "norm"}.get(kind, kind)
+
+
+def _frac(a, b):
+    """fraction of the elements where a and b differ (bit-exact classes' wrong references)"""
+    return (a.to(b.device) != b).double().mean().item()
+
+
+_HED = ("maxpool2x2", "hed_project", "hed_fuse")
 
 
 class Auditor:
@@ -82,6 +95,7 @@ class Auditor:
         self.worst_label = {}
         self.wrong = collections.defaultdict(collections.Counter)
         self.other = collections.Counter()
+        self.labels = collections.Counter()     # (class, first word of the label)
         self.lnstat = 0.0
         self.pending = None
 
@@ -103,14 +117,17 @@ class Auditor:
             self.pending = None
         torch.cuda.synchronize()
 
-    def _record(self, cls, label, units, wrongs):
+    def _record(self, cls, label, units, wrongs, exact=False):
+        """units: error in tolerance units (bit-exact classes: 0, or inf on any difference); wrongs: name -> the wrong
+        reference's distance in tolerance units (bit-exact classes: the fraction of outputs where it differs)."""
         self.launches[cls] += 1
-        atol, rtol = R.TOL[cls]
-        assert units <= 1.0, f"{label}: error {units:.3g}x the {cls} tolerance ({atol} rms + {rtol} |ref|)"
+        self.labels[cls, label.split(" ")[0]] += 1
+        need = 0.01 if exact else 10.0
+        assert units <= 1.0, f"{label}: error {units:.3g}x the {cls} tolerance {R.TOL.get(cls, 'bit-exact')}"
         best = max(wrongs.values()) if wrongs else 0.0
-        assert wrongs and best >= 10.0, f"{label}: no wrong reference lands >= 10x the tolerance away ({wrongs})"
+        assert wrongs and best >= need, f"{label}: no wrong reference lands far enough away ({need}: {wrongs})"
         for name, m in wrongs.items():
-            if m >= 10.0:
+            if m >= need:
                 self.wrong[cls][name] += 1
         self.checked[cls] += 1
         if units >= self.worst[cls]:
@@ -256,8 +273,190 @@ class Auditor:
                 f"{label}: stray write into the spare columns"
         self._record("norm", label, R.tol_units(got, ref, atol, rtol), wrongs)
 
+    # ---- smallconv --------------------------------------------------------------------------------------------------------
+    def _before_smallconv(self, rec):
+        a = R.as_dict(rec.smallconv)
+        f, nb, cin = a["flags"], a["nb"], a["cin"]
+        if f & (R.SC_IN_F32_NCHW | R.SC_IN_F16_NCHW):
+            dt = torch.float32 if f & R.SC_IN_F32_NCHW else torch.float16
+            x = _snap(a["x"], nb * cin * a["in_h"], a["in_w"], a["in_w"], dt).reshape(nb, cin, a["in_h"], a["in_w"])
+        else:
+            dt = torch.uint8 if f & R.SC_IN_U8 else torch.float16
+            x = _snap(a["x"], nb * a["in_h"] * a["in_w"], cin, cin, dt).reshape(nb, a["in_h"], a["in_w"], cin)
+        hw = a["h"] * a["w"]
+        res = None
+        if a["res"]:
+            items = nb if a["res_bstride"] else 1
+            res = torch.stack([_snap(a["res"] + 2 * n * a["res_bstride"], hw, a["cout"], a["ldr"]) for n in range(items)])
+        return {"x": x, "wt": _snap(a["wt"], 9 * cin, a["cout"], a["cout"], torch.float32), "bias": _vec(a["bias"], a["cout"]),
+                "in_off": _vec(a["in_off"], 3), "res": res, "spare": _spare(a["y"], nb * hw, a["cout"], a["ldy"])}
+
+    def _after_smallconv(self, rec, kind, label, s):
+        a = R.as_dict(rec.smallconv)
+        atol, rtol = R.TOL["smallconv"]
+        rows = a["nb"] * a["h"] * a["w"]
+
+        def ref(**kw):
+            return R.smallconv_ref(a, s["x"], s["wt"], s["bias"], s["res"], s["in_off"], **kw)
+        want = ref()
+        got = _dev(a["y"], rows, a["cout"], a["ldy"])
+        wrongs = {"3x3 taps mirrored": R.tol_units(ref(mirrored=True), want, atol, rtol)}
+        if (a["in_h"] != a["h"] or a["in_w"] != a["w"]) and not (
+                torch.equal(R.nearest_index(a["in_h"], a["h"]), R.nearest_index(a["in_h"], a["h"], exact_integer=True)) and
+                torch.equal(R.nearest_index(a["in_w"], a["w"]), R.nearest_index(a["in_w"], a["w"], exact_integer=True))):
+            wrongs["exact-integer resize rule"] = R.tol_units(ref(exact_integer=True), want, atol, rtol)
+        if s["res"] is not None:
+            wrongs["residual omitted"] = R.tol_units(ref(no_res=True), want, atol, rtol)
+            if a["res_bstride"] and a["nb"] > 1:
+                wrongs["item 0's residual for every item"] = R.tol_units(ref(res_item0=True), want, atol, rtol)
+        if a["flags"] & R.SC_IN_OFFSET:
+            wrongs["offset applied after the zero padding"] = R.tol_units(ref(offset_after_pad=True), want, atol, rtol)
+        if s["spare"] is not None:
+            now = _dev(a["y"], rows - 1, a["ldy"], a["ldy"])[:, a["cout"]:].view(torch.int16)
+            assert torch.equal(now, s["spare"]), f"{label}: stray write into the spare columns [{a['cout']}, {a['ldy']})"
+        self._record("smallconv", label, R.tol_units(got, want, atol, rtol), wrongs)
+
+    # ---- upsample2x / maxpool2x2 (bit-exact) ------------------------------------------------------------------------------
+    def _before_upsample2x(self, rec):
+        a = R.as_dict(rec.upsample2x)
+        return {"x": _snap(a["x"], a["nb"] * a["h"] * a["w"], a["c"], a["c"]).reshape(a["nb"], a["h"], a["w"], a["c"])}
+
+    def _after_upsample2x(self, rec, kind, label, s):
+        a = R.as_dict(rec.upsample2x)
+        want = R.upsample2x_ref(s["x"])
+        got = _dev(a["y"], a["nb"] * 4 * a["h"] * a["w"], a["c"], a["c"]).reshape(want.shape)
+        ok = torch.equal(got.view(torch.int16), want.view(torch.int16))
+        self._record("upsample2x", label, 0.0 if ok else float("inf"),
+                     {"source row (y+1)//2": _frac(R.upsample2x_ref(s["x"], shifted=True), want)}, exact=True)
+
+    def _before_maxpool2x2(self, rec):
+        a = R.as_dict(rec.maxpool2x2)
+        return {"x": _snap(a["x"], a["nb"] * a["h"] * a["w"], a["c"], a["c"]).reshape(a["nb"], a["h"], a["w"], a["c"])}
+
+    def _after_maxpool2x2(self, rec, kind, label, s):
+        a = R.as_dict(rec.maxpool2x2)
+        want = R.maxpool2x2_ref(s["x"])
+        got = _dev(a["y"], a["nb"] * (a["h"] // 2) * (a["w"] // 2), a["c"], a["c"]).reshape(want.shape)
+        ok = torch.equal(got.view(torch.int16), want.view(torch.int16))
+        self._record("maxpool2x2", label, 0.0 if ok else float("inf"),
+                     {"average pooling": _frac(R.maxpool2x2_ref(s["x"], average=True), want),
+                      "window shifted by one": _frac(R.maxpool2x2_ref(s["x"], shifted=True), want)}, exact=True)
+
+    # ---- HED ----------------------------------------------------------------------------------------------------------------
+    def _before_hed_project(self, rec):
+        a = R.as_dict(rec.hed_project)
+        return {"x": _snap(a["x"], a["npix"], a["c"], a["ldx"]), "w": _vec(a["w"], a["c"]), "bias": _vec(a["bias"], 1)}
+
+    def _after_hed_project(self, rec, kind, label, s):
+        a = R.as_dict(rec.hed_project)
+        atol, rtol = R.TOL["hed_project"]
+        want = R.hed_project_ref(s["x"], s["w"], s["bias"])
+        got = _dev(a["out"], 1, a["npix"], a["npix"], torch.float32).flatten()
+        wrongs = {"bias omitted": R.tol_units(R.hed_project_ref(s["x"], s["w"], s["bias"], no_bias=True), want, atol, rtol),
+                  "channel pairs swapped": R.tol_units(R.hed_project_ref(s["x"], s["w"], s["bias"], swap_pairs=True), want, atol, rtol)}
+        self._record("hed_project", label, R.tol_units(got, want, atol, rtol), wrongs)
+
+    def _before_hed_fuse(self, rec):
+        a = R.as_dict(rec.hed_fuse)
+        return {"maps": [_snap(a["maps"][k], a["hs"][k], a["ws"][k], a["ws"][k], torch.float32) for k in range(a["levels"])]}
+
+    def _after_hed_fuse(self, rec, kind, label, s):
+        a = R.as_dict(rec.hed_fuse)
+        h, w = a["h"], a["w"]
+        got = _dev(a["out"], h * w, 3, 3, torch.uint8)
+        assert torch.equal(got[:, 1], got[:, 0]) and torch.equal(got[:, 2], got[:, 0]), f"{label}: the 3 channels differ"
+        u = got[:, 0].reshape(h, w)
+        if a["edge_f16"]:
+            assert torch.equal(_dev(a["edge_f16"], h * w, 1, 1).reshape(h, w), u.half()), f"{label}: edge_f16 != the u8 value"
+        nbad, near = R.hed_fuse_mismatch(u, s["maps"], h, w)
+        assert near, f"{label}: a pixel off by more than 1, or away from an integer boundary"
+        want = R.hed_fuse_ref(s["maps"], h, w)
+        self._record("hed_fuse", label, nbad / (1e-3 * h * w),
+                     {"align_corners=True": _frac(R.hed_fuse_ref(s["maps"], h, w, align_corners=True), want),
+                      "rounding instead of truncation": _frac(R.hed_fuse_ref(s["maps"], h, w, rounding=True), want)}, exact=True)
+
+    # ---- scheduler step (rewrites the stream-batch buffer in place) ----------------------------------------------------------
+    def _before_lcm_step(self, rec):
+        a = R.as_dict(rec.lcm_step)
+        n = a["T"] * a["hw"]
+        return {"x": _snap(a["x"], n, 4, 4), "eps": _snap(a["eps"], n, 4, 4), "noise": _snap(a["noise"], n, 4, 4),
+                "coef": _vec(a["coef"], 4 * a["T"])}
+
+    def _after_lcm_step(self, rec, kind, label, s):
+        a = R.as_dict(rec.lcm_step)
+        T, hw = a["T"], a["hw"]
+        atol, rtol = R.TOL["lcm_step"]
+        noise = s["noise"] if s["noise"] is not None else torch.zeros_like(s["x"])
+        args = (a, s["x"].reshape(T, hw, 4), s["eps"].reshape(T, hw, 4), noise.reshape(T, hw, 4), s["coef"])
+        out, x = R.lcm_step_ref(*args)
+        got_out = _dev(a["out_latent"], hw, 4, 4)
+        got_x = _dev(a["x"], T * hw, 4, 4).reshape(T, hw, 4)
+
+        def units(go, gx):   # distance of (out_latent, x) from the reference, in tolerance units
+            u = R.tol_units(go, out, atol, rtol)
+            return max(u, R.tol_units(gx[1:], x[1:], atol, rtol)) if T > 1 else u
+        assert torch.equal(got_x[0].view(torch.int16), s["x"][:hw].view(torch.int16)), f"{label}: slot 0 of x changed"
+        assert torch.equal(_dev(a["eps"], T * hw, 4, 4), s["eps"]), f"{label}: eps changed"
+        if s["noise"] is not None:
+            assert torch.equal(_dev(a["noise"], T * hw, 4, 4), s["noise"]), f"{label}: noise changed"
+        wrongs = {"c_skip / c_out swapped": units(*R.lcm_step_ref(*args, swap_cskip_cout=True))}
+        if T > 1:
+            wrongs["slot i re-noised from its own x0"] = units(*R.lcm_step_ref(*args, own_x0=True))
+        self._record("lcm_step", label, units(got_out, got_x), wrongs)
+
+    # ---- post_u8 (bit-exact) ------------------------------------------------------------------------------------------------
+    def _before_post_u8(self, rec):
+        a = R.as_dict(rec.post_u8)
+        return {"y": _snap(a["y"], a["nb"] * a["h"] * a["w"], 3, a["ldy"])}
+
+    def _after_post_u8(self, rec, kind, label, s):
+        a = R.as_dict(rec.post_u8)
+        want = R.post_u8_ref(a, s["y"])
+        got = _dev(a["out"], a["nb"] * 3 * a["h"], a["w"], a["w"], torch.uint8).reshape(want.shape)
+        self._record("post_u8", label, 0.0 if torch.equal(got, want) else float("inf"),
+                     {"rounding instead of truncation": _frac(R.post_u8_ref(a, s["y"], rounding=True), want),
+                      "BGR channel order": _frac(R.post_u8_ref(a, s["y"], bgr=True), want)}, exact=True)
+
+    # ---- prepare-time: time embedding ---------------------------------------------------------------------------------------
+    def _before_small_linear(self, rec):
+        a = R.as_dict(rec.small_linear)
+        return {"x": _snap(a["in"], a["nb"], a["k"], a["in_ld"], torch.float32), "w": _snap(a["w"], a["n"], a["k"], a["k"]),
+                "bias": _vec(a["bias"], a["n"])}
+
+    def _after_small_linear(self, rec, kind, label, s):
+        a = R.as_dict(rec.small_linear)
+        atol, rtol = R.TOL["small_linear"]
+
+        def ref(**kw):
+            return R.small_linear_ref(a, s["x"], s["w"], s["bias"], **kw)
+        want = ref()
+        got = _dev(a["out"], a["nb"], a["n"], a["out_ld"], torch.float32)
+        wrongs = {}
+        if a["silu_in"]:
+            wrongs["SiLU omitted"] = R.tol_units(ref(no_silu=True), want, atol, rtol)
+        if s["bias"] is not None:
+            wrongs["bias omitted"] = R.tol_units(ref(no_bias=True), want, atol, rtol)
+        if a["nb"] > 1:
+            wrongs["slot 0's input for every slot"] = R.tol_units(ref(slot0=True), want, atol, rtol)
+        self._record("small_linear", label, R.tol_units(got, want, atol, rtol), wrongs)
+
+    def _before_timestep_embedding(self, rec):
+        a = R.as_dict(rec.timestep_embedding)
+        return {"t": _vec(a["t"], a["nb"])}
+
+    def _after_timestep_embedding(self, rec, kind, label, s):
+        a = R.as_dict(rec.timestep_embedding)
+        want = R.timestep_embedding_ref(s["t"], a["dim"])
+        got = _dev(a["out"], a["nb"], a["dim"], a["dim"], torch.float32).double()
+
+        def units(x):
+            return (x - want).abs().max().item() / R.TEMB_ATOL
+        self._record("timestep_embedding", label, units(got),
+                     {"[sin | cos] order": units(R.timestep_embedding_ref(s["t"], a["dim"], sin_first=True)),
+                      "exponent over half - 1": units(R.timestep_embedding_ref(s["t"], a["dim"], half_minus_one=True))})
+
     def table(self, name):
-        lines = [f"launch audit {name}: {self.calls} launches",
+        lines = [f"launch audit {name}: {self.calls} launches, {sum(self.other.values())} other",
                  f"  {'class':16s} {'launches':>8s} {'checked':>8s} {'worst/tol':>9s}  wrong references applied (worst launch)"]
         for cls in sorted(self.launches):
             wr = ", ".join(f"{k}: {v}" for k, v in sorted(self.wrong[cls].items()))
@@ -295,7 +494,8 @@ def _engine(turbo, tl, hw, full=False, concurrency=1, cn=False, hed=False, kl=Fa
     # the audited engine's policy, so that the two compute bit-identical frames
     lane.set_concurrency(concurrency)
     lane._prepare_like(sd)
-    return sd, lane
+    keys = list(usd) + (list(cn16) if cn else [])   # the UNet's and the ControlNet's parameters
+    return sd, lane, keys
 
 
 _TINY = [
@@ -304,6 +504,9 @@ _TINY = [
     pytest.param(dict(turbo=False, tl=_T4, hw=192), id="tiny-sd15-T4-192"),             # unfolded transformer program: 36 / 9 tokens
     pytest.param(dict(turbo=True, tl=[32], hw=192, cn=True, hed=True), id="tiny-turbo-T1-192-cn-hed"),
     pytest.param(dict(turbo=False, tl=_T4, hw=128, kl=True), id="tiny-sd15-T4-128-kl"),
+    # a camera-sized frame: the heads resize 300x400 -> 128x192 (400 -> 192: torch's rule and the integer rule differ), and
+    # the ControlNet head writes 16 channels into a 64-wide buffer
+    pytest.param(dict(turbo=True, tl=[32], hw=(128, 192), cn=True, frame=(300, 400)), id="tiny-turbo-T1-128x192-cn-300x400"),
 ]
 _FULL = [
     pytest.param(dict(turbo=True, tl=[32], hw=512, concurrency=1), id="turbo-T1-512-c1"),
@@ -313,6 +516,9 @@ _FULL = [
     pytest.param(dict(turbo=False, tl=_T4, hw=448, concurrency=1), id="sd15-T4-448-c1"),   # unfolded program at 14x14 (level 2)
     pytest.param(dict(turbo=True, tl=[32], hw=512, cn=True, hed=True), id="turbo-T1-512-cn-hed"),
     pytest.param(dict(turbo=True, tl=[32], hw=512, kl=True), id="turbo-T1-512-kl"),
+    # 720 -> 448 is a pair where torch's rule and the integer rule differ; the 448x768 head runs 64-channel groups and the
+    # grid-stride loop
+    pytest.param(dict(turbo=True, tl=[32], hw=(448, 768), frame=(720, 1280)), id="turbo-T1-448x768-720x1280"),
 ]
 
 
@@ -331,25 +537,49 @@ def _audit(cuda, name, cfg, full):
     sd = lane = None
     _release_device_memory()
     free0 = torch.cuda.mem_get_info()[0]
+    cfg = dict(cfg)
+    frame_hw = cfg.pop("frame", None)
     try:
         t0 = time.time()
-        sd, lane = _engine(full=full, **cfg)
-        height, width = sd.height, sd.width
+        sd, lane, keys = _engine(full=full, **cfg)
+        fh, fw = frame_hw or (sd.height, sd.width)
         nframes = 2 if len(cfg["tl"]) > 1 else 1      # T = 4: the second frame runs on a non-zero latent buffer
-        frames = [ow.make_frame(height, width, seed=300 + i).cuda() for i in range(nframes)]
+        frames = [ow.make_frame(fh, fw, seed=300 + i).cuda() for i in range(nframes)]
         for f in frames[:-1]:
             sd.step_u8(f)
             lane.step_u8(f)
+        # the refresh recomputes sd's time biases and prompt K / V^T: the bit-identity with the lane below also shows that
+        # it is deterministic
+        ref_aud = Auditor()
+        sd.audit_refresh(ref_aud)
         aud = Auditor()
         got = sd.audit_step(frames[-1], aud).clone()
         want = lane.step_u8(frames[-1])
         torch.cuda.synchronize()
-        print("\n" + aud.table(name) + f"\n  wall time {time.time() - t0:.1f} s, "
+        print("\n" + ref_aud.table(name + " refresh") + "\n" + aud.table(name) + f"\n  wall time {time.time() - t0:.1f} s, "
               f"free HBM at the start {free0 / 2**30:.1f} GiB")
+        for a in (ref_aud, aud):
+            assert not a.other, f"launches without a record: {dict(a.other)}"
+            for cls in a.launches:
+                assert a.checked[cls] == a.launches[cls], cls
+            assert a.calls == sum(a.checked.values())
+        # the frame: every class it must have, the scheduler step and the tail exactly once, HED only with HED
         assert aud.calls == sd.launches_per_step, (aud.calls, sd.launches_per_step)
-        for cls in aud.launches:
-            assert aud.checked[cls] == aud.launches[cls], cls
-        assert {"contraction", "attention", "norm"} <= set(aud.checked), dict(aud.checked)
+        assert {"contraction", "attention", "norm", "smallconv", "upsample2x", "lcm_step", "post_u8"} <= set(aud.checked), \
+            dict(aud.checked)
+        assert aud.checked["lcm_step"] == 1 and aud.checked["post_u8"] == 1, dict(aud.checked)
+        hed = {k: aud.checked[k] for k in _HED if aud.checked[k]}
+        assert hed == ({"maxpool2x2": 4, "hed_project": 5, "hed_fuse": 1} if cfg.get("hed") else {}), hed
+        # the refresh, tied to the model: one time-bias projection per resnet with a time embedding, one time MLP (two
+        # linears) per model, and the K and V^T projections of every cross attention
+        n_temb = sum(k.endswith("time_emb_proj.weight") for k in keys)
+        n_attn2 = sum(k.endswith("attn2.to_k.weight") for k in keys)
+        nets = 2 if cfg.get("cn") else 1
+        assert ref_aud.checked["timestep_embedding"] == 1, dict(ref_aud.checked)
+        assert ref_aud.labels["small_linear", "temb"] == n_temb > 0, (dict(ref_aud.labels), n_temb)
+        assert ref_aud.checked["small_linear"] == n_temb + 2 * nets, (dict(ref_aud.checked), n_temb)
+        assert ref_aud.checked["contraction"] == 2 * n_attn2 > 0, (dict(ref_aud.checked), n_attn2)
+        assert set(ref_aud.checked) == {"timestep_embedding", "small_linear", "contraction"}, dict(ref_aud.checked)
         assert torch.equal(got, want), "the audited frame differs from a graph step of an identical lane"
     finally:
         torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = prev
@@ -360,10 +590,10 @@ def _audit(cuda, name, cfg, full):
 
 
 @pytest.mark.parametrize("cfg", _TINY)
-def test_launch_audit_tiny(cuda, request, cfg):
+def test_frame_and_refresh_launch_audit_tiny(cuda, request, cfg):
     _audit(cuda, request.node.callspec.id, cfg, full=False)
 
 
 @pytest.mark.parametrize("cfg", _FULL)
-def test_launch_audit_full_size(cuda, request, cfg):
+def test_frame_and_refresh_launch_audit_full_size(cuda, request, cfg):
     _audit(cuda, request.node.callspec.id, cfg, full=True)

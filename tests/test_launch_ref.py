@@ -183,3 +183,176 @@ def test_tolerance_units():
     assert abs(R.tol_units(got, ref, 3e-3, 3e-3) - 1.0) < 1e-9
     got[0] = float("nan")
     assert R.tol_units(got, ref, 3e-3, 3e-3) == float("inf")
+
+
+# ---- the elementwise kernels and the prepare-time launches ------------------------------------------------------------------
+def _sc_args(nb, h, w, cin, cout, in_h, in_w, flags, res_bstride=0):
+    return {"nb": nb, "h": h, "w": w, "cin": cin, "cout": cout, "in_h": in_h, "in_w": in_w, "flags": flags,
+            "res_bstride": res_bstride}
+
+
+def _wt(w_oihw):
+    """OIHW -> smallconv's prepared fp32 [cin*9][cout], k = tap*cin + c"""
+    o, c = w_oihw.shape[:2]
+    return w_oihw.permute(2, 3, 1, 0).reshape(9 * c, o)
+
+
+def test_smallconv_u8_head_with_resize():
+    """u8 NHWC frame / 255 (rounded to fp16), resized 720x20 -> 448x12 with torch's nearest rule, 3x3 conv + bias + ReLU ->
+    F.interpolate(size=...) + F.conv2d.  720 -> 448 is a pair where torch's rule and the exact-integer rule differ."""
+    g = torch.Generator().manual_seed(40)
+    x = torch.randint(0, 256, (1, 720, 20, 3), generator=g, dtype=torch.uint8)
+    w, b = _rand((64, 3, 3, 3), 41, 0.3), _rand((64,), 42)
+    a = _sc_args(1, 448, 12, 3, 64, 720, 20, R.SC_IN_U8 | R.SC_OUT_RELU)
+    got = R.smallconv_ref(a, x, _wt(w), b)
+    v = (x.float() * (1.0 / 255.0)).half().float().permute(0, 3, 1, 2)   # fp32: torch's rule for float64 scales in float64
+    ref = _rows(F.relu(F.conv2d(F.interpolate(v, size=(448, 12), mode="nearest").double(), w, b, padding=1)))
+    torch.testing.assert_close(got, ref, rtol=1e-12, atol=1e-12)
+    assert not torch.equal(R.nearest_index(720, 448), R.nearest_index(720, 448, exact_integer=True))
+    assert (R.smallconv_ref(a, x, _wt(w), b, exact_integer=True) - ref).abs().max() > 0.1
+    assert (R.smallconv_ref(a, x, _wt(w), b, mirrored=True) - ref).abs().max() > 0.1
+
+
+def test_smallconv_offset_input_pads_in_the_shifted_domain():
+    """HED's first conv / the AutoencoderKL head: u8 - in_off[c], zero padding applied after the shift; SiLU epilogue."""
+    g = torch.Generator().manual_seed(43)
+    x = torch.randint(0, 256, (1, 9, 11, 3), generator=g, dtype=torch.uint8)
+    off = torch.tensor([122.7, 116.6, 104.0])
+    w, b = _rand((16, 3, 3, 3), 44, 0.02), _rand((16,), 45)
+    a = _sc_args(1, 9, 11, 3, 16, 9, 11, R.SC_IN_U8 | R.SC_IN_OFFSET | R.SC_OUT_SILU)
+    got = R.smallconv_ref(a, x, _wt(w), b, in_off=off)
+    v = (x.float() - off).half().double().permute(0, 3, 1, 2)
+    ref = _rows(F.silu(F.conv2d(v, w, b, padding=1)))
+    torch.testing.assert_close(got, ref, rtol=1e-12, atol=1e-12)
+    wrong = R.smallconv_ref(a, x, _wt(w), b, in_off=off, offset_after_pad=True).reshape(9, 11, 16)
+    assert (wrong - ref.reshape(9, 11, 16))[0].abs().max() > 0.1                                # the border moves
+    torch.testing.assert_close(wrong[1:-1, 1:-1], ref.reshape(9, 11, 16)[1:-1, 1:-1], rtol=1e-12, atol=1e-12)
+
+
+def test_smallconv_fp16_tanh_input_and_per_item_residual():
+    """fp16 latent through tanh(x/3)*3 (DecoderTiny), per-item residual (item n at n * res_bstride), batch 2."""
+    nb, h, w = 2, 6, 5
+    x = (_rand((nb, h, w, 4), 46) * 4).half()
+    wc, b = _rand((32, 4, 3, 3), 47, 0.2), _rand((32,), 48)
+    res = _rand((nb, h * w, 32), 49).half()
+    a = _sc_args(nb, h, w, 4, 32, h, w, R.SC_IN_TANH3, res_bstride=h * w * 32)
+    got = R.smallconv_ref(a, x, _wt(wc), b, res=res)
+    v = (torch.tanh(x.float() / 3) * 3).half().double().permute(0, 3, 1, 2)
+    ref = _rows(F.conv2d(v, wc, b, padding=1)) + res.double().reshape(nb * h * w, 32)
+    torch.testing.assert_close(got, ref, rtol=1e-6, atol=1e-6)   # fp32 tanh vs the fp32 x/3 product: rare fp16 ties
+    assert (R.smallconv_ref(a, x, _wt(wc), b, res=res, res_item0=True) - ref)[h * w:].abs().max() > 0.1
+    assert (R.smallconv_ref(a, x, _wt(wc), b, res=res, no_res=True) - ref).abs().max() > 0.1
+
+
+def _frac_differ(a, b):
+    return (a != b).double().mean().item()
+
+
+def test_upsample2x_and_maxpool2x2():
+    x = _rand((2, 5, 7, 16), 50).half()
+    ref = F.interpolate(x.permute(0, 3, 1, 2).double(), scale_factor=2, mode="nearest").permute(0, 2, 3, 1)
+    got = R.upsample2x_ref(x)
+    assert torch.equal(got.double(), ref)
+    assert _frac_differ(R.upsample2x_ref(x, shifted=True), got) >= 0.01
+    ref = F.max_pool2d(x.permute(0, 3, 1, 2).double(), 2).permute(0, 2, 3, 1)
+    got = R.maxpool2x2_ref(x[:, :4, :6])
+    assert torch.equal(got.double(), F.max_pool2d(x[:, :4, :6].permute(0, 3, 1, 2).double(), 2).permute(0, 2, 3, 1))
+    assert ref.shape[1] == 2 and got.shape[1:3] == (2, 3)
+    for wrong in (R.maxpool2x2_ref(x[:, :4, :6], average=True), R.maxpool2x2_ref(x[:, :4, :6], shifted=True)):
+        assert _frac_differ(wrong, got) >= 0.01
+
+
+def test_hed_project_reference():
+    x, w, b = _rand((40, 64), 51).half(), _rand((64,), 52), _rand((1,), 53)
+    got = R.hed_project_ref(x, w, b)
+    ref = F.conv2d(x.double().T.reshape(1, 64, 40, 1), w.reshape(1, 64, 1, 1), b).reshape(40)
+    torch.testing.assert_close(got, ref, rtol=1e-12, atol=1e-12)
+    for wrong in (R.hed_project_ref(x, w, b, no_bias=True), R.hed_project_ref(x, w, b, swap_pairs=True)):
+        assert (wrong - ref).abs().max() > 0.1
+
+
+def test_hed_fuse_matches_the_oracle_post_processing(monkeypatch):
+    """Five side outputs at h / 2^k -> oracle/hed.py's detect tail (F.interpolate bilinear, align_corners=False, mean,
+    sigmoid, * 255, clamp, u8 cast); the oracle's own code, fed these maps."""
+    from oracle import hed as ohed
+    h, w = 48, 80
+    maps = [_rand((h >> k, w >> k), 54 + k, 2.0) for k in range(5)]
+    monkeypatch.setattr(ohed, "side_outputs", lambda sd, x: [m[None, None] for m in maps])
+    ref = ohed.detect(None, torch.zeros(1, 3, h, w, dtype=torch.float64))[0, 0]
+    got = R.hed_fuse_ref(maps, h, w)
+    assert torch.equal(got, ref)
+    assert R.hed_fuse_mismatch(got, maps, h, w) == (0, True)
+    for wrong in (R.hed_fuse_ref(maps, h, w, align_corners=True), R.hed_fuse_ref(maps, h, w, rounding=True)):
+        assert _frac_differ(wrong, got) >= 0.01
+
+
+def test_lcm_step_matches_the_oracle_scheduler_and_buffer_update():
+    """oracle/stream.py scheduler_step_batch + predict_x0_batch's buffer update (T = 4, with and without the noise term)."""
+    from types import SimpleNamespace
+
+    from oracle import stream as ostream
+    T, h, w = 4, 3, 5
+    x, eps, noise = (_rand((T, 4, h, w), s) for s in (60, 61, 62))
+    coef = torch.cat([0.5 + 0.5 * torch.rand(T, dtype=torch.float64), 0.2 + 0.7 * torch.rand(T, dtype=torch.float64),
+                      0.3 * torch.rand(T, dtype=torch.float64), 0.5 + torch.rand(T, dtype=torch.float64)])
+    c = coef.reshape(4, T)
+    for dan in (1, 0):
+        ns = SimpleNamespace(denoising_steps_num=T, x_t_latent_buffer=x[1:].clone(), init_noise=noise,
+                             stock_noise=noise.clone(), do_add_noise=bool(dan), static_buffers=False, last={},
+                             alpha_prod_t_sqrt=c[0].view(T, 1, 1, 1), beta_prod_t_sqrt=c[1].view(T, 1, 1, 1),
+                             c_skip=c[2].view(T, 1, 1, 1), c_out=c[3].view(T, 1, 1, 1))
+        ns.unet_step = lambda xx, ns=ns: (ostream.StreamOracle.scheduler_step_batch(ns, eps, xx), eps)
+        out = ostream.StreamOracle.predict_x0_batch(ns, x[:1])
+
+        def flat(t):
+            return t.permute(0, 2, 3, 1).reshape(t.shape[0], h * w, 4)
+        a = {"T": T, "do_add_noise": dan}
+        got_out, got_x = R.lcm_step_ref(a, flat(x), flat(eps), flat(noise), coef)
+        torch.testing.assert_close(got_out, flat(out)[0], rtol=1e-12, atol=1e-12)
+        torch.testing.assert_close(got_x[1:], flat(ns.x_t_latent_buffer), rtol=1e-12, atol=1e-12)
+        assert torch.equal(got_x[0], flat(x)[0])
+        w_out, _ = R.lcm_step_ref(a, flat(x), flat(eps), flat(noise), coef, swap_cskip_cout=True)
+        _, w_x = R.lcm_step_ref(a, flat(x), flat(eps), flat(noise), coef, own_x0=True)
+        assert (w_out - got_out).abs().max() > 0.1 and (w_x - got_x).abs().max() > 0.1
+
+
+def test_post_u8_matches_torch_half_ops():
+    nb, h, w = 2, 16, 24
+    y = (torch.rand(nb * h * w, 3, generator=torch.Generator().manual_seed(63), dtype=torch.float64) * 1.4 - 0.2).half()
+    y[:6, 0] = torch.tensor([-0.5, 0.0, 0.5, 1.0, 1.5, 0.25], dtype=torch.float16)
+    a = {"nb": nb, "h": h, "w": w}
+    got = R.post_u8_ref(a, y)
+    v = y.reshape(nb, h, w, 3).permute(0, 3, 1, 2)
+    v = v * 2 - 1
+    v = v / 2 + 0.5
+    v = v.clamp(0, 1) * 255
+    ref = v.clamp(0, 255).to(torch.uint8)
+    assert v.dtype == torch.float16 and torch.equal(got, ref)
+    for wrong in (R.post_u8_ref(a, y, rounding=True), R.post_u8_ref(a, y, bgr=True)):
+        assert _frac_differ(wrong, got) >= 0.01
+
+
+def test_timestep_embedding_and_time_mlp_match_the_oracle():
+    """timestep_embedding vs oracle.unet.timestep_embedding; the time MLP (linear_1, SiLU, linear_2) as two small_linear
+    launches vs oracle.unet.time_embed; a resnet's time bias conv1.bias + time_emb_proj(silu(emb)) vs F.linear."""
+    from oracle import unet as ounet
+    t = torch.tensor([999.0, 261.0, 35.0, 1.0])
+    c0 = 64
+    emb = R.timestep_embedding_ref(t, c0)
+    torch.testing.assert_close(emb, ounet.timestep_embedding(t, c0).double(), rtol=0, atol=R.TEMB_ATOL)
+    for wrong in (R.timestep_embedding_ref(t, c0, sin_first=True), R.timestep_embedding_ref(t, c0, half_minus_one=True)):
+        assert (wrong - emb).abs().max() > 0.1
+    td = 4 * c0
+    sd = {"time_embedding.linear_1.weight": _rand((td, c0), 64, 0.2).half().double(),
+          "time_embedding.linear_1.bias": _rand((td,), 65), "time_embedding.linear_2.weight": _rand((td, td), 66, 0.1).half().double(),
+          "time_embedding.linear_2.bias": _rand((td,), 67)}
+    l1 = {"k": c0, "silu_in": 0}
+    l2 = {"k": td, "silu_in": 1}
+    hid = R.small_linear_ref(l1, emb, sd["time_embedding.linear_1.weight"], sd["time_embedding.linear_1.bias"])
+    out = R.small_linear_ref(l2, hid, sd["time_embedding.linear_2.weight"], sd["time_embedding.linear_2.bias"])
+    torch.testing.assert_close(out, ounet.time_embed(sd, ounet.tiny_config(True), t), rtol=1e-4, atol=1e-4)
+    wp, bp = _rand((128, td), 68, 0.1).half(), _rand((128,), 69)
+    bias = R.small_linear_ref(l2, out, wp, bp)
+    torch.testing.assert_close(bias, F.linear(F.silu(out), wp.double(), bp), rtol=1e-12, atol=1e-12)
+    for kw in ({"no_silu": True}, {"no_bias": True}, {"slot0": True}):
+        assert (R.small_linear_ref(l2, out, wp, bp, **kw) - bias).abs().max() > 0.1

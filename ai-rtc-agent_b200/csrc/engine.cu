@@ -294,6 +294,16 @@ struct WeightStore {
     std::map<std::string, size_t> packed_bytes, fvec_bytes;   // their sizes (b2sd_export_packed)
 };
 
+// One temporal stream's stream-batch state (b2sd_state_*): slots 1 .. T-1 of the UNet input batch, NHWC fp16, stream-ordered
+// allocation.  It remembers the weight store, batch and size it was made for; the weak reference does not keep weights alive.
+struct b2sd_state {
+    std::weak_ptr<WeightStore> ws;
+    int batch = 0, height = 0, width = 0;
+    size_t bytes = 0;
+    __half* buf = nullptr;
+    cudaEvent_t done = nullptr;   // recorded after each step's copy-out; the next step of this stream waits on it
+};
+
 struct b2sd_engine {
     b2sd_config cfg{};
     int lh = 0, lw = 0;  // latent extents
@@ -343,11 +353,11 @@ struct b2sd_engine {
     bool allow_swap = false;  // builders enable the swapped GEMM orientation for UNet contractions (never TAESD / V^T / GEGLU)
     cudaGraphExec_t graph_exec = nullptr;
     cudaGraph_t graph = nullptr;
-    // Stage pipelining of a stateful (T > 1) stream over lanes that SHARE the stream-batch state (b2sd_share_stream_state): the
-    // frame program is cut into [TAESD encoder body | last encoder conv + UNet + scheduler step | TAESD decoder], three CUDA
-    // graphs; only the middle stage touches the shared x_in, and the lanes chain it through one event.
-    struct StageGroup { cudaEvent_t unet_done = nullptr; ~StageGroup() { if (unet_done) cudaEventDestroy(unet_done); } };
-    std::shared_ptr<StageGroup> group;
+    // Stepping a stream state (b2sd_step_state): the frame program is cut into [encoder body | last encoder conv + UNet +
+    // scheduler step | decoder], three CUDA graphs captured on first use.  Only the middle stage reads and writes slots 1.. of
+    // x_in, so the state is copied in before it and out after it, and steps of one state chain through the state's event.
+    // An engine of a b2sd_share_stream_state pair steps pair_state (created by the owner, shared with the lane) every frame.
+    std::shared_ptr<b2sd_state> pair_state;
     size_t idx_enc_end = 0, idx_unet_end = 0;          // stage boundaries inside prog_frame
     cudaGraphExec_t stage_exec[3] = {nullptr, nullptr, nullptr};
     cudaGraph_t stage_graph[3] = {nullptr, nullptr, nullptr};
@@ -1720,6 +1730,51 @@ int b2sd_engine::build_program(cudaStream_t s) {
     return 0;
 }
 
+// ---- stream states -------------------------------------------------------------------------------
+static size_t state_bytes(const b2sd_engine* h) { return (size_t)(h->cfg.batch - 1) * h->lh * h->lw * 4 * sizeof(__half); }
+
+static int state_new(const b2sd_engine* h, cudaStream_t s, b2sd_state** out) {
+    b2sd_state* st = new b2sd_state;
+    st->ws = h->ws;
+    st->batch = h->cfg.batch; st->height = h->cfg.height; st->width = h->cfg.width;
+    st->bytes = state_bytes(h);
+    cudaError_t e = cudaEventCreateWithFlags(&st->done, cudaEventDisableTiming);
+    if (e == cudaSuccess && st->bytes) e = cudaMallocAsync(reinterpret_cast<void**>(&st->buf), st->bytes, s);
+    if (e == cudaSuccess && st->bytes) e = cudaMemsetAsync(st->buf, 0, st->bytes, s);
+    if (e == cudaSuccess) e = cudaEventRecord(st->done, s);
+    if (e != cudaSuccess) {
+        b2_set_error("b2sd_state_create: %s", cudaGetErrorString(e));
+        if (st->buf) cudaFreeAsync(st->buf, s);
+        if (st->done) cudaEventDestroy(st->done);
+        delete st;
+        return -1;
+    }
+    *out = st;
+    return 0;
+}
+
+static int state_free(b2sd_state* st, cudaStream_t s) {
+    cudaError_t e = cudaSuccess;
+    if (st->buf) {
+        e = cudaStreamWaitEvent(s, st->done, 0);
+        if (e == cudaSuccess) e = cudaFreeAsync(st->buf, s);
+    }
+    cudaEventDestroy(st->done);   // a recorded, not yet completed event is released once the device reaches it
+    delete st;
+    if (e != cudaSuccess) {
+        b2_set_error("b2sd_state_destroy: %s", cudaGetErrorString(e));
+        return -1;
+    }
+    return 0;
+}
+
+static int state_reset(b2sd_state* st, cudaStream_t s) {
+    CUDA_OK(cudaStreamWaitEvent(s, st->done, 0));
+    if (st->bytes) CUDA_OK(cudaMemsetAsync(st->buf, 0, st->bytes, s));
+    CUDA_OK(cudaEventRecord(st->done, s));
+    return 0;
+}
+
 // ================================================================================================
 extern "C" {
 
@@ -1971,6 +2026,7 @@ int b2sd_prepare(b2sd_handle h, const void* prompt_embeds, const float* timestep
     }
     // x_t_latent_buffer = zeros (StreamDiffusion.prepare); slot 0 is overwritten by every frame
     CUDA_OK(cudaMemsetAsync(h->x_in.p, 0, (size_t)h->x_in.elems() * 2, s));
+    if (h->pair_state) TRY(state_reset(h->pair_state.get(), s));
     TRY(h->build_program(s));
     TRY(h->run(h->prog_prompt, s));
     TRY(refresh_time(h, s));
@@ -2170,17 +2226,8 @@ int b2sd_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* fra
     return b2sd_step_ex(h, frame_in, B2SD_IN_U8_NHWC, in_h, in_w, frame_out, B2SD_OUT_U8_NCHW, stream);
 }
 
-int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int in_w, void* frame_out, int out_kind,
-                 void* stream) {
-    if (!h || !h->built) {
-        b2_set_error("b2sd_step: call b2sd_prepare first");
-        return -1;
-    }
-    if (!frame_in || !frame_out || in_h < 1 || in_w < 1) {
-        b2_set_error("b2sd_step: bad frame arguments");
-        return -1;
-    }
-    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+// the input heads of a frame: the encoder head, and the ControlNet / HED head that reads the frame
+static int step_heads(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int in_w, cudaStream_t s) {
     SmallConvArgs a = h->head;
     a.x = frame_in; a.in_h = in_h; a.in_w = in_w;
     const int in_flags = in_kind == B2SD_IN_U8_NHWC ? SC_IN_U8 : (in_kind == B2SD_IN_F32_NCHW ? SC_IN_F32_NCHW : SC_IN_F16_NCHW);
@@ -2194,32 +2241,67 @@ int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int
         c.x = frame_in; c.in_h = in_h; c.in_w = in_w; c.flags = in_flags | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
         TRY(smallconv_launch(c, s));
     }
-    if (h->group) {
-        // stage-pipelined lanes of one stateful stream: encoder body | [wait previous frame's UNet stage] last encoder conv,
-        // UNet, scheduler step [signal] | decoder.  Lanes run on different streams; only the middle stage is serialised.
-        const size_t cut[4] = {0, h->idx_enc_end, h->idx_unet_end, h->prog_frame.size()};
-        for (int st = 0; st < 3; ++st) {
-            if (st == 1) CUDA_OK(cudaStreamWaitEvent(s, h->group->unet_done, 0));
-            if (h->cfg.use_cuda_graph) {
-                if (!h->stage_exec[st]) {
-                    cudaStream_t cs;
-                    CUDA_OK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-                    CUDA_OK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-                    int rc = h->run_range(h->prog_frame, cut[st], cut[st + 1], cs);
-                    cudaError_t ec = cudaStreamEndCapture(cs, &h->stage_graph[st]);
-                    cudaStreamDestroy(cs);
-                    if (rc || ec != cudaSuccess || cudaGraphInstantiate(&h->stage_exec[st], h->stage_graph[st], 0) != cudaSuccess) {
-                        if (!rc) b2_set_error("b2sd_step: CUDA graph capture of stage %d failed: %s", st, cudaGetErrorString(ec != cudaSuccess ? ec : cudaGetLastError()));
-                        h->drop_graphs();
-                        return -1;
-                    }
-                }
-                CUDA_OK(cudaGraphLaunch(h->stage_exec[st], s));
-            } else {
-                TRY(h->run_range(h->prog_frame, cut[st], cut[st + 1], s));
-            }
-            if (st == 1) CUDA_OK(cudaEventRecord(h->group->unet_done, s));
+    return 0;
+}
+
+// the frame program on a stream state: encoder body | [wait for the state's previous step, state -> slots 1..T-1] last encoder
+// conv, UNet, scheduler step [slots 1..T-1 -> state, signal] | decoder.  Only the middle stage is serialised per state: the
+// stages of other states, and the other stages of this one, overlap on other lanes.  The copies and the wait stay outside the
+// stage graphs because the state changes from frame to frame.
+static int step_stages(b2sd_handle h, b2sd_state* state, cudaStream_t s) {
+    const size_t cut[4] = {0, h->idx_enc_end, h->idx_unet_end, h->prog_frame.size()};
+    __half* slots = h->x_in.p + (size_t)h->lh * h->lw * 4;   // slot 1
+    for (int st = 0; st < 3; ++st) {
+        if (st == 1) {
+            CUDA_OK(cudaStreamWaitEvent(s, state->done, 0));
+            if (state->bytes) CUDA_OK(cudaMemcpyAsync(slots, state->buf, state->bytes, cudaMemcpyDeviceToDevice, s));
         }
+        if (h->cfg.use_cuda_graph) {
+            if (!h->stage_exec[st]) {
+                cudaStream_t cs;
+                CUDA_OK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+                CUDA_OK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
+                int rc = h->run_range(h->prog_frame, cut[st], cut[st + 1], cs);
+                cudaError_t ec = cudaStreamEndCapture(cs, &h->stage_graph[st]);
+                cudaStreamDestroy(cs);
+                if (rc || ec != cudaSuccess || cudaGraphInstantiate(&h->stage_exec[st], h->stage_graph[st], 0) != cudaSuccess) {
+                    if (!rc) b2_set_error("b2sd_step: CUDA graph capture of stage %d failed: %s", st, cudaGetErrorString(ec != cudaSuccess ? ec : cudaGetLastError()));
+                    h->drop_graphs();
+                    return -1;
+                }
+            }
+            CUDA_OK(cudaGraphLaunch(h->stage_exec[st], s));
+        } else {
+            TRY(h->run_range(h->prog_frame, cut[st], cut[st + 1], s));
+        }
+        if (st == 1) {
+            if (state->bytes) CUDA_OK(cudaMemcpyAsync(state->buf, slots, state->bytes, cudaMemcpyDeviceToDevice, s));
+            CUDA_OK(cudaEventRecord(state->done, s));
+        }
+    }
+    return 0;
+}
+
+static int step_tail(b2sd_handle h, void* frame_out, int out_kind, cudaStream_t s) {
+    if (out_kind == B2SD_OUT_F16_NCHW)
+        return post_f16_launch(h->image.p, h->image.ld, static_cast<__half*>(frame_out), 1, h->cfg.height, h->cfg.width, s);
+    return post_u8_launch(h->image.p, h->image.ld, static_cast<uint8_t*>(frame_out), 1, h->cfg.height, h->cfg.width, s);
+}
+
+int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int in_w, void* frame_out, int out_kind,
+                 void* stream) {
+    if (!h || !h->built) {
+        b2_set_error("b2sd_step: call b2sd_prepare first");
+        return -1;
+    }
+    if (!frame_in || !frame_out || in_h < 1 || in_w < 1) {
+        b2_set_error("b2sd_step: bad frame arguments");
+        return -1;
+    }
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    TRY(step_heads(h, frame_in, in_kind, in_h, in_w, s));
+    if (h->pair_state) {
+        TRY(step_stages(h, h->pair_state.get(), s));
     } else if (h->cfg.use_cuda_graph) {
         if (!h->graph_exec) {
             cudaStream_t cs;
@@ -2240,9 +2322,59 @@ int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int
     } else {
         TRY(h->run(h->prog_frame, s));
     }
-    if (out_kind == B2SD_OUT_F16_NCHW)
-        return post_f16_launch(h->image.p, h->image.ld, static_cast<__half*>(frame_out), 1, h->cfg.height, h->cfg.width, s);
-    return post_u8_launch(h->image.p, h->image.ld, static_cast<uint8_t*>(frame_out), 1, h->cfg.height, h->cfg.width, s);
+    return step_tail(h, frame_out, out_kind, s);
+}
+
+int b2sd_state_create(b2sd_handle h, b2sd_state_handle* out, void* stream) {
+    if (!h || !out || !h->built) {
+        b2_set_error("b2sd_state_create: null argument, or b2sd_prepare not called");
+        return -1;
+    }
+    if (h->pair_state) {
+        b2_set_error("b2sd_state_create: the engine is part of a b2sd_share_stream_state pair, which steps its own state");
+        return -1;
+    }
+    return state_new(h, reinterpret_cast<cudaStream_t>(stream), out);
+}
+
+int b2sd_state_reset(b2sd_state_handle state, void* stream) {
+    if (!state) {
+        b2_set_error("b2sd_state_reset: null state");
+        return -1;
+    }
+    return state_reset(state, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2sd_state_destroy(b2sd_state_handle state, void* stream) {
+    return state ? state_free(state, reinterpret_cast<cudaStream_t>(stream)) : 0;
+}
+
+int b2sd_step_state(b2sd_handle h, b2sd_state_handle state, const void* frame_in, int in_kind, int in_h, int in_w,
+                    void* frame_out, int out_kind, void* stream) {
+    if (!h || !h->built || !state) {
+        b2_set_error("b2sd_step_state: null argument, or b2sd_prepare not called");
+        return -1;
+    }
+    if (h->pair_state) {
+        b2_set_error("b2sd_step_state: the engine is part of a b2sd_share_stream_state pair, which steps its own state");
+        return -1;
+    }
+    if (state->ws.lock() != h->ws || state->batch != h->cfg.batch || state->height != h->cfg.height ||
+        state->width != h->cfg.width) {
+        b2_set_error("b2sd_step_state: the state was made for another weight store, batch or size (state: batch %d, %dx%d; "
+                     "engine: batch %d, %dx%d)", state->batch, state->height, state->width, h->cfg.batch, h->cfg.height,
+                     h->cfg.width);
+        return -1;
+    }
+    if (!state->bytes) return b2sd_step_ex(h, frame_in, in_kind, in_h, in_w, frame_out, out_kind, stream);
+    if (!frame_in || !frame_out || in_h < 1 || in_w < 1) {
+        b2_set_error("b2sd_step_state: bad frame arguments");
+        return -1;
+    }
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    TRY(step_heads(h, frame_in, in_kind, in_h, in_w, s));
+    TRY(step_stages(h, state, s));
+    return step_tail(h, frame_out, out_kind, s);
 }
 
 int b2sd_get_tensor(b2sd_handle h, const char* name, void* dst, int64_t capacity, int64_t* count, int* dims4, void* stream) {
@@ -2372,7 +2504,7 @@ int b2sd_audit_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, voi
         b2_set_error("b2sd_audit_step: bad arguments (or b2sd_prepare not called)");
         return -1;
     }
-    if (h->group) {
+    if (h->pair_state) {
         b2_set_error("b2sd_audit_step: stage-pipelined lanes (b2sd_share_stream_state) are not supported");
         return -1;
     }
@@ -2498,12 +2630,12 @@ int b2sd_share_stream_state(b2sd_handle lane, b2sd_handle owner) {
         b2_set_error("b2sd_share_stream_state: engines must be lanes of one weight store with the same batch and size");
         return -1;
     }
-    if (!owner->group) {
-        owner->group = std::make_shared<b2sd_engine::StageGroup>();
-        CUDA_OK(cudaEventCreateWithFlags(&owner->group->unet_done, cudaEventDisableTiming));
+    if (!owner->pair_state) {
+        b2sd_state* st = nullptr;
+        TRY(state_new(owner, nullptr, &st));
+        owner->pair_state = std::shared_ptr<b2sd_state>(st, [](b2sd_state* p) { state_free(p, nullptr); });
     }
-    lane->group = owner->group;
-    lane->x_in.p = owner->x_in.p;        // the UNet input batch: slot 0 = fresh x_t, slots 1.. = x_t_latent_buffer
+    lane->pair_state = owner->pair_state;
     lane->built = false;
     owner->built = false;
     return 0;

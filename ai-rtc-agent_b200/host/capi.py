@@ -218,6 +218,12 @@ def lib() -> C.CDLL:
         _lib.b2sd_share_stream_state.restype = C.c_int
         _lib.b2sd_set_concurrency.argtypes = [vp, ci]
         _lib.b2sd_set_concurrency.restype = C.c_int
+        _lib.b2sd_state_create.argtypes = [vp, C.POINTER(vp), vp]
+        _lib.b2sd_state_reset.argtypes = [vp, vp]
+        _lib.b2sd_state_destroy.argtypes = [vp, vp]
+        _lib.b2sd_step_state.argtypes = [vp, vp, vp, ci, ci, ci, vp, ci, vp]
+        for name in ("state_create", "state_reset", "state_destroy", "step_state"):
+            getattr(_lib, "b2sd_" + name).restype = C.c_int
         _lib.b2sd_profile.argtypes = [vp, vp, ci, ci, vp, ci, C.c_char_p, i64, vp]
         _lib.b2sd_profile.restype = C.c_int
         _lib.b2sd_profile_kind.argtypes = [vp, C.c_char_p, ci, C.POINTER(C.c_double), C.POINTER(ci), C.POINTER(C.c_double), vp]

@@ -28,6 +28,20 @@ DEFAULT_GUIDANCE_SCALE = 0.0
 DEFAULT_LANES_ONE_STEP = 8    # frames in flight for a 1-step stream batch (measured with the throughput launch policy: 4 -> 409, 6 -> 470,
                               # 8 -> 483, 10 -> 481, 12 -> 486 fps; p50 submit -> result 10.4 / 13.5 / 16.8 / 17.8 / 18.7 ms; lanes=1: 241 fps, 4.2 ms)
 DEFAULT_LANES_STATEFUL = 2    # T > 1: stage pipelining over two lanes that share the stream-batch state
+DEFAULT_LANES_PER_PEER = 2    # T > 1 with per-peer streams: independent lanes, any of which steps any peer's state (SD-1.5 T=4
+                              # 512x512, tools/bench_peers.py: 2 lanes 47.0 / 54.3 fps at 1 / 2+ peers, p50 42.5 / 36.8 ms; 3 lanes
+                              # 47.1 / 56.1 fps at 1 / 4+ peers but p50 63.7 / 53.4 ms and 3 GB more; 4 lanes no faster)
+PER_PEER_STREAMS_ENV = "B200SD_PER_PEER_STREAMS"
+
+
+def env_flag(name: str) -> bool:
+    """A boolean environment switch: unset, "", 0, false, no, off -> False; 1, true, yes, on -> True; anything else raises."""
+    v = os.getenv(name, "").strip().lower()
+    if v in ("", "0", "false", "no", "off"):
+        return False
+    if v in ("1", "true", "yes", "on"):
+        return True
+    raise ValueError(f"${name}={os.getenv(name)!r}: expected 1/0, true/false, yes/no or on/off")
 
 
 def _is_video_frame(frame) -> bool:
@@ -55,13 +69,25 @@ def _as_torch_u8_nhwc(frame, device) -> torch.Tensor:
 
 
 class StreamDiffusionPipeline:
+    per_peer_streams = False
+    _own_state = None   # the StreamState enqueue() steps with per-peer streams; None: the engines' own shared state
+
     def __init__(self, model_id: str, t_index_list: Optional[List[int]] = None, width: int = 512, height: int = 512,
-                 prompt: str = DEFAULT_PROMPT, lanes: Optional[int] = None):
+                 prompt: str = DEFAULT_PROMPT, lanes: Optional[int] = None, per_peer_streams: Optional[bool] = None):
         """lanes: frames in flight for enqueue() ($B200SD_LANES overrides the default).  With a 1-step stream batch (SD-Turbo)
         consecutive frames are independent: DEFAULT_LANES_ONE_STEP lanes process frame n+1.. while frame n is still on the GPU.
         With T > 1 the stream batch carries state from frame to frame: two lanes share that state and are stage-pipelined (TAESD
         encoder of frame n+1 and decoder of frame n-1 overlap the UNet of frame n).  Both are bit-identical to submitting the
-        same frames one at a time."""
+        same frames one at a time.
+
+        per_peer_streams (None: $B200SD_PER_PEER_STREAMS, default off): one pipeline serves several viewers, each with its own
+        temporal stream.  open_stream() gives a viewer a PeerStream whose frames carry that viewer's stream-batch state only;
+        pipeline(frame) / enqueue(frame) keep stepping the pipeline's own stream.  The lanes are then independent
+        (DEFAULT_LANES_PER_PEER for T > 1) and any lane steps any viewer's state.  Off, every caller of the pipeline shares one
+        temporal stream, as in the reference: with T > 1 a frame's output then mixes in frames of the other callers."""
+        if per_peer_streams is None:
+            per_peer_streams = env_flag(PER_PEER_STREAMS_ENV)
+        self.per_peer_streams = bool(per_peer_streams)
         self.prompt = prompt
         self.t_index_list = list(t_index_list) if t_index_list is not None else DEFAULT_T_INDEX_LIST
         self.device = "cuda"
@@ -82,9 +108,11 @@ class StreamDiffusionPipeline:
             engine_dir=os.getenv("TRT_ENGINES_CACHE", "./models/engines"),
         )
         stateful = len(self.t_index_list) > 1     # x_t_latent_buffer chains frame n+1 to frame n
+        shared = stateful and not self.per_peer_streams   # lanes stage-pipeline one shared stream-batch state
         if lanes is None:
-            lanes = int(os.getenv("B200SD_LANES", "0")) or (DEFAULT_LANES_STATEFUL if stateful else DEFAULT_LANES_ONE_STEP)
-        if stateful:
+            default = (DEFAULT_LANES_PER_PEER if self.per_peer_streams else DEFAULT_LANES_STATEFUL) if stateful else DEFAULT_LANES_ONE_STEP
+            lanes = int(os.getenv("B200SD_LANES", "0")) or default
+        if shared:
             lanes = min(lanes, 2)   # three stages, the middle one serial: a third lane has nothing to overlap
         # launch policy = number of frames in flight ($B200SD_POLICY_FRAMES overrides it for profiling: a single lane running the
         # throughput policy's launches gives ncu a clean one-frame launch list)
@@ -92,7 +120,9 @@ class StreamDiffusionPipeline:
         self.model.prepare(prompt=self.prompt, num_inference_steps=DEFAULT_NUM_INFERENCE_STEPS,
                            guidance_scale=DEFAULT_GUIDANCE_SCALE)
         sd = self.model.stream
-        self._engines = [sd] + [sd.add_lane(share_state=stateful) for _ in range(max(1, lanes) - 1)]
+        self._engines = [sd] + [sd.add_lane(share_state=shared) for _ in range(max(1, lanes) - 1)]
+        # per-peer mode: enqueue() steps this state, so the pipeline's own stream is one more peer of the lane pool
+        self._own_state = sd.new_state() if self.per_peer_streams else None
         # one lane: frames run on the caller's stream, exactly as before.  Several lanes: every lane has its own stream (a lane on
         # the caller's stream would order the other lanes' "input ready" events behind its frames and serialise them)
         self._lane_streams = [None] if len(self._engines) == 1 else [torch.cuda.Stream(sd.device) for _ in self._engines]
@@ -159,11 +189,22 @@ class StreamDiffusionPipeline:
     def __call__(self, frame):
         """lib/pipeline.py:76-96, blocking semantics preserved: the result is complete when the call returns only in the
         software-encode branch (`.cpu()`); with NVENC set the CUDA tensor is returned stream-ordered, like the reference."""
-        ticket = self.enqueue(frame)
+        return self._call(frame, self._own_state)
+
+    def _call(self, frame, state):
+        ticket = self._enqueue(frame, state)
         if os.getenv("NVENC"):
             ticket.wait(torch.cuda.current_stream(self.model.stream.device))   # stream-ordered result, whichever lane ran it
             return ticket.result(wait=False)
         return ticket.result()
+
+    def open_stream(self) -> "PeerStream":
+        """A new viewer's temporal stream (per_peer_streams only): its frames carry its own stream-batch state, starting from
+        zeros, whatever other viewers submit in between."""
+        if not self.per_peer_streams:
+            raise RuntimeError("open_stream() needs per_peer_streams=True (or $B200SD_PER_PEER_STREAMS=1): without it every "
+                               "caller of this pipeline shares one temporal stream")
+        return PeerStream(self)
 
     # ---- non-blocking entry (SURVEY.md 8f-2): everything is queued on CUDA streams and a ticket comes back at once ------
     def enqueue(self, frame) -> "FrameTicket":
@@ -171,6 +212,11 @@ class StreamDiffusionPipeline:
         stream.  av.VideoFrame input is staged through a pinned ring and copied on a separate copy stream, so the upload of
         frame n+1 overlaps the compute of frame n; with NVENC unset the download of the result is queued the same way.
         Tickets complete in submission order (one temporal stream per pipeline, like the reference)."""
+        return self._enqueue(frame, self._own_state)
+
+    def _enqueue(self, frame, state) -> "FrameTicket":
+        """enqueue() on `state` (a StreamState, or None for the engines' own shared stream).  Lanes rotate over all submissions;
+        frames of one state are ordered on the device by the state's event."""
         if not _is_gpu_frame(frame) and not _is_video_frame(frame):
             raise Exception("invalid frame type")
         dev = self.model.stream.device
@@ -205,7 +251,7 @@ class StreamDiffusionPipeline:
             if compute is not caller:
                 rgb.record_stream(compute)
         with torch.cuda.stream(compute):
-            post_output = engine.step_u8(rgb)
+            post_output = engine.step_u8(rgb, state=state)
         if compute is not caller:
             post_output.record_stream(caller)
         if slot is not None:
@@ -269,3 +315,39 @@ class FrameTicket:
         out.pts = self._src.pts
         out.time_base = self._src.time_base
         return out
+
+
+class PeerStream:
+    """One viewer's temporal stream on a per-peer pipeline (StreamDiffusionPipeline.open_stream): enqueue() / __call__ behave
+    as the pipeline's, with this viewer's own stream-batch state.  close() frees the state after its last frame, without a
+    host synchronisation."""
+
+    def __init__(self, pipeline: StreamDiffusionPipeline):
+        self._pipeline = pipeline
+        self._state = pipeline.model.stream.new_state()
+
+    @property
+    def closed(self) -> bool:
+        return self._state is None
+
+    def _live_state(self):
+        if self._state is None:
+            raise RuntimeError("the peer stream is closed")
+        return self._state
+
+    def enqueue(self, frame) -> FrameTicket:
+        return self._pipeline._enqueue(frame, self._live_state())
+
+    def __call__(self, frame):
+        return self._pipeline._call(frame, self._live_state())
+
+    def close(self) -> None:
+        if self._state is not None:
+            state, self._state = self._state, None
+            state.close()
+
+    def __enter__(self) -> "PeerStream":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()

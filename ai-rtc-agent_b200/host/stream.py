@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import weakref
 from typing import Callable, Dict, List, Optional
 
 import numpy as np
@@ -112,8 +113,6 @@ class StreamDiffusion:
         self.image_processor = ImageProcessor(8)
         self.prompt_encoder = prompt_encoder
         self.text_encoder = prompt_encoder
-        self.unet = self
-        self.vae = self
         self._handle = C.c_void_p()
         self._prepared = False
         self._lib = capi.lib()
@@ -143,8 +142,11 @@ class StreamDiffusion:
                           use_denoising_batch=use_denoising_batch, frame_buffer_size=frame_buffer_size, cfg_type=cfg_type,
                           device=device, use_cuda_graph=use_cuda_graph, use_tiny_vae=use_tiny_vae,
                           vae_scaling_factor=vae_scaling_factor)
-        self.lanes: List["StreamDiffusion"] = []     # extra engines over this one's weights (add_lane)
-        self._parent = parent
+        # extra engines over this one's weights (add_lane).  A lane keeps no reference to its parent: an engine and its lanes then
+        # form no reference cycle, so their device memory is released as soon as the last reference goes, not at the next
+        # run of the garbage collector
+        self.lanes: List["StreamDiffusion"] = []
+        self._states = parent._states if parent is not None else weakref.WeakSet()   # live StreamStates of the engine and its lanes
         if parent is not None:
             # a lane: shares the parent's weights in HBM, owns its activations / stream state / CUDA graph
             capi.check(self._lib.b2sd_create_lane(parent._handle, C.byref(cfg), C.byref(self._handle)), "b2sd_create_lane")
@@ -158,6 +160,16 @@ class StreamDiffusion:
             self._load("vae.", vae_sd)
             self._load("controlnet.", controlnet_sd or {})
             self._load("hed.", hed_sd or {})
+
+    # the reference reaches the UNet and the VAE as `stream.unet` / `stream.vae`; both are this engine.  Properties, not attributes
+    # holding self: a self-reference would keep every engine's device memory until the garbage collector runs
+    @property
+    def unet(self) -> "StreamDiffusion":
+        return self
+
+    @property
+    def vae(self) -> "StreamDiffusion":
+        return self
 
     def set_concurrency(self, frames_in_flight: int) -> None:
         """Tell the engine how many frames will be in flight on this GPU (before prepare()): > 1 selects the throughput
@@ -225,6 +237,9 @@ class StreamDiffusion:
         self._engine_prepare()
         for lane in self.lanes:
             lane._prepare_like(self)
+        for state in list(self._states):   # as prepare zeroes the engines' own latent buffers
+            if not state.closed:
+                state.reset()
 
     _SCHEDULE_ATTRS = ("generator", "guidance_scale", "delta", "prompt_embeds", "timesteps", "sub_timesteps", "sub_timesteps_tensor",
                        "init_noise", "stock_noise", "c_skip", "c_out", "alpha_prod_t_sqrt", "beta_prod_t_sqrt")
@@ -261,6 +276,14 @@ class StreamDiffusion:
         self.lanes.append(lane)
         return lane
 
+    def new_state(self) -> "StreamState":
+        """A fresh temporal stream (zeroed x_t_latent_buffer) that this engine and every lane of its weights can step:
+        pass it as `state=` to step_u8 / step_u8_into / __call__.  prepare() resets it.  Not for share_state lanes."""
+        self._check()
+        state = StreamState(self)
+        self._states.add(state)
+        return state
+
     def _encode(self, prompt: str) -> torch.Tensor:
         e = self.prompt_encoder(prompt)
         if e.dim() == 2:
@@ -293,9 +316,19 @@ class StreamDiffusion:
         if not self._prepared:
             raise RuntimeError("StreamDiffusion.prepare() must be called before frames are processed")
 
+    def _step(self, frame_ptr: int, in_kind: int, in_h: int, in_w: int, out_ptr: int, out_kind: int,
+              state: Optional["StreamState"]) -> None:
+        if state is None:
+            capi.check(self._lib.b2sd_step_ex(self._handle, frame_ptr, in_kind, in_h, in_w, out_ptr, out_kind, self._stream()),
+                       "b2sd_step_ex")
+        else:
+            capi.check(self._lib.b2sd_step_state(self._handle, state.handle, frame_ptr, in_kind, in_h, in_w, out_ptr, out_kind,
+                                                 self._stream()), "b2sd_step_state")
+
     @torch.no_grad()
-    def __call__(self, x: torch.Tensor) -> torch.Tensor:
-        """x: (3,H',W') or (1,3,H',W') float tensor in [0,1] on the GPU -> (1,3,H,W) fp16 image in ~[-1,1]."""
+    def __call__(self, x: torch.Tensor, state: Optional["StreamState"] = None) -> torch.Tensor:
+        """x: (3,H',W') or (1,3,H',W') float tensor in [0,1] on the GPU -> (1,3,H,W) fp16 image in ~[-1,1].
+        state: step that stream state (new_state) instead of this engine's own."""
         self._check()
         if x.dim() == 3:
             x = x.unsqueeze(0)
@@ -315,8 +348,7 @@ class StreamDiffusion:
         x = x.contiguous()
         out = torch.empty((1, 3, self.height, self.width), dtype=torch.float16, device=self.device)
         t0 = self._tick()
-        capi.check(self._lib.b2sd_step_ex(self._handle, x.data_ptr(), kind, x.shape[-2], x.shape[-1], out.data_ptr(),
-                                          capi.OUT_F16_NCHW, self._stream()), "b2sd_step_ex")
+        self._step(x.data_ptr(), kind, x.shape[-2], x.shape[-1], out.data_ptr(), capi.OUT_F16_NCHW, state)
         self._tock(t0)
         self.prev_image_result = out
         return out
@@ -347,23 +379,23 @@ class StreamDiffusion:
             self._ev_pending = pair
 
     @torch.no_grad()
-    def step_u8(self, frame_nhwc: torch.Tensor) -> torch.Tensor:
+    def step_u8(self, frame_nhwc: torch.Tensor, state: Optional["StreamState"] = None) -> torch.Tensor:
         """Fused fast path of lib/pipeline.py:76-96: u8 NHWC (1,H',W',3) CUDA tensor in, u8 NCHW (1,3,H,W) out,
-        one engine call, no intermediate tensors."""
+        one engine call, no intermediate tensors.  state: step that stream state (new_state) instead of this engine's own."""
         self._check()
         if frame_nhwc.dtype != torch.uint8 or frame_nhwc.dim() != 4 or frame_nhwc.shape[-1] != 3 or not frame_nhwc.is_cuda:
             raise TypeError("expected a CUDA uint8 tensor shaped (1,H,W,3)")
         frame_nhwc = frame_nhwc.contiguous()
         out = torch.empty((1, 3, self.height, self.width), dtype=torch.uint8, device=self.device)
         t0 = self._tick()
-        capi.check(self._lib.b2sd_step(self._handle, frame_nhwc.data_ptr(), frame_nhwc.shape[1], frame_nhwc.shape[2],
-                                       out.data_ptr(), self._stream()), "b2sd_step")
+        self._step(frame_nhwc.data_ptr(), capi.IN_U8_NHWC, frame_nhwc.shape[1], frame_nhwc.shape[2], out.data_ptr(),
+                   capi.OUT_U8_NCHW, state)
         self._tock(t0)
         return out
 
-    def step_u8_into(self, frame_nhwc: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
-        capi.check(self._lib.b2sd_step(self._handle, frame_nhwc.data_ptr(), frame_nhwc.shape[1], frame_nhwc.shape[2],
-                                       out.data_ptr(), self._stream()), "b2sd_step")
+    def step_u8_into(self, frame_nhwc: torch.Tensor, out: torch.Tensor, state: Optional["StreamState"] = None) -> torch.Tensor:
+        self._step(frame_nhwc.data_ptr(), capi.IN_U8_NHWC, frame_nhwc.shape[1], frame_nhwc.shape[2], out.data_ptr(),
+                   capi.OUT_U8_NCHW, state)
         return out
 
     def get_tensor(self, name: str) -> torch.Tensor:
@@ -446,3 +478,47 @@ class StreamDiffusion:
     @property
     def launches_per_step(self) -> int:
         return self._lib.b2sd_launches_per_step(self._handle)
+
+
+class StreamState:
+    """One temporal stream's stream-batch state (x_t_latent_buffer), apart from the engines that step it (b2sd_state_*): any
+    lane of the creating engine's weights steps it, so several video streams share a pool of lanes without mixing their
+    frames.  (T-1)*(h/8)*(w/8)*4 fp16 values on the device; nothing at T = 1.  Made by StreamDiffusion.new_state()."""
+
+    def __init__(self, engine: StreamDiffusion):
+        self._engine = engine          # keeps the engine (and its stream / library) alive while the state exists
+        self._lib = engine._lib
+        self._handle = C.c_void_p()
+        capi.check(self._lib.b2sd_state_create(engine._handle, C.byref(self._handle), engine._stream()), "b2sd_state_create")
+
+    @property
+    def handle(self) -> C.c_void_p:
+        if not self._handle.value:
+            raise RuntimeError("the stream state is closed")
+        return self._handle
+
+    @property
+    def closed(self) -> bool:
+        return not self._handle.value
+
+    def reset(self) -> None:
+        """Zero the state after its last step (stream-ordered, no host synchronisation)."""
+        capi.check(self._lib.b2sd_state_reset(self.handle, self._engine._stream()), "b2sd_state_reset")
+
+    def close(self) -> None:
+        """Free the state after its last step, stream-ordered, without a host synchronisation.  Idempotent."""
+        if self._handle.value:
+            h, self._handle = self._handle, C.c_void_p()
+            capi.check(self._lib.b2sd_state_destroy(h, self._engine._stream()), "b2sd_state_destroy")
+
+    def __enter__(self) -> "StreamState":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -42,11 +42,39 @@ class VideoStreamTrack(_Base):
         self.warmup_frames = int(os.getenv("WARMUP_FRAMES", 10))
         self.drop_frames = int(os.getenv("DROP_FRAMES", 0))
         self.poll_interval = poll_interval
+        # a pipeline with per-peer streams gives this track its own temporal stream, opened at the first frame
+        self._per_peer = bool(getattr(pipeline, "per_peer_streams", False))
+        self._peer = None
+
+    def _target(self):
+        if not self._per_peer:
+            return self.pipeline
+        if self._peer is None:
+            self._peer = self.pipeline.open_stream()
+        return self._peer
+
+    def _close_stream(self):
+        """Free this track's stream state (stream-ordered after its last frame: no device or host synchronisation)."""
+        if self._peer is not None:
+            peer, self._peer = self._peer, None
+            peer.close()
+
+    def stop(self):
+        super().stop()
+        self._close_stream()
+
+    async def _recv_source(self):
+        try:
+            return await self.track.recv()
+        except BaseException:   # the source ended (aiortc raises MediaStreamError) or the coroutine was cancelled
+            self._close_stream()
+            raise
 
     async def _process(self, frame):
-        enqueue = getattr(self.pipeline, "enqueue", None)
+        target = self._target()
+        enqueue = getattr(target, "enqueue", None)
         if enqueue is None:                      # any callable pipeline works; it is then called synchronously like the reference
-            return self.pipeline(frame)
+            return target(frame)
         ticket = enqueue(frame)
         while not ticket.done():
             await asyncio.sleep(self.poll_interval)   # let the event loop run while the GPU works
@@ -55,13 +83,13 @@ class VideoStreamTrack(_Base):
     async def recv(self):
         while self.warmup_frame_idx < self.warmup_frames:
             logger.info(f"dropping warmup frames {self.warmup_frame_idx}")
-            frame = await self.track.recv()
+            frame = await self._recv_source()
             await self._process(frame)
             self.warmup_frame_idx += 1
 
         # Frame dropping (lib/tracks.py:27-31): skipping source frames can help playback with some encoders
         for _ in range(self.drop_frames):
-            await self.track.recv()
+            await self._recv_source()
 
-        frame = await self.track.recv()
+        frame = await self._recv_source()
         return await self._process(frame)

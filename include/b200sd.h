@@ -388,8 +388,28 @@ int b2sd_audit_refresh(b2sd_handle h, b2sd_audit_fn fn, void* user, void* stream
  * simply alternate): `lane` shares `owner`'s stream-batch state; the frame program of each is cut into TAESD encoder body |
  * last encoder conv + UNet + scheduler step | TAESD decoder, and only the middle stage is serialised between the lanes (one
  * CUDA event), so the encoder of frame n+1 and the decoder of frame n-1 overlap the UNet of frame n.  Both engines must be
- * lanes of one weight store with equal batch / size; call before b2sd_prepare; submit frames alternately, in order. */
+ * lanes of one weight store with equal batch / size; call before b2sd_prepare; submit frames alternately, in order.
+ * Both engines then step one stream state (b2sd_state_*) that `owner` creates; b2sd_prepare of either zeroes it. */
 int b2sd_share_stream_state(b2sd_handle lane, b2sd_handle owner);
+
+/* Stream states: the stream-batch state of one temporal stream (x_t_latent_buffer, slots 1 .. T-1 of the UNet input batch,
+ * (T-1) * (h/8) * (w/8) * 4 fp16 values; nothing at T = 1) kept apart from the engines that step it.  Any engine of the
+ * state's weight store with the state's batch and size can step it, so several video streams (one state each) share a pool
+ * of lanes: frames of different states overlap completely, and consecutive frames of one state are stage-pipelined across
+ * lanes as with b2sd_share_stream_state.  A state carries one CUDA event that orders its steps; submit the frames of one
+ * state in order from one host thread.  Engines that are part of a b2sd_share_stream_state pair refuse these calls. */
+typedef struct b2sd_state* b2sd_state_handle;
+/* a zeroed state sized for h's batch and size (h prepared); allocated stream-ordered on `stream` */
+int b2sd_state_create(b2sd_handle h, b2sd_state_handle* out, void* stream);
+/* zero the state (what b2sd_prepare does to an engine's own latent buffer), after its last step, on `stream` */
+int b2sd_state_reset(b2sd_state_handle state, void* stream);
+/* free the state on `stream` after its last step, without a host synchronisation; NULL is a no-op */
+int b2sd_state_destroy(b2sd_state_handle state, void* stream);
+/* b2sd_step_ex on `state`: input heads, encoder body | wait for the state's previous step, copy the state into slots 1 .. T-1,
+ * latent conv + UNet (+ ControlNet) + scheduler step, copy slots 1 .. T-1 back, record the state's event | decoder, tail.
+ * At T = 1 the state is empty and this is b2sd_step_ex. */
+int b2sd_step_state(b2sd_handle h, b2sd_state_handle state, const void* frame_in, int in_kind, int in_h, int in_w,
+                    void* frame_out, int out_kind, void* stream);
 /* How many frames will be in flight on this GPU (lanes / independent streams).  1 (default): launch policy tuned for the
  * latency of a single frame; > 1: policy tuned for throughput (smaller operand rings so CTAs of different frames share an
  * SM; from 4 frames in flight on, contractions are launched as CTA pairs -- tcgen05.mma.cta_group::2 -- without split-K: least

@@ -1,5 +1,5 @@
-// Epilogue helpers shared by the wgmma contraction kernels (igemm.cu, tconv.cu): accumulator fragment (registers) or staged
-// fp32 row -> bias / scale / residual / ReLU / GEGLU -> fp16 NHWC stores.
+// Epilogue helpers of the wgmma contraction kernels (igemm.cu; tconv.cu has its own, staged through shared memory): accumulator
+// fragment (registers) or staged fp32 row -> bias / scale / residual / ReLU / GEGLU -> fp16 NHWC stores.
 #pragma once
 #include "igemm.cuh"
 #include "ptx.cuh"

@@ -130,6 +130,26 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
         : "memory");
 }
 
+// Shared -> global tensor store, tracked by the issuing thread's bulk async-groups; elements outside the tensor are not written.
+// The writers of the source tile must have run fence_proxy_async_smem() (and synchronised with the issuing thread) first.
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(reinterpret_cast<uint64_t>(m)),
+                 "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's committed stores still read their shared-memory source (the source may then be overwritten)
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's committed stores are still incomplete (their writes are not yet performed)
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+
+// barrier over `count` threads (a multiple of 32) under id `id` (1..15; 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 // Multicast form (CTA pairs): the box lands at the same shared-memory offset in every CTA of `cta_mask` (cluster ranks),
 // and each destination's mbarrier at `bar`'s offset receives the complete_tx of its bytes.
 __device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, uint16_t cta_mask) {

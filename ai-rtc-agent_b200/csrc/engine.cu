@@ -292,6 +292,45 @@ struct WeightStore {
     std::map<std::string, __half*> packed;   // cache of packed weight matrices
     std::map<std::string, float*> fvec;      // cache of fp32 vectors
     std::map<std::string, size_t> packed_bytes, fvec_bytes;   // their sizes (b2sd_export_packed)
+    std::shared_ptr<struct CondPool> cond_pool;   // made by the first conditioning override of a state of this store
+};
+
+enum { COND_PROMPT = 0, COND_TIME = 1 };
+static const uint64_t COND_GLOBAL = 0, COND_UNKNOWN = ~0ull;   // what a lane's block holds, besides an override's id
+
+// Where the conditioning overrides of a weight store's states live and are freed.  The pool never makes an allocation wait for
+// a free on another stream (no internal dependencies), and the frees run on a stream of their own: so neither the update that
+// replaces an override nor the next one ever makes a lane's stream wait for the frames queued on another lane.
+struct CondPool {
+    cudaMemPool_t pool = nullptr;
+    cudaStream_t reaper = nullptr;
+    ~CondPool() {
+        if (reaper) cudaStreamDestroy(reaper);   // returns at once; pending frees still run
+        if (pool) cudaMemPoolDestroy(pool);      // released once its last allocation is freed
+    }
+};
+
+// One state's own copy of one conditioning block (b2sd_state_set_prompt_embeds / _set_timesteps).  Immutable once published: an
+// update makes a new one, since a lane that is behind on the device may still copy out of the old one.  The destructor frees it
+// on the pool's reaper stream after the copy that computed it and after the latest copy out of it on every stream.
+struct CondOverride {
+    uint64_t id = 0;
+    void* buf = nullptr;
+    size_t bytes = 0;
+    cudaEvent_t ready = nullptr;   // recorded once buf holds the block
+    std::vector<std::pair<cudaStream_t, cudaEvent_t>> uses;   // per stream, recorded after its latest copy out of buf
+    std::shared_ptr<CondPool> pool;
+    ~CondOverride() {
+        if (!pool) return;   // the pool could not be made: nothing was allocated
+        const cudaStream_t r = pool->reaper;
+        if (ready) cudaStreamWaitEvent(r, ready, 0);
+        for (auto& u : uses) {
+            cudaStreamWaitEvent(r, u.second, 0);
+            cudaEventDestroy(u.second);
+        }
+        if (buf) cudaFreeAsync(buf, r);
+        if (ready) cudaEventDestroy(ready);
+    }
 };
 
 // One temporal stream's stream-batch state (b2sd_state_*): slots 1 .. T-1 of the UNet input batch, NHWC fp16, stream-ordered
@@ -302,6 +341,7 @@ struct b2sd_state {
     size_t bytes = 0;
     __half* buf = nullptr;
     cudaEvent_t done = nullptr;   // recorded after each step's copy-out; the next step of this stream waits on it
+    std::unique_ptr<CondOverride> cond[2];   // the state's own prompt / time block; none: the stepping engine's global values
 };
 
 struct b2sd_engine {
@@ -337,6 +377,30 @@ struct b2sd_engine {
     float* gn_ws = nullptr;    // GroupNorm chunk partials (shared: launches are stream-ordered)
     int* tile_counters = nullptr;
     float coef_host[4][64]{};
+
+    __half* ctx_global = nullptr;   // the global prompt embeddings and timesteps: ctx / tsteps again after a state's refresh
+    float* tsteps_global = nullptr;
+
+    // The conditioning the frame program reads, as two contiguous blocks: [COND_PROMPT] every cross-attention K / V^T cache
+    // (UNet and ControlNet), [COND_TIME] every resnet's per-slot time bias.  A step first makes each block hold what its state
+    // is stepped with (the state's override, else this lane's global values), with one copy when it holds something else.
+    struct CondBlock {
+        char* p = nullptr;        // read by the frame program
+        char* global = nullptr;   // this lane's copy of its global values (b2sd_prepare, b2sd_set_prompt_embeds / _timesteps)
+        size_t cap = 0, used = 0;
+        uint64_t held = 0;        // what p holds: COND_GLOBAL, the id of an override, or COND_UNKNOWN
+        void* take(size_t bytes) {
+            bytes = (bytes + 1023) & ~size_t(1023);
+            if (used + bytes > cap) {
+                b2_set_error("conditioning block of %zu bytes exhausted", cap);
+                return nullptr;
+            }
+            void* r = p + used;
+            used += bytes;
+            return r;
+        }
+    } cond[2];
+    int64_t cond_binds = 0;   // copies into a block by a step (b2sd_conditioning_binds)
 
     unsigned long long* ln_stats = nullptr;   // slab of per-row LayerNorm statistics [rows][2] (see IgEpilogue::rowstat_out)
     size_t ln_stats_cap = 0, ln_stats_used = 0;   // in 64-bit words
@@ -752,7 +816,7 @@ int b2sd_engine::build_resnet(const std::string& p, const Act& xa, const Act* xb
         if (!wp) return -1;
         const float* colbias = nullptr;
         if (emb) {
-            float* cb = static_cast<float*>(prog.alloc((size_t)B * cout * sizeof(float)));
+            float* cb = static_cast<float*>(cond[COND_TIME].take((size_t)B * cout * sizeof(float)));
             const float* bsum = vec({p + "conv1.bias", p + "time_emb_proj.bias"});
             const Raw* wt = get(p + "time_emb_proj.weight");
             if (!cb || !bsum || !wt) return -1;
@@ -925,9 +989,10 @@ int b2sd_engine::build_transformer(const std::string& p, const Act& x, int heads
     __half* wk2 = pack_rows(t + "attn2.k", {{t + "attn2.to_k.weight", head_perm(0)}}, D, s);
     __half* wv2 = pack_rows(t + "attn2.v", {{t + "attn2.to_v.weight", head_perm(0)}}, D, s);
     if (!wk2 || !wv2) return -1;
-    __half* kc = static_cast<__half*>(prog.alloc((size_t)L * Cp * 2));
+    __half* kc = static_cast<__half*>(cond[COND_PROMPT].take((size_t)L * Cp * 2));
     const int Lpad = 128 * ((L + 127) / 128);
-    __half* vct = static_cast<__half*>(prog.alloc((size_t)Cp * Lpad * 2));
+    __half* vct = static_cast<__half*>(cond[COND_PROMPT].take((size_t)Cp * Lpad * 2));
+    if (!kc || !vct) return -1;
     {
         allow_swap = false;
         ActView ctxv{ctx, 1, 1, L, D, D};
@@ -1522,6 +1587,37 @@ int b2sd_engine::build_program(cudaStream_t s) {
         ln_stats = static_cast<unsigned long long*>(prog.alloc(ln_stats_cap * sizeof(unsigned long long)));
         if (!ln_stats) return -1;
     }
+    {
+        // the conditioning blocks, sized from the shapes build_transformer (K [L][Cp], V^T [Cp][Lpad] per block) and build_resnet
+        // (time bias [B][cout] per resnet) take from them, and zeroed once (V^T's pad columns are never written)
+        const int L = cfg.ctx_tokens, Lpad = 128 * ((L + 127) / 128), lpb = cfg.layers_per_block, cn = cfg.controlnet ? 1 : 0;
+        auto r = [](size_t b) { return (b + 1023) & ~size_t(1023); };
+        size_t bytes[2] = {0, 0};
+        for (int i = 0; i < nlev; ++i) {
+            const int d_real = ch[i] / cfg.heads[i], dp = d_real <= 64 ? 64 : (d_real <= 128 ? 128 : 192);
+            const size_t Cp = (size_t)cfg.heads[i] * dp;
+            // UNet down + up blocks (and the ControlNet's down blocks) of this level, the mid blocks at the last one
+            int transformers = cfg.down_attn[i] ? lpb + (lpb + 1) + cn * lpb : 0;
+            int resnets = lpb + (lpb + 1) + cn * lpb;
+            if (i == nlev - 1) {
+                transformers += 1 + cn;
+                resnets += 2 * (1 + cn);
+            }
+            bytes[COND_PROMPT] += transformers * (r(L * Cp * 2) + r(Cp * Lpad * 2));
+            bytes[COND_TIME] += resnets * r((size_t)B * ch[i] * sizeof(float));
+        }
+        for (int k = 0; k < 2; ++k) {
+            CondBlock& b = cond[k];
+            b.cap = bytes[k];
+            b.used = 0;
+            b.held = COND_UNKNOWN;
+            b.p = static_cast<char*>(prog.alloc(b.cap));
+            b.global = static_cast<char*>(prog.alloc(b.cap));
+            if (!b.p || !b.global) return -1;
+            CUDA_OK(cudaMemsetAsync(b.p, 0, b.cap, s));
+            CUDA_OK(cudaMemsetAsync(b.global, 0, b.cap, s));
+        }
+    }
 
     allow_swap = false;
     const bool kl = cfg.vae == B2SD_VAE_KL;
@@ -1775,6 +1871,97 @@ static int state_reset(b2sd_state* st, cudaStream_t s) {
     return 0;
 }
 
+// ---- conditioning blocks ----------------------------------------------------------------------------
+// Block k now holds the lane's global values (after b2sd_prepare / b2sd_set_*, which computed them into it): keep a copy to rebind.
+static int keep_global(b2sd_engine* h, int k, cudaStream_t s) {
+    auto& b = h->cond[k];
+    CUDA_OK(cudaMemcpyAsync(b.global, b.p, b.used, cudaMemcpyDeviceToDevice, s));
+    b.held = COND_GLOBAL;
+    return 0;
+}
+
+// Make the blocks hold what `st` is stepped with (nullptr: a step without a state), before the frame program reads them
+static int bind_conditioning(b2sd_engine* h, const b2sd_state* st, cudaStream_t s) {
+    for (int k = 0; k < 2; ++k) {
+        auto& b = h->cond[k];
+        CondOverride* ov = st ? st->cond[k].get() : nullptr;
+        const uint64_t want = ov ? ov->id : COND_GLOBAL;
+        if (b.held == want) continue;
+        b.held = COND_UNKNOWN;
+        if (ov) {
+            CUDA_OK(cudaStreamWaitEvent(s, ov->ready, 0));
+            CUDA_OK(cudaMemcpyAsync(b.p, ov->buf, b.used, cudaMemcpyDeviceToDevice, s));
+            cudaEvent_t* use = nullptr;
+            for (auto& u : ov->uses)
+                if (u.first == s) use = &u.second;
+            if (!use) {
+                ov->uses.emplace_back(s, nullptr);
+                use = &ov->uses.back().second;
+                CUDA_OK(cudaEventCreateWithFlags(use, cudaEventDisableTiming));
+            }
+            CUDA_OK(cudaEventRecord(*use, s));
+        } else {
+            CUDA_OK(cudaMemcpyAsync(b.p, b.global, b.used, cudaMemcpyDeviceToDevice, s));
+        }
+        b.held = want;
+        ++h->cond_binds;
+    }
+    return 0;
+}
+
+static std::shared_ptr<CondPool> cond_pool(b2sd_engine* h) {
+    std::shared_ptr<CondPool>& cp = h->ws->cond_pool;
+    if (cp) return cp;
+    auto p = std::make_shared<CondPool>();
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    cudaMemPoolProps props{};
+    props.allocType = cudaMemAllocationTypePinned;
+    props.location.type = cudaMemLocationTypeDevice;
+    props.location.id = dev;
+    int no = 0;
+    // Keep the memory of a few overrides across synchronisations (the default threshold, 0, hands freed memory back to the
+    // driver at every one, and the next override maps it again inside cudaMallocFromPoolAsync); it is released with the pool.
+    uint64_t keep = 4 * (uint64_t)(h->cond[COND_PROMPT].cap + h->cond[COND_TIME].cap);
+    if (keep < (64ull << 20)) keep = 64ull << 20;   // the pool maps memory in chunks of tens of MiB
+    if (e == cudaSuccess) e = cudaMemPoolCreate(&p->pool, &props);
+    if (e == cudaSuccess) e = cudaMemPoolSetAttribute(p->pool, cudaMemPoolReuseAllowInternalDependencies, &no);
+    if (e == cudaSuccess) e = cudaMemPoolSetAttribute(p->pool, cudaMemPoolAttrReleaseThreshold, &keep);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&p->reaper, cudaStreamNonBlocking);
+    if (e != cudaSuccess) {
+        b2_set_error("conditioning override pool: %s", cudaGetErrorString(e));
+        return nullptr;
+    }
+    cp = p;
+    return cp;
+}
+
+// The prompt / time program has just computed `st`'s values into h's block k on s: copy them into a new override of the state
+// (h's block holds it).  The override it replaces is freed after every copy out of it.
+static int publish_override(b2sd_engine* h, b2sd_state* st, int k, cudaStream_t s) {
+    static std::atomic<uint64_t> next_id{1};
+    auto& b = h->cond[k];
+    std::unique_ptr<CondOverride> ov(new CondOverride);
+    ov->pool = cond_pool(h);
+    if (!ov->pool) return -1;
+    ov->id = next_id++;
+    ov->bytes = b.used;
+    cudaError_t e = cudaEventCreateWithFlags(&ov->ready, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaMallocFromPoolAsync(&ov->buf, ov->bytes, ov->pool->pool, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ov->buf, b.p, b.used, cudaMemcpyDeviceToDevice, s);
+    if (ov->ready) {
+        const cudaError_t er = cudaEventRecord(ov->ready, s);
+        if (e == cudaSuccess) e = er;
+    }
+    if (e != cudaSuccess) {
+        b2_set_error("conditioning override of %zu bytes: %s", ov->bytes, cudaGetErrorString(e));
+        return -1;
+    }
+    b.held = ov->id;
+    st->cond[k] = std::move(ov);
+    return 0;
+}
+
 // ================================================================================================
 extern "C" {
 
@@ -1873,7 +2060,9 @@ static int create_engine(const b2sd_config* cfg, std::shared_ptr<WeightStore> st
     e->gn_ws = static_cast<float*>(e->state.alloc(groupnorm_partial_floats(B, cfg->norm_groups) * sizeof(float)));
     e->tile_counters = static_cast<int*>(e->state.alloc(65536 * sizeof(int)));
     if (e->tile_counters) cudaMemset(e->tile_counters, 0, 65536 * sizeof(int));
-    if (!e->x_in.p || !e->noise || !e->coef || !e->tsteps || !e->ctx || !e->temb || !e->gn_ws ||
+    e->ctx_global = static_cast<__half*>(e->state.alloc((size_t)cfg->ctx_tokens * cfg->cross_attention_dim * 2));
+    e->tsteps_global = static_cast<float*>(e->state.alloc(B * sizeof(float)));
+    if (!e->x_in.p || !e->noise || !e->coef || !e->tsteps || !e->ctx || !e->temb || !e->gn_ws || !e->ctx_global || !e->tsteps_global ||
         (cfg->controlnet && (!e->cn_temb_h || !e->cn_temb))) {
         b2_set_error("b2sd_create: cudaMalloc failed");
         delete e;
@@ -2030,6 +2219,11 @@ int b2sd_prepare(b2sd_handle h, const void* prompt_embeds, const float* timestep
     TRY(h->build_program(s));
     TRY(h->run(h->prog_prompt, s));
     TRY(refresh_time(h, s));
+    CUDA_OK(cudaMemcpyAsync(h->ctx_global, h->ctx, (size_t)h->cfg.ctx_tokens * h->cfg.cross_attention_dim * 2,
+                            cudaMemcpyDeviceToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(h->tsteps_global, h->tsteps, B * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    TRY(keep_global(h, COND_PROMPT, s));
+    TRY(keep_global(h, COND_TIME, s));
     CUDA_OK(cudaStreamSynchronize(s));
     // Every pack-only parameter now exists in its kernel-native layout: drop the raw copies (about half of the UNet's
     // 1.73 GB).  Later prepares hit the packed caches and never touch them.
@@ -2205,10 +2399,13 @@ int b2sd_set_prompt_embeds(b2sd_handle h, const void* prompt_embeds, void* strea
         return -1;
     }
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    CUDA_OK(cudaMemcpyAsync(h->ctx, prompt_embeds, (size_t)h->cfg.ctx_tokens * h->cfg.cross_attention_dim * 2,
-                            cudaMemcpyHostToDevice, s));
+    const size_t bytes = (size_t)h->cfg.ctx_tokens * h->cfg.cross_attention_dim * 2;
+    CUDA_OK(cudaMemcpyAsync(h->ctx, prompt_embeds, bytes, cudaMemcpyHostToDevice, s));
     CUDA_OK(cudaStreamSynchronize(s));
-    return h->run(h->prog_prompt, s);
+    CUDA_OK(cudaMemcpyAsync(h->ctx_global, h->ctx, bytes, cudaMemcpyDeviceToDevice, s));
+    h->cond[COND_PROMPT].held = COND_UNKNOWN;
+    TRY(h->run(h->prog_prompt, s));
+    return keep_global(h, COND_PROMPT, s);
 }
 
 int b2sd_set_timesteps(b2sd_handle h, const float* timesteps, void* stream) {
@@ -2219,8 +2416,73 @@ int b2sd_set_timesteps(b2sd_handle h, const float* timesteps, void* stream) {
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     CUDA_OK(cudaMemcpyAsync(h->tsteps, timesteps, h->cfg.batch * sizeof(float), cudaMemcpyHostToDevice, s));
     CUDA_OK(cudaStreamSynchronize(s));
-    return refresh_time(h, s);
+    CUDA_OK(cudaMemcpyAsync(h->tsteps_global, h->tsteps, h->cfg.batch * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    h->cond[COND_TIME].held = COND_UNKNOWN;
+    TRY(refresh_time(h, s));
+    return keep_global(h, COND_TIME, s);
 }
+
+// ---- per-state conditioning --------------------------------------------------------------------------
+// What every call that runs a state on an engine refuses
+static int check_state(const char* fn, b2sd_handle h, const b2sd_state* state) {
+    if (!h || !h->built || !state) {
+        b2_set_error("%s: null argument, or b2sd_prepare not called", fn);
+        return -1;
+    }
+    if (h->pair_state) {
+        b2_set_error("%s: the engine is part of a b2sd_share_stream_state pair, which steps its own state", fn);
+        return -1;
+    }
+    if (state->ws.lock() != h->ws || state->batch != h->cfg.batch || state->height != h->cfg.height ||
+        state->width != h->cfg.width) {
+        b2_set_error("%s: the state was made for another weight store, batch or size (state: batch %d, %dx%d; "
+                     "engine: batch %d, %dx%d)", fn, state->batch, state->height, state->width, h->cfg.batch, h->cfg.height,
+                     h->cfg.width);
+        return -1;
+    }
+    return 0;
+}
+
+// Run h's prompt (k = COND_PROMPT) or time refresh on s with `input` (device) in place of the global embeddings / timesteps,
+// put the global ones back, and publish the block as the state's override.  Stream-ordered after the frames queued on s, and
+// no host synchronisation: the refresh writes only h's block, which no other stream reads.
+static int state_refresh(const char* fn, b2sd_handle h, b2sd_state* state, int k, const void* input, cudaStream_t s) {
+    TRY(check_state(fn, h, state));
+    if (!input) {
+        b2_set_error("%s: null argument", fn);
+        return -1;
+    }
+    void* dst = k == COND_PROMPT ? (void*)h->ctx : (void*)h->tsteps;
+    const void* global = k == COND_PROMPT ? (const void*)h->ctx_global : (const void*)h->tsteps_global;
+    const size_t bytes = k == COND_PROMPT ? (size_t)h->cfg.ctx_tokens * h->cfg.cross_attention_dim * 2
+                                          : (size_t)h->cfg.batch * sizeof(float);
+    h->cond[k].held = COND_UNKNOWN;
+    CUDA_OK(cudaMemcpyAsync(dst, input, bytes, cudaMemcpyDeviceToDevice, s));
+    const int rc = k == COND_PROMPT ? h->run(h->prog_prompt, s) : refresh_time(h, s);
+    CUDA_OK(cudaMemcpyAsync(dst, global, bytes, cudaMemcpyDeviceToDevice, s));
+    TRY(rc);
+    return publish_override(h, state, k, s);
+}
+
+int b2sd_state_set_prompt_embeds(b2sd_handle h, b2sd_state_handle state, const void* prompt_embeds, void* stream) {
+    return state_refresh("b2sd_state_set_prompt_embeds", h, state, COND_PROMPT, prompt_embeds,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2sd_state_set_timesteps(b2sd_handle h, b2sd_state_handle state, const float* timesteps, void* stream) {
+    return state_refresh("b2sd_state_set_timesteps", h, state, COND_TIME, timesteps, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2sd_state_clear_conditioning(b2sd_state_handle state, int which) {
+    if (!state || (which != COND_PROMPT && which != COND_TIME)) {
+        b2_set_error("b2sd_state_clear_conditioning: null state, or which is not 0 (prompt) or 1 (time)");
+        return -1;
+    }
+    state->cond[which].reset();
+    return 0;
+}
+
+int64_t b2sd_conditioning_binds(b2sd_handle h) { return h ? h->cond_binds : -1; }
 
 int b2sd_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* frame_out, void* stream) {
     return b2sd_step_ex(h, frame_in, B2SD_IN_U8_NHWC, in_h, in_w, frame_out, B2SD_OUT_U8_NCHW, stream);
@@ -2255,6 +2517,7 @@ static int step_stages(b2sd_handle h, b2sd_state* state, cudaStream_t s) {
         if (st == 1) {
             CUDA_OK(cudaStreamWaitEvent(s, state->done, 0));
             if (state->bytes) CUDA_OK(cudaMemcpyAsync(slots, state->buf, state->bytes, cudaMemcpyDeviceToDevice, s));
+            TRY(bind_conditioning(h, state, s));
         }
         if (h->cfg.use_cuda_graph) {
             if (!h->stage_exec[st]) {
@@ -2288,8 +2551,9 @@ static int step_tail(b2sd_handle h, void* frame_out, int out_kind, cudaStream_t 
     return post_u8_launch(h->image.p, h->image.ld, static_cast<uint8_t*>(frame_out), 1, h->cfg.height, h->cfg.width, s);
 }
 
-int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int in_w, void* frame_out, int out_kind,
-                 void* stream) {
+// b2sd_step_ex with the conditioning of `cond` (nullptr: the engine's global values) bound before the whole-frame program
+static int step_whole(b2sd_handle h, const b2sd_state* cond, const void* frame_in, int in_kind, int in_h, int in_w,
+                      void* frame_out, int out_kind, void* stream) {
     if (!h || !h->built) {
         b2_set_error("b2sd_step: call b2sd_prepare first");
         return -1;
@@ -2302,7 +2566,10 @@ int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int
     TRY(step_heads(h, frame_in, in_kind, in_h, in_w, s));
     if (h->pair_state) {
         TRY(step_stages(h, h->pair_state.get(), s));
-    } else if (h->cfg.use_cuda_graph) {
+        return step_tail(h, frame_out, out_kind, s);
+    }
+    TRY(bind_conditioning(h, cond, s));
+    if (h->cfg.use_cuda_graph) {
         if (!h->graph_exec) {
             cudaStream_t cs;
             CUDA_OK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
@@ -2323,6 +2590,11 @@ int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int
         TRY(h->run(h->prog_frame, s));
     }
     return step_tail(h, frame_out, out_kind, s);
+}
+
+int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int in_w, void* frame_out, int out_kind,
+                 void* stream) {
+    return step_whole(h, nullptr, frame_in, in_kind, in_h, in_w, frame_out, out_kind, stream);
 }
 
 int b2sd_state_create(b2sd_handle h, b2sd_state_handle* out, void* stream) {
@@ -2351,22 +2623,8 @@ int b2sd_state_destroy(b2sd_state_handle state, void* stream) {
 
 int b2sd_step_state(b2sd_handle h, b2sd_state_handle state, const void* frame_in, int in_kind, int in_h, int in_w,
                     void* frame_out, int out_kind, void* stream) {
-    if (!h || !h->built || !state) {
-        b2_set_error("b2sd_step_state: null argument, or b2sd_prepare not called");
-        return -1;
-    }
-    if (h->pair_state) {
-        b2_set_error("b2sd_step_state: the engine is part of a b2sd_share_stream_state pair, which steps its own state");
-        return -1;
-    }
-    if (state->ws.lock() != h->ws || state->batch != h->cfg.batch || state->height != h->cfg.height ||
-        state->width != h->cfg.width) {
-        b2_set_error("b2sd_step_state: the state was made for another weight store, batch or size (state: batch %d, %dx%d; "
-                     "engine: batch %d, %dx%d)", state->batch, state->height, state->width, h->cfg.batch, h->cfg.height,
-                     h->cfg.width);
-        return -1;
-    }
-    if (!state->bytes) return b2sd_step_ex(h, frame_in, in_kind, in_h, in_w, frame_out, out_kind, stream);
+    TRY(check_state("b2sd_step_state", h, state));
+    if (!state->bytes) return step_whole(h, state, frame_in, in_kind, in_h, in_w, frame_out, out_kind, stream);
     if (!frame_in || !frame_out || in_h < 1 || in_w < 1) {
         b2_set_error("b2sd_step_state: bad frame arguments");
         return -1;
@@ -2411,6 +2669,7 @@ int b2sd_profile(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* 
         return -1;
     }
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    TRY(bind_conditioning(h, nullptr, s));
     const size_t nops = h->prog_frame.size() + 2;
     std::vector<cudaEvent_t> ev(nops + 1);
     for (auto& e : ev) CUDA_OK(cudaEventCreate(&e));
@@ -2509,6 +2768,7 @@ int b2sd_audit_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, voi
         return -1;
     }
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    TRY(bind_conditioning(h, nullptr, s));   // the engine's own stream: its global conditioning
     Audited au{"b2sd_audit_step", fn, user, s};
     // the input heads and the tail as b2sd_step_ex launches them for a u8 frame, with the caller's frame and size
     SmallConvArgs a = h->head;
@@ -2541,9 +2801,12 @@ int b2sd_audit_refresh(b2sd_handle h, b2sd_audit_fn fn, void* user, void* stream
     Audited au{"b2sd_audit_refresh", fn, user, reinterpret_cast<cudaStream_t>(stream)};
     std::vector<Op> time_ops;
     TRY(time_embedding_ops(h, &time_ops));
+    h->cond[COND_PROMPT].held = h->cond[COND_TIME].held = COND_UNKNOWN;
     TRY(au.program(h->prog_prompt));
     TRY(au.program(time_ops));
-    return au.program(h->prog_time);
+    TRY(au.program(h->prog_time));
+    h->cond[COND_PROMPT].held = h->cond[COND_TIME].held = COND_GLOBAL;   // recomputed from the global embeddings / timesteps
+    return 0;
 }
 
 // Start gate for concurrent b2sd_profile_kind calls (one host thread per lane): every call finishes its capture / instantiation /

@@ -159,6 +159,7 @@ IG_SILU = 8
 IG_PAD0 = 16
 SC_IN_U8, SC_IN_TANH3, SC_OUT_RELU, SC_OUT_SILU, SC_IN_OFFSET = 1, 2, 4, 32, 64
 CONTROL_FRAME, CONTROL_HED = 0, 1
+COND_PROMPT, COND_TIME = 0, 1      # b2sd_state_clear_conditioning
 VAE_TINY, VAE_KL = 0, 1
 IG_TCONV = 64
 IG_PAIR = 128
@@ -222,8 +223,14 @@ def lib() -> C.CDLL:
         _lib.b2sd_state_reset.argtypes = [vp, vp]
         _lib.b2sd_state_destroy.argtypes = [vp, vp]
         _lib.b2sd_step_state.argtypes = [vp, vp, vp, ci, ci, ci, vp, ci, vp]
-        for name in ("state_create", "state_reset", "state_destroy", "step_state"):
+        _lib.b2sd_state_set_prompt_embeds.argtypes = [vp, vp, vp, vp]
+        _lib.b2sd_state_set_timesteps.argtypes = [vp, vp, vp, vp]
+        _lib.b2sd_state_clear_conditioning.argtypes = [vp, ci]
+        for name in ("state_create", "state_reset", "state_destroy", "step_state", "state_set_prompt_embeds", "state_set_timesteps",
+                     "state_clear_conditioning"):
             getattr(_lib, "b2sd_" + name).restype = C.c_int
+        _lib.b2sd_conditioning_binds.argtypes = [vp]
+        _lib.b2sd_conditioning_binds.restype = i64
         _lib.b2sd_profile.argtypes = [vp, vp, ci, ci, vp, ci, C.c_char_p, i64, vp]
         _lib.b2sd_profile.restype = C.c_int
         _lib.b2sd_profile_kind.argtypes = [vp, C.c_char_p, ci, C.POINTER(C.c_double), C.POINTER(ci), C.POINTER(C.c_double), vp]

@@ -159,14 +159,25 @@ class StreamDiffusionPipeline:
                 st.wait_event(done)
 
     def update_prompt(self, prompt: str):
+        """The global prompt: every stream's, including open peer streams with a prompt of their own (PeerStream.update_prompt)."""
         cur = self._quiesce()
         self.model.stream.update_prompt(prompt)
         self._release(cur)
 
     def update_t_index_list(self, t_index_list: List[int]):
+        """The global t_index_list: every stream's, including open peer streams with one of their own."""
         cur = self._quiesce()
         self.model.update_t_index_list(t_index_list)
+        self.model.stream.clear_overrides(prompt=False, t_index_list=True)   # also when the global list was already this one
         self._release(cur)
+
+    def _update_state(self, update) -> None:
+        """update(engine) refreshes one peer's conditioning on the lane that takes the next submission, on that lane's stream:
+        stream-ordered after the frames queued there, with no host wait and no wait on the other lanes."""
+        lane = self._next_lane
+        compute = self._lane_streams[lane] or torch.cuda.current_stream(self.model.stream.device)
+        with torch.cuda.stream(compute):
+            update(self._engines[lane])
 
     # ---- reference-shaped stages ----------------------------------------------------------------------
     def preprocess(self, frame) -> torch.Tensor:
@@ -319,8 +330,9 @@ class FrameTicket:
 
 class PeerStream:
     """One viewer's temporal stream on a per-peer pipeline (StreamDiffusionPipeline.open_stream): enqueue() / __call__ behave
-    as the pipeline's, with this viewer's own stream-batch state.  close() frees the state after its last frame, without a
-    host synchronisation."""
+    as the pipeline's, with this viewer's own stream-batch state, and with this viewer's own prompt / t_index_list once it sets
+    them (update_prompt / update_t_index_list; until then the pipeline's).  close() frees the state after its last frame,
+    without a host synchronisation."""
 
     def __init__(self, pipeline: StreamDiffusionPipeline):
         self._pipeline = pipeline
@@ -337,6 +349,30 @@ class PeerStream:
 
     def enqueue(self, frame) -> FrameTicket:
         return self._pipeline._enqueue(frame, self._live_state())
+
+    @property
+    def prompt(self) -> str:
+        """This viewer's prompt: its own (update_prompt) or the pipeline's global one"""
+        own = self._live_state().own_prompt
+        return own if own is not None else self._pipeline.model.stream.prompt
+
+    @property
+    def t_index_list(self) -> List[int]:
+        own = self._live_state().own_t_index_list
+        return list(own if own is not None else self._pipeline.model.stream.t_list)
+
+    def update_prompt(self, prompt: str) -> None:
+        """This viewer's own prompt: its frames enqueued after the call use it, whichever lane runs them; frames already
+        queued, and every other viewer's frames, are unaffected.  Does not wait for queued frames.  A later global
+        pipeline.update_prompt replaces it."""
+        state = self._live_state()
+        self._pipeline._update_state(lambda engine: state.set_prompt(prompt, engine=engine))
+
+    def update_t_index_list(self, t_index_list: List[int]) -> None:
+        """This viewer's own t_index_list, with the semantics of the global update_t_index_list (only the time embedding's
+        timesteps change) and update_prompt's ordering."""
+        state = self._live_state()
+        self._pipeline._update_state(lambda engine: state.set_t_index_list(t_index_list, engine=engine))
 
     def __call__(self, frame):
         return self._pipeline._call(frame, self._live_state())

@@ -219,6 +219,7 @@ class StreamDiffusion:
                                       "(lib/pipeline.py:14 passes 0.0)")
         self.delta = delta
         T = self.denoising_steps_num
+        self.prompt = prompt
         self.prompt_embeds = self._encode(prompt).repeat(self.batch_size, 1, 1)
         self.timesteps = lcm_timestep_table(num_inference_steps)
         self.sub_timesteps = [self.timesteps[t] for t in self.t_list]
@@ -237,11 +238,12 @@ class StreamDiffusion:
         self._engine_prepare()
         for lane in self.lanes:
             lane._prepare_like(self)
-        for state in list(self._states):   # as prepare zeroes the engines' own latent buffers
+        for state in list(self._states):   # as prepare zeroes the engines' own latent buffers, and follows its conditioning
             if not state.closed:
                 state.reset()
+                state.clear_overrides()
 
-    _SCHEDULE_ATTRS = ("generator", "guidance_scale", "delta", "prompt_embeds", "timesteps", "sub_timesteps", "sub_timesteps_tensor",
+    _SCHEDULE_ATTRS = ("generator", "guidance_scale", "delta", "prompt", "prompt_embeds", "timesteps", "sub_timesteps", "sub_timesteps_tensor",
                        "init_noise", "stock_noise", "c_skip", "c_out", "alpha_prod_t_sqrt", "beta_prod_t_sqrt")
 
     def _engine_prepare(self) -> None:
@@ -284,6 +286,14 @@ class StreamDiffusion:
         self._states.add(state)
         return state
 
+    _enc_stream = None
+
+    def _encoder_stream(self):
+        """the CUDA stream per-state prompts are encoded on (_encode_beside)"""
+        if self._enc_stream is None:
+            self._enc_stream = torch.cuda.Stream(self.device)
+        return self._enc_stream
+
     def _encode(self, prompt: str) -> torch.Tensor:
         e = self.prompt_encoder(prompt)
         if e.dim() == 2:
@@ -294,22 +304,41 @@ class StreamDiffusion:
 
     @torch.no_grad()
     def update_prompt(self, prompt: str) -> None:
+        """The global prompt: this engine's, its lanes' and every live state's (a state's own prompt is dropped)."""
+        self.prompt = prompt
         self.prompt_embeds = self._encode(prompt).repeat(self.batch_size, 1, 1)
         emb = self.prompt_embeds[0].cpu().contiguous()
         for eng in [self] + self.lanes:
-            eng.prompt_embeds = self.prompt_embeds
+            eng.prompt, eng.prompt_embeds = prompt, self.prompt_embeds
             capi.check(self._lib.b2sd_set_prompt_embeds(eng._handle, emb.data_ptr(), self._stream()), "b2sd_set_prompt_embeds")
+        self.clear_overrides(prompt=True, t_index_list=False)
 
-    def sync_timesteps(self) -> None:
-        """Push self.sub_timesteps to the engine (called after lib/wrapper.py:389-407 style updates).  As in the
-        reference only the timestep embedding changes; alpha/beta/c_skip/c_out keep their prepare() values."""
-        t = torch.tensor([float(v) for v in self.sub_timesteps], dtype=torch.float32)
+    def _timestep_tensor(self, sub_timesteps: List[int]) -> torch.Tensor:
+        t = torch.tensor([float(v) for v in sub_timesteps], dtype=torch.float32)
         if t.numel() != self.batch_size:
             raise ValueError(f"t_index_list length {t.numel()} != stream batch {self.batch_size} (static batch, as the "
                              "reference's TensorRT engines)")
+        return t
+
+    def sync_timesteps(self) -> None:
+        """Push self.sub_timesteps to the engine (called after lib/wrapper.py:389-407 style updates).  As in the
+        reference only the timestep embedding changes; alpha/beta/c_skip/c_out keep their prepare() values.  Every live
+        state's own t_index_list is dropped."""
+        t = self._timestep_tensor(self.sub_timesteps)
         for eng in [self] + self.lanes:
             eng.t_list, eng.sub_timesteps, eng.sub_timesteps_tensor = self.t_list, self.sub_timesteps, self.sub_timesteps_tensor
             capi.check(self._lib.b2sd_set_timesteps(eng._handle, t.data_ptr(), self._stream()), "b2sd_set_timesteps")
+        self.clear_overrides(prompt=False, t_index_list=True)
+
+    def clear_overrides(self, prompt: bool = True, t_index_list: bool = True) -> None:
+        """Every live state of this engine's weights follows the global prompt and / or t_index_list again."""
+        for state in list(self._states):
+            if not state.closed:
+                state.clear_overrides(prompt=prompt, t_index_list=t_index_list)
+
+    def conditioning_binds(self) -> int:
+        """How many conditioning block copies this engine's steps have issued (b2sd_conditioning_binds).  Test aid."""
+        return self._lib.b2sd_conditioning_binds(self._handle)
 
     # ---- per frame ---------------------------------------------------------------------------------
     def _check(self):
@@ -480,16 +509,76 @@ class StreamDiffusion:
         return self._lib.b2sd_launches_per_step(self._handle)
 
 
+def _on_device(t: torch.Tensor, device: torch.device) -> torch.Tensor:
+    """t on `device`, copied on the current stream without a host wait (a host tensor goes through pinned memory)"""
+    if t.is_cuda:
+        return t.to(device).contiguous()
+    return t.contiguous().pin_memory().to(device, non_blocking=True)
+
+
+def _encode_beside(eng: StreamDiffusion, prompt: str) -> torch.Tensor:
+    """eng's embedding of `prompt`, [ctx_tokens][D] on the device, ready for the current stream's later work.  The encoder runs
+    on a stream of its own: the current stream may have frames queued (a lane's), and an encoder that synchronises its stream
+    (CLIP's blocking upload of the token ids) or launches kernels then waits only for earlier encodes, never for those frames."""
+    cur = torch.cuda.current_stream(eng.device)
+    side = eng._encoder_stream()
+    with torch.cuda.stream(side):
+        emb = _on_device(eng._encode(prompt)[0], eng.device)
+        ready = torch.cuda.Event()
+        ready.record(side)
+    cur.wait_event(ready)
+    emb.record_stream(cur)
+    return emb
+
+
 class StreamState:
     """One temporal stream's stream-batch state (x_t_latent_buffer), apart from the engines that step it (b2sd_state_*): any
     lane of the creating engine's weights steps it, so several video streams share a pool of lanes without mixing their
-    frames.  (T-1)*(h/8)*(w/8)*4 fp16 values on the device; nothing at T = 1.  Made by StreamDiffusion.new_state()."""
+    frames.  (T-1)*(h/8)*(w/8)*4 fp16 values on the device; nothing at T = 1.  Made by StreamDiffusion.new_state().
+
+    A state may also have its own prompt and its own t_index_list (set_prompt / set_t_index_list): a device copy of the
+    conditioning blocks the engines compute from them (cross-attention K / V^T, resnet time biases), which a lane copies in
+    before it steps the state.  Without them the state follows the engines' global prompt and t_index_list."""
+
+    own_prompt: Optional[str] = None               # None: the global prompt
+    own_t_index_list: Optional[List[int]] = None   # None: the global t_index_list
 
     def __init__(self, engine: StreamDiffusion):
         self._engine = engine          # keeps the engine (and its stream / library) alive while the state exists
         self._lib = engine._lib
         self._handle = C.c_void_p()
         capi.check(self._lib.b2sd_state_create(engine._handle, C.byref(self._handle), engine._stream()), "b2sd_state_create")
+
+    @torch.no_grad()
+    def set_prompt(self, prompt: str, engine: Optional[StreamDiffusion] = None) -> None:
+        """This stream's own prompt, for the steps submitted after the call.  Computed on `engine` (any lane of the creating
+        engine's weights; default the creating engine) on the current CUDA stream, after the frames queued there, with no host
+        synchronisation besides the prompt encoder's own, which runs on a stream of its own (_encode_beside) and so never waits
+        for queued frames."""
+        eng = engine or self._engine
+        emb = _encode_beside(eng, prompt)
+        capi.check(self._lib.b2sd_state_set_prompt_embeds(eng._handle, self.handle, emb.data_ptr(), eng._stream()),
+                   "b2sd_state_set_prompt_embeds")
+        self.own_prompt = prompt
+
+    @torch.no_grad()
+    def set_t_index_list(self, t_index_list: List[int], engine: Optional[StreamDiffusion] = None) -> None:
+        """This stream's own t_index_list, as StreamDiffusion.sync_timesteps applies one: only the timesteps of the time
+        embedding change (alpha / beta / c_skip / c_out keep their prepare() values).  Same stream and synchronisation rules as
+        set_prompt."""
+        eng = engine or self._engine
+        t_index_list = list(t_index_list)
+        t = _on_device(eng._timestep_tensor([eng.timesteps[i] for i in t_index_list]), eng.device)
+        capi.check(self._lib.b2sd_state_set_timesteps(eng._handle, self.handle, t.data_ptr(), eng._stream()),
+                   "b2sd_state_set_timesteps")
+        self.own_t_index_list = t_index_list
+
+    def clear_overrides(self, prompt: bool = True, t_index_list: bool = True) -> None:
+        """Follow the global prompt and / or t_index_list again from the next step on (no device work)."""
+        for on, which, attr in ((prompt, capi.COND_PROMPT, "own_prompt"), (t_index_list, capi.COND_TIME, "own_t_index_list")):
+            if on:
+                capi.check(self._lib.b2sd_state_clear_conditioning(self.handle, which), "b2sd_state_clear_conditioning")
+                setattr(self, attr, None)
 
     @property
     def handle(self) -> C.c_void_p:

@@ -45,6 +45,7 @@ class VideoStreamTrack(_Base):
         # a pipeline with per-peer streams gives this track its own temporal stream, opened at the first frame
         self._per_peer = bool(getattr(pipeline, "per_peer_streams", False))
         self._peer = None
+        self._stopped = False
 
     def _target(self):
         if not self._per_peer:
@@ -61,7 +62,19 @@ class VideoStreamTrack(_Base):
 
     def stop(self):
         super().stop()
+        self._stopped = True
         self._close_stream()
+
+    def update_prompt(self, prompt: str) -> None:
+        """A config message's prompt: this track's viewer only with per-peer streams (the stream is opened if no frame has
+        arrived yet), else the pipeline's global prompt.  A no-op once the track is stopped."""
+        if not self._stopped:
+            self._target().update_prompt(prompt)
+
+    def update_t_index_list(self, t_index_list) -> None:
+        """As update_prompt, for the t_index_list"""
+        if not self._stopped:
+            self._target().update_t_index_list(t_index_list)
 
     async def _recv_source(self):
         try:

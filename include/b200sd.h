@@ -245,10 +245,11 @@ int b2sd_import_packed(b2sd_handle h, const char* path);
  * Synchronises `stream`. */
 int b2sd_prepare(b2sd_handle h, const void* prompt_embeds, const float* timesteps, const float* coef,
                  const void* init_noise, void* stream);
-/* StreamDiffusion.update_prompt (lib/pipeline.py:44-45): refresh the per-layer cross-attention K/V cache */
+/* StreamDiffusion.update_prompt (lib/pipeline.py:44-45): refresh the per-layer cross-attention K/V cache (the engine's global
+ * prompt block, see b2sd_state_set_prompt_embeds) */
 int b2sd_set_prompt_embeds(b2sd_handle h, const void* prompt_embeds, void* stream);
 /* lib/wrapper.py:389-407 update_t_index_list: only sub_timesteps change (alpha/beta/c_skip/c_out keep the
- * values given to b2sd_prepare -- reference behaviour) */
+ * values given to b2sd_prepare -- reference behaviour); refreshes the engine's global time block */
 int b2sd_set_timesteps(b2sd_handle h, const float* timesteps, void* stream);
 
 /* One StreamDiffusionPipeline.__call__ (lib/pipeline.py:76-96, NVENC branch): frame_in = device u8 NHWC
@@ -403,13 +404,40 @@ typedef struct b2sd_state* b2sd_state_handle;
 int b2sd_state_create(b2sd_handle h, b2sd_state_handle* out, void* stream);
 /* zero the state (what b2sd_prepare does to an engine's own latent buffer), after its last step, on `stream` */
 int b2sd_state_reset(b2sd_state_handle state, void* stream);
-/* free the state on `stream` after its last step, without a host synchronisation; NULL is a no-op */
+/* free the state (and its conditioning overrides) on `stream` after its last step, without a host synchronisation; NULL is a
+ * no-op */
 int b2sd_state_destroy(b2sd_state_handle state, void* stream);
 /* b2sd_step_ex on `state`: input heads, encoder body | wait for the state's previous step, copy the state into slots 1 .. T-1,
  * latent conv + UNet (+ ControlNet) + scheduler step, copy slots 1 .. T-1 back, record the state's event | decoder, tail.
  * At T = 1 the state is empty and this is b2sd_step_ex. */
 int b2sd_step_state(b2sd_handle h, b2sd_state_handle state, const void* frame_in, int in_kind, int in_h, int in_w,
                     void* frame_out, int out_kind, void* stream);
+
+/* Per-state conditioning: a state may carry its own prompt and its own timesteps, so each viewer of a lane pool sees its own
+ * prompt and t_index_list.  An engine keeps what its frame program reads of the conditioning in two contiguous blocks: the
+ * prompt block (every cross-attention K / V^T cache, UNet and ControlNet) and the time block (every resnet's per-slot time
+ * bias).  A state's override of a block is a device copy of it computed for that state.  Before the UNet stage of a step, each
+ * block is made to hold what the state is stepped with -- its override, or the engine's global values (b2sd_prepare /
+ * b2sd_set_prompt_embeds / b2sd_set_timesteps) -- with one device-to-device copy when it holds something else; so lanes whose
+ * states never override copy nothing.  b2sd_step_ex and the other calls without a state use the global values.
+ * An override is immutable: an update makes a new one, and the one it replaces is freed after the last step that copies it.
+ * The calls refuse what b2sd_step_state refuses (null handles, a state of another store / batch / size, an engine of a
+ * b2sd_share_stream_state pair, an unprepared engine).  A state's bookkeeping is host state without a lock: calls that take
+ * one state (b2sd_step_state and the three below) must not run concurrently, from whichever engine or thread; calls on
+ * different states may.  The overrides of a weight store's states share a memory pool that keeps a few blocks' worth of
+ * memory across synchronisations; it is released when the last engine of the store and the last override are gone. */
+/* Compute `state`'s prompt block from embeddings in DEVICE memory, fp16 [ctx_tokens][cross_attention_dim], on engine h (any
+ * engine that may step the state), stream-ordered on `stream` after the frames queued there, without a host synchronisation.
+ * Steps of the state submitted after this call use it, on any engine. */
+int b2sd_state_set_prompt_embeds(b2sd_handle h, b2sd_state_handle state, const void* prompt_embeds, void* stream);
+/* The same for the time block from the state's per-slot timesteps in DEVICE memory, fp32 [batch]; as b2sd_set_timesteps, only
+ * the time embedding changes (alpha / beta / c_skip / c_out keep their b2sd_prepare values). */
+int b2sd_state_set_timesteps(b2sd_handle h, b2sd_state_handle state, const float* timesteps, void* stream);
+/* Drop the state's override of the prompt (which = 0) or time (which = 1) block: later steps use the engines' global values.
+ * No device work; the override is freed after the steps already submitted with it. */
+int b2sd_state_clear_conditioning(b2sd_state_handle state, int which);
+/* Test aid: how many block copies the steps of engine h have issued to bind a state's (or the global) conditioning */
+int64_t b2sd_conditioning_binds(b2sd_handle h);
 /* How many frames will be in flight on this GPU (lanes / independent streams).  1 (default): launch policy tuned for the
  * latency of a single frame; > 1: policy tuned for throughput (smaller operand rings so CTAs of different frames share an
  * SM; from 4 frames in flight on, contractions are launched as CTA pairs -- tcgen05.mma.cta_group::2 -- without split-K: least

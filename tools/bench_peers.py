@@ -14,7 +14,14 @@ hbm_per_peer_kb: device memory the peers' streams take (cudaMemGetInfo around op
 payload, (T-1) * 64 * 64 * 4 fp16 values.  The shared mode with one peer and the per-peer mode with one peer are measured
 alternately, `repeats` times each, so that their spread is measured in the same run.  `lanes` (T > 1 only) lists the lane
 counts of the per-peer pool to measure; the default lane count for T = 1 is the shared mode's.  The card's name and power
-limit are read in the same run."""
+limit are read in the same run.
+
+With --conditioning same,distinct,changing only the per-peer pool with the default lane count (or the first of --lanes) is
+measured, at every peer count of --peers from 2 on, the modes alternately, `repeats` times each:
+  * same: every viewer has the pipeline's prompt and t_index_list (no conditioning copies);
+  * distinct: every viewer has its own prompt (PeerStream.update_prompt) and, at T > 1, its own t_index_list;
+  * changing: as distinct, and viewer 0 changes its prompt every 10 of its frames; update_ms: host time of those calls
+    (synthetic prompt encoder)."""
 from __future__ import annotations
 
 import argparse
@@ -56,12 +63,19 @@ def build(model: str, tl, per_peer: bool, lanes, hw: int = 512):
     return pipe, (free0 - torch.cuda.mem_get_info()[0]) / 2 ** 20
 
 
-def measure(pipe, peers: int, frames, n: int, warmup: int) -> dict:
-    """peers = 0: the pipeline's own stream (pipeline.enqueue); else that many PeerStreams, round-robin"""
+def measure(pipe, peers: int, frames, n: int, warmup: int, conditioning: str = "same") -> dict:
+    """peers = 0: the pipeline's own stream (pipeline.enqueue); else that many PeerStreams, round-robin, with the
+    conditioning mode of the module docstring"""
     import torch
     torch.cuda.synchronize()
     free0 = torch.cuda.mem_get_info()[0]
     targets = [pipe.open_stream() for _ in range(peers)] if peers else [pipe]
+    if conditioning != "same":
+        for k, t in enumerate(targets):
+            t.update_prompt(f"viewer {k}")
+            if len(pipe.t_index_list) > 1:
+                t.update_t_index_list([v - 1 - k % 8 for v in pipe.t_index_list])
+    update_ms = []
     torch.cuda.synchronize()
     hbm = (free0 - torch.cuda.mem_get_info()[0]) / max(1, peers) / 1024
     pending_max = pipe.lanes
@@ -77,6 +91,11 @@ def measure(pipe, peers: int, frames, n: int, warmup: int) -> dict:
                 lat[p].append((time.perf_counter() - t0) * 1e3)
         for i in range(count):
             p = i % len(targets)
+            if conditioning == "changing" and p == 0 and i % (10 * len(targets)) == 0:
+                t1 = time.perf_counter()
+                targets[0].update_prompt(f"viewer 0, frame {i}")
+                if record:
+                    update_ms.append((time.perf_counter() - t1) * 1e3)
             pend.append((p, time.perf_counter(), targets[p].enqueue(frames[i % len(frames)])))
             while len(pend) >= pending_max:
                 retire()
@@ -90,8 +109,11 @@ def measure(pipe, peers: int, frames, n: int, warmup: int) -> dict:
     if peers:
         for t in targets:
             t.close()
-    return {"fps": round(n / wall, 2), "p50_ms": round(max(statistics.median(v) for v in lat.values()), 3),
-            "p99_ms": round(max(_pct(v, 0.99) for v in lat.values()), 3), "hbm_per_peer_kb": round(hbm, 1) if peers else None}
+    out = {"fps": round(n / wall, 2), "p50_ms": round(max(statistics.median(v) for v in lat.values()), 3),
+           "p99_ms": round(max(_pct(v, 0.99) for v in lat.values()), 3), "hbm_per_peer_kb": round(hbm, 1) if peers else None}
+    if update_ms:
+        out.update(update_ms_p50=round(statistics.median(update_ms), 3), update_ms_max=round(max(update_ms), 3))
+    return out
 
 
 def run_model(model: str, tl, args, info) -> dict:
@@ -109,6 +131,27 @@ def run_model(model: str, tl, args, info) -> dict:
         print(json.dumps(row), flush=True)
 
     lane_counts = args.lanes if T > 1 else [None]
+    if args.conditioning:
+        from ai_rtc_agent_b200.host.pipeline import DEFAULT_LANES_PER_PEER
+        pool, pool_mb = build(model, tl, True, (DEFAULT_LANES_PER_PEER if DEFAULT_LANES_PER_PEER in lane_counts else lane_counts[0])
+                              if T > 1 else None)
+        for p in (p for p in args.peers if p >= 2):
+            for r in range(args.repeats):
+                for mode in args.conditioning:
+                    emit(dict(mode="per_peer", conditioning=mode, peers=p, lanes=pool.lanes, repeat=r, pool_mb=round(pool_mb),
+                              **measure(pool, p, frames, args.frames, args.warmup, mode)))
+        fps = collections.defaultdict(list)
+        for r in rows:
+            fps[(r["peers"], r["conditioning"])].append(r["fps"])
+        summary = {**base, "summary": True, "lanes": pool.lanes,
+                   "fps": {f"{p}:{m}": [min(v), max(v)] for (p, m), v in sorted(fps.items())}}
+        print(json.dumps(summary), flush=True)
+        del pool
+        from ai_rtc_agent_b200.host import weights as W
+        W._PRELOADED.pop(model, None)
+        torch.cuda.synchronize()
+        torch.cuda.empty_cache()
+        return summary
     shared, shared_mb = build(model, tl, False, None)
     pools = {}
     for lanes in lane_counts:
@@ -144,7 +187,11 @@ def main(argv=None) -> int:
     ap.add_argument("--peers", default="1,2,4,8")
     ap.add_argument("--lanes", default="2,3,4", help="per-peer lane counts to measure at T > 1")
     ap.add_argument("--models", default="all", choices=["all", "sd15", "turbo"])
+    ap.add_argument("--conditioning", default="", help="compare these conditioning modes (same, distinct, changing) instead")
     args = ap.parse_args(argv)
+    args.conditioning = [v for v in args.conditioning.split(",") if v]
+    if any(v not in ("same", "distinct", "changing") for v in args.conditioning):
+        ap.error("--conditioning takes same, distinct and changing")
     args.peers = [int(v) for v in args.peers.split(",")]
     args.lanes = [int(v) for v in args.lanes.split(",")]
     os.environ.setdefault("B200SD_SYNTHETIC_WEIGHTS", "1")

@@ -79,6 +79,7 @@ static void fill_plan_info(const IgemmPlan& plan, b2sd_igemm_plan_info* out) {
     out->m_tiles = plan.p.tiles_w * plan.p.tiles_h * plan.p.tiles_n;
     out->smem_bytes = (int64_t)plan.smem;
     out->rows_total = plan.rows_total;
+    out->tw = plan.p.tw; out->th = plan.p.th; out->tn = plan.p.tn;
 }
 
 }  // extern "C"

@@ -42,6 +42,7 @@ class IgemmPlanInfo(C.Structure):
         ("num_stages", C.c_int), ("acc_bufs", C.c_int), ("total_kb", C.c_int), ("kb_per_split", C.c_int),
         ("tmem_cols", C.c_int), ("m_tiles", C.c_int),
         ("smem_bytes", C.c_int64), ("rows_total", C.c_int64),
+        ("tw", C.c_int), ("th", C.c_int), ("tn", C.c_int),
     ]
 
 

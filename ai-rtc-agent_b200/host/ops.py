@@ -19,6 +19,13 @@ def pack_conv_weight(w_oihw: torch.Tensor) -> torch.Tensor:
     return w_oihw.permute(0, 2, 3, 1).reshape(o, kh * kw * i).contiguous().to(torch.float16)
 
 
+def _pitch(t: torch.Tensor) -> int:
+    """elements between consecutive pixels of an NHWC view: the stride of its innermost dimension with more than one index
+    (torch gives a size-1 dimension an arbitrary stride, e.g. W = 1 in the 1 x 1 output of a stride-2 conv)"""
+    n, h, w, _ = t.shape
+    return t.stride(2) if w > 1 or (h == 1 and n == 1) else (t.stride(1) if h > 1 else t.stride(0))
+
+
 def _view(t: torch.Tensor) -> capi.ActView:
     assert t.dtype == torch.float16 and t.is_cuda and t.dim() == 4
     n, h, w, c = t.shape
@@ -71,7 +78,7 @@ def _igemm_desc(srcs, w, out, *, stride=1, colbias=None, res=None, acc_scale=1.0
     d.nb, d.ho, d.wo = nb, ho, wo
     d.bn, d.splits = bn, splits
     d.swap = int(swap)
-    d.out, d.ldc = out.data_ptr(), out.stride(2)
+    d.out, d.ldc = out.data_ptr(), _pitch(out)
     nv = n_valid if n_valid is not None else out.shape[3]
     d.n_valid = nv
     if timeline is not None:
@@ -82,7 +89,7 @@ def _igemm_desc(srcs, w, out, *, stride=1, colbias=None, res=None, acc_scale=1.0
         d.colbias_bstride = colbias.shape[1] if colbias.dim() == 2 and colbias.shape[0] > 1 else 0
     if res is not None:
         assert res.dtype == torch.float16
-        d.res, d.ldr = res.data_ptr(), res.stride(2)
+        d.res, d.ldr = res.data_ptr(), _pitch(res)
     d.acc_scale, d.res_scale = acc_scale, res_scale
     d.flags = (capi.IG_RELU if relu else 0) | (capi.IG_GEGLU if geglu else 0) | (capi.IG_TCONV if tconv else 0) | (capi.IG_PAIR if pair else 0) \
         | (capi.IG_SILU if silu else 0) | (capi.IG_PAD0 if pad0 else 0)

@@ -106,6 +106,7 @@ typedef struct {
     int tmem_cols;
     int m_tiles;       /* 128-row output tiles */
     int64_t smem_bytes, rows_total;
+    int tw, th, tn;    /* pixel tile: tn images x th rows x tw columns of the output (swapped orientation: the N-side tile) */
 } b2sd_igemm_plan_info;
 int b2sd_igemm_plan_dry(const b2sd_igemm_desc* d, int autotile, int allow_swap, b2sd_igemm_plan_info* out);
 

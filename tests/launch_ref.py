@@ -174,24 +174,19 @@ def contraction_ref(d, snap: Dict[str, torch.Tensor], kmask=None, bias0=False, s
     return epilogue(d, acc, cb, None if no_res else snap.get("res"), rs, snap.get("colsum"))
 
 
-def split_k_lost_mask(d, total_kb: int, kb_per_split: int, device) -> torch.Tensor:
-    """[K] mask without the last cluster rank's K slice."""
+def k_block_mask(d, kb0: int, kb1: int, device) -> torch.Tensor:
+    """[K] mask without the 64-wide K blocks [kb0, kb1) (a split-K rank's slice, or one block)."""
     k = sum(nt * c for _, _, nt, c in k_segments(d))
     m = torch.ones(k, dtype=torch.float64, device=device)
-    splits = -(-total_kb // kb_per_split)
-    m[(splits - 1) * kb_per_split * 64:] = 0
+    m[kb0 * 64:kb1 * 64] = 0
     return m
 
 
-def last_block_mask(d, w: torch.Tensor) -> torch.Tensor:
-    """[K] mask without the last 64-wide K block whose weights are not all zero (narrow layers pad K with zero weights)."""
+def nonzero_blocks(d, w: torch.Tensor) -> List[int]:
+    """the 64-wide K blocks whose weights are not all zero, in K order"""
     k = sum(nt * c for _, _, nt, c in k_segments(d))
     W = w[:n_gemm(d), :k]
-    nz = (W != 0).reshape(W.shape[0], k // 64, 64).any(dim=2).any(dim=0)
-    last = int(nz.nonzero().max())
-    m = torch.ones(k, dtype=torch.float64, device=w.device)
-    m[last * 64:(last + 1) * 64] = 0
-    return m
+    return (W != 0).reshape(W.shape[0], k // 64, 64).any(dim=2).any(dim=0).nonzero().flatten().tolist()
 
 
 def split_out2(d, y: torch.Tensor):

@@ -49,9 +49,35 @@ def _conv(srcs, ws, stride):
     return acc
 
 
-@pytest.mark.parametrize("nb", [1, 4])
-@pytest.mark.parametrize("height,width,chs", [(384, 512, SD_CHS), (448, 768, SD_CHS), (768, 448, SD_CHS), (128, 192, TINY_CHS)],
-                         ids=["384x512", "448x768", "768x448", "tiny-128x192"])
+PLANS = ((1, True), (1, False), (2, True))   # (autotile, allow_swap) of the engine's tile policy
+
+
+def _case(height, width, chs, nb, name):
+    return pytest.param(height, width, chs, nb, id=f"{name}-{nb}")
+
+
+# Beyond the non-square sizes: the sizes the engine accepts at its edges and the tile regimes only they reach
+# (tests/test_config_space.py) -- 64 x 64 (1 x 1 deepest level: the 128 x 1 row tile, four 1-pixel images in one M tile, the
+# swapped orientation at 2 x 2), 576 (9 x 9 level: 117-row tiles; 18-wide level: a 16-wide tile with 2 valid columns),
+# 704 x 320 at batch 5 (11 x 5 level: 2 images per tile, the last one a phantom), 960 x 832 (15 x 13 level) and 1024 at
+# batch 3.  Batches 3 and 5 leave a phantom image in the last M tile; batch 16 fills several tiles with images.
+CASES = [_case(h, w, chs, nb, name) for (h, w, chs, name) in
+         ((384, 512, SD_CHS, "384x512"), (448, 768, SD_CHS, "448x768"), (768, 448, SD_CHS, "768x448"),
+          (128, 192, TINY_CHS, "tiny-128x192")) for nb in (1, 4)] + [
+    _case(64, 64, SD_CHS, 1, "64"), _case(64, 64, SD_CHS, 4, "64"), _case(64, 64, TINY_CHS, 16, "tiny-64"),
+    _case(512, 512, TINY_CHS, 3, "tiny-512"), _case(448, 448, TINY_CHS, 3, "tiny-448"),
+    _case(576, 576, TINY_CHS, 1, "tiny-576"), _case(704, 320, TINY_CHS, 5, "tiny-704x320"),
+    _case(960, 832, TINY_CHS, 1, "tiny-960x832"), _case(1024, 1024, TINY_CHS, 3, "tiny-1024"),
+    _case(128, 128, TINY_CHS, 16, "tiny-128"),
+    # extreme aspect ratios: levels a few rows high and 16 or more columns wide put several images into one 16- or 8-wide
+    # tile, and take the swapped orientation to 16-wide pixel tiles
+    _case(64, 576, TINY_CHS, 3, "tiny-64x576"), _case(64, 1024, SD_CHS, 3, "64x1024"), _case(64, 320, TINY_CHS, 4, "tiny-64x320"),
+    _case(64, 768, TINY_CHS, 4, "tiny-64x768"), _case(64, 576, SD_CHS, 1, "64x576"), _case(64, 512, TINY_CHS, 1, "tiny-64x512"),
+    _case(192, 768, TINY_CHS, 3, "tiny-192x768"), _case(128, 64, SD_CHS, 1, "128x64"), _case(64, 256, SD_CHS, 1, "64x256"),
+]
+
+
+@pytest.mark.parametrize("height,width,chs,nb", CASES)
 def test_igemm_nonsquare_levels(cuda, height, width, chs, nb):
     from ai_rtc_agent_b200.host import ops
     seen = set()
@@ -66,10 +92,11 @@ def test_igemm_nonsquare_levels(cuda, height, width, chs, nb):
         wp = torch.cat([ops.pack_conv_weight(wt) for wt in ws], dim=1).contiguous()
         bias = hetero((nb, cout), (0,), 1000 + seed, cuda, offset=2.0, scale=(0.5, 2.0), dtype=torch.float32).contiguous()
         ho, wo = h // stride, w // stride
-        out = guarded((nb * ho * wo, cout), pitch=cout + 64, device=cuda)
+        # the tail band holds every phantom image a partial last M tile can reach past the batch (< 4 tile-fulls of one image)
+        out = guarded((nb * ho * wo, cout), pitch=cout + 64, device=cuda, tail=max(64, 3 * ho * wo))
         o4 = out.view.view(nb, ho, wo, cout)
         src_taps = [(x, t) for x, (_, t) in zip(srcs, segs)]
-        for autotile, allow_swap in ((1, True), (1, False), (2, True)):
+        for autotile, allow_swap in PLANS:
             info = ops.igemm_engine_plan(src_taps, wp, o4, autotile=autotile, allow_swap=allow_swap, stride=stride, colbias=bias)
             key = (tuple(t for _, t in segs), stride, ho, wo, nb, info.bn, info.splits, info.swap, info.mode)
             if key in seen:
@@ -84,11 +111,14 @@ def test_igemm_nonsquare_levels(cuda, height, width, chs, nb):
             acc = _conv(srcs, ws, stride)
             bd = bias.double()[:, None, None, :]
             ref = acc + bd
-            if any(t == 9 for _, t in segs):
+            if any(t == 9 for _, t in segs) and h != w:
                 hw_swapped = _conv([x.reshape(nb, w, h, -1) for x in srcs], ws, stride).reshape(nb, ho, wo, cout) + bd
                 assert_discriminates(o4, ref, hw_swapped, 4e-3, 3e-3, what, "H and W swapped")
-            else:   # a 1x1 contraction gives the same pixels whichever way they are laid out
-                assert_discriminates(o4, ref, ref.roll(1, 2), 4e-3, 3e-3, what, "pixels shifted by one column")
+            elif any(t == 9 for _, t in segs) and h > 1:   # square level: H and W swapped = the image transposed
+                transposed = _conv([x.transpose(1, 2) for x in srcs], ws, stride).transpose(1, 2) + bd
+                assert_discriminates(o4, ref, transposed, 4e-3, 3e-3, what, "H and W swapped")
+            elif ho * wo > 1:   # a 1x1 contraction gives the same pixels whichever way they are laid out
+                assert_discriminates(o4, ref, ref.roll(1, 2 if wo > 1 else 1), 4e-3, 3e-3, what, "pixels shifted by one")
             if nb > 1:
                 assert_discriminates(o4, ref, acc + bd[:1], 4e-3, 3e-3, what, "image 0's bias for every image")
                 first = _conv([x[:1].expand_as(x) for x in srcs], ws, stride) + bd

@@ -27,7 +27,7 @@ def _rand(shape, dev, seed, scale=1.0):
     return (torch.randn(shape, generator=g) * scale).to(dev)
 
 
-@pytest.mark.parametrize("nb,heads,seq,d,dp", [
+SELF_ATTENTION_CASES = [
     (1, 1, 128, 64, 64),     # one q tile, one kv block
     (1, 2, 256, 64, 64),     # two kv blocks: online-softmax rescale, S double buffer
     (1, 5, 4096, 64, 64),    # SD-Turbo 64x64 latent self-attention
@@ -37,7 +37,14 @@ def _rand(shape, dev, seed, scale=1.0):
     (1, 8, 256, 40, 64),     # SD-1.5 head dim 40 zero-padded to 64
     (1, 8, 256, 80, 128),    # SD-1.5 head dim 80 -> 128
     (2, 8, 384, 160, 192),   # SD-1.5 head dim 160 -> 192 (BKV 64 variant)
-])
+    (1, 5, 16384, 64, 64),   # SD-Turbo 1024x1024 level 0: 128 q tiles, 128 kv blocks
+    (3, 8, 1024, 40, 64),    # stream batch 3
+    (2, 2, 14400, 64, 64),   # 960 x 960 level 0 at batch 2: a long sequence whose last KV tile reaches into the next image
+    (1, 8, 4, 40, 64),       # 128 x 128 mid block: 4 tokens, fewer than one 8-column V^T group
+]
+
+
+@pytest.mark.parametrize("nb,heads,seq,d,dp", SELF_ATTENTION_CASES)
 def test_self_attention(cuda, nb, heads, seq, d, dp):
     ops = _ops()
     q = _rand((nb, heads, seq, d), cuda, 1).half()
@@ -48,11 +55,12 @@ def test_self_attention(cuda, nb, heads, seq, d, dp):
     kp = torch.zeros_like(qp)
     qp[..., :d] = q.permute(0, 2, 1, 3)
     kp[..., :d] = k.permute(0, 2, 1, 3)
-    vt = torch.zeros(heads, dp, nb, seq, dtype=torch.float16, device=cuda)
-    vt[:, :d] = v.permute(1, 3, 0, 2)
+    cols = -(-nb * seq // 8) * 8   # V^T row pitch: a multiple of 8 (16-byte rows for the TMA unit)
+    vt = torch.zeros(heads, dp, cols, dtype=torch.float16, device=cuda)
+    vt[:, :d, :nb * seq] = v.permute(1, 3, 0, 2).reshape(heads, d, nb * seq)
     out = torch.full((nb * seq, heads * d), float("nan"), dtype=torch.float16, device=cuda)
     ops.attention(qp.reshape(nb * seq, heads * dp), kp.reshape(nb * seq, heads * dp),
-                  vt.reshape(heads * dp, nb * seq), out, nb=nb, heads=heads, sq=seq, skv=seq, d_real=d, dp=dp,
+                  vt.reshape(heads * dp, cols)[:, :nb * seq], out, nb=nb, heads=heads, sq=seq, skv=seq, d_real=d, dp=dp,
                   k_bstride=seq, vt_bstride=seq)
     ref = F.scaled_dot_product_attention(q.float(), k.float(), v.float())  # (nb,heads,seq,d)
     ref = ref.permute(0, 2, 1, 3).reshape(nb * seq, heads * d)
@@ -114,7 +122,10 @@ def _vt_layout(v, dp, pitch=None):
     return vt.reshape(heads * dp, cols)
 
 
-@pytest.mark.parametrize("seq", [144, 576, 4096 + 64])
+BATCH_TAIL_SEQS = [144, 576, 4096 + 64]
+
+
+@pytest.mark.parametrize("seq", BATCH_TAIL_SEQS)
 @pytest.mark.parametrize("d,dp", [(64, 64), (80, 128), (160, 192)])
 def test_self_attention_batch_tail_poisoned(cuda, seq, d, dp):
     """Four batch items packed with k_bstride = vt_bstride = seq, as the engine packs them: the tail KV tile of batch item b
@@ -158,7 +169,16 @@ def test_self_attention_batch_tail_poisoned(cuda, seq, d, dp):
     assert_discriminates(out.view, ref, wrong_v, *ATTN_TOL, what, "batch item 0's values for every item")
 
 
-@pytest.mark.parametrize("seq", [36, 196])
+# the mid-block token counts of the smallest engines (64 x 64: 1, 128 x 128: 4, 128 x 192: 6), at stream batch 3: fewer
+# tokens than one 8-column V^T group, and a batch that is not a power of two
+PADDED_VT_SEQS = [36, 196, 1, 4, 6]
+
+
+def _padded_vt_batch(seq):
+    return 4 if seq >= 8 else 3
+
+
+@pytest.mark.parametrize("seq", PADDED_VT_SEQS)
 @pytest.mark.parametrize("d,dp", [(40, 64), (80, 128), (160, 192)])
 def test_self_attention_padded_vt_batch_stride(cuda, seq, d, dp):
     """The transformer program for token counts that are not a multiple of 8 with several images (SD-1.5 at 192x192: 36 and 9
@@ -170,7 +190,7 @@ def test_self_attention_padded_vt_batch_stride(cuda, seq, d, dp):
     keys leaking in."""
     ops = _ops()
     from tests import launch_ref as R
-    nb, heads = 4, 2
+    nb, heads = _padded_vt_batch(seq), 2
     seqp = -(-seq // 8) * 8
     bkv = _bkv(dp)
     tail = -(-seq // bkv) * bkv - seq
@@ -200,9 +220,11 @@ def test_self_attention_padded_vt_batch_stride(cuda, seq, d, dp):
     what = f"self-attn nb={nb} seq={seq} (V^T stride {seqp}) d={d}/{dp}"
     assert_discriminates(out.view, ref, R.attention_ref(dict(a, vt_bstride=seq), qb, kb, vt), *ATTN_TOL, what,
                          "V^T addressed with the K batch stride")
-    assert_discriminates(out.view, ref, R.attention_ref(dict(a, k_bstride=seqp), qb, torch.cat([kb, torch.zeros_like(kb)]), vt),
-                         *ATTN_TOL, what, "K addressed with the V^T batch stride")
-    assert_discriminates(out.view, ref, R.attention_ref(dict(a, skv=seqp), qb, torch.cat([kb, torch.zeros_like(kb[:8])]), vt),
+    if seq > 1:   # one key per image: the output does not depend on which key it is
+        assert_discriminates(out.view, ref, R.attention_ref(dict(a, k_bstride=seqp), qb,
+                                                            torch.cat([kb, kb.new_zeros((nb * seqp, kb.shape[1]))]), vt),
+                             *ATTN_TOL, what, "K addressed with the V^T batch stride")
+    assert_discriminates(out.view, ref, R.attention_ref(dict(a, skv=seqp), qb, torch.cat([kb, kb.new_zeros((8, kb.shape[1]))]), vt),
                          *ATTN_TOL, what, "V^T pad columns (and the keys past seq) not masked")
 
 
@@ -363,6 +385,7 @@ GN_PATH_CASES = [
     ("cluster", 4, 1, 64, 64, 320, 0, 1e-5), ("cluster", 4, 4, 64, 64, 320, 0, 1e-5),
     ("cluster", 8, 1, 64, 64, 640, 320, 1e-5), ("cluster", 8, 4, 64, 64, 640, 320, 1e-6),   # groups of 30 straddle the concat
     ("cluster", 4, 2, 32, 32, 1280, 640, 1e-5),                                              # groups of 60 straddle the concat
+    ("cluster", 1, 4, 1, 1, 1280, 0, 1e-5),                                                  # 64 x 64 engine: 1-pixel images
     ("fused", None, 1, 96, 96, 640, 0, 1e-5), ("fused", None, 1, 96, 96, 640, 0, 1e-6),
     ("fused", None, 1, 72, 72, 640, 320, 1e-5),                                              # fused, straddling groups
     ("stats+apply", None, 1, 96, 96, 640, 320, 1e-5),                                        # straddling groups

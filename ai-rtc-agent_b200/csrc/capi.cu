@@ -317,4 +317,9 @@ int b2sd_op_post_u8(const void* y_nhwc, int ldy, void* out_nchw_u8, int nb, int 
                           h, w, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int b2sd_op_post_f16(const void* y_nhwc, int ldy, void* out_nchw_f16, int nb, int h, int w, void* stream) {
+    return post_f16_launch(reinterpret_cast<const __half*>(y_nhwc), ldy, reinterpret_cast<__half*>(out_nchw_f16), nb, h, w,
+                           reinterpret_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

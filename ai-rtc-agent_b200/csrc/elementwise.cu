@@ -3,6 +3,8 @@
 
 #include <stdio.h>
 
+#include <utility>
+
 #include "igemm.cuh"  // b2_set_error
 #include "launch.cuh"
 #include "ptx.cuh"
@@ -60,11 +62,19 @@ __device__ __forceinline__ T block_reduce_sum(T v, T* scratch) {
 }
 
 // ------------------------------------------------------------------------------------------ GroupNorm
+// Every path sums x - pilot and (x - pilot)^2, the pilot being the group's first channel at the image's first pixel, which
+// every CTA reads without talking to the others.  The pilot lies within a few standard deviations of the group mean, so
+// var = E[(x-p)^2] - E[x-p]^2 keeps fp32 precision however far the mean sits from zero (raw sums lose ~(mean/std)^2 of it).
 // Pass 1: grid (chunks, nb); a CTA owns `ppc` consecutive pixels x all channels (fully coalesced 16-byte
-// loads), reduces per channel, then per group, and writes one (sum, sumsq) pair per (chunk, group).
+// loads), reduces per channel, then per group, and writes one (sum, sumsq) pair per (chunk, group) of x - pilot.
 // Pass 2: every CTA re-derives mean/rstd of its batch item from the <=128 chunk partials (fixed summation
 // order => deterministic), then normalises 8 channels per thread.
 constexpr int GN_MAX_CHUNKS = 128;
+
+__device__ __forceinline__ float gn_pilot(const GroupNormArgs& a, int b, int g) {
+    const int c = g * ((a.ca + a.cb) / a.groups);
+    return __half2float(c < a.ca ? a.xa[(long)b * a.hw * a.lda + c] : a.xb[(long)b * a.hw * a.ldb + (c - a.ca)]);
+}
 
 __global__ void __launch_bounds__(512) gn_stats_kernel(GroupNormArgs a, int ppc, int vc, int rpi) {
     B2_PDL_ENTRY();
@@ -79,9 +89,12 @@ __global__ void __launch_bounds__(512) gn_stats_kernel(GroupNormArgs a, int ppc,
     const int ld = from_a ? a.lda : a.ldb;
     const int p_begin = chunk * ppc;
     const int p_end = min(a.hw, p_begin + ppc);
-    float s[8], q[8];
+    float s[8], q[8], pil[8];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) s[i] = q[i] = 0.f;
+    for (int i = 0; i < 8; ++i) {
+        s[i] = q[i] = 0.f;
+        pil[i] = prow < rpi ? gn_pilot(a, b, (c0 + i) / ((a.ca + a.cb) / a.groups)) : 0.f;
+    }
     if (prow < rpi) {
         for (int p = p_begin + prow; p < p_end; p += rpi) {
             const uint4 u = *reinterpret_cast<const uint4*>(base + ((long)b * a.hw + p) * ld);
@@ -89,8 +102,9 @@ __global__ void __launch_bounds__(512) gn_stats_kernel(GroupNormArgs a, int ppc,
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const float2 f = __half22float2(h[i]);
-                s[2 * i] += f.x; q[2 * i] += f.x * f.x;
-                s[2 * i + 1] += f.y; q[2 * i + 1] += f.y * f.y;
+                const float d0 = f.x - pil[2 * i], d1 = f.y - pil[2 * i + 1];
+                s[2 * i] += d0; q[2 * i] += d0 * d0;
+                s[2 * i + 1] += d1; q[2 * i + 1] += d1 * d1;
             }
         }
 #pragma unroll
@@ -125,7 +139,7 @@ __global__ void __launch_bounds__(512) gn_stats_kernel(GroupNormArgs a, int ppc,
     }
 }
 
-// mean / rstd of every group of batch item b from the per-chunk partial sums (layout [b][group][chunk]): one warp
+// mean / rstd of every group of batch item b from the per-chunk partial sums of x - pilot (layout [b][group][chunk]): one warp
 // per group reads the chunk partials with coalesced loads (all in flight at once) and reduces them with a fixed
 // shuffle tree, so the result is deterministic and costs about one L2 round trip.
 __device__ __forceinline__ void gn_finalize_stats(const GroupNormArgs& a, int b, int nchunks, float* /*scratch*/,
@@ -152,9 +166,9 @@ __device__ __forceinline__ void gn_finalize_stats(const GroupNormArgs& a, int b,
             gq += __shfl_xor_sync(0xffffffffu, gq, o);
         }
         if (lane == 0) {
-            const float mean = gs * inv_n;
-            s_mean[g] = mean;
-            s_rstd[g] = rsqrtf(fmaxf(gq * inv_n - mean * mean, 0.f) + a.eps);
+            const float m = gs * inv_n;   // mean of x - pilot
+            s_mean[g] = gn_pilot(a, b, g) + m;
+            s_rstd[g] = rsqrtf(fmaxf(gq * inv_n - m * m, 0.f) + a.eps);
         }
     }
     __syncthreads();
@@ -225,9 +239,12 @@ __global__ void __launch_bounds__(512) gn_fused_kernel(GroupNormArgs a, int ppc,
     const int ld = from_a ? a.lda : a.ldb;
     const int p_begin = chunk * ppc, p_end = min(a.hw, p_begin + ppc);
     uint4 cache[GN_CACHE];
-    float s[8], q[8];
+    float s[8], q[8], pil[8];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) s[i] = q[i] = 0.f;
+    for (int i = 0; i < 8; ++i) {
+        s[i] = q[i] = 0.f;
+        pil[i] = prow < rpi ? gn_pilot(a, b, (c0 + i) / ((a.ca + a.cb) / a.groups)) : 0.f;
+    }
     if (prow < rpi) {
 #pragma unroll
         for (int it = 0; it < GN_CACHE; ++it) {
@@ -239,8 +256,9 @@ __global__ void __launch_bounds__(512) gn_fused_kernel(GroupNormArgs a, int ppc,
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                     const float2 f = __half22float2(h[i]);
-                    s[2 * i] += f.x; q[2 * i] += f.x * f.x;
-                    s[2 * i + 1] += f.y; q[2 * i + 1] += f.y * f.y;
+                    const float d0 = f.x - pil[2 * i], d1 = f.y - pil[2 * i + 1];
+                    s[2 * i] += d0; q[2 * i] += d0 * d0;
+                    s[2 * i + 1] += d1; q[2 * i + 1] += d1 * d1;
                 }
             }
         }
@@ -369,6 +387,7 @@ __global__ void __launch_bounds__(GNC_THREADS, 2) gn_cluster_kernel(GroupNormArg
     B2_PDL_ENTRY();
     const int p0 = rank * ppc, p1 = min(a.hw, p0 + ppc);
     const long rowbase = (long)b * a.hw;
+    const float pil = gn_pilot(a, b, g);
     uint32_t v[GNC_ITEMS];
 #pragma unroll
     for (int k = 0; k < GNC_ITEMS; ++k) {
@@ -378,10 +397,13 @@ __global__ void __launch_bounds__(GNC_THREADS, 2) gn_cluster_kernel(GroupNormArg
     }
     float s = 0.f, q = 0.f;
 #pragma unroll
-    for (int k = 0; k < GNC_ITEMS; ++k) {   // out-of-range items are zero: they add nothing
-        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&v[k]));
-        s += f.x + f.y;
-        q += f.x * f.x + f.y * f.y;
+    for (int k = 0; k < GNC_ITEMS; ++k) {
+        if (p0 + prow + k * pstep < p1) {
+            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&v[k]));
+            const float d0 = f.x - pil, d1 = f.y - pil;
+            s += d0 + d1;
+            q += d0 * d0 + d1 * d1;
+        }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -406,8 +428,9 @@ __global__ void __launch_bounds__(GNC_THREADS, 2) gn_cluster_kernel(GroupNormArg
     float S = 0.f, Q = 0.f;
     for (int r = 0; r < nrank; ++r) { S += part[r].x; Q += part[r].y; }   // fixed order => deterministic
     const float inv_n = 1.0f / ((float)a.hw * (float)cpg);
-    const float mean = S * inv_n;
-    const float rstd = rsqrtf(fmaxf(Q * inv_n - mean * mean, 0.f) + a.eps);
+    const float m = S * inv_n;   // mean of x - pilot
+    const float rstd = rsqrtf(fmaxf(Q * inv_n - m * m, 0.f) + a.eps);
+    const float mean = pil + m;
     const float ax = rstd * gm.x, ay = rstd * gm.y;
     const float bx = bt.x - mean * ax, by = bt.y - mean * ay;
     __half* dst = a.y + c;
@@ -460,6 +483,18 @@ int groupnorm_launch(const GroupNormArgs& a, cudaStream_t s) {
         !a.partial) {
         b2_set_error("groupnorm: unsupported channels %d+%d groups %d (need multiples of 8 and a workspace)", a.ca, a.cb,
                      a.groups);
+        return -1;
+    }
+    // every path centres its statistics on a value of x (gn_pilot) that some CTAs read after others have written y
+    const auto span = [&](const void* p, int ld, int c) {
+        return std::make_pair((const char*)p, (const char*)p + (((long)a.nb * a.hw - 1) * ld + c) * sizeof(__half));
+    };
+    const auto overlap = [](std::pair<const char*, const char*> u, std::pair<const char*, const char*> v) {
+        return u.first < v.second && v.first < u.second;
+    };
+    const auto ys = span(a.y, a.ldy, C);
+    if (overlap(ys, span(a.xa, a.lda, a.ca)) || (a.cb && overlap(ys, span(a.xb, a.ldb, a.cb)))) {
+        b2_set_error("groupnorm: the output overlaps an input (in-place GroupNorm is not supported)");
         return -1;
     }
     if (const int cl = gn_cluster_size(a)) {
@@ -555,15 +590,20 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict
         xv[k] = make_uint4(0, 0, 0, 0);
         if (ch < chunks) xv[k] = reinterpret_cast<const uint4*>(xr)[ch];
     }
+    // statistics of x - x[0] (the row's pilot, see GroupNorm): fp32 precision however far the row mean sits from zero
+    const float pil = __half2float(__ushort_as_half((unsigned short)(__shfl_sync(0xffffffffu, xv[0].x, 0) & 0xffffu)));
     float s = 0.f, ss = 0.f;
 #pragma unroll
-    for (int k = 0; k < LN_MAXK; ++k) {   // absent chunks are zero: they add nothing
-        const __half2* h = reinterpret_cast<const __half2*>(&xv[k]);
+    for (int k = 0; k < LN_MAXK; ++k) {
+        if (lane + 32 * k < chunks) {
+            const __half2* h = reinterpret_cast<const __half2*>(&xv[k]);
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float2 f = __half22float2(h[i]);
-            s += f.x + f.y;
-            ss += f.x * f.x + f.y * f.y;
+            for (int i = 0; i < 4; ++i) {
+                const float2 f = __half22float2(h[i]);
+                const float d0 = f.x - pil, d1 = f.y - pil;
+                s += d0 + d1;
+                ss += d0 * d0 + d1 * d1;
+            }
         }
     }
 #pragma unroll
@@ -571,8 +611,9 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict
         s += __shfl_xor_sync(0xffffffffu, s, o);
         ss += __shfl_xor_sync(0xffffffffu, ss, o);
     }
-    const float mean = s / c;
-    const float rstd = rsqrtf(fmaxf(ss / c - mean * mean, 0.f) + eps);
+    const float m = s / c;
+    const float rstd = rsqrtf(fmaxf(ss / c - m * m, 0.f) + eps);
+    const float mean = pil + m;
     __half* yr = y + row * ldy;
 #pragma unroll
     for (int k = 0; k < LN_MAXK; ++k) {

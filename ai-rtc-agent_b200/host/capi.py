@@ -200,6 +200,7 @@ def lib() -> C.CDLL:
         _lib.b2sd_op_hed_fuse.argtypes = [C.POINTER(vp), C.POINTER(ci), C.POINTER(ci), ci, ci, ci, vp, vp, vp]
         _lib.b2sd_op_lcm_step.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, vp]
         _lib.b2sd_op_post_u8.argtypes = [vp, ci, vp, ci, ci, ci, vp]
+        _lib.b2sd_op_post_f16.argtypes = [vp, ci, vp, ci, ci, ci, vp]
         _lib.b2sd_op_nv12_to_rgb.argtypes = [vp, ci, vp, ci, vp, ci, ci, ci, vp]
         _lib.b2sd_op_rgb_to_nv12.argtypes = [vp, vp, ci, vp, ci, ci, ci, ci, vp]
         _lib.b2sd_codec_probe.restype = C.c_int
@@ -245,7 +246,7 @@ def lib() -> C.CDLL:
         for name in ("create", "create_lane", "destroy", "load_tensor", "prepare", "export_packed", "import_packed", "set_prompt_embeds", "set_timesteps", "step",
                      "step_ex", "get_tensor", "launches_per_step"):
             getattr(_lib, "b2sd_" + name).restype = C.c_int
-        for name in ("attention", "groupnorm", "layernorm", "upsample2x", "smallconv", "smallconv_ex", "maxpool2x2", "hed_project", "hed_fuse", "lcm_step", "post_u8", "nv12_to_rgb", "rgb_to_nv12"):
+        for name in ("attention", "groupnorm", "layernorm", "upsample2x", "smallconv", "smallconv_ex", "maxpool2x2", "hed_project", "hed_fuse", "lcm_step", "post_u8", "post_f16", "nv12_to_rgb", "rgb_to_nv12"):
             getattr(_lib, "b2sd_op_" + name).restype = C.c_int
     return _lib
 

@@ -214,3 +214,10 @@ def post_u8(y, out):
     nb, h, w, _ = y.shape
     capi.check(capi.lib().b2sd_op_post_u8(y.data_ptr(), y.stride(2), out.data_ptr(), nb, h, w, _sp()), "b2sd_op_post_u8")
     return out
+
+
+def post_f16(y, out):
+    """y: NHWC fp16 [nb, h, w, >= 3]; out: fp16 NCHW [nb, 3, h, w] = y * 2 - 1 (the float entry's tail)"""
+    nb, h, w, _ = y.shape
+    capi.check(capi.lib().b2sd_op_post_f16(y.data_ptr(), y.stride(2), out.data_ptr(), nb, h, w, _sp()), "b2sd_op_post_f16")
+    return out

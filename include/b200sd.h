@@ -129,7 +129,8 @@ typedef struct {
 } b2sd_attn_desc;
 int b2sd_op_attention(const b2sd_attn_desc* d, void* stream);
 
-/* GroupNorm(+SiLU) over the channel concatenation [xa | xb] (xb may be NULL), NHWC fp16. */
+/* GroupNorm(+SiLU) over the channel concatenation [xa | xb] (xb may be NULL), NHWC fp16.  y must not overlap xa or xb
+ * (the statistics are centred on a value of x that other CTAs read after some have written y): refused. */
 int b2sd_op_groupnorm(const void* xa, int ca, int lda, const void* xb, int cb, int ldb, const float* gamma,
                       const float* beta, void* y, int ldy, int nb, int hw, int groups, float eps, int silu,
                       void* stream);
@@ -170,6 +171,8 @@ int b2sd_op_rgb_to_nv12(const void* rgb_nchw, void* y, int y_pitch, void* uv, in
 int b2sd_codec_probe(void);
 /* decoder tail + lib/pipeline.py:72-74 on the fp16 grid -> u8 NCHW */
 int b2sd_op_post_u8(const void* y_nhwc, int ldy, void* out_nchw_u8, int nb, int h, int w, void* stream);
+/* the float entry's tail: y * 2 - 1 in fp16 -> fp16 NCHW */
+int b2sd_op_post_f16(const void* y_nhwc, int ldy, void* out_nchw_f16, int nb, int h, int w, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Engine level: one handle == one temporal stream (one StreamDiffusion instance, lib/wrapper.py:168).

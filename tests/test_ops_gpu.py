@@ -432,9 +432,11 @@ def test_groupnorm_paths_discriminate(cuda, path, cl, nb, h, w, ca, cb, eps, sil
     (1, 96, 96, 640, 0, "fused"), (1, 96, 96, 640, 320, "stats+apply"),
 ])
 def test_groupnorm_offset_heavy(cuda, nb, h, w, ca, cb, path):
-    """Groups whose mean is 30-100 standard deviations away from zero (within fp16 range).  Every GroupNorm kernel computes the
-    variance as E[x^2] - mean^2 in fp32; this pins |mean|/std <= 100 as the operating range in which that holds the usual
-    tolerance.  The case's error, in units of the tolerance, is printed."""
+    """Groups whose mean is 30-100 standard deviations away from zero (within fp16 range).  Every GroupNorm kernel sums
+    x - pilot and (x - pilot)^2 in fp32, the pilot being the group's first channel at the image's first pixel, so the
+    variance keeps fp32 precision however far the mean is from zero, as long as the pilot lies within a few standard
+    deviations of the mean; test_precision_gpu.test_floor_groupnorm holds every path to the fp16 floor for |mean|/std up to
+    100 on such data, and test_precision_audit_gpu measures the pilot's distance on real activations (at most 3.3 std).  The case's error, in units of the tolerance, is printed."""
     ops = _ops()
     c = ca + cb
     g = torch.Generator().manual_seed(11)
@@ -480,8 +482,10 @@ def test_layernorm(cuda, rows, c):
 
 @pytest.mark.parametrize("rows,c", [(1024, 320), (256, 1280)])
 def test_layernorm_offset_heavy(cuda, rows, c):
-    """Rows with |mean|/std of 30..100: layernorm_kernel computes the variance as E[x^2] - mean^2 in fp32; this pins that
-    range as the one in which it holds the usual tolerance.  The error, in units of the tolerance, is printed."""
+    """Rows with |mean|/std of 30..100: layernorm_kernel sums x - x[0] and (x - x[0])^2 in fp32, so the variance keeps fp32
+    precision however far the mean is from zero while x[0] lies within a few standard deviations of the mean;
+    test_precision_gpu.test_floor_layernorm holds it to the fp16 floor for |mean|/std up to 100 on such rows.
+    The error, in units of the tolerance, is printed."""
     ops = _ops()
     x = offset_heavy_rows(rows, c, cuda)
     gamma = (1 + 0.1 * _rand((c,), cuda, 2)).float()

@@ -471,7 +471,8 @@ static int gn_cluster_size(const GroupNormArgs& a) {
 int groupnorm_plan(const GroupNormArgs& a, int* threads, int* pixels_per_cta) {
     const int cl = gn_cluster_size(a);
     if (threads) *threads = cl ? GNC_THREADS : 0;
-    if (pixels_per_cta) *pixels_per_cta = cl ? (a.hw + cl - 1) / cl : 0;
+    // the non-cluster kernels split each image into GN_MAX_CHUNKS chunks of pixels, one CTA each (groupnorm_launch)
+    if (pixels_per_cta) *pixels_per_cta = cl ? (a.hw + cl - 1) / cl : (a.hw + GN_MAX_CHUNKS - 1) / GN_MAX_CHUNKS;
     return cl;
 }
 

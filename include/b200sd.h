@@ -111,7 +111,8 @@ typedef struct {
 int b2sd_igemm_plan_dry(const b2sd_igemm_desc* d, int autotile, int allow_swap, b2sd_igemm_plan_info* out);
 
 /* Host-only: launch shape of GroupNorm over [ca | cb] channels, hw pixels per image: cluster = CTAs per (image, group) of the
- * cluster kernel (0 = whole-grid cooperative kernel), threads per CTA, pixels per CTA. */
+ * cluster kernel (0 = the non-cluster kernels: fused cooperative, or statistics + apply), threads per CTA of the cluster kernel,
+ * pixels per CTA (cluster = 0: pixels per chunk of the non-cluster kernels). */
 int b2sd_groupnorm_plan_dry(int ca, int cb, int groups, int hw, int* cluster, int* threads, int* pixels_per_cta);
 uint64_t b2sd_igemm_partial_floats(int splits, int64_t rows_total, int n_valid);   /* legacy sizing helper, unused by the cluster split-K */
 

@@ -248,9 +248,12 @@ def groupnorm_ref(g, xa: torch.Tensor, xb: Optional[torch.Tensor], gamma, beta, 
     return y
 
 
-def layernorm_ref(l, x: torch.Tensor, gamma, beta, shift_rows=False) -> torch.Tensor:
-    """LayerNorm over the c columns of x [rows, c] -> float64; shift_rows: the neighbouring row's statistics (wrong reference)."""
+def layernorm_ref(l, x: torch.Tensor, gamma, beta, shift_rows=False, shift_affine=False) -> torch.Tensor:
+    """LayerNorm over the c columns of x [rows, c] -> float64; wrong references: shift_rows, the neighbouring row's statistics;
+    shift_affine, the neighbouring column's gamma and beta."""
     x = x.double()
+    if shift_affine:
+        gamma, beta = torch.roll(gamma, 1), torch.roll(beta, 1)
     mean = x.mean(dim=1, keepdim=True)
     var = x.var(dim=1, unbiased=False, keepdim=True)
     if shift_rows:

@@ -76,12 +76,18 @@ def groupnorm_regime(ca, cb, hw):
     return f"gn:cl{cl.value}" + ("+hw<8" if hw < 8 else "")
 
 
+def variant_prefix(flags):
+    """the kernel variant of a contraction with these epilogue flags: "pad0:" (igemm_pad0_kernel, the tap origin at the output
+    pixel), "silu:" (the SiLU-epilogue instantiations), "" (the plain kernels)"""
+    return "pad0:" if flags & capi.IG_PAD0 else ("silu:" if flags & capi.IG_SILU else "")
+
+
 @functools.lru_cache(maxsize=None)
-def _planned(nb, h, w, srcs, cout, stride, geglu, allow_swap, autotile):
-    d, _ = _desc(nb, h, w, list(srcs), cout, stride=stride, geglu=geglu)
+def _planned(nb, h, w, srcs, cout, stride, geglu, allow_swap, autotile, flags=0):
+    d, _ = _desc(nb, h, w, list(srcs), cout, stride=stride, geglu=geglu, flags=flags)
     info = capi.IgemmPlanInfo()
     assert capi.lib().b2sd_igemm_plan_dry(C.byref(d), autotile, int(allow_swap), C.byref(info)) == 0, capi.lib().b2sd_last_error()
-    return contraction_regime(d.nb, d.ho, d.wo, info.tw, info.th, info.tn, info.swap)
+    return variant_prefix(flags) + contraction_regime(d.nb, d.ho, d.wo, info.tw, info.th, info.tn, info.swap)
 
 
 def plan_regime(info, nb, ho, wo):
@@ -234,8 +240,8 @@ def test_gpu_lists_cover_the_configuration_space():
     missing = sorted(space_eng - set().union(*(eng(r) for _, _, r in engines)))
     assert not missing, f"regimes no engine configuration reaches: {missing}"
     # Each configuration of the sweep earns its GPU time: a regime that no other engine configuration reaches.  (The
-    # full-size audit entries are there for the real models' channel counts, launch policies and networks -- ControlNet,
-    # HED, AutoencoderKL, frame resizing -- which this model does not describe.)
+    # full-size audit entries are also there for frame resizing, which this model does not describe; the ControlNet, HED and
+    # AutoencoderKL branches are modelled by tests/test_config_space_branches.py.)
     dead = []
     for i, (lst, name, regs) in enumerate(engines):
         others = set().union(*(eng(r) for j, (_, _, r) in enumerate(engines) if j != i))

@@ -20,8 +20,9 @@ def _full_ring_stages(info):
     return max(2, min(8, RING_KB * 1024 // stage, max(2, info.kb_per_split)))
 
 
-def _desc(nb, h, w, srcs, cout, stride=1, bn=0, splits=1, swap=0, geglu=False, res=False):
-    """srcs: [(channels, ntap)], output h/stride x w/stride x cout"""
+def _desc(nb, h, w, srcs, cout, stride=1, bn=0, splits=1, swap=0, geglu=False, res=False, flags=0):
+    """srcs: [(channels, ntap)], output h/stride x w/stride x cout; flags: further epilogue / kernel-variant flags (IG_SILU,
+    IG_PAD0), which restrict the planner's choices as they do in the engine"""
     d = capi.IgemmDesc()
     d.nseg = len(srcs)
     k = 0
@@ -39,7 +40,7 @@ def _desc(nb, h, w, srcs, cout, stride=1, bn=0, splits=1, swap=0, geglu=False, r
     if res:
         d.res, d.ldr = 0xC000000, cout
     d.acc_scale = d.res_scale = 1.0
-    d.flags = capi.IG_GEGLU if geglu else 0
+    d.flags = (capi.IG_GEGLU if geglu else 0) | flags
     d.n_valid = cout
     return d, k // 64
 

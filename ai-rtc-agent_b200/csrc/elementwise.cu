@@ -1065,6 +1065,37 @@ int gather_rows_launch(const __half* src, int src_ld, const int* perm, __half* d
     return 0;
 }
 
+// ---- LoRA factors as igemm operands (b2sd_apply_lora) ---------------------------------------------------------------------
+// dst[i][p*rank + k] = part p of src(i, k) for k < rank, zero for the columns up to kp; src(i, k) = src[i*si + k*sk].  fp16
+// sources have one part.  fp32 sources have three, hi = fp16(x) or lo = fp16(x - hi) as bit p of lo_mask says, so that
+// [uh | ul | uh] . [dh ; dh ; dl] = (uh + ul)(dh + dl) - ul dl carries the fp32 factors to about 2^-22.
+__global__ void lora_factor_kernel(const void* __restrict__ src, int f32, long n, int rank, long si, long sk, int lo_mask,
+                                   __half* __restrict__ dst, int kp) {
+    const long total = n * kp;
+    for (long e = (long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long)gridDim.x * blockDim.x) {
+        const int c = (int)(e % kp);
+        const long i = e / kp;
+        const int p = c / rank, k = c - p * rank;
+        __half v = __float2half(0.f);
+        if (p < (f32 ? 3 : 1)) {
+            if (f32) {
+                const float x = static_cast<const float*>(src)[i * si + k * sk];
+                const __half hi = __float2half_rn(x);
+                v = (lo_mask >> p) & 1 ? __float2half_rn(x - __half2float(hi)) : hi;
+            } else {
+                v = static_cast<const __half*>(src)[i * si + k * sk];
+            }
+        }
+        dst[e] = v;
+    }
+}
+int lora_factor_launch(const void* src, int f32, long n, int rank, long si, long sk, int lo_mask, __half* dst, int kp,
+                       cudaStream_t s) {
+    lora_factor_kernel<<<grid_for(n * kp), 256, 0, s>>>(src, f32, n, rank, si, sk, lo_mask, dst, kp);
+    B2_CHECK_LAUNCH("lora_factor");
+    return 0;
+}
+
 // ---- LayerNorm folded into the consumer GEMM (load-time preparation; one warp per weight row) -----------------------
 __global__ void scale_cols_kernel(__half* w, long rows, int k, const float* __restrict__ g) {
     const long r = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);

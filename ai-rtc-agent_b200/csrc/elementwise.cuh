@@ -104,6 +104,10 @@ int pack_conv_weight_launch(const __half* w_oihw, __half* dst, int dst_ld, int k
 // copy rows with a row permutation: dst[r][:] = src[perm[r]][:]
 int gather_rows_launch(const __half* src, int src_ld, const int* perm, __half* dst, int dst_ld, int rows, int cols,
                        cudaStream_t s);
+// One LoRA factor as a zero-padded fp16 igemm operand [n][kp] (b2sd_apply_lora): row i, column k < rank from
+// src[i*si + k*sk] (fp16, or f32 = 1: fp32 split into three hi / lo parts, see the kernel)
+int lora_factor_launch(const void* src, int f32, long n, int rank, long si, long sk, int lo_mask, __half* dst, int kp,
+                       cudaStream_t s);
 
 // LayerNorm folded into its consumer GEMM, load-time preparation on packed [rows][k] fp16 weights:
 //   scale_cols: W'[n][k] = W[n][k] * gamma[k];  row_sum: s[n] = sum_k W'[n][k];  row_dot: b'[n] = sum_k W[n][k] * beta[k] (+ bias[n])

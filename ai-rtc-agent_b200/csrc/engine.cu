@@ -10,6 +10,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <functional>
@@ -293,6 +294,30 @@ struct WeightStore {
     std::map<std::string, float*> fvec;      // cache of fp32 vectors
     std::map<std::string, size_t> packed_bytes, fvec_bytes;   // their sizes (b2sd_export_packed)
     std::shared_ptr<struct CondPool> cond_pool;   // made by the first conditioning override of a state of this store
+
+    // ---- live parameters (b2sd_set_live_params / b2sd_apply_lora) ----
+    // How each packed / fp32-vector cache entry derived from raw parameters is rebuilt in place: recorded when it is first
+    // made (in every mode; it is host state only).  `keys` are the raw parameters it reads through src().
+    struct Rebuild {
+        std::vector<std::string> keys;
+        std::function<int(cudaStream_t)> fn;
+    };
+    std::map<std::string, Rebuild> rebuild;
+    std::map<std::string, const __half*> src_override;   // during b2sd_apply_lora: fused matrices the rebuilds read instead
+    const __half* src(const std::string& key) const {
+        auto o = src_override.find(key);
+        if (o != src_override.end()) return o->second;
+        auto it = raw.find(key);
+        return it == raw.end() ? nullptr : it->second.p;
+    }
+    bool live = false;           // keep the base parameters; parameters may be re-fused at run time
+    bool live_ready = false;     // the first prepare has made the base copies below
+    Arena base_arena{256u << 20};
+    std::map<std::string, __half*> base;   // base values of the UNet matrices kernels read raw (their live copy is raw[key].p)
+    std::vector<std::string> fused;        // keys whose live values differ from the base (the last b2sd_apply_lora)
+    void* scratch = nullptr;               // factor operands and fused matrices of b2sd_apply_lora, grown stream-ordered
+    size_t scratch_cap = 0;
+    ~WeightStore() { if (scratch) cudaFree(scratch); }
 };
 
 enum { COND_PROMPT = 0, COND_TIME = 1 };
@@ -476,16 +501,34 @@ struct b2sd_engine {
         return d;
     }
 
+    // A raw parameter a packing kernel is about to read (its fused value while b2sd_apply_lora rebuilds a cache entry)
+    const Raw* pack_source(const std::string& key) {
+        const Raw* r = get(key);
+        if (r && !r->p) {
+            b2_set_error("parameter '%s' was released after the first prepare and is not in the packed cache", key.c_str());
+            return nullptr;
+        }
+        return r;
+    }
+    // Make a cache entry: record how to rebuild it from its raw parameters (b2sd_apply_lora), then build it once
+    int record_rebuild(const std::string& name, std::vector<std::string> keys, std::function<int(cudaStream_t)> fn, cudaStream_t s) {
+        WeightStore::Rebuild& rb = ws->rebuild[name];
+        rb.keys = std::move(keys);
+        rb.fn = std::move(fn);
+        return rb.fn(s);
+    }
+
     // fp32 [cin*9][cout] weights of a tiny-Cin conv (cached)
     const float* small_w(const std::string& key, cudaStream_t s) {
         auto it = fvec.find("sw:" + key);
         if (it != fvec.end()) return it->second;
-        const Raw* r = get(key);
+        const Raw* r = pack_source(key);
         if (!r) return nullptr;
-        if (!r->p) { b2_set_error("parameter '%s' was released after the first prepare and is not in the packed cache", key.c_str()); return nullptr; }
         const int cout = (int)r->shape[0], cin = (int)r->shape[1];
         float* d = static_cast<float*>(weights.alloc((size_t)cin * 9 * cout * sizeof(float)));
-        if (!d || smallconv_prep_launch(r->p, d, cout, cin, s)) return nullptr;
+        WeightStore* w = ws.get();
+        if (!d || record_rebuild("sw:" + key, {key}, [=](cudaStream_t st) { return smallconv_prep_launch(w->src(key), d, cout, cin, st); }, s))
+            return nullptr;
         fvec["sw:" + key] = d;
         fvec_bytes["sw:" + key] = (size_t)cin * 9 * cout * sizeof(float);
         return d;
@@ -503,21 +546,61 @@ struct b2sd_engine {
         const int rows_pad = (rows + 15) / 16 * 16;
         __half* dst = static_cast<__half*>(weights.alloc((size_t)rows_pad * K * 2));
         if (!dst) return nullptr;
-        cudaMemsetAsync(dst, 0, (size_t)rows_pad * K * 2, s);
-        int koff = 0;
+        std::vector<std::string> keys;
+        std::vector<int> cin_total;
         for (auto& g : segs) {
-            const Raw* r = get(g.key);
+            const Raw* r = pack_source(g.key);
             if (!r) return nullptr;
-            if (!r->p) { b2_set_error("parameter '%s' was released after the first prepare and is not in the packed cache", g.key.c_str()); return nullptr; }
-            const int cin_total = (int)r->shape[1];
-            if (pack_conv_weight_launch(r->p, dst, K, koff, rows, cin_total, g.taps, g.c0, g.cn, s)) return nullptr;
-            koff += g.taps * g.cn;
+            keys.push_back(g.key);
+            cin_total.push_back((int)r->shape[1]);
         }
+        WeightStore* w = ws.get();
+        const size_t bytes = (size_t)rows_pad * K * 2;
+        if (record_rebuild(name, keys, [=](cudaStream_t st) {
+                if (cudaMemsetAsync(dst, 0, bytes, st) != cudaSuccess) return -1;
+                int koff = 0;
+                for (size_t i = 0; i < segs.size(); ++i) {
+                    const ConvSeg& g = segs[i];
+                    if (pack_conv_weight_launch(w->src(g.key), dst, K, koff, rows, cin_total[i], g.taps, g.c0, g.cn, st)) return -1;
+                    koff += g.taps * g.cn;
+                }
+                return 0;
+            }, s))
+            return nullptr;
         packed[name] = dst;
-        packed_bytes[name] = (size_t)rows_pad * K * 2;
+        packed_bytes[name] = bytes;
         return dst;
     }
-    // rows gathered from one or more [*, K] matrices: spec = list of (key, perm)
+    // rows gathered from one or more [*, K] matrices: spec = list of (key, perm).  The gathers of an entry, as a rebuild step.
+    std::function<int(cudaStream_t)> gather_fn(const std::vector<std::pair<std::string, std::vector<int>>>& parts, int K,
+                                               __half* dst, size_t bytes, cudaStream_t s) {
+        std::vector<std::pair<std::string, const int*>> dparts;
+        std::vector<int> counts;
+        for (auto& p : parts) {
+            if (!pack_source(p.first)) return nullptr;
+            int* dperm = static_cast<int*>(weights.alloc(p.second.size() * sizeof(int)));
+            if (!dperm) return nullptr;
+            cudaMemcpyAsync(dperm, p.second.data(), p.second.size() * sizeof(int), cudaMemcpyHostToDevice, s);
+            cudaStreamSynchronize(s);  // host vector may die before the copy otherwise
+            dparts.emplace_back(p.first, dperm);
+            counts.push_back((int)p.second.size());
+        }
+        WeightStore* w = ws.get();
+        return [=](cudaStream_t st) {
+            if (cudaMemsetAsync(dst, 0, bytes, st) != cudaSuccess) return -1;
+            size_t r0 = 0;
+            for (size_t i = 0; i < dparts.size(); ++i) {
+                if (gather_rows_launch(w->src(dparts[i].first), K, dparts[i].second, dst + r0 * K, K, counts[i], K, st)) return -1;
+                r0 += counts[i];
+            }
+            return 0;
+        };
+    }
+    static std::vector<std::string> part_keys(const std::vector<std::pair<std::string, std::vector<int>>>& parts) {
+        std::vector<std::string> k;
+        for (auto& p : parts) k.push_back(p.first);
+        return k;
+    }
     __half* pack_rows(const std::string& name, const std::vector<std::pair<std::string, std::vector<int>>>& parts,
                       int K, cudaStream_t s) {
         auto it = packed.find(name);
@@ -527,19 +610,8 @@ struct b2sd_engine {
         const size_t rows_pad = (rows + 15) / 16 * 16;
         __half* dst = static_cast<__half*>(weights.alloc(rows_pad * K * 2));
         if (!dst) return nullptr;
-        cudaMemsetAsync(dst, 0, rows_pad * K * 2, s);
-        size_t r0 = 0;
-        for (auto& p : parts) {
-            const Raw* r = get(p.first);
-            if (!r) return nullptr;
-            if (!r->p) { b2_set_error("parameter '%s' was released after the first prepare and is not in the packed cache", p.first.c_str()); return nullptr; }
-            int* dperm = static_cast<int*>(weights.alloc(p.second.size() * sizeof(int)));
-            if (!dperm) return nullptr;
-            cudaMemcpyAsync(dperm, p.second.data(), p.second.size() * sizeof(int), cudaMemcpyHostToDevice, s);
-            cudaStreamSynchronize(s);  // host vector may die before the copy otherwise
-            if (gather_rows_launch(r->p, K, dperm, dst + r0 * K, K, (int)p.second.size(), K, s)) return nullptr;
-            r0 += p.second.size();
-        }
+        auto gather = gather_fn(parts, K, dst, rows_pad * K * 2, s);
+        if (!gather || record_rebuild(name, part_keys(parts), gather, s)) return nullptr;
         packed[name] = dst;
         packed_bytes[name] = rows_pad * K * 2;
         return dst;
@@ -554,22 +626,28 @@ struct b2sd_engine {
         for (auto& p : parts) rows += p.second.size();
         const size_t rows_pad = (rows + 15) / 16 * 16;
         const bool done = packed.count(name) && fvec.count(name + ":cs") && fvec.count(name + ":b");
-        __half* w = pack_rows(name, parts, K, s);
-        if (!w) return -1;
         if (!done) {
+            // one rebuild step for the three entries: the gathered rows, then the fold on them
+            __half* w = static_cast<__half*>(weights.alloc(rows_pad * K * 2));
+            if (!w) return -1;
+            auto gather = gather_fn(parts, K, w, rows_pad * K * 2, s);
             const float* gamma = vec({ln_prefix + ".weight"});
             const float* beta = vec({ln_prefix + ".bias"});
             float* cs = static_cast<float*>(weights.alloc(rows_pad * sizeof(float)));
             float* bb = static_cast<float*>(weights.alloc(rows_pad * sizeof(float)));
-            if (!gamma || !beta || !cs || !bb) return -1;
-            cudaMemsetAsync(bb, 0, rows_pad * sizeof(float), s);
-            TRY(row_dot_launch(w, (long)rows, K, beta, bias_vec, bb, s));     // on the un-scaled rows
-            TRY(scale_cols_launch(w, (long)rows_pad, K, gamma, s));
-            TRY(row_sum_launch(w, (long)rows_pad, K, cs, s));
+            if (!gather || !gamma || !beta || !cs || !bb) return -1;
+            TRY(record_rebuild(name, part_keys(parts), [=](cudaStream_t st) {
+                TRY(gather(st));
+                if (cudaMemsetAsync(bb, 0, rows_pad * sizeof(float), st) != cudaSuccess) return -1;
+                TRY(row_dot_launch(w, (long)rows, K, beta, bias_vec, bb, st));     // on the un-scaled rows
+                TRY(scale_cols_launch(w, (long)rows_pad, K, gamma, st));
+                return row_sum_launch(w, (long)rows_pad, K, cs, st);
+            }, s));
+            packed[name] = w; packed_bytes[name] = rows_pad * K * 2;
             fvec[name + ":cs"] = cs; fvec_bytes[name + ":cs"] = rows_pad * sizeof(float);
             fvec[name + ":b"] = bb; fvec_bytes[name + ":b"] = rows_pad * sizeof(float);
         }
-        out->w = w;
+        out->w = packed[name];
         out->colsum = fvec[name + ":cs"];
         out->bias = fvec[name + ":b"];
         return 0;
@@ -2104,6 +2182,11 @@ int b2sd_load_tensor(b2sd_handle h, const char* key, const void* ptr, int dtype,
                      "load different parameters (or set B2_KEEP_RAW=1 before the first prepare)", key);
         return -1;
     }
+    if (h->ws->live_ready) {
+        b2_set_error("b2sd_load_tensor(%s): the engine's parameters are live (b2sd_set_live_params) and prepared; change them "
+                     "with b2sd_apply_lora", key);
+        return -1;
+    }
     r.pack_only = is_pack_only(key, shape, ndim);
     auto old = h->raw.find(key);
     if (old != h->raw.end()) {
@@ -2187,6 +2270,31 @@ static int refresh_time(b2sd_handle h, cudaStream_t s) {
     return h->run(h->prog_time, s);
 }
 
+// A UNet matrix a LoRA may re-fuse: a loaded (not derived) parameter without a sub-network prefix, 2-D or 4-D
+static bool lora_target(const std::string& key, const Raw& r) {
+    for (const char* pre : {"vae.", "controlnet.", "hed."})
+        if (key.compare(0, strlen(pre), pre) == 0) return false;
+    return !r.derived && r.shape.size() >= 2;
+}
+
+// Live mode, after the first prepare: the raw copies of the pack-only UNet matrices are kept as their base values (the packed
+// entries are rebuilt from them), and every UNet matrix a kernel reads raw gets a base copy beside it, so that its live copy
+// can be re-fused at the address the frame program holds.
+static int make_live_base(b2sd_handle h) {
+    WeightStore& w = *h->ws;
+    if (w.live_ready) return 0;
+    for (auto& kv : w.raw) {
+        if (kv.second.pack_only || !lora_target(kv.first, kv.second)) continue;
+        const size_t bytes = (size_t)kv.second.numel() * 2;
+        __half* b = static_cast<__half*>(w.base_arena.alloc(bytes));
+        if (!b) return -1;
+        CUDA_OK(cudaMemcpy(b, kv.second.p, bytes, cudaMemcpyDeviceToDevice));
+        w.base[kv.first] = b;
+    }
+    w.live_ready = true;
+    return 0;
+}
+
 int b2sd_prepare(b2sd_handle h, const void* prompt_embeds, const float* timesteps, const float* coef,
                  const void* init_noise, void* stream) {
     if (!h || !prompt_embeds || !timesteps || !coef || !init_noise) {
@@ -2216,7 +2324,14 @@ int b2sd_prepare(b2sd_handle h, const void* prompt_embeds, const float* timestep
     // x_t_latent_buffer = zeros (StreamDiffusion.prepare); slot 0 is overwritten by every frame
     CUDA_OK(cudaMemsetAsync(h->x_in.p, 0, (size_t)h->x_in.elems() * 2, s));
     if (h->pair_state) TRY(state_reset(h->pair_state.get(), s));
+    const size_t rebuilds = h->ws->rebuild.size();
     TRY(h->build_program(s));
+    if (h->ws->rebuild.size() != rebuilds && !h->ws->fused.empty()) {
+        // new packed entries (a lane with another weight layout) were made from the base values, not the fused ones
+        b2_set_error("b2sd_prepare: this engine needs packed weights the store did not have when b2sd_apply_lora ran; prepare "
+                     "every lane before the first b2sd_apply_lora, or apply the LoRAs again");
+        return -1;
+    }
     TRY(h->run(h->prog_prompt, s));
     TRY(refresh_time(h, s));
     CUDA_OK(cudaMemcpyAsync(h->ctx_global, h->ctx, (size_t)h->cfg.ctx_tokens * h->cfg.cross_attention_dim * 2,
@@ -2225,6 +2340,7 @@ int b2sd_prepare(b2sd_handle h, const void* prompt_embeds, const float* timestep
     TRY(keep_global(h, COND_PROMPT, s));
     TRY(keep_global(h, COND_TIME, s));
     CUDA_OK(cudaStreamSynchronize(s));
+    if (h->ws->live) return make_live_base(h);
     // Every pack-only parameter now exists in its kernel-native layout: drop the raw copies (about half of the UNet's
     // 1.73 GB).  Later prepares hit the packed caches and never touch them.
     static const bool keep_raw = getenv("B2_KEEP_RAW") != nullptr;
@@ -2318,6 +2434,11 @@ int b2sd_import_packed(b2sd_handle h, const char* path) {
     }
     if (!h->raw.empty()) {
         b2_set_error("b2sd_import_packed: the engine already holds parameters");
+        return -1;
+    }
+    if (h->ws->live) {
+        b2_set_error("b2sd_import_packed: the engine's parameters are live (b2sd_set_live_params): a blob does not carry the "
+                     "base parameters they are re-fused from; load them with b2sd_load_tensor");
         return -1;
     }
     FILE* f = fopen(path, "rb");
@@ -2419,6 +2540,171 @@ int b2sd_set_timesteps(b2sd_handle h, const float* timesteps, void* stream) {
     CUDA_OK(cudaMemcpyAsync(h->tsteps_global, h->tsteps, h->cfg.batch * sizeof(float), cudaMemcpyDeviceToDevice, s));
     h->cond[COND_TIME].held = COND_UNKNOWN;
     TRY(refresh_time(h, s));
+    return keep_global(h, COND_TIME, s);
+}
+
+// ---- live parameters ------------------------------------------------------------------------------------------------------
+int b2sd_set_live_params(b2sd_handle h, int on) {
+    if (!h) {
+        b2_set_error("b2sd_set_live_params: null handle");
+        return -1;
+    }
+    WeightStore& w = *h->ws;
+    if (w.raw_released || w.imported || w.live_ready) {
+        b2_set_error("b2sd_set_live_params: call it before the first b2sd_prepare of the weight store, on parameters loaded with "
+                     "b2sd_load_tensor");
+        return -1;
+    }
+    w.live = on != 0;
+    return 0;
+}
+
+static size_t align256(size_t b) { return (b + 255) & ~size_t(255); }
+
+int b2sd_apply_lora(b2sd_handle h, int n, const b2sd_lora_factor* f, void* stream) {
+    if (!h || n < 0 || (n > 0 && !f)) {
+        b2_set_error("b2sd_apply_lora: bad argument");
+        return -1;
+    }
+    WeightStore& w = *h->ws;
+    if (!w.live || !w.live_ready) {
+        b2_set_error("b2sd_apply_lora: the weight store is not live (b2sd_set_live_params before the first b2sd_prepare)");
+        return -1;
+    }
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    // ---- validate everything before the first device operation
+    struct Job { Raw* r = nullptr; long rows = 0, cols = 0; std::vector<const b2sd_lora_factor*> fs; };
+    std::map<std::string, Job> jobs;
+    size_t a_bytes = 0, b_bytes = 0, tmp_bytes = 0;
+    for (int i = 0; i < n; ++i) {
+        const b2sd_lora_factor& fc = f[i];
+        auto it = fc.key ? w.raw.find(fc.key) : w.raw.end();
+        if (it == w.raw.end() || !lora_target(it->first, it->second)) {
+            b2_set_error("b2sd_apply_lora: factor %d: '%s' is not a UNet weight matrix of this engine", i, fc.key ? fc.key : "(null)");
+            return -1;
+        }
+        if (!fc.up || !fc.down || fc.rank < 1 || fc.rank > 4096 || (fc.dtype != 0 && fc.dtype != 1) || !isfinite(fc.scale)) {
+            b2_set_error("b2sd_apply_lora: factor %d (%s): null factor, rank %d outside 1..4096, dtype %d or a non-finite scale", i,
+                         fc.key, fc.rank, fc.dtype);
+            return -1;
+        }
+        Job& j = jobs[it->first];
+        j.r = &it->second;
+        j.rows = it->second.shape[0];
+        j.cols = it->second.numel() / j.rows;
+        j.fs.push_back(&fc);
+        const size_t kp = (size_t)((fc.dtype ? 3 : 1) * fc.rank + IG_BK - 1) / IG_BK * IG_BK;
+        a_bytes = std::max(a_bytes, align256(j.rows * kp * 2));
+        b_bytes = std::max(b_bytes, align256(j.cols * kp * 2));
+        tmp_bytes = std::max(tmp_bytes, align256((size_t)j.rows * j.cols * 2));
+    }
+    // the keys that change: listed ones, and those the previous call fused that now revert to their base
+    std::map<std::string, bool> touched;   // key -> listed
+    for (auto& kv : jobs) touched[kv.first] = true;
+    for (auto& k : w.fused) touched.emplace(k, false);
+    // packed entries to rebuild, and the fused matrices each needs at once
+    std::vector<WeightStore::Rebuild*> entries;
+    size_t slot_bytes = 0;
+    for (auto& kv : w.rebuild) {
+        size_t need = 0;
+        bool hit = false;
+        for (auto& k : kv.second.keys) {
+            auto t = touched.find(k);
+            if (t == touched.end()) continue;
+            hit = true;
+            if (t->second) need += align256((size_t)jobs[k].rows * jobs[k].cols * 2);
+        }
+        if (hit) entries.push_back(&kv.second);
+        slot_bytes = std::max(slot_bytes, need);
+    }
+    // ---- scratch: [up operand | down operand | two chain buffers | fused matrices of one entry]
+    const size_t need = a_bytes + b_bytes + 2 * tmp_bytes + slot_bytes;
+    if (need > w.scratch_cap) {
+        if (w.scratch) CUDA_OK(cudaFreeAsync(w.scratch, s));
+        w.scratch = nullptr;
+        w.scratch_cap = 0;
+        CUDA_OK(cudaMallocAsync(&w.scratch, need, s));
+        w.scratch_cap = need;
+    }
+    char* sp = static_cast<char*>(w.scratch);
+    __half* opa = reinterpret_cast<__half*>(sp);
+    __half* opb = reinterpret_cast<__half*>(sp + a_bytes);
+    __half* tmp[2] = {reinterpret_cast<__half*>(sp + a_bytes + b_bytes), reinterpret_cast<__half*>(sp + a_bytes + b_bytes + tmp_bytes)};
+    char* slots = sp + a_bytes + b_bytes + 2 * tmp_bytes;
+    // from here on a failure leaves any touched key possibly fused: the next call restores all of them
+    std::vector<std::string> now;
+    for (auto& kv : touched) now.push_back(kv.first);
+    w.fused = now;
+
+    // out = base + sum of the key's deltas in order, rounded to fp16 after each: one igemm per factor, M = rows, N = cols,
+    // K = rank (three parts for fp32 factors) zero-padded to the K block, epilogue scale * acc + residual
+    auto fuse = [&](const Job& j, const __half* base, __half* out) -> int {
+        const __half* prev = base;
+        for (size_t i = 0; i < j.fs.size(); ++i) {
+            const b2sd_lora_factor& fc = *j.fs[i];
+            __half* dst = i + 1 == j.fs.size() ? out : tmp[i & 1];
+            const int kp = ((fc.dtype ? 3 : 1) * fc.rank + IG_BK - 1) / IG_BK * IG_BK;
+            TRY(lora_factor_launch(fc.up, fc.dtype, j.rows, fc.rank, fc.rank, 1, 2, opa, kp, s));     // up[r][k]
+            TRY(lora_factor_launch(fc.down, fc.dtype, j.cols, fc.rank, 1, j.cols, 4, opb, kp, s));    // down[k][c], transposed
+            IgemmDesc d{};
+            d.nseg = 1; d.src[0] = ActView{opa, 1, 1, (int)j.rows, kp, kp}; d.ntap[0] = 1;
+            d.w = opb; d.w_rows = (int)j.cols; d.w_ld = kp; d.stride = 1;
+            d.Nb = 1; d.Ho = 1; d.Wo = (int)j.rows;
+            d.epi.out = dst; d.epi.ldc = (int)j.cols;
+            d.epi.res = prev; d.epi.ldr = (int)j.cols;
+            d.epi.acc_scale = fc.scale; d.epi.res_scale = 1.f;
+            d.epi.n_valid = (int)j.cols;
+            IgemmPlan plan;
+            TRY(igemm_plan(d, &plan));
+            TRY(igemm_launch(plan, s));
+            prev = dst;
+        }
+        return 0;
+    };
+    // matrices the kernels read raw: fused in place (the frame program holds their address), or copied back from the base
+    for (auto& kv : touched) {
+        Raw& r = w.raw[kv.first];
+        if (r.pack_only) continue;
+        __half* base = w.base[kv.first];
+        if (kv.second) TRY(fuse(jobs[kv.first], base, r.p));
+        else CUDA_OK(cudaMemcpyAsync(r.p, base, (size_t)r.numel() * 2, cudaMemcpyDeviceToDevice, s));
+    }
+    // packed entries: rebuilt in place from the fused matrices of their listed keys and the base of the others
+    for (WeightStore::Rebuild* e : entries) {
+        size_t off = 0;
+        w.src_override.clear();
+        for (auto& k : e->keys) {
+            auto t = touched.find(k);
+            if (t == touched.end() || !t->second || w.src_override.count(k)) continue;
+            __half* out = reinterpret_cast<__half*>(slots + off);
+            off += align256((size_t)jobs[k].rows * jobs[k].cols * 2);
+            TRY(fuse(jobs[k], w.raw[k].p, out));
+            w.src_override[k] = out;
+        }
+        const int rc = e->fn(s);
+        w.src_override.clear();
+        TRY(rc);
+    }
+    now.clear();
+    for (auto& kv : jobs) now.push_back(kv.first);
+    w.fused = now;
+    return 0;
+}
+
+int b2sd_refresh_conditioning(b2sd_handle h, void* stream) {
+    if (!h || !h->built) {
+        b2_set_error("b2sd_refresh_conditioning: call b2sd_prepare first");
+        return -1;
+    }
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    CUDA_OK(cudaMemcpyAsync(h->ctx, h->ctx_global, (size_t)h->cfg.ctx_tokens * h->cfg.cross_attention_dim * 2,
+                            cudaMemcpyDeviceToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(h->tsteps, h->tsteps_global, h->cfg.batch * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    h->cond[COND_PROMPT].held = COND_UNKNOWN;
+    h->cond[COND_TIME].held = COND_UNKNOWN;
+    TRY(h->run(h->prog_prompt, s));
+    TRY(refresh_time(h, s));
+    TRY(keep_global(h, COND_PROMPT, s));
     return keep_global(h, COND_TIME, s);
 }
 

@@ -152,6 +152,12 @@ class EngineConfig(C.Structure):
     ]
 
 
+class LoraFactor(C.Structure):
+    """b2sd_lora_factor: delta = scale * up @ down on one UNet parameter (factors in device memory)"""
+    _fields_ = [("key", C.c_char_p), ("up", C.c_void_p), ("down", C.c_void_p), ("rank", C.c_int), ("dtype", C.c_int),
+                ("scale", C.c_float)]
+
+
 IN_U8_NHWC, IN_F32_NCHW, IN_F16_NCHW = 0, 1, 2
 OUT_U8_NCHW, OUT_F16_NCHW = 0, 1
 IG_RELU = 1
@@ -230,6 +236,11 @@ def lib() -> C.CDLL:
         _lib.b2sd_state_clear_conditioning.argtypes = [vp, ci]
         for name in ("state_create", "state_reset", "state_destroy", "step_state", "state_set_prompt_embeds", "state_set_timesteps",
                      "state_clear_conditioning"):
+            getattr(_lib, "b2sd_" + name).restype = C.c_int
+        _lib.b2sd_set_live_params.argtypes = [vp, ci]
+        _lib.b2sd_apply_lora.argtypes = [vp, ci, C.POINTER(LoraFactor), vp]
+        _lib.b2sd_refresh_conditioning.argtypes = [vp, vp]
+        for name in ("set_live_params", "apply_lora", "refresh_conditioning"):
             getattr(_lib, "b2sd_" + name).restype = C.c_int
         _lib.b2sd_conditioning_binds.argtypes = [vp]
         _lib.b2sd_conditioning_binds.restype = i64

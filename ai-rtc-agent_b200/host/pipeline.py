@@ -14,12 +14,12 @@ separately with the reference's tensor contracts."""
 from __future__ import annotations
 
 import os
-from typing import List, Optional
+from typing import Dict, List, Optional
 
 import numpy as np
 import torch
 
-from .wrapper import StreamDiffusionWrapper
+from .wrapper import LIVE_LORA_ENV, StreamDiffusionWrapper
 
 DEFAULT_PROMPT = "fireworks in the night sky"
 DEFAULT_T_INDEX_LIST = [18, 26, 35, 45]
@@ -73,7 +73,8 @@ class StreamDiffusionPipeline:
     _own_state = None   # the StreamState enqueue() steps with per-peer streams; None: the engines' own shared state
 
     def __init__(self, model_id: str, t_index_list: Optional[List[int]] = None, width: int = 512, height: int = 512,
-                 prompt: str = DEFAULT_PROMPT, lanes: Optional[int] = None, per_peer_streams: Optional[bool] = None):
+                 prompt: str = DEFAULT_PROMPT, lanes: Optional[int] = None, per_peer_streams: Optional[bool] = None,
+                 live_lora: Optional[bool] = None):
         """lanes: frames in flight for enqueue() ($B200SD_LANES overrides the default).  With a 1-step stream batch (SD-Turbo)
         consecutive frames are independent: DEFAULT_LANES_ONE_STEP lanes process frame n+1.. while frame n is still on the GPU.
         With T > 1 the stream batch carries state from frame to frame: two lanes share that state and are stage-pipelined (TAESD
@@ -84,14 +85,21 @@ class StreamDiffusionPipeline:
         temporal stream.  open_stream() gives a viewer a PeerStream whose frames carry that viewer's stream-batch state only;
         pipeline(frame) / enqueue(frame) keep stepping the pipeline's own stream.  The lanes are then independent
         (DEFAULT_LANES_PER_PEER for T > 1) and any lane steps any viewer's state.  Off, every caller of the pipeline shares one
-        temporal stream, as in the reference: with T > 1 a frame's output then mixes in frames of the other callers."""
+        temporal stream, as in the reference: with T > 1 a frame's output then mixes in frames of the other callers.
+
+        live_lora (None: $B200SD_LIVE_LORA, default off): update_lora() switches style LoRAs while the pipeline runs.  The base
+        weights stay on the device (more HBM, see README), and the packed-weight blob is neither read nor written."""
         if per_peer_streams is None:
             per_peer_streams = env_flag(PER_PEER_STREAMS_ENV)
         self.per_peer_streams = bool(per_peer_streams)
         self.prompt = prompt
         self.t_index_list = list(t_index_list) if t_index_list is not None else DEFAULT_T_INDEX_LIST
         self.device = "cuda"
-        self.model = StreamDiffusionWrapper(
+        if live_lora is None:
+            live_lora = env_flag(LIVE_LORA_ENV)
+        self.model = StreamDiffusionWrapper.__new__(StreamDiffusionWrapper)
+        self.model.live_lora = bool(live_lora)
+        self.model.__init__(
             model_id_or_path=model_id,
             device=self.device,
             dtype=torch.float16,
@@ -163,6 +171,19 @@ class StreamDiffusionPipeline:
         cur = self._quiesce()
         self.model.stream.update_prompt(prompt)
         self._release(cur)
+
+    def update_lora(self, lora_dict: Optional[Dict[str, float]]):
+        """The style LoRAs ({safetensors path: scale}, the wrapper's lora_dict form; None or {}: none) of every stream: the
+        pipeline's own and every open peer stream, each keeping its own prompt / t_index_list.  Frames enqueued before the
+        call use the old weights and frames enqueued after it the new ones.  Needs live_lora=True; errors are raised before
+        anything changes."""
+        if not self.model.live_lora:
+            raise RuntimeError("update_lora needs StreamDiffusionPipeline(live_lora=True) (or $B200SD_LIVE_LORA=1)")
+        cur = self._quiesce()
+        try:
+            self.model.update_lora(lora_dict)
+        finally:
+            self._release(cur)
 
     def update_t_index_list(self, t_index_list: List[int]):
         """The global t_index_list: every stream's, including open peer streams with one of their own."""

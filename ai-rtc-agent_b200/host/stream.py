@@ -8,6 +8,7 @@ frame_buffer_size=1, cfg_type "self"/"none" with guidance_scale <= 1.0 (no CFG a
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 import weakref
 from typing import Callable, Dict, List, Optional
@@ -78,12 +79,16 @@ class StreamDiffusion:
                  packed_blob: Optional[str] = None, parent: Optional["StreamDiffusion"] = None,
                  controlnet_sd: Optional[Dict[str, torch.Tensor]] = None,
                  hed_sd: Optional[Dict[str, torch.Tensor]] = None, use_tiny_vae: bool = True,
-                 vae_scaling_factor: float = 0.18215):
+                 vae_scaling_factor: float = 0.18215, live_lora: bool = False):
         """vae_sd: TAESD (use_tiny_vae=True) or the model's own AutoencoderKL (use_tiny_vae=False: latents = vae_scaling_factor
         times the mean of the encoder's distribution, decoded from x0 / vae_scaling_factor).
         controlnet_sd: a diffusers ControlNetModel state dict (empty when the weights come from packed_blob); every
         stream-batch slot is then conditioned on the current frame's control image: the frame itself, or with hed_sd (a
-        ControlNetHED.pth state dict, empty with packed_blob) its HED edge map.  Lanes inherit their parent's ControlNet."""
+        ControlNetHED.pth state dict, empty with packed_blob) its HED edge map.  Lanes inherit their parent's ControlNet.
+        live_lora: keep the base UNet weights on the device so that apply_lora() can switch LoRAs at run time (not with
+        packed_blob; lanes inherit it)."""
+        if live_lora and packed_blob is not None:
+            raise ValueError("live_lora needs the weights themselves: a packed blob does not carry the base weights")
         if hed_sd is not None and controlnet_sd is None:
             raise ValueError("the HED processor needs a ControlNet")
         if frame_buffer_size != 1:
@@ -141,7 +146,8 @@ class StreamDiffusion:
         self._ctor = dict(torch_dtype=torch_dtype, width=width, height=height, do_add_noise=do_add_noise,
                           use_denoising_batch=use_denoising_batch, frame_buffer_size=frame_buffer_size, cfg_type=cfg_type,
                           device=device, use_cuda_graph=use_cuda_graph, use_tiny_vae=use_tiny_vae,
-                          vae_scaling_factor=vae_scaling_factor)
+                          vae_scaling_factor=vae_scaling_factor, live_lora=live_lora)
+        self.live_lora = bool(live_lora)
         # extra engines over this one's weights (add_lane).  A lane keeps no reference to its parent: an engine and its lanes then
         # form no reference cycle, so their device memory is released as soon as the last reference goes, not at the next
         # run of the garbage collector
@@ -152,6 +158,9 @@ class StreamDiffusion:
             capi.check(self._lib.b2sd_create_lane(parent._handle, C.byref(cfg), C.byref(self._handle)), "b2sd_create_lane")
             return
         capi.check(self._lib.b2sd_create(C.byref(cfg), C.byref(self._handle)), "b2sd_create")
+        if live_lora:
+            capi.check(self._lib.b2sd_set_live_params(self._handle, 1), "b2sd_set_live_params")
+            self._unet_shapes = {k: tuple(v.shape) for k, v in unet_sd.items()}
         if packed_blob is not None:
             # kernel-native weights written by export_packed() / `python -m ai_rtc_agent_b200.pack`: no state dicts, no repacking
             capi.check(self._lib.b2sd_import_packed(self._handle, os.fsencode(packed_blob)), f"b2sd_import_packed({packed_blob})")
@@ -336,6 +345,39 @@ class StreamDiffusion:
             if not state.closed:
                 state.clear_overrides(prompt=prompt, t_index_list=t_index_list)
 
+    @torch.no_grad()
+    def apply_lora(self, lora_dict: Optional[Dict[str, float]]) -> None:
+        """Switch the style LoRAs (live_lora engines): from now on the UNet computes with the base weights plus the LoRAs of
+        lora_dict ({safetensors path: scale}, fused in order, as the constructor's lora_dict would have; None / {}: the base).
+        The files are read and every pair checked before anything changes on the device.  The weights are re-fused on the
+        device on the current CUDA stream, then the conditioning of this engine, its lanes and every live state (its own prompt
+        / t_index_list included) is recomputed with them; the caller orders the stream after the frames in flight and before
+        later ones.  No host synchronisation besides the upload of the factors and the prompt encoder's own."""
+        from .weights import lora_factors
+        if not self.live_lora:
+            raise RuntimeError("apply_lora needs an engine built with live_lora=True (StreamDiffusionPipeline(live_lora=True) or "
+                               "$B200SD_LIVE_LORA=1)")
+        self._check()
+        factors = lora_factors(self._unet_shapes, lora_dict)
+        keep = []   # the device factors stay referenced until the call has enqueued the work that reads them
+        arr = (capi.LoraFactor * max(1, len(factors)))()
+        for i, (key, up, down, scale) in enumerate(factors):
+            up, down, scale = _factor_operands(up, down, scale)
+            up, down = _on_device(up, self.device), _on_device(down, self.device)
+            keep += [up, down]
+            arr[i] = capi.LoraFactor(key.encode(), up.data_ptr(), down.data_ptr(), up.shape[1],
+                                     0 if up.dtype == torch.float16 else 1, scale)
+        capi.check(self._lib.b2sd_apply_lora(self._handle, len(factors), arr, self._stream()), "b2sd_apply_lora")
+        for eng in [self] + self.lanes:
+            capi.check(self._lib.b2sd_refresh_conditioning(eng._handle, self._stream()), "b2sd_refresh_conditioning")
+        for state in list(self._states):
+            if state.closed:
+                continue
+            if state.own_prompt is not None:
+                state.set_prompt(state.own_prompt, engine=self)
+            if state.own_t_index_list is not None:
+                state.set_t_index_list(state.own_t_index_list, engine=self)
+
     def conditioning_binds(self) -> int:
         """How many conditioning block copies this engine's steps have issued (b2sd_conditioning_binds).  Test aid."""
         return self._lib.b2sd_conditioning_binds(self._handle)
@@ -514,6 +556,24 @@ def _on_device(t: torch.Tensor, device: torch.device) -> torch.Tensor:
     if t.is_cuda:
         return t.to(device).contiguous()
     return t.contiguous().pin_memory().to(device, non_blocking=True)
+
+
+def _factor_operands(up: torch.Tensor, down: torch.Tensor, scale: float):
+    """A LoRA pair as the engine takes it: two fp16 factors as they are (exact operands), anything else as fp32 with each
+    factor scaled by a power of two to a largest magnitude in [1, 2) and `scale` compensated (exact), so that the engine's
+    fp16 hi / lo split of the factors keeps their small elements."""
+    if up.dtype == torch.float16 and down.dtype == torch.float16:
+        return up.contiguous(), down.contiguous(), float(scale)
+    out = []
+    for t in (up, down):
+        t = t.float().contiguous()
+        amax = float(t.abs().max()) if t.numel() else 0.0
+        if amax > 0 and math.isfinite(amax):
+            e = math.frexp(amax)[1] - 1        # amax in [2^e, 2^(e+1))
+            t = t * 2.0 ** -e
+            scale = scale * 2.0 ** e
+        out.append(t)
+    return out[0], out[1], float(scale)
 
 
 def _encode_beside(eng: StreamDiffusion, prompt: str) -> torch.Tensor:

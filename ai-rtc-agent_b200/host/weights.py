@@ -5,8 +5,9 @@ from __future__ import annotations
 
 import glob
 import logging
+import math
 import os
-from typing import Dict, Optional, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
@@ -139,11 +140,12 @@ def resolve_hed(synthetic_ok: bool) -> Dict[str, torch.Tensor]:
                             "synthetic weights")
 
 
-def fuse_lora(unet_sd: Dict[str, torch.Tensor], lora_sd: Dict[str, torch.Tensor], scale: float = 1.0, strict: bool = True) -> int:
-    """W += scale * (alpha / rank) * up @ down for every UNet module the LoRA names (diffusers/peft key styles
-    `...to_q.lora_A.weight` / `lora.down.weight`, and kohya `lora_unet_*`).  Returns the number of fused layers.
-    This is the weight-prep step the reference performs with pipe.fuse_lora() before building engines.  strict (default):
-    every UNet LoRA pair must land on a parameter, otherwise KeyError."""
+def resolve_lora(unet_keys, lora_sd: Dict[str, torch.Tensor], strict: bool = True
+                 ) -> List[Tuple[str, torch.Tensor, torch.Tensor, float, int]]:
+    """The UNet parameters a LoRA state dict names: [(parameter key, up, down, alpha, rank)] in the state dict's order, for the
+    diffusers/peft key styles `...to_q.lora_A.weight` / `lora.down.weight` and kohya `lora_unet_*` + `.alpha` (LoCon 3x3
+    downs included).  unet_keys: the UNet's parameter names.  strict (default): every UNet LoRA pair must land on a parameter,
+    and at least one must, otherwise KeyError; text-encoder pairs are skipped."""
     pairs: Dict[str, Dict[str, torch.Tensor]] = {}
     for k, v in lora_sd.items():
         base = None
@@ -161,8 +163,10 @@ def fuse_lora(unet_sd: Dict[str, torch.Tensor], lora_sd: Dict[str, torch.Tensor]
                 pairs.setdefault(k[: -len(".alpha")], {})["alpha"] = v
             continue
         pairs.setdefault(base, {})[role] = v
-    index = {k[: -len(".weight")].replace(".", "_"): k for k in unet_sd if k.endswith(".weight")}
-    fused = 0
+    keys = list(unet_keys)
+    index = {k[: -len(".weight")].replace(".", "_"): k for k in keys if k.endswith(".weight")}
+    keys = set(keys)
+    found = []
     unmatched = []
     for base, d in pairs.items():
         if "up" not in d or "down" not in d:
@@ -172,22 +176,63 @@ def fuse_lora(unet_sd: Dict[str, torch.Tensor], lora_sd: Dict[str, torch.Tensor]
             if name.startswith(prefix):
                 name = name[len(prefix):]
         name = name.replace(".processor", "").replace("to_out_lora", "to_out.0").replace("_lora", "")
-        key = name + ".weight" if (name + ".weight") in unet_sd else index.get(name.replace(".", "_"))
+        key = name + ".weight" if (name + ".weight") in keys else index.get(name.replace(".", "_"))
         if key is None:
             if not base.startswith(("lora_te_", "text_encoder.", "lora_te1_", "lora_te2_")):   # text-encoder LoRA: not on this path
                 unmatched.append(base)
             continue
-        up, down = d["up"].float(), d["down"].float()
-        rank = down.shape[0]
+        rank = d["down"].shape[0]
         alpha = float(d["alpha"]) if "alpha" in d else float(rank)
-        delta = (up.flatten(1) @ down.flatten(1)) * (scale * alpha / rank)
+        found.append((key, d["up"], d["down"], alpha, rank))
+    if strict and (not found or unmatched):
+        # a LoRA that silently does not apply leaves e.g. SD-1.5 un-distilled while it is run at 4 steps
+        raise KeyError(f"LoRA fusing matched {len(found)} of {len(found) + len(unmatched)} UNet modules; unmatched (first 5): "
+                       f"{unmatched[:5]}")
+    return found
+
+
+def fuse_lora(unet_sd: Dict[str, torch.Tensor], lora_sd: Dict[str, torch.Tensor], scale: float = 1.0, strict: bool = True) -> int:
+    """W += scale * (alpha / rank) * up @ down for every UNet module the LoRA names (resolve_lora's key styles).  Returns the
+    number of fused layers.  This is the weight-prep step the reference performs with pipe.fuse_lora() before building
+    engines.  strict (default): every UNet LoRA pair must land on a parameter, otherwise KeyError."""
+    found = resolve_lora(unet_sd.keys(), lora_sd, strict)
+    for key, up, down, alpha, rank in found:
+        delta = (up.float().flatten(1) @ down.float().flatten(1)) * (scale * alpha / rank)
         w = unet_sd[key]
         unet_sd[key] = (w.float() + delta.reshape(w.shape)).to(w.dtype)
-        fused += 1
-    if strict and (fused == 0 or unmatched):
-        # a LoRA that silently does not apply leaves e.g. SD-1.5 un-distilled while it is run at 4 steps
-        raise KeyError(f"LoRA fusing matched {fused} of {fused + len(unmatched)} UNet modules; unmatched (first 5): {unmatched[:5]}")
-    return fused
+    return len(found)
+
+
+def load_lora_file(path: str) -> Dict[str, torch.Tensor]:
+    """A LoRA file's state dict.  Only safetensors are read (never a pickle, which can run code): anything else is a
+    ValueError."""
+    if not str(path).endswith(".safetensors"):
+        raise ValueError(f"LoRA {path}: only .safetensors files are read")
+    try:
+        return _load_safetensors(path)
+    except FileNotFoundError:
+        raise
+    except Exception as exc:   # noqa: BLE001 - safetensors raises its own error type on a file that is not safetensors
+        raise ValueError(f"LoRA {path}: not a safetensors file ({exc})") from exc
+
+
+def lora_factors(unet_shapes: Dict[str, Tuple[int, ...]], lora_dict: Optional[Dict[str, float]]
+                 ) -> List[Tuple[str, torch.Tensor, torch.Tensor, float]]:
+    """What fusing `lora_dict` ({path: scale}, in order) on the base weights means, as factors for the engine's live re-fusing:
+    [(parameter key, up [rows][rank], down [rank][cols], scale * alpha / rank)] with cols = the product of the parameter's
+    other dimensions.  Reads every file and checks every pair (resolve_lora's strict rule, and each pair's shape against its
+    parameter) before returning, so an error leaves nothing half applied."""
+    out = []
+    for path, scale in (lora_dict or {}).items():
+        for key, up, down, alpha, rank in resolve_lora(unet_shapes.keys(), load_lora_file(path)):
+            shape = tuple(unet_shapes[key])
+            rows, cols = shape[0], math.prod(shape[1:])
+            up2, down2 = up.flatten(1), down.flatten(1)
+            if up2.shape[0] != rows or down2.shape[1] != cols or up2.shape[1] != down2.shape[0]:
+                raise ValueError(f"LoRA {path}: the pair on {key} has up {tuple(up.shape)} / down {tuple(down.shape)}, which do not "
+                                 f"fit the parameter's shape {shape}")
+            out.append((key, up2, down2, scale * alpha / rank))
+    return out
 
 
 def layout_variant(batch: int, height: int, width: int) -> str:

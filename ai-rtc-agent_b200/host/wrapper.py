@@ -49,7 +49,15 @@ def postprocess_image(image: torch.Tensor, output_type: str = "pil"):
     raise ValueError(f"unknown output_type {output_type}")
 
 
+LIVE_LORA_ENV = "B200SD_LIVE_LORA"
+
+
 class StreamDiffusionWrapper:
+    # Live LoRA mode (update_lora): None reads $B200SD_LIVE_LORA.  An attribute, not a constructor keyword, so that the
+    # constructor keeps the reference's signature; StreamDiffusionPipeline(live_lora=...) sets it on the instance before
+    # __init__ runs.
+    live_lora: Optional[bool] = None
+
     def __init__(
         self,
         model_id_or_path: str,
@@ -127,6 +135,11 @@ class StreamDiffusionWrapper:
         self.engine_dir = engine_dir
         self.packed_blob = None
         self._blob_to_write = None
+        if self.live_lora is None:
+            from .pipeline import env_flag
+            self.live_lora = env_flag(LIVE_LORA_ENV)
+        self.live_lora = bool(self.live_lora)
+        self._pending_lora = lora_dict if self.live_lora else None   # live mode: applied on the device by the first prepare()
         self.cuda_stream = CudaStreamPtr(cuda_stream_handle) if cuda_stream_handle is not None else None
         self._ext_stream = (torch.cuda.ExternalStream(cuda_stream_handle) if cuda_stream_handle is not None else None)
 
@@ -140,7 +153,9 @@ class StreamDiffusionWrapper:
                     use_lcm_lora, cfg_type, controlnet_id_or_path=None, controlnet_processor_id=None) -> StreamDiffusion:
         """Like the reference (lib/wrapper.py:583-615): first try the cached artefact under `engine_dir` -- there TensorRT engine
         files, here the packed-weight blob -- and on any failure fall through to the full path (load weights, fuse LoRAs),
-        after which the blob is written for the next start (lib/wrapper.py:889-910 moves the engines into the cache)."""
+        after which the blob is written for the next start (lib/wrapper.py:889-910 moves the engines into the cache).
+        Live LoRA mode neither reads nor writes the blob (it does not carry the base weights): the weights are loaded without
+        lora_dict, which the first prepare() then fuses on the device."""
         import os
         from . import arch as A
         from . import weights as W
@@ -162,7 +177,7 @@ class StreamDiffusionWrapper:
         # blobs are kept for real checkpoints; seeded synthetic weights (benchmarks, tests) only with B200SD_PACK_CACHE=synthetic
         mode = os.getenv("B200SD_PACK_CACHE", "1")
         use_cache = self.engine_dir is not None and mode != "0" and model_id_or_path not in W._PRELOADED and \
-            (have_ckpt or mode == "synthetic")
+            (have_ckpt or mode == "synthetic") and not self.live_lora
         if use_cache:
             blob = W.packed_blob_path(self.engine_dir, model_id_or_path, arch.name, use_lcm_lora and not self.sd_turbo, lcm_lora_id,
                                       lora_dict, vae_id, synthetic=not have_ckpt,
@@ -179,12 +194,13 @@ class StreamDiffusionWrapper:
                 return sd
             except Exception as exc:   # noqa: BLE001 - same policy as lib/wrapper.py:611-615
                 logger.warning("packed-weight blob %s unusable (%s); rebuilding from the checkpoint", blob, exc)
-        arch, unet_sd, vae_sd, repo = resolve_weights(model_id_or_path, vae_id, lcm_lora_id, use_lcm_lora, lora_dict,
-                                                      self.sd_turbo, use_tiny_vae=tiny_vae)
+        arch, unet_sd, vae_sd, repo = resolve_weights(model_id_or_path, vae_id, lcm_lora_id, use_lcm_lora,
+                                                      None if self.live_lora else lora_dict, self.sd_turbo, use_tiny_vae=tiny_vae)
         cn_sd = W.resolve_controlnet(controlnet_id_or_path, arch, synthetic_ok) if cn else None
         hed_sd = W.resolve_hed(synthetic_ok) if hed else None
         self._blob_to_write = blob
-        return StreamDiffusion(arch, unet_sd, vae_sd, t_index_list, encoder, controlnet_sd=cn_sd, hed_sd=hed_sd, **kw)
+        return StreamDiffusion(arch, unet_sd, vae_sd, t_index_list, encoder, controlnet_sd=cn_sd, hed_sd=hed_sd,
+                               live_lora=self.live_lora, **kw)
 
     def _on_stream(self):
         return torch.cuda.stream(self._ext_stream) if self._ext_stream is not None else _NullCtx()
@@ -199,6 +215,9 @@ class StreamDiffusionWrapper:
         with self._on_stream():
             self.stream.prepare(prompt, negative_prompt, num_inference_steps=num_inference_steps,
                                 guidance_scale=guidance_scale, delta=delta)
+            if self._pending_lora:
+                self.stream.apply_lora(self._pending_lora)
+            self._pending_lora = None
         if self._blob_to_write is not None:
             # first start from a checkpoint: leave the packed blob behind (the reference moves its freshly built engines into
             # the cache directory, lib/wrapper.py:889-910); failures only cost the next start its speed-up
@@ -241,6 +260,18 @@ class StreamDiffusionWrapper:
     def postprocess_image(self, image_tensor: torch.Tensor, output_type: str = "pil"):
         out = postprocess_image(image_tensor, output_type=output_type)
         return out if self.frame_buffer_size > 1 else out[0]
+
+    def update_lora(self, lora_dict: Optional[Dict[str, float]]) -> None:
+        """Switch the style LoRAs of a live-LoRA wrapper ($B200SD_LIVE_LORA=1, or StreamDiffusionPipeline(live_lora=True)):
+        frames computed after the call use the checkpoint (with the LCM-LoRA, as at construction) plus the LoRAs of lora_dict
+        ({safetensors path: scale}, the constructor's form, fused in order); None or {} returns to the base weights.  Errors
+        (a file that is not safetensors, a pair that does not fit its parameter, a LoRA that matches no UNet module) are
+        raised before anything changes.  See StreamDiffusion.apply_lora for the stream ordering."""
+        if not self.live_lora:
+            raise RuntimeError("update_lora needs live LoRA mode, chosen at construction: $B200SD_LIVE_LORA=1 or "
+                               "StreamDiffusionPipeline(live_lora=True)")
+        with self._on_stream():
+            self.stream.apply_lora(lora_dict)
 
     def update_t_index_list(self, t_index_list: List[int]) -> None:
         """lib/wrapper.py:389-407: swaps the sub-timesteps only."""

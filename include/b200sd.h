@@ -229,8 +229,39 @@ int b2sd_create_lane(b2sd_handle parent, const b2sd_config* cfg, b2sd_handle* ou
  * ("controlnet.controlnet_cond_embedding.conv_in.weight").  ptr may be host or device memory.
  * dtype: 0 = fp16, 1 = fp32.  Replaces the ONNX export + TensorRT build of lib/wrapper.py:785-910.
  * After the first b2sd_prepare the raw copies of parameters that only feed the packing kernels are released (set
- * B2_KEEP_RAW=1 to keep them); loading further tensors into such an engine is an error. */
+ * B2_KEEP_RAW=1 to keep them); loading further tensors into such an engine is an error.  So is loading into a prepared
+ * engine with live parameters (b2sd_set_live_params): b2sd_apply_lora changes those. */
 int b2sd_load_tensor(b2sd_handle h, const char* key, const void* ptr, int dtype, const int64_t* shape, int ndim);
+
+/* Live parameters: LoRAs switched on a running engine (b2sd_apply_lora).  on = 1 puts h's weight store in live mode; call it
+ * before the store's first b2sd_prepare, on parameters loaded with b2sd_load_tensor.  Lanes share the store and so the mode.
+ * The first prepare then keeps the loaded (base) UNet parameters: the raw copies of the pack-only ones are not released, and
+ * every UNet matrix a kernel reads as loaded gets a second, base copy.  b2sd_import_packed refuses a live store (a blob does
+ * not carry the base). */
+int b2sd_set_live_params(b2sd_handle h, int on);
+/* One LoRA pair on one UNet matrix: delta = scale * up @ down, with up [rows][rank] and down [rank][cols] in DEVICE memory,
+ * rows = the parameter's first dimension and cols = the product of the others (Cin * kh * kw for a convolution, as
+ * W.flatten(1)).  scale is the LoRA's scale times alpha / rank. */
+typedef struct b2sd_lora_factor {
+    const char* key;      /* the parameter, e.g. "up_blocks.1.attentions.0.transformer_blocks.0.attn2.to_k.weight" */
+    const void* up;
+    const void* down;
+    int rank;
+    int dtype;            /* of both factors: 0 = fp16, 1 = fp32 */
+    float scale;
+} b2sd_lora_factor;
+/* Re-fuse the live UNet parameters of h's weight store: every key of f becomes base + the deltas of its factors, in the given
+ * order, rounded to fp16 after each (as fusing LoRAs one after another on the host does); every other parameter reverts to its
+ * base value, which is never written (n = 0: the base weights).  The deltas run on the tensor cores; every packed and fp32
+ * entry derived from a changed parameter is rebuilt in place, so addresses, frame programs and CUDA graphs stay valid.  All of
+ * it is enqueued on `stream` without a host synchronisation: the caller orders it after the frames in flight on the store's
+ * engines and before later ones, keeps the factors alive until it has run, and then refreshes each engine's conditioning
+ * (b2sd_refresh_conditioning) and each state's own (b2sd_state_set_*).  Arguments are checked before any device work.  A store
+ * scratch holds the factor operands and fused matrices; it grows only when a call needs more than any before it. */
+int b2sd_apply_lora(b2sd_handle h, int n, const b2sd_lora_factor* f, void* stream);
+/* Recompute h's global prompt and time blocks (cross-attention K / V^T, time embeddings, resnet time biases) from its global
+ * prompt embeddings and timesteps with the current parameters, on `stream`, without a host synchronisation */
+int b2sd_refresh_conditioning(b2sd_handle h, void* stream);
 
 /* Packed-weight blob: the kernel-native layouts b2sd_prepare derives from the parameters (reordered convolution
  * matrices, per-head q/k/v gathers, GEGLU interleave, fused bias vectors), written once and loaded instead of

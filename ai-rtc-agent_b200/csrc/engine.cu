@@ -72,6 +72,11 @@ class Arena {
   public:
     explicit Arena(size_t slab) : slab_(slab) {}
     ~Arena() { release(); }
+    // Stream-ordered mode (a style's store and lanes, b2sd_create_style): slabs come from `pool` on `order` and are freed on
+    // it, so releasing them never synchronises the device; whoever frees first makes `order` wait for the last work that
+    // reads them (b2sd_release).  The pool must not reuse memory across streams by waiting (no internal dependencies): the
+    // host waits for each allocation, and so would wait for the frames of whatever stream freed it.  Set before the first alloc.
+    void set_order(cudaStream_t order, cudaMemPool_t pool) { order_ = order; pool_ = pool; }
     void* alloc(size_t bytes) {
         bytes = (bytes + 1023) & ~size_t(1023);
         if (cur_ < 0 || off_ + bytes > sizes_[cur_]) {
@@ -81,7 +86,8 @@ class Arena {
             if (next >= (int)slabs_.size()) {
                 size_t sz = bytes > slab_ ? bytes : slab_;
                 void* p = nullptr;
-                const cudaError_t e = cudaMalloc(&p, sz);
+                cudaError_t e = order_ ? cudaMallocFromPoolAsync(&p, sz, pool_, order_) : cudaMalloc(&p, sz);
+                if (e == cudaSuccess && order_) e = cudaStreamSynchronize(order_);   // usable on any stream from here on
                 if (e != cudaSuccess) {   // callers only see nullptr: say why, or the caller reports a stale message
                     b2_set_error("device allocation of %zu bytes failed: %s", sz, cudaGetErrorString(e));
                     return nullptr;
@@ -99,7 +105,7 @@ class Arena {
     }
     void reset() { cur_ = slabs_.empty() ? -1 : 0; off_ = 0; }
     void release() {
-        for (void* p : slabs_) cudaFree(p);
+        for (void* p : slabs_) order_ ? cudaFreeAsync(p, order_) : cudaFree(p);
         slabs_.clear();
         sizes_.clear();
         cur_ = -1;
@@ -108,6 +114,8 @@ class Arena {
 
   private:
     size_t slab_;
+    cudaStream_t order_ = nullptr;
+    cudaMemPool_t pool_ = nullptr;
     std::vector<void*> slabs_;
     std::vector<size_t> sizes_;
     int cur_ = -1;
@@ -285,6 +293,26 @@ static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_o
 // path, so several engines ("lanes", b2sd_create_lane) share one store: one copy of the 1.7 GB UNet in HBM however many
 // frames are in flight.
 struct WeightStore {
+    // ---- styles (b2sd_create_style).  Declared first, so destroyed last: the arenas below free on `order`, and a style reads
+    // its parent's base values until then.
+    std::shared_ptr<WeightStore> parent;   // a style: the live store whose base values it reads in place
+    struct OrderStream {
+        cudaStream_t s = nullptr;
+        cudaMemPool_t pool = nullptr;
+        ~OrderStream() {
+            if (s) cudaStreamDestroy(s);         // returns at once; the frees queued on it still run
+            if (pool) cudaMemPoolDestroy(pool);  // released once its last allocation is freed
+        }
+    } order;                               // a style: the stream and pool its memory is allocated and freed with
+    const uint64_t id = next_id();         // tells the stores apart (the overrides computed with their parameters)
+    uint64_t family = id;                  // a store and the styles derived from it: their states may move between them
+    struct Copy { __half* dst; const __half* src; size_t bytes; };
+    std::vector<Copy> pending;             // a style: base values copied into its own matrices by its first prepare
+    static uint64_t next_id() {
+        static std::atomic<uint64_t> n{1};
+        return n++;
+    }
+
     std::map<std::string, Raw> raw;
     Arena weights{256u << 20};   // packed parameters + the raw ones kernels read directly (live for the store's lifetime)
     Arena raw_only{256u << 20};  // raw parameters that only feed the packing kernels: released after the first prepare
@@ -317,7 +345,9 @@ struct WeightStore {
     std::vector<std::string> fused;        // keys whose live values differ from the base (the last b2sd_apply_lora)
     void* scratch = nullptr;               // factor operands and fused matrices of b2sd_apply_lora, grown stream-ordered
     size_t scratch_cap = 0;
-    ~WeightStore() { if (scratch) cudaFree(scratch); }
+    ~WeightStore() {
+        if (scratch) order.s ? cudaFreeAsync(scratch, order.s) : cudaFree(scratch);
+    }
 };
 
 enum { COND_PROMPT = 0, COND_TIME = 1 };
@@ -340,6 +370,7 @@ struct CondPool {
 // on the pool's reaper stream after the copy that computed it and after the latest copy out of it on every stream.
 struct CondOverride {
     uint64_t id = 0;
+    uint64_t store = 0;            // WeightStore::id of the parameters it was computed with
     void* buf = nullptr;
     size_t bytes = 0;
     cudaEvent_t ready = nullptr;   // recorded once buf holds the block
@@ -359,9 +390,10 @@ struct CondOverride {
 };
 
 // One temporal stream's stream-batch state (b2sd_state_*): slots 1 .. T-1 of the UNet input batch, NHWC fp16, stream-ordered
-// allocation.  It remembers the weight store, batch and size it was made for; the weak reference does not keep weights alive.
+// allocation.  It remembers the family of weight stores (a store and its styles), batch and size it was made for; any engine of
+// the family may step it.
 struct b2sd_state {
-    std::weak_ptr<WeightStore> ws;
+    uint64_t family = 0;
     int batch = 0, height = 0, width = 0;
     size_t bytes = 0;
     __half* buf = nullptr;
@@ -1909,7 +1941,7 @@ static size_t state_bytes(const b2sd_engine* h) { return (size_t)(h->cfg.batch -
 
 static int state_new(const b2sd_engine* h, cudaStream_t s, b2sd_state** out) {
     b2sd_state* st = new b2sd_state;
-    st->ws = h->ws;
+    st->family = h->ws->family;
     st->batch = h->cfg.batch; st->height = h->cfg.height; st->width = h->cfg.width;
     st->bytes = state_bytes(h);
     cudaError_t e = cudaEventCreateWithFlags(&st->done, cudaEventDisableTiming);
@@ -1965,6 +1997,11 @@ static int bind_conditioning(b2sd_engine* h, const b2sd_state* st, cudaStream_t 
         CondOverride* ov = st ? st->cond[k].get() : nullptr;
         const uint64_t want = ov ? ov->id : COND_GLOBAL;
         if (b.held == want) continue;
+        if (ov && ov->store != h->ws->id) {
+            b2_set_error("the state's own %s was computed with another weight store's parameters (a style's or its parent's): "
+                         "set it again on an engine of this store", k == COND_PROMPT ? "prompt" : "timesteps");
+            return -1;
+        }
         b.held = COND_UNKNOWN;
         if (ov) {
             CUDA_OK(cudaStreamWaitEvent(s, ov->ready, 0));
@@ -2023,6 +2060,7 @@ static int publish_override(b2sd_engine* h, b2sd_state* st, int k, cudaStream_t 
     ov->pool = cond_pool(h);
     if (!ov->pool) return -1;
     ov->id = next_id++;
+    ov->store = h->ws->id;
     ov->bytes = b.used;
     cudaError_t e = cudaEventCreateWithFlags(&ov->ready, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaMallocFromPoolAsync(&ov->buf, ov->bytes, ov->pool->pool, s);
@@ -2118,6 +2156,10 @@ static int create_engine(const b2sd_config* cfg, std::shared_ptr<WeightStore> st
     }
     if (igemm_init() || attn_init() || tconv_init()) return -1;
     b2sd_engine* e = new b2sd_engine(std::move(store));
+    if (e->ws->order.s) {
+        e->state.set_order(e->ws->order.s, e->ws->order.pool);
+        e->prog.set_order(e->ws->order.s, e->ws->order.pool);
+    }
     e->cfg = *cfg;
     e->lh = cfg->height / 8;
     e->lw = cfg->width / 8;
@@ -2324,6 +2366,9 @@ int b2sd_prepare(b2sd_handle h, const void* prompt_embeds, const float* timestep
     // x_t_latent_buffer = zeros (StreamDiffusion.prepare); slot 0 is overwritten by every frame
     CUDA_OK(cudaMemsetAsync(h->x_in.p, 0, (size_t)h->x_in.elems() * 2, s));
     if (h->pair_state) TRY(state_reset(h->pair_state.get(), s));
+    for (auto& c : h->ws->pending)   // a style's own UNet matrices start as the base values, before anything packs them
+        CUDA_OK(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToDevice, s));
+    h->ws->pending.clear();
     const size_t rebuilds = h->ws->rebuild.size();
     TRY(h->build_program(s));
     if (h->ws->rebuild.size() != rebuilds && !h->ws->fused.empty()) {
@@ -2623,7 +2668,7 @@ int b2sd_apply_lora(b2sd_handle h, int n, const b2sd_lora_factor* f, void* strea
         if (w.scratch) CUDA_OK(cudaFreeAsync(w.scratch, s));
         w.scratch = nullptr;
         w.scratch_cap = 0;
-        CUDA_OK(cudaMallocAsync(&w.scratch, need, s));
+        CUDA_OK(w.order.pool ? cudaMallocFromPoolAsync(&w.scratch, need, w.order.pool, s) : cudaMallocAsync(&w.scratch, need, s));
         w.scratch_cap = need;
     }
     char* sp = static_cast<char*>(w.scratch);
@@ -2708,6 +2753,115 @@ int b2sd_refresh_conditioning(b2sd_handle h, void* stream) {
     return keep_global(h, COND_TIME, s);
 }
 
+// ---- styles ---------------------------------------------------------------------------------------------------------------
+// Whether a packed / fp32 cache entry is derived from a UNet matrix a LoRA may change (a style then needs its own copy)
+static bool lora_derived(const WeightStore& w, std::string name) {
+    auto rb = w.rebuild.find(name);
+    if (rb == w.rebuild.end()) {   // the LayerNorm fold's column sums and biases are rebuilt with the gathered rows
+        for (const char* suffix : {":cs", ":b"}) {
+            const size_t n = strlen(suffix);
+            if (name.size() > n && name.compare(name.size() - n, n, suffix) == 0) {
+                rb = w.rebuild.find(name.substr(0, name.size() - n));
+                break;
+            }
+        }
+    }
+    if (rb == w.rebuild.end()) return false;
+    for (auto& k : rb->second.keys) {
+        auto it = w.raw.find(k);
+        if (it != w.raw.end() && lora_target(k, it->second)) return true;
+    }
+    return false;
+}
+
+int b2sd_create_style(b2sd_handle parent, b2sd_handle* out) {
+    if (!parent || !out) {
+        b2_set_error("b2sd_create_style: null argument");
+        return -1;
+    }
+    // derive from the family's root: its base values are the ones every style reads
+    std::shared_ptr<WeightStore> root = parent->ws->parent ? parent->ws->parent : parent->ws;
+    if (!root->live || !root->live_ready) {
+        b2_set_error("b2sd_create_style: the parent's weight store is not live and prepared (b2sd_set_live_params before its "
+                     "first b2sd_prepare)");
+        return -1;
+    }
+    auto st = std::make_shared<WeightStore>();
+    st->parent = root;
+    st->family = root->family;
+    st->live = st->live_ready = true;
+    {   // the style's own pool, which never makes an allocation wait for a free on another stream (as CondPool)
+        int dev = 0, no = 0;
+        cudaError_t e = cudaGetDevice(&dev);
+        cudaMemPoolProps props{};
+        props.allocType = cudaMemAllocationTypePinned;
+        props.location.type = cudaMemLocationTypeDevice;
+        props.location.id = dev;
+        if (e == cudaSuccess) e = cudaMemPoolCreate(&st->order.pool, &props);
+        if (e == cudaSuccess) e = cudaMemPoolSetAttribute(st->order.pool, cudaMemPoolReuseAllowInternalDependencies, &no);
+        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&st->order.s, cudaStreamNonBlocking);
+        if (e != cudaSuccess) {
+            b2_set_error("b2sd_create_style: %s", cudaGetErrorString(e));
+            return -1;
+        }
+    }
+    st->weights.set_order(st->order.s, st->order.pool);
+    st->raw_only.set_order(st->order.s, st->order.pool);
+    st->base_arena.set_order(st->order.s, st->order.pool);
+    // Parameters: the raw map's entries point at the root's memory (its base values for the pack-only UNet matrices), except
+    // the UNet matrices kernels read raw, which get copies of their own, filled with the base values by the first prepare.
+    st->raw = root->raw;
+    for (auto& kv : st->raw) {
+        Raw& r = kv.second;
+        if (r.pack_only || !lora_target(kv.first, r)) continue;
+        auto base = root->base.find(kv.first);
+        if (base == root->base.end()) {
+            b2_set_error("b2sd_create_style: the parent's store has no base value of '%s'", kv.first.c_str());
+            return -1;
+        }
+        const size_t bytes = (size_t)r.numel() * 2;
+        __half* p = static_cast<__half*>(st->weights.alloc(bytes));
+        if (!p) return -1;
+        st->base[kv.first] = base->second;
+        st->pending.push_back({p, base->second, bytes});
+        r.p = p;
+    }
+    // Cache entries no UNet LoRA reaches are shared; the others are made by the style's first prepare, from its own parameters
+    for (auto& kv : root->packed)
+        if (!lora_derived(*root, kv.first)) {
+            st->packed[kv.first] = kv.second;
+            st->packed_bytes[kv.first] = root->packed_bytes.at(kv.first);
+        }
+    for (auto& kv : root->fvec)
+        if (!lora_derived(*root, kv.first)) {
+            st->fvec[kv.first] = kv.second;
+            st->fvec_bytes[kv.first] = root->fvec_bytes.at(kv.first);
+        }
+    if (create_engine(&parent->cfg, st, out)) return -1;
+    (*out)->concurrency = parent->concurrency;
+    return 0;
+}
+
+int b2sd_release(b2sd_handle h, void* stream) {
+    if (!h) return 0;
+    const cudaStream_t order = h->ws->order.s;
+    if (!order) {
+        b2_set_error("b2sd_release: the engine's weight store is not a style (b2sd_create_style); use b2sd_destroy");
+        return -1;
+    }
+    cudaEvent_t last = nullptr;
+    cudaError_t e = cudaEventCreateWithFlags(&last, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventRecord(last, reinterpret_cast<cudaStream_t>(stream));
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(order, last, 0);
+    if (last) cudaEventDestroy(last);
+    if (e != cudaSuccess) {
+        b2_set_error("b2sd_release: %s", cudaGetErrorString(e));
+        return -1;
+    }
+    delete h;   // its memory, and its store's once no engine holds it, is freed on `order` after the work queued on `stream`
+    return 0;
+}
+
 // ---- per-state conditioning --------------------------------------------------------------------------
 // What every call that runs a state on an engine refuses
 static int check_state(const char* fn, b2sd_handle h, const b2sd_state* state) {
@@ -2719,7 +2873,7 @@ static int check_state(const char* fn, b2sd_handle h, const b2sd_state* state) {
         b2_set_error("%s: the engine is part of a b2sd_share_stream_state pair, which steps its own state", fn);
         return -1;
     }
-    if (state->ws.lock() != h->ws || state->batch != h->cfg.batch || state->height != h->cfg.height ||
+    if (state->family != h->ws->family || state->batch != h->cfg.batch || state->height != h->cfg.height ||
         state->width != h->cfg.width) {
         b2_set_error("%s: the state was made for another weight store, batch or size (state: batch %d, %dx%d; "
                      "engine: batch %d, %dx%d)", fn, state->batch, state->height, state->width, h->cfg.batch, h->cfg.height,

@@ -240,7 +240,9 @@ def lib() -> C.CDLL:
         _lib.b2sd_set_live_params.argtypes = [vp, ci]
         _lib.b2sd_apply_lora.argtypes = [vp, ci, C.POINTER(LoraFactor), vp]
         _lib.b2sd_refresh_conditioning.argtypes = [vp, vp]
-        for name in ("set_live_params", "apply_lora", "refresh_conditioning"):
+        _lib.b2sd_create_style.argtypes = [vp, C.POINTER(vp)]
+        _lib.b2sd_release.argtypes = [vp, vp]
+        for name in ("set_live_params", "apply_lora", "refresh_conditioning", "create_style", "release"):
             getattr(_lib, "b2sd_" + name).restype = C.c_int
         _lib.b2sd_conditioning_binds.argtypes = [vp]
         _lib.b2sd_conditioning_binds.restype = i64

@@ -13,8 +13,10 @@ u8 NHWC in -> u8 NCHW out, nothing leaves HBM).  preprocess / predict / postproc
 separately with the reference's tensor contracts."""
 from __future__ import annotations
 
+import collections
 import os
-from typing import Dict, List, Optional
+import weakref
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -32,6 +34,9 @@ DEFAULT_LANES_PER_PEER = 2    # T > 1 with per-peer streams: independent lanes, 
                               # 512x512, tools/bench_peers.py: 2 lanes 47.0 / 54.3 fps at 1 / 2+ peers, p50 42.5 / 36.8 ms; 3 lanes
                               # 47.1 / 56.1 fps at 1 / 4+ peers but p50 63.7 / 53.4 ms and 3 GB more; 4 lanes no faster)
 PER_PEER_STREAMS_ENV = "B200SD_PER_PEER_STREAMS"
+MAX_STYLES_ENV = "B200SD_MAX_STYLES"
+DEFAULT_MAX_STYLES = 4        # viewers' own styles held at once (PeerStream.update_lora); each holds a UNet copy and its lanes
+STYLE_LANES = DEFAULT_LANES_PER_PEER   # lanes of each such style
 
 
 def env_flag(name: str) -> bool:
@@ -68,9 +73,37 @@ def _as_torch_u8_nhwc(frame, device) -> torch.Tensor:
     return t
 
 
+def _max_styles() -> int:
+    return int(os.getenv(MAX_STYLES_ENV, "0")) or DEFAULT_MAX_STYLES
+
+
+def style_key(lora_dict: Optional[Dict[str, float]]) -> Tuple[Tuple[str, int, int, float], ...]:
+    """What a lora_dict means, for the style pool: its (real path, file size, mtime in ns, scale) in order, so that a replaced
+    file or another order or scale is another style.  A missing file raises."""
+    key = []
+    for path, scale in (lora_dict or {}).items():
+        st = os.stat(path)
+        key.append((os.path.realpath(path), st.st_size, st.st_mtime_ns, float(scale)))
+    return tuple(key)
+
+
+class _Style:
+    """A style of the pipeline's weights (StreamDiffusion.add_style) and its lanes, with their own streams: the lane pool of the
+    viewers whose own lora_dict it is.  The same attributes as the pipeline's own lane pool, so _enqueue runs on either."""
+
+    def __init__(self, key, lora_dict, engines, streams):
+        self.key, self.lora_dict = key, dict(lora_dict or {})
+        self._engines, self._lane_streams = engines, streams
+        self._lane_done = [None] * len(engines)
+        self._next_lane = 0
+        self.users = 0   # open viewers on it
+
+
 class StreamDiffusionPipeline:
     per_peer_streams = False
     _own_state = None   # the StreamState enqueue() steps with per-peer streams; None: the engines' own shared state
+    _lora = None        # the global lora_dict (update_lora)
+    _lora_key = ()      # its style_key
 
     def __init__(self, model_id: str, t_index_list: Optional[List[int]] = None, width: int = 512, height: int = 512,
                  prompt: str = DEFAULT_PROMPT, lanes: Optional[int] = None, per_peer_streams: Optional[bool] = None,
@@ -92,6 +125,8 @@ class StreamDiffusionPipeline:
         if per_peer_streams is None:
             per_peer_streams = env_flag(PER_PEER_STREAMS_ENV)
         self.per_peer_streams = bool(per_peer_streams)
+        self._styles = collections.OrderedDict()   # style_key -> _Style of viewers' own styles, least recently used first
+        self._peer_set = weakref.WeakSet()         # open PeerStreams
         self.prompt = prompt
         self.t_index_list = list(t_index_list) if t_index_list is not None else DEFAULT_T_INDEX_LIST
         self.device = "cuda"
@@ -136,35 +171,33 @@ class StreamDiffusionPipeline:
         self._lane_streams = [None] if len(self._engines) == 1 else [torch.cuda.Stream(sd.device) for _ in self._engines]
         self._lane_done = [None] * len(self._engines)     # completion event of the last frame given to each lane
         self._next_lane = 0
-        # Every frame's output is a fresh tensor allocated on its lane's stream (the caller owns it and may hold it across calls,
-        # SURVEY 8b "Ownership").  Give each lane stream's allocator pool a few output-sized blocks now: the first cudaMalloc a
-        # lane needed in the middle of a stream otherwise synchronises the device, i.e. stalls every frame in flight once
-        # (seen as a single 2x latency spike, 33 ms instead of 17 ms, some 50-80 frames into a run with 10 frames pending).
-        for st in self._lane_streams:
-            if st is not None:
-                with torch.cuda.stream(st):
-                    prime = [torch.empty((1, 3, self.model.height, self.model.width), dtype=torch.uint8, device=sd.device)
-                             for _ in range(4)]
-                    del prime
+        self._prime(self._lane_streams)
 
     @property
     def lanes(self) -> int:
         return len(self._engines)
 
+    def _pools(self):
+        """the pipeline's lane pool and every style's"""
+        return [self] + list(self._styles.values())
+
     def _quiesce(self):
-        """Every lane finishes its queued frames before a prompt / timestep update touches the shared schedule."""
+        """Every lane (the styles' too) finishes its queued frames before a prompt / timestep update touches the shared
+        schedule."""
         cur = torch.cuda.current_stream(self.model.stream.device)
-        for ev in self._lane_done:
-            if ev is not None:
-                cur.wait_event(ev)
+        for pool in self._pools():
+            for ev in pool._lane_done:
+                if ev is not None:
+                    cur.wait_event(ev)
         return cur
 
     def _release(self, cur):
         done = torch.cuda.Event()
         done.record(cur)
-        for st in self._lane_streams:
-            if st is not None:
-                st.wait_event(done)
+        for pool in self._pools():
+            for st in pool._lane_streams:
+                if st is not None:
+                    st.wait_event(done)
 
     def update_prompt(self, prompt: str):
         """The global prompt: every stream's, including open peer streams with a prompt of their own (PeerStream.update_prompt)."""
@@ -182,8 +215,114 @@ class StreamDiffusionPipeline:
         cur = self._quiesce()
         try:
             self.model.update_lora(lora_dict)
+            # every viewer follows the new global style, as a global prompt replaces viewers' own (the update above has set
+            # their own prompt / t_index_list again on the pipeline's engines); cached styles stay valid for later requests
+            for peer in list(self._peer_set):
+                self._leave_style(peer)
+            self._lora, self._lora_key = dict(lora_dict or {}), style_key(lora_dict)
         finally:
             self._release(cur)
+
+    # ---- viewers' own styles (PeerStream.update_lora) ------------------------------------------------------------------
+    def _leave_style(self, peer) -> None:
+        if peer._style is not None:
+            peer._style.users -= 1
+            peer._style, peer._lora = None, None
+
+    def _set_peer_style(self, peer, lora_dict: Optional[Dict[str, float]]) -> None:
+        """Move `peer` to the lane pool of lora_dict's style (the pipeline's own when it is the global one), building the style
+        when it is not cached.  Everything that can fail is checked before anything changes; unused styles beyond
+        $B200SD_MAX_STYLES are evicted only once the switch has succeeded, so a build briefly holds one style more."""
+        from .weights import lora_factors
+        state = peer._live_state()
+        if not self.model.live_lora:
+            raise RuntimeError("PeerStream.update_lora needs StreamDiffusionPipeline(live_lora=True) (or $B200SD_LIVE_LORA=1)")
+        key = style_key(lora_dict)
+        if key == self._lora_key:
+            target = None
+        elif key in self._styles:
+            target = self._styles[key]
+        else:
+            sd = self.model.stream
+            factors = lora_factors(sd._unet_shapes, lora_dict)   # reads the files and checks every pair
+            limit = _max_styles()
+            unused = any(st.users == 0 for st in self._styles.values())
+            leaving = peer._style is not None and peer._style.users == 1   # the viewer's style, which it alone uses
+            if len(self._styles) >= limit and not unused and not leaving:
+                raise RuntimeError(f"every one of the {limit} viewer styles (${MAX_STYLES_ENV}) is in use")
+            target = self._build_style(key, lora_dict, factors)
+        if target is peer._style:
+            return
+        if target is not None:
+            self._styles[target.key] = self._styles.pop(target.key)   # most recently used
+        # the viewer's own conditioning is computed again with the new weights, on the lane that takes its next frame
+        pool = target or self
+        if state.own_prompt is not None or state.own_t_index_list is not None:
+            prompt, t_index_list = state.own_prompt, state.own_t_index_list
+
+            def rebind(engine):
+                if prompt is not None:
+                    state.set_prompt(prompt, engine=engine)
+                if t_index_list is not None:
+                    state.set_t_index_list(t_index_list, engine=engine)
+            self._update_state(rebind, pool)
+        self._leave_style(peer)
+        if target is not None:
+            target.users += 1
+            peer._style, peer._lora = target, dict(lora_dict or {})
+        # back within the bound: unused styles, least recently used first, each freed after its last frames
+        for k in [k for k, st in self._styles.items() if st.users == 0]:
+            if len(self._styles) <= _max_styles():
+                break
+            self._evict(k)
+
+    def _build_style(self, key, lora_dict, factors) -> _Style:
+        """A style and its lanes, made, prepared and fused on a stream of their own: no wait for any queued frame."""
+        sd = self.model.stream
+        streams = [torch.cuda.Stream(sd.device) for _ in range(STYLE_LANES)]
+        with torch.cuda.stream(streams[0]):
+            style = sd.add_style()
+            try:
+                engines = [style] + [style.add_lane() for _ in range(STYLE_LANES - 1)]
+                style.apply_factors(factors)
+            except BaseException:
+                sd.drop_style(style, streams[0])
+                raise
+        done = torch.cuda.Event()
+        done.record(streams[0])
+        for st in streams[1:]:
+            st.wait_event(done)
+        self._prime(streams)
+        pool = self._styles[key] = _Style(key, lora_dict, engines, streams)
+        return pool
+
+    def _evict(self, key) -> None:
+        """Free a cached style no viewer uses, after its lanes' last frames: stream-ordered, no host or device wait."""
+        pool = self._styles.pop(key)
+        after = torch.cuda.Stream(self.model.stream.device)
+        for st in pool._lane_streams:   # the style's build and every frame given to it
+            after.wait_stream(st)
+        for ev in pool._lane_done:      # and their downloads
+            if ev is not None:
+                after.wait_event(ev)
+        self.model.stream.drop_style(pool._engines[0], after)
+
+    def _prime(self, streams) -> None:
+        """Every frame's output is a fresh tensor allocated on its lane's stream (the caller owns it and may hold it across
+        calls, SURVEY 8b "Ownership").  Give each lane stream's allocator pool a few output-sized blocks now: the first
+        cudaMalloc a lane needed in the middle of a stream otherwise synchronises the device, i.e. stalls every frame in flight
+        once (seen as a single 2x latency spike, 33 ms instead of 17 ms, some 50-80 frames into a run with 10 frames pending)."""
+        for st in streams:
+            if st is not None:
+                with torch.cuda.stream(st):
+                    prime = [torch.empty((1, 3, self.model.height, self.model.width), dtype=torch.uint8,
+                                         device=self.model.stream.device) for _ in range(4)]
+                    del prime
+
+    @property
+    def styles(self) -> int:
+        """viewers' own styles held (PeerStream.update_lora), in use or cached"""
+        return len(self._styles)
 
     def update_t_index_list(self, t_index_list: List[int]):
         """The global t_index_list: every stream's, including open peer streams with one of their own."""
@@ -192,13 +331,15 @@ class StreamDiffusionPipeline:
         self.model.stream.clear_overrides(prompt=False, t_index_list=True)   # also when the global list was already this one
         self._release(cur)
 
-    def _update_state(self, update) -> None:
-        """update(engine) refreshes one peer's conditioning on the lane that takes the next submission, on that lane's stream:
-        stream-ordered after the frames queued there, with no host wait and no wait on the other lanes."""
-        lane = self._next_lane
-        compute = self._lane_streams[lane] or torch.cuda.current_stream(self.model.stream.device)
+    def _update_state(self, update, pool=None) -> None:
+        """update(engine) refreshes one peer's conditioning on the lane of `pool` (a style's lanes, default the pipeline's) that
+        takes the next submission, on that lane's stream: stream-ordered after the frames queued there, with no host wait and no
+        wait on the other lanes."""
+        pool = pool or self
+        lane = pool._next_lane
+        compute = pool._lane_streams[lane] or torch.cuda.current_stream(self.model.stream.device)
         with torch.cuda.stream(compute):
-            update(self._engines[lane])
+            update(pool._engines[lane])
 
     # ---- reference-shaped stages ----------------------------------------------------------------------
     def preprocess(self, frame) -> torch.Tensor:
@@ -223,8 +364,8 @@ class StreamDiffusionPipeline:
         software-encode branch (`.cpu()`); with NVENC set the CUDA tensor is returned stream-ordered, like the reference."""
         return self._call(frame, self._own_state)
 
-    def _call(self, frame, state):
-        ticket = self._enqueue(frame, state)
+    def _call(self, frame, state, pool=None):
+        ticket = self._enqueue(frame, state, pool)
         if os.getenv("NVENC"):
             ticket.wait(torch.cuda.current_stream(self.model.stream.device))   # stream-ordered result, whichever lane ran it
             return ticket.result(wait=False)
@@ -246,17 +387,19 @@ class StreamDiffusionPipeline:
         Tickets complete in submission order (one temporal stream per pipeline, like the reference)."""
         return self._enqueue(frame, self._own_state)
 
-    def _enqueue(self, frame, state) -> "FrameTicket":
-        """enqueue() on `state` (a StreamState, or None for the engines' own shared stream).  Lanes rotate over all submissions;
-        frames of one state are ordered on the device by the state's event."""
+    def _enqueue(self, frame, state, pool=None) -> "FrameTicket":
+        """enqueue() on `state` (a StreamState, or None for the engines' own shared stream) on the lanes of `pool` (a viewer's
+        style, default the pipeline's).  Lanes rotate over all submissions to the pool; frames of one state are ordered on the
+        device by the state's event."""
         if not _is_gpu_frame(frame) and not _is_video_frame(frame):
             raise Exception("invalid frame type")
+        pool = pool or self
         dev = self.model.stream.device
         caller = torch.cuda.current_stream(dev)
-        lane = self._next_lane
-        self._next_lane = (lane + 1) % len(self._engines)
-        engine = self._engines[lane]
-        compute = self._lane_streams[lane] or caller
+        lane = pool._next_lane
+        pool._next_lane = (lane + 1) % len(pool._engines)
+        engine = pool._engines[lane]
+        compute = pool._lane_streams[lane] or caller
         if compute is not caller:
             ready = torch.cuda.Event()
             ready.record(caller)          # whatever produced the frame on the caller's stream
@@ -291,7 +434,7 @@ class StreamDiffusionPipeline:
         done = torch.cuda.Event()
         if os.getenv("NVENC"):
             done.record(compute)
-            self._lane_done[lane] = done
+            pool._lane_done[lane] = done
             return FrameTicket(post_output, done, None, None)
         # software-encode branch (lib/pipeline.py:83-94): hand back an av.VideoFrame with the input's timing
         assert _is_video_frame(frame)
@@ -304,7 +447,7 @@ class StreamDiffusionPipeline:
             host_out.copy_(post_output, non_blocking=True)
             post_output.record_stream(self._copy_stream)
             done.record(self._copy_stream)
-        self._lane_done[lane] = done
+        pool._lane_done[lane] = done
         return FrameTicket(post_output, done, host_out, frame)
 
     def _ensure_staging(self, dev) -> None:
@@ -355,9 +498,13 @@ class PeerStream:
     them (update_prompt / update_t_index_list; until then the pipeline's).  close() frees the state after its last frame,
     without a host synchronisation."""
 
+    _style = None   # the pipeline's _Style this viewer's frames run on; None: the pipeline's lanes
+    _lora = None    # this viewer's own lora_dict (update_lora), with _style
+
     def __init__(self, pipeline: StreamDiffusionPipeline):
         self._pipeline = pipeline
         self._state = pipeline.model.stream.new_state()
+        pipeline._peer_set.add(self)
 
     @property
     def closed(self) -> bool:
@@ -369,7 +516,7 @@ class PeerStream:
         return self._state
 
     def enqueue(self, frame) -> FrameTicket:
-        return self._pipeline._enqueue(frame, self._live_state())
+        return self._pipeline._enqueue(frame, self._live_state(), self._style)
 
     @property
     def prompt(self) -> str:
@@ -387,20 +534,38 @@ class PeerStream:
         queued, and every other viewer's frames, are unaffected.  Does not wait for queued frames.  A later global
         pipeline.update_prompt replaces it."""
         state = self._live_state()
-        self._pipeline._update_state(lambda engine: state.set_prompt(prompt, engine=engine))
+        self._pipeline._update_state(lambda engine: state.set_prompt(prompt, engine=engine), self._style)
 
     def update_t_index_list(self, t_index_list: List[int]) -> None:
         """This viewer's own t_index_list, with the semantics of the global update_t_index_list (only the time embedding's
         timesteps change) and update_prompt's ordering."""
         state = self._live_state()
-        self._pipeline._update_state(lambda engine: state.set_t_index_list(t_index_list, engine=engine))
+        self._pipeline._update_state(lambda engine: state.set_t_index_list(t_index_list, engine=engine), self._style)
+
+    @property
+    def lora(self) -> Dict[str, float]:
+        """This viewer's style LoRAs: its own (update_lora) or the pipeline's global ones"""
+        self._live_state()
+        return dict(self._lora if self._style is not None else (self._pipeline._lora or {}))
+
+    def update_lora(self, lora_dict: Optional[Dict[str, float]]) -> None:
+        """This viewer's own style: the base weights plus the LoRAs of lora_dict ({safetensors path: scale}, fused in order, the
+        constructor's form; None or {}: the base weights).  Its frames enqueued after the call use it and frames already queued
+        the old one; the stream state carries across, and the viewer keeps its own prompt / t_index_list.  Every other viewer
+        is unaffected.  Viewers with the same lora_dict share one style; the global lora_dict is the pipeline's own lanes.  A
+        style is built (on streams of its own, waiting for no queued frame) when no cached one matches; $B200SD_MAX_STYLES
+        bounds how many are held, the least recently used unused one making room.  Needs live_lora=True.  Errors (a closed
+        stream, a bad file, a pair that does not fit, a LoRA matching no module, every style in use) are raised before anything
+        changes.  A later global pipeline.update_lora replaces it."""
+        self._pipeline._set_peer_style(self, lora_dict)
 
     def __call__(self, frame):
-        return self._pipeline._call(frame, self._live_state())
+        return self._pipeline._call(frame, self._live_state(), self._style)
 
     def close(self) -> None:
         if self._state is not None:
             state, self._state = self._state, None
+            self._pipeline._leave_style(self)
             state.close()
 
     def __enter__(self) -> "PeerStream":
@@ -408,3 +573,10 @@ class PeerStream:
 
     def __exit__(self, *exc) -> None:
         self.close()
+
+    def __del__(self):
+        # a viewer dropped without close(): its style is no longer in use, and its state is freed after its last frame
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -71,6 +71,9 @@ class ImageProcessor:
 
 
 class StreamDiffusion:
+    styles = ()          # instances made by __init__ get a list (add_style)
+    _is_style = False
+
     def __init__(self, arch: UNetArch, unet_sd: Dict[str, torch.Tensor], vae_sd: Dict[str, torch.Tensor],
                  t_index_list: List[int], prompt_encoder: Callable[[str], torch.Tensor],
                  torch_dtype: torch.dtype = torch.float16, width: int = 512, height: int = 512,
@@ -79,14 +82,15 @@ class StreamDiffusion:
                  packed_blob: Optional[str] = None, parent: Optional["StreamDiffusion"] = None,
                  controlnet_sd: Optional[Dict[str, torch.Tensor]] = None,
                  hed_sd: Optional[Dict[str, torch.Tensor]] = None, use_tiny_vae: bool = True,
-                 vae_scaling_factor: float = 0.18215, live_lora: bool = False):
+                 vae_scaling_factor: float = 0.18215, live_lora: bool = False, style_of: Optional["StreamDiffusion"] = None):
         """vae_sd: TAESD (use_tiny_vae=True) or the model's own AutoencoderKL (use_tiny_vae=False: latents = vae_scaling_factor
         times the mean of the encoder's distribution, decoded from x0 / vae_scaling_factor).
         controlnet_sd: a diffusers ControlNetModel state dict (empty when the weights come from packed_blob); every
         stream-batch slot is then conditioned on the current frame's control image: the frame itself, or with hed_sd (a
         ControlNetHED.pth state dict, empty with packed_blob) its HED edge map.  Lanes inherit their parent's ControlNet.
         live_lora: keep the base UNet weights on the device so that apply_lora() can switch LoRAs at run time (not with
-        packed_blob; lanes inherit it)."""
+        packed_blob; lanes inherit it).
+        style_of: make a style of that live engine instead (add_style)."""
         if live_lora and packed_blob is not None:
             raise ValueError("live_lora needs the weights themselves: a packed blob does not carry the base weights")
         if hed_sd is not None and controlnet_sd is None:
@@ -152,7 +156,17 @@ class StreamDiffusion:
         # form no reference cycle, so their device memory is released as soon as the last reference goes, not at the next
         # run of the garbage collector
         self.lanes: List["StreamDiffusion"] = []
-        self._states = parent._states if parent is not None else weakref.WeakSet()   # live StreamStates of the engine and its lanes
+        # styles of this engine's weights (add_style); like lanes they keep no reference to it
+        self.styles: List["StreamDiffusion"] = []
+        self._is_style = style_of is not None
+        # live StreamStates of the engine, its lanes and its styles: any of them may step any of these states
+        family = parent if parent is not None else style_of
+        self._states = family._states if family is not None else weakref.WeakSet()
+        if style_of is not None:
+            # a style: the UNet weights of style_of's base plus LoRAs of its own (apply_lora), everything else shared
+            capi.check(self._lib.b2sd_create_style(style_of._handle, C.byref(self._handle)), "b2sd_create_style")
+            self._unet_shapes = style_of._unet_shapes
+            return
         if parent is not None:
             # a lane: shares the parent's weights in HBM, owns its activations / stream state / CUDA graph
             capi.check(self._lib.b2sd_create_lane(parent._handle, C.byref(cfg), C.byref(self._handle)), "b2sd_create_lane")
@@ -245,7 +259,7 @@ class StreamDiffusion:
         self.alpha_prod_t_sqrt = torch.stack([ac[t].sqrt() for t in self.sub_timesteps]).to(self.dtype).view(T, 1, 1, 1)
         self.beta_prod_t_sqrt = torch.stack([(1 - ac[t]).sqrt() for t in self.sub_timesteps]).to(self.dtype).view(T, 1, 1, 1)
         self._engine_prepare()
-        for lane in self.lanes:
+        for lane in self._family()[1:]:
             lane._prepare_like(self)
         for state in list(self._states):   # as prepare zeroes the engines' own latent buffers, and follows its conditioning
             if not state.closed:
@@ -287,6 +301,35 @@ class StreamDiffusion:
         self.lanes.append(lane)
         return lane
 
+    def add_style(self) -> "StreamDiffusion":
+        """A style of this live engine (b2sd_create_style): an engine whose UNet is this engine's base weights plus LoRAs of its
+        own (its apply_lora), sharing every other weight with it, prepared like this engine on the current CUDA stream.  Give
+        it lanes with its add_lane().  Later prepare() / update_prompt() / timestep updates on this object reach the style and
+        its lanes; apply_lora() on this object does not.  Every state of this engine's weights may be stepped by the style's
+        engines, but a state's own prompt / t_index_list must be set again on a style engine before it steps there.  Free the
+        style with drop_style()."""
+        self._check()
+        if not self.live_lora or self._is_style:
+            raise RuntimeError("add_style needs a live_lora engine that is not itself a style")
+        style = StreamDiffusion(self.arch, {}, {}, self.t_list, self.prompt_encoder, style_of=self, **self._ctor)
+        style._prepare_like(self)
+        self.styles.append(style)
+        return style
+
+    def drop_style(self, style: "StreamDiffusion", after: "torch.cuda.Stream") -> None:
+        """Free a style of this engine and its lanes after the work queued on `after` (which the caller makes wait for their
+        last frames), stream-ordered: no host or device synchronisation (b2sd_release)."""
+        self.styles.remove(style)
+        for eng in [style] + style.lanes:
+            if eng._handle.value:
+                h, eng._handle = eng._handle, C.c_void_p()
+                capi.check(self._lib.b2sd_release(h, after.cuda_stream), "b2sd_release")
+        style.lanes = []
+
+    def _family(self) -> List["StreamDiffusion"]:
+        """this engine, its lanes, its styles and their lanes: every engine a global prompt / timestep update reaches"""
+        return [self] + self.lanes + [e for st in self.styles for e in [st] + st.lanes]
+
     def new_state(self) -> "StreamState":
         """A fresh temporal stream (zeroed x_t_latent_buffer) that this engine and every lane of its weights can step:
         pass it as `state=` to step_u8 / step_u8_into / __call__.  prepare() resets it.  Not for share_state lanes."""
@@ -317,7 +360,7 @@ class StreamDiffusion:
         self.prompt = prompt
         self.prompt_embeds = self._encode(prompt).repeat(self.batch_size, 1, 1)
         emb = self.prompt_embeds[0].cpu().contiguous()
-        for eng in [self] + self.lanes:
+        for eng in self._family():
             eng.prompt, eng.prompt_embeds = prompt, self.prompt_embeds
             capi.check(self._lib.b2sd_set_prompt_embeds(eng._handle, emb.data_ptr(), self._stream()), "b2sd_set_prompt_embeds")
         self.clear_overrides(prompt=True, t_index_list=False)
@@ -334,7 +377,7 @@ class StreamDiffusion:
         reference only the timestep embedding changes; alpha/beta/c_skip/c_out keep their prepare() values.  Every live
         state's own t_index_list is dropped."""
         t = self._timestep_tensor(self.sub_timesteps)
-        for eng in [self] + self.lanes:
+        for eng in self._family():
             eng.t_list, eng.sub_timesteps, eng.sub_timesteps_tensor = self.t_list, self.sub_timesteps, self.sub_timesteps_tensor
             capi.check(self._lib.b2sd_set_timesteps(eng._handle, t.data_ptr(), self._stream()), "b2sd_set_timesteps")
         self.clear_overrides(prompt=False, t_index_list=True)
@@ -358,7 +401,12 @@ class StreamDiffusion:
             raise RuntimeError("apply_lora needs an engine built with live_lora=True (StreamDiffusionPipeline(live_lora=True) or "
                                "$B200SD_LIVE_LORA=1)")
         self._check()
-        factors = lora_factors(self._unet_shapes, lora_dict)
+        self.apply_factors(lora_factors(self._unet_shapes, lora_dict))
+
+    @torch.no_grad()
+    def apply_factors(self, factors) -> None:
+        """apply_lora with the factors weights.lora_factors made from a lora_dict (checked already).  On a style only the style's
+        engines are refreshed: the states stepped on it have their own prompt / t_index_list set again by whoever moves them."""
         keep = []   # the device factors stay referenced until the call has enqueued the work that reads them
         arr = (capi.LoraFactor * max(1, len(factors)))()
         for i, (key, up, down, scale) in enumerate(factors):
@@ -370,6 +418,8 @@ class StreamDiffusion:
         capi.check(self._lib.b2sd_apply_lora(self._handle, len(factors), arr, self._stream()), "b2sd_apply_lora")
         for eng in [self] + self.lanes:
             capi.check(self._lib.b2sd_refresh_conditioning(eng._handle, self._stream()), "b2sd_refresh_conditioning")
+        if self._is_style:
+            return
         for state in list(self._states):
             if state.closed:
                 continue

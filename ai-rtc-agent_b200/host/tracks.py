@@ -76,6 +76,12 @@ class VideoStreamTrack(_Base):
         if not self._stopped:
             self._target().update_t_index_list(t_index_list)
 
+    def update_lora(self, lora_dict) -> None:
+        """As update_prompt, for the style LoRAs ({safetensors path: scale}; None or {}: none): this viewer's own style with
+        per-peer streams (PeerStream.update_lora), else the pipeline's global one"""
+        if not self._stopped:
+            self._target().update_lora(lora_dict)
+
     async def _recv_source(self):
         try:
             return await self.track.recv()

@@ -263,6 +263,22 @@ int b2sd_apply_lora(b2sd_handle h, int n, const b2sd_lora_factor* f, void* strea
  * prompt embeddings and timesteps with the current parameters, on `stream`, without a host synchronisation */
 int b2sd_refresh_conditioning(b2sd_handle h, void* stream);
 
+/* Styles: one engine's UNet with its own LoRAs beside the parent's, sharing everything a UNet LoRA does not reach.
+ * b2sd_create_style makes an engine over a new weight store derived from parent's, which must be live and prepared
+ * (b2sd_set_live_params before its first b2sd_prepare).  The style reads the parent's base parameters in place (they are never
+ * written) and keeps the parent's store alive; it owns copies of the UNet matrices kernels read as loaded and the packed /
+ * fp32 entries derived from UNet matrices, and shares by pointer the VAE, ControlNet, HED and every other entry.  It has the
+ * parent's configuration and concurrency.  Prepare it and its lanes (b2sd_create_lane(style, ...)) like any engine, before its
+ * first b2sd_apply_lora, which then fuses LoRAs relative to the shared base.  A store and the styles derived from it form a
+ * family: a state of any of them may be stepped by an engine of any other (same batch and size), but a state's own prompt /
+ * timesteps are bound only on engines of the store they were computed on (set them again after a move).
+ * The style's memory is allocated and freed stream-ordered, from a pool of its own that never makes an allocation wait for a
+ * free on another stream, on a stream of its own: nothing about it synchronises the device or waits for other engines' work.
+ * Free its engines with b2sd_release(h, stream), whose frees run after the work queued on `stream` at the call (make it wait
+ * for the last frames of every engine of the style first); the store goes with its last engine. */
+int b2sd_create_style(b2sd_handle parent, b2sd_handle* out);
+int b2sd_release(b2sd_handle h, void* stream);
+
 /* Packed-weight blob: the kernel-native layouts b2sd_prepare derives from the parameters (reordered convolution
  * matrices, per-head q/k/v gathers, GEGLU interleave, fused bias vectors), written once and loaded instead of
  * b2sd_load_tensor + repacking.  Replaces the reference's cached TensorRT engine files `engines--<model>/...engine`

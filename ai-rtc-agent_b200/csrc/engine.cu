@@ -472,23 +472,17 @@ struct b2sd_engine {
     int launches = 0;
     std::string cur;   // name prefix of the layer being built (debug / profiling labels)
     bool allow_swap = false;  // builders enable the swapped GEMM orientation for UNet contractions (never TAESD / V^T / GEGLU)
-    cudaGraphExec_t graph_exec = nullptr;
-    cudaGraph_t graph = nullptr;
     // Stepping a stream state (b2sd_step_state): the frame program is cut into [encoder body | last encoder conv + UNet +
-    // scheduler step | decoder], three CUDA graphs captured on first use.  Only the middle stage reads and writes slots 1.. of
-    // x_in, so the state is copied in before it and out after it, and steps of one state chain through the state's event.
-    // An engine of a b2sd_share_stream_state pair steps pair_state (created by the owner, shared with the lane) every frame.
-    std::shared_ptr<b2sd_state> pair_state;
+    // scheduler step | decoder].  Only the middle stage reads and writes slots 1.. of x_in, so the state is copied in before it
+    // and out after it, and steps of one state chain through the state's event.
     size_t idx_enc_end = 0, idx_unet_end = 0;          // stage boundaries inside prog_frame
-    cudaGraphExec_t stage_exec[3] = {nullptr, nullptr, nullptr};
-    cudaGraph_t stage_graph[3] = {nullptr, nullptr, nullptr};
+    // the CUDA graph of each program range run_frame is called with, captured on first use: GRAPH_WHOLE is all of prog_frame
+    // (b2sd_step_ex), GRAPH_STAGE + i the i-th stage of a state's step
+    enum { GRAPH_WHOLE = 0, GRAPH_STAGE = 1, NUM_GRAPHS = 4 };
+    cudaGraphExec_t graph_exec[NUM_GRAPHS] = {};
     void drop_graphs() {
-        if (graph_exec) { cudaGraphExecDestroy(graph_exec); graph_exec = nullptr; }
-        if (graph) { cudaGraphDestroy(graph); graph = nullptr; }
-        for (int i = 0; i < 3; ++i) {
-            if (stage_exec[i]) { cudaGraphExecDestroy(stage_exec[i]); stage_exec[i] = nullptr; }
-            if (stage_graph[i]) { cudaGraphDestroy(stage_graph[i]); stage_graph[i] = nullptr; }
-        }
+        for (auto& g : graph_exec)
+            if (g) { cudaGraphExecDestroy(g); g = nullptr; }
     }
 
     ~b2sd_engine() { drop_graphs(); }
@@ -877,31 +871,27 @@ struct b2sd_engine {
     int build_transformer(const std::string& p, const Act& x, int heads, Act* out, cudaStream_t s);
     int build_taesd_block(const std::string& p, const Act& x, Act* out, cudaStream_t s);
     int build_program(cudaStream_t s);
-    int run_range(std::vector<Op>& ops, size_t a, size_t b, cudaStream_t s) {
-        for (size_t i = a; i < b && i < ops.size(); ++i) TRY(ops[i](s));
-        return 0;
-    }
-    int run(std::vector<Op>& ops, cudaStream_t s) {
+    // ops[a, b) on s
+    int run(std::vector<Op>& ops, cudaStream_t s, size_t a = 0, size_t b = SIZE_MAX) {
         static const bool dbg = getenv("B200SD_DEBUG_SYNC") != nullptr;
         static const char* skip = getenv("B200SD_SKIP");  // debug: "groupnorm,attn" drops those launches (timing only)
         static const char* skip_name = getenv("B200SD_SKIP_NAME");  // debug: drop launches whose label contains this substring
-        int idx = 0;
-        for (auto& op : ops) {
+        for (size_t idx = a; idx < b && idx < ops.size(); ++idx) {
+            Op& op = ops[idx];
             if (skip) {
                 const std::string kind = op.name.substr(0, op.name.find(' '));
-                if (!kind.empty() && std::string(skip).find(kind) != std::string::npos) { ++idx; continue; }
+                if (!kind.empty() && std::string(skip).find(kind) != std::string::npos) continue;
             }
-            if (skip_name && op.name.find(skip_name) != std::string::npos) { ++idx; continue; }
+            if (skip_name && op.name.find(skip_name) != std::string::npos) continue;
             TRY(op(s));
             if (dbg) {
                 cudaError_t e = cudaStreamSynchronize(s);
                 if (e != cudaSuccess) {
-                    b2_set_error("op %d '%s' failed: %s", idx, op.name.c_str(), cudaGetErrorString(e));
-                    fprintf(stderr, "b2sd: op %d '%s' failed: %s\n", idx, op.name.c_str(), cudaGetErrorString(e));
+                    b2_set_error("op %zu '%s' failed: %s", idx, op.name.c_str(), cudaGetErrorString(e));
+                    fprintf(stderr, "b2sd: op %zu '%s' failed: %s\n", idx, op.name.c_str(), cudaGetErrorString(e));
                     return -1;
                 }
             }
-            ++idx;
         }
         return 0;
     }
@@ -2308,7 +2298,7 @@ static int time_embedding_ops(b2sd_handle h, std::vector<Op>* ops) {
 static int refresh_time(b2sd_handle h, cudaStream_t s) {
     std::vector<Op> ops;
     TRY(time_embedding_ops(h, &ops));
-    TRY(h->run_range(ops, 0, ops.size(), s));
+    TRY(h->run(ops, s));
     return h->run(h->prog_time, s);
 }
 
@@ -2365,7 +2355,6 @@ int b2sd_prepare(b2sd_handle h, const void* prompt_embeds, const float* timestep
     }
     // x_t_latent_buffer = zeros (StreamDiffusion.prepare); slot 0 is overwritten by every frame
     CUDA_OK(cudaMemsetAsync(h->x_in.p, 0, (size_t)h->x_in.elems() * 2, s));
-    if (h->pair_state) TRY(state_reset(h->pair_state.get(), s));
     for (auto& c : h->ws->pending)   // a style's own UNet matrices start as the base values, before anything packs them
         CUDA_OK(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToDevice, s));
     h->ws->pending.clear();
@@ -2869,10 +2858,6 @@ static int check_state(const char* fn, b2sd_handle h, const b2sd_state* state) {
         b2_set_error("%s: null argument, or b2sd_prepare not called", fn);
         return -1;
     }
-    if (h->pair_state) {
-        b2_set_error("%s: the engine is part of a b2sd_share_stream_state pair, which steps its own state", fn);
-        return -1;
-    }
     if (state->family != h->ws->family || state->batch != h->cfg.batch || state->height != h->cfg.height ||
         state->width != h->cfg.width) {
         b2_set_error("%s: the state was made for another weight store, batch or size (state: batch %d, %dx%d; "
@@ -2928,21 +2913,68 @@ int b2sd_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* fra
     return b2sd_step_ex(h, frame_in, B2SD_IN_U8_NHWC, in_h, in_w, frame_out, B2SD_OUT_U8_NCHW, stream);
 }
 
-// the input heads of a frame: the encoder head, and the ControlNet / HED head that reads the frame
-static int step_heads(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int in_w, cudaStream_t s) {
-    SmallConvArgs a = h->head;
-    a.x = frame_in; a.in_h = in_h; a.in_w = in_w;
+// The input heads of a frame, in launch order: the encoder head, and with a ControlNet the head that reads the frame as the
+// control image -- the frame itself in [0, 1] at the engine's size (same nearest resize), or HED's edge map, whose first conv
+// reads the frame here and whose remaining layers run in stage 1
+struct InputHeads {
+    SmallConvArgs conv[2];
+    const char* label[2];
+    int n = 0;
+};
+
+static InputHeads input_heads(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int in_w) {
     const int in_flags = in_kind == B2SD_IN_U8_NHWC ? SC_IN_U8 : (in_kind == B2SD_IN_F32_NCHW ? SC_IN_F32_NCHW : SC_IN_F16_NCHW);
-    a.flags = in_flags | (h->head.flags & SC_IN_OFFSET);   // AutoencoderKL: 2x - 1 as the offset input mode
-    TRY(smallconv_launch(a, s));
-    if (h->cfg.controlnet) {   // the control image is the frame itself in [0, 1], at the engine's size (same nearest resize)
-        // the control image is the frame itself in [0, 1] at the engine's size (same nearest resize), or HED's edge map, whose
-        // first conv reads the frame here and whose remaining layers run in stage 1
+    InputHeads in;
+    in.conv[0] = h->head;
+    in.conv[0].flags = in_flags | (h->head.flags & SC_IN_OFFSET);   // AutoencoderKL: 2x - 1 as the offset input mode
+    in.label[0] = "smallconv head";
+    in.n = 1;
+    if (h->cfg.controlnet) {
         const bool hed = h->cfg.control_processor == B2SD_CONTROL_HED;
-        SmallConvArgs c = hed ? h->hed_head : h->cn_head;
-        c.x = frame_in; c.in_h = in_h; c.in_w = in_w; c.flags = in_flags | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
-        TRY(smallconv_launch(c, s));
+        in.conv[1] = hed ? h->hed_head : h->cn_head;
+        in.conv[1].flags = in_flags | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
+        in.label[1] = hed ? "smallconv hed head" : "smallconv controlnet head";
+        in.n = 2;
     }
+    for (int i = 0; i < in.n; ++i) {
+        in.conv[i].x = frame_in; in.conv[i].in_h = in_h; in.conv[i].in_w = in_w;
+    }
+    return in;
+}
+
+static int step_heads(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int in_w, cudaStream_t s) {
+    const InputHeads in = input_heads(h, frame_in, in_kind, in_h, in_w);
+    for (int i = 0; i < in.n; ++i) TRY(smallconv_launch(in.conv[i], s));
+    return 0;
+}
+
+// prog_frame[a, b) on s: with use_cuda_graph as the CUDA graph h->graph_exec[slot], captured and instantiated on first use
+static int run_frame(b2sd_handle h, int slot, size_t a, size_t b, cudaStream_t s) {
+    if (!h->cfg.use_cuda_graph) return h->run(h->prog_frame, s, a, b);
+    cudaGraphExec_t& exec = h->graph_exec[slot];
+    if (!exec) {
+        cudaStream_t cs;   // the caller's stream may be the legacy default stream, which cannot capture
+        CUDA_OK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+        CUDA_OK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
+        const int rc = h->run(h->prog_frame, cs, a, b);
+        cudaGraph_t graph = nullptr;
+        const cudaError_t ec = cudaStreamEndCapture(cs, &graph);
+        cudaStreamDestroy(cs);
+        const bool ok = !rc && ec == cudaSuccess && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess;
+        if (graph) cudaGraphDestroy(graph);   // the executable graph does not need it
+        if (!ok) {
+            exec = nullptr;   // a failed capture must not leave a half-built graph behind
+            if (!rc) {
+                const char* why = cudaGetErrorString(ec != cudaSuccess ? ec : cudaGetLastError());
+                if (slot == b2sd_engine::GRAPH_WHOLE)
+                    b2_set_error("b2sd_step: CUDA graph capture / instantiation failed: %s", why);
+                else
+                    b2_set_error("b2sd_step: CUDA graph capture of stage %d failed: %s", slot - b2sd_engine::GRAPH_STAGE, why);
+            }
+            return -1;
+        }
+    }
+    CUDA_OK(cudaGraphLaunch(exec, s));
     return 0;
 }
 
@@ -2959,24 +2991,7 @@ static int step_stages(b2sd_handle h, b2sd_state* state, cudaStream_t s) {
             if (state->bytes) CUDA_OK(cudaMemcpyAsync(slots, state->buf, state->bytes, cudaMemcpyDeviceToDevice, s));
             TRY(bind_conditioning(h, state, s));
         }
-        if (h->cfg.use_cuda_graph) {
-            if (!h->stage_exec[st]) {
-                cudaStream_t cs;
-                CUDA_OK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-                CUDA_OK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-                int rc = h->run_range(h->prog_frame, cut[st], cut[st + 1], cs);
-                cudaError_t ec = cudaStreamEndCapture(cs, &h->stage_graph[st]);
-                cudaStreamDestroy(cs);
-                if (rc || ec != cudaSuccess || cudaGraphInstantiate(&h->stage_exec[st], h->stage_graph[st], 0) != cudaSuccess) {
-                    if (!rc) b2_set_error("b2sd_step: CUDA graph capture of stage %d failed: %s", st, cudaGetErrorString(ec != cudaSuccess ? ec : cudaGetLastError()));
-                    h->drop_graphs();
-                    return -1;
-                }
-            }
-            CUDA_OK(cudaGraphLaunch(h->stage_exec[st], s));
-        } else {
-            TRY(h->run_range(h->prog_frame, cut[st], cut[st + 1], s));
-        }
+        TRY(run_frame(h, b2sd_engine::GRAPH_STAGE + st, cut[st], cut[st + 1], s));
         if (st == 1) {
             if (state->bytes) CUDA_OK(cudaMemcpyAsync(state->buf, slots, state->bytes, cudaMemcpyDeviceToDevice, s));
             CUDA_OK(cudaEventRecord(state->done, s));
@@ -3004,31 +3019,8 @@ static int step_whole(b2sd_handle h, const b2sd_state* cond, const void* frame_i
     }
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     TRY(step_heads(h, frame_in, in_kind, in_h, in_w, s));
-    if (h->pair_state) {
-        TRY(step_stages(h, h->pair_state.get(), s));
-        return step_tail(h, frame_out, out_kind, s);
-    }
     TRY(bind_conditioning(h, cond, s));
-    if (h->cfg.use_cuda_graph) {
-        if (!h->graph_exec) {
-            cudaStream_t cs;
-            CUDA_OK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-            CUDA_OK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-            int rc = h->run(h->prog_frame, cs);
-            cudaError_t ec = cudaStreamEndCapture(cs, &h->graph);
-            cudaStreamDestroy(cs);
-            if (rc || ec != cudaSuccess || cudaGraphInstantiate(&h->graph_exec, h->graph, 0) != cudaSuccess) {
-                if (h->graph) cudaGraphDestroy(h->graph);   // a failed capture must not leave a half-built graph behind
-                h->graph = nullptr;
-                h->graph_exec = nullptr;
-                if (!rc) b2_set_error("b2sd_step: CUDA graph capture / instantiation failed: %s", cudaGetErrorString(ec != cudaSuccess ? ec : cudaGetLastError()));
-                return -1;
-            }
-        }
-        CUDA_OK(cudaGraphLaunch(h->graph_exec, s));
-    } else {
-        TRY(h->run(h->prog_frame, s));
-    }
+    TRY(run_frame(h, b2sd_engine::GRAPH_WHOLE, 0, h->prog_frame.size(), s));
     return step_tail(h, frame_out, out_kind, s);
 }
 
@@ -3040,10 +3032,6 @@ int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int
 int b2sd_state_create(b2sd_handle h, b2sd_state_handle* out, void* stream) {
     if (!h || !out || !h->built) {
         b2_set_error("b2sd_state_create: null argument, or b2sd_prepare not called");
-        return -1;
-    }
-    if (h->pair_state) {
-        b2_set_error("b2sd_state_create: the engine is part of a b2sd_share_stream_state pair, which steps its own state");
         return -1;
     }
     return state_new(h, reinterpret_cast<cudaStream_t>(stream), out);
@@ -3114,17 +3102,9 @@ int b2sd_profile(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* 
     std::vector<cudaEvent_t> ev(nops + 1);
     for (auto& e : ev) CUDA_OK(cudaEventCreate(&e));
     std::vector<double> acc(nops, 0.0);
-    SmallConvArgs a = h->head;
-    a.x = frame_in; a.in_h = in_h; a.in_w = in_w; a.flags = SC_IN_U8 | (h->head.flags & SC_IN_OFFSET);
     for (int it = 0; it < iters + 1; ++it) {  // first iteration is a warm-up
         CUDA_OK(cudaEventRecord(ev[0], s));
-        TRY(smallconv_launch(a, s));
-        if (h->cfg.controlnet) {
-            const bool hed = h->cfg.control_processor == B2SD_CONTROL_HED;
-            SmallConvArgs c = hed ? h->hed_head : h->cn_head;
-            c.x = frame_in; c.in_h = in_h; c.in_w = in_w; c.flags = SC_IN_U8 | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
-            TRY(smallconv_launch(c, s));
-        }
+        TRY(step_heads(h, frame_in, B2SD_IN_U8_NHWC, in_h, in_w, s));
         CUDA_OK(cudaEventRecord(ev[1], s));
         size_t i = 1;
         for (auto& op : h->prog_frame) {
@@ -3203,23 +3183,14 @@ int b2sd_audit_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, voi
         b2_set_error("b2sd_audit_step: bad arguments (or b2sd_prepare not called)");
         return -1;
     }
-    if (h->pair_state) {
-        b2_set_error("b2sd_audit_step: stage-pipelined lanes (b2sd_share_stream_state) are not supported");
-        return -1;
-    }
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     TRY(bind_conditioning(h, nullptr, s));   // the engine's own stream: its global conditioning
     Audited au{"b2sd_audit_step", fn, user, s};
     // the input heads and the tail as b2sd_step_ex launches them for a u8 frame, with the caller's frame and size
-    SmallConvArgs a = h->head;
-    a.x = frame_in; a.in_h = in_h; a.in_w = in_w; a.flags = SC_IN_U8 | (h->head.flags & SC_IN_OFFSET);
-    TRY(au.launch(smallconv_record(a), "smallconv head", [&] { return smallconv_launch(a, s); }));
-    if (h->cfg.controlnet) {
-        const bool hed = h->cfg.control_processor == B2SD_CONTROL_HED;
-        SmallConvArgs c = hed ? h->hed_head : h->cn_head;
-        c.x = frame_in; c.in_h = in_h; c.in_w = in_w; c.flags = SC_IN_U8 | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
-        TRY(au.launch(smallconv_record(c), hed ? "smallconv hed head" : "smallconv controlnet head",
-                      [&] { return smallconv_launch(c, s); }));
+    const InputHeads in = input_heads(h, frame_in, B2SD_IN_U8_NHWC, in_h, in_w);
+    for (int i = 0; i < in.n; ++i) {
+        const SmallConvArgs& a = in.conv[i];
+        TRY(au.launch(smallconv_record(a), in.label[i], [&] { return smallconv_launch(a, s); }));
     }
     TRY(au.program(h->prog_frame));
     uint8_t* out = static_cast<uint8_t*>(frame_out);
@@ -3322,27 +3293,6 @@ int b2sd_profile_kind(b2sd_handle h, const char* kind, int iters, double* ms_per
 }
 
 int b2sd_launches_per_step(b2sd_handle h) { return h ? h->launches : 0; }
-
-/* Make `lane` continue the SAME temporal stream as `owner` (both engines of one weight store, same batch and size): they
- * share the stream-batch state (x_t_latent_buffer) and are stage-pipelined -- while one lane runs the UNet stage of frame n,
- * the other runs the TAESD encoder body of frame n+1 / the decoder of frame n-1.  Frames must be submitted alternately, in
- * order, from one host thread.  Call before either engine's b2sd_prepare. */
-int b2sd_share_stream_state(b2sd_handle lane, b2sd_handle owner) {
-    if (!lane || !owner || lane == owner || lane->ws != owner->ws || lane->cfg.batch != owner->cfg.batch ||
-        lane->cfg.height != owner->cfg.height || lane->cfg.width != owner->cfg.width) {
-        b2_set_error("b2sd_share_stream_state: engines must be lanes of one weight store with the same batch and size");
-        return -1;
-    }
-    if (!owner->pair_state) {
-        b2sd_state* st = nullptr;
-        TRY(state_new(owner, nullptr, &st));
-        owner->pair_state = std::shared_ptr<b2sd_state>(st, [](b2sd_state* p) { state_free(p, nullptr); });
-    }
-    lane->pair_state = owner->pair_state;
-    lane->built = false;
-    owner->built = false;
-    return 0;
-}
 
 int b2sd_set_concurrency(b2sd_handle h, int frames_in_flight) {
     if (!h || frames_in_flight < 1) {

@@ -223,8 +223,6 @@ def lib() -> C.CDLL:
         _lib.b2sd_step_ex.argtypes = [vp, vp, ci, ci, ci, vp, ci, vp]
         _lib.b2sd_get_tensor.argtypes = [vp, C.c_char_p, vp, i64, C.POINTER(i64), C.POINTER(ci), vp]
         _lib.b2sd_launches_per_step.argtypes = [vp]
-        _lib.b2sd_share_stream_state.argtypes = [vp, vp]
-        _lib.b2sd_share_stream_state.restype = C.c_int
         _lib.b2sd_set_concurrency.argtypes = [vp, ci]
         _lib.b2sd_set_concurrency.restype = C.c_int
         _lib.b2sd_state_create.argtypes = [vp, C.POINTER(vp), vp]

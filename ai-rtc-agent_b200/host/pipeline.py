@@ -29,14 +29,13 @@ DEFAULT_NUM_INFERENCE_STEPS = 50
 DEFAULT_GUIDANCE_SCALE = 0.0
 DEFAULT_LANES_ONE_STEP = 8    # frames in flight for a 1-step stream batch (measured with the throughput launch policy: 4 -> 409, 6 -> 470,
                               # 8 -> 483, 10 -> 481, 12 -> 486 fps; p50 submit -> result 10.4 / 13.5 / 16.8 / 17.8 / 18.7 ms; lanes=1: 241 fps, 4.2 ms)
-DEFAULT_LANES_STATEFUL = 2    # T > 1: stage pipelining over two lanes that share the stream-batch state
-DEFAULT_LANES_PER_PEER = 2    # T > 1 with per-peer streams: independent lanes, any of which steps any peer's state (SD-1.5 T=4
-                              # 512x512, tools/bench_peers.py: 2 lanes 47.0 / 54.3 fps at 1 / 2+ peers, p50 42.5 / 36.8 ms; 3 lanes
-                              # 47.1 / 56.1 fps at 1 / 4+ peers but p50 63.7 / 53.4 ms and 3 GB more; 4 lanes no faster)
+DEFAULT_LANES_STATEFUL = 2    # T > 1: lanes stage-pipeline each stream state they step (SD-1.5 T=4 512x512, tools/bench_peers.py:
+                              # 2 lanes 47.0 / 54.3 fps at 1 / 2+ peers, p50 42.5 / 36.8 ms; 3 lanes 47.1 / 56.1 fps at 1 / 4+
+                              # peers but p50 63.7 / 53.4 ms and 3 GB more; 4 lanes no faster)
 PER_PEER_STREAMS_ENV = "B200SD_PER_PEER_STREAMS"
 MAX_STYLES_ENV = "B200SD_MAX_STYLES"
 DEFAULT_MAX_STYLES = 4        # viewers' own styles held at once (PeerStream.update_lora); each holds a UNet copy and its lanes
-STYLE_LANES = DEFAULT_LANES_PER_PEER   # lanes of each such style
+STYLE_LANES = DEFAULT_LANES_STATEFUL   # lanes of each such style
 
 
 def env_flag(name: str) -> bool:
@@ -101,7 +100,7 @@ class _Style:
 
 class StreamDiffusionPipeline:
     per_peer_streams = False
-    _own_state = None   # the StreamState enqueue() steps with per-peer streams; None: the engines' own shared state
+    _own_state = None   # the StreamState enqueue() steps (per-peer streams, or T > 1 on several lanes); None: the engines' own
     _lora = None        # the global lora_dict (update_lora)
     _lora_key = ()      # its style_key
 
@@ -110,15 +109,15 @@ class StreamDiffusionPipeline:
                  live_lora: Optional[bool] = None):
         """lanes: frames in flight for enqueue() ($B200SD_LANES overrides the default).  With a 1-step stream batch (SD-Turbo)
         consecutive frames are independent: DEFAULT_LANES_ONE_STEP lanes process frame n+1.. while frame n is still on the GPU.
-        With T > 1 the stream batch carries state from frame to frame: two lanes share that state and are stage-pipelined (TAESD
-        encoder of frame n+1 and decoder of frame n-1 overlap the UNet of frame n).  Both are bit-identical to submitting the
-        same frames one at a time.
+        With T > 1 the stream batch carries state from frame to frame: the pipeline's stream is then a stream state that two lanes
+        step in turn, stage-pipelined (TAESD encoder of frame n+1 and decoder of frame n-1 overlap the UNet of frame n).  Both
+        are bit-identical to submitting the same frames one at a time.
 
         per_peer_streams (None: $B200SD_PER_PEER_STREAMS, default off): one pipeline serves several viewers, each with its own
         temporal stream.  open_stream() gives a viewer a PeerStream whose frames carry that viewer's stream-batch state only;
-        pipeline(frame) / enqueue(frame) keep stepping the pipeline's own stream.  The lanes are then independent
-        (DEFAULT_LANES_PER_PEER for T > 1) and any lane steps any viewer's state.  Off, every caller of the pipeline shares one
-        temporal stream, as in the reference: with T > 1 a frame's output then mixes in frames of the other callers.
+        pipeline(frame) / enqueue(frame) keep stepping the pipeline's own stream.  Any lane steps any viewer's state
+        (DEFAULT_LANES_STATEFUL lanes for T > 1).  Off, every caller of the pipeline shares one temporal stream, as in the
+        reference: with T > 1 a frame's output then mixes in frames of the other callers.
 
         live_lora (None: $B200SD_LIVE_LORA, default off): update_lora() switches style LoRAs while the pipeline runs.  The base
         weights stay on the device (more HBM, see README), and the packed-weight blob is neither read nor written."""
@@ -151,21 +150,20 @@ class StreamDiffusionPipeline:
             engine_dir=os.getenv("TRT_ENGINES_CACHE", "./models/engines"),
         )
         stateful = len(self.t_index_list) > 1     # x_t_latent_buffer chains frame n+1 to frame n
-        shared = stateful and not self.per_peer_streams   # lanes stage-pipeline one shared stream-batch state
         if lanes is None:
-            default = (DEFAULT_LANES_PER_PEER if self.per_peer_streams else DEFAULT_LANES_STATEFUL) if stateful else DEFAULT_LANES_ONE_STEP
-            lanes = int(os.getenv("B200SD_LANES", "0")) or default
-        if shared:
-            lanes = min(lanes, 2)   # three stages, the middle one serial: a third lane has nothing to overlap
+            lanes = int(os.getenv("B200SD_LANES", "0")) or (DEFAULT_LANES_STATEFUL if stateful else DEFAULT_LANES_ONE_STEP)
+        if stateful and not self.per_peer_streams:
+            lanes = min(lanes, 2)   # one stream in three stages, the middle one serial: a third lane has nothing to overlap
         # launch policy = number of frames in flight ($B200SD_POLICY_FRAMES overrides it for profiling: a single lane running the
         # throughput policy's launches gives ncu a clean one-frame launch list)
         self.model.stream.set_concurrency(max(1, int(os.environ.get("B200SD_POLICY_FRAMES", lanes))))
         self.model.prepare(prompt=self.prompt, num_inference_steps=DEFAULT_NUM_INFERENCE_STEPS,
                            guidance_scale=DEFAULT_GUIDANCE_SCALE)
         sd = self.model.stream
-        self._engines = [sd] + [sd.add_lane(share_state=shared) for _ in range(max(1, lanes) - 1)]
-        # per-peer mode: enqueue() steps this state, so the pipeline's own stream is one more peer of the lane pool
-        self._own_state = sd.new_state() if self.per_peer_streams else None
+        self._engines = [sd] + [sd.add_lane() for _ in range(max(1, lanes) - 1)]
+        # enqueue() steps this state: lanes take turns on one T > 1 stream, or the pipeline's stream is one more peer of the pool
+        if self.per_peer_streams or (stateful and len(self._engines) > 1):
+            self._own_state = sd.new_state()
         # one lane: frames run on the caller's stream, exactly as before.  Several lanes: every lane has its own stream (a lane on
         # the caller's stream would order the other lanes' "input ready" events behind its frames and serialise them)
         self._lane_streams = [None] if len(self._engines) == 1 else [torch.cuda.Stream(sd.device) for _ in self._engines]
@@ -388,7 +386,7 @@ class StreamDiffusionPipeline:
         return self._enqueue(frame, self._own_state)
 
     def _enqueue(self, frame, state, pool=None) -> "FrameTicket":
-        """enqueue() on `state` (a StreamState, or None for the engines' own shared stream) on the lanes of `pool` (a viewer's
+        """enqueue() on `state` (a StreamState, or None for the engines' own stream) on the lanes of `pool` (a viewer's
         style, default the pipeline's).  Lanes rotate over all submissions to the pool; frames of one state are ordered on the
         device by the state's event."""
         if not _is_gpu_frame(frame) and not _is_video_frame(frame):

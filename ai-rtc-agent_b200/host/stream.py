@@ -285,18 +285,14 @@ class StreamDiffusion:
         self.t_list = list(other.t_list)
         self._engine_prepare()
 
-    def add_lane(self, share_state: bool = False) -> "StreamDiffusion":
+    def add_lane(self) -> "StreamDiffusion":
         """Another engine over the same weights, prepared identically (same prompt embedding, schedule and seed-2 noise):
         frames may be alternated between this engine and its lanes on different CUDA streams.  Later prepare() /
-        update_prompt() / timestep updates on this object reach every lane.
-        share_state=False: the lane is an independent temporal stream (or, for a 1-step stream batch, simply the next frame).
-        share_state=True: the lane continues THIS stream -- it shares the stream-batch state and is stage-pipelined with it
-        (b2sd_share_stream_state): required for T > 1, where frame n+1 needs frame n's x_t_latent_buffer."""
+        update_prompt() / timestep updates on this object reach every lane.  Stepped without a state, the lane is an
+        independent temporal stream (or, for a 1-step stream batch, simply the next frame); to continue one stream with T > 1
+        on several lanes, step one new_state() on each in turn."""
         self._check()
         lane = StreamDiffusion(self.arch, {}, {}, self.t_list, self.prompt_encoder, parent=self, **self._ctor)
-        if share_state:
-            capi.check(self._lib.b2sd_share_stream_state(lane._handle, self._handle), "b2sd_share_stream_state")
-            self._engine_prepare()          # the owner's frame program is rebuilt as three stages (packed weights are cached)
         lane._prepare_like(self)
         self.lanes.append(lane)
         return lane
@@ -332,7 +328,7 @@ class StreamDiffusion:
 
     def new_state(self) -> "StreamState":
         """A fresh temporal stream (zeroed x_t_latent_buffer) that this engine and every lane of its weights can step:
-        pass it as `state=` to step_u8 / step_u8_into / __call__.  prepare() resets it.  Not for share_state lanes."""
+        pass it as `state=` to step_u8 / step_u8_into / __call__.  prepare() resets it."""
         self._check()
         state = StreamState(self)
         self._states.add(state)

@@ -437,20 +437,15 @@ int b2sd_audit_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, voi
  * b2sd_audit_step; index counts the refresh's kernel launches.  It recomputes what b2sd_prepare computed from the same inputs. */
 int b2sd_audit_refresh(b2sd_handle h, b2sd_audit_fn fn, void* user, void* stream);
 
-/* Stage pipelining of ONE stateful stream (stream batch T > 1, where frame n+1 needs frame n's latent buffer and lanes cannot
- * simply alternate): `lane` shares `owner`'s stream-batch state; the frame program of each is cut into TAESD encoder body |
- * last encoder conv + UNet + scheduler step | TAESD decoder, and only the middle stage is serialised between the lanes (one
- * CUDA event), so the encoder of frame n+1 and the decoder of frame n-1 overlap the UNet of frame n.  Both engines must be
- * lanes of one weight store with equal batch / size; call before b2sd_prepare; submit frames alternately, in order.
- * Both engines then step one stream state (b2sd_state_*) that `owner` creates; b2sd_prepare of either zeroes it. */
-int b2sd_share_stream_state(b2sd_handle lane, b2sd_handle owner);
-
 /* Stream states: the stream-batch state of one temporal stream (x_t_latent_buffer, slots 1 .. T-1 of the UNet input batch,
  * (T-1) * (h/8) * (w/8) * 4 fp16 values; nothing at T = 1) kept apart from the engines that step it.  Any engine of the
  * state's weight store with the state's batch and size can step it, so several video streams (one state each) share a pool
  * of lanes: frames of different states overlap completely, and consecutive frames of one state are stage-pipelined across
- * lanes as with b2sd_share_stream_state.  A state carries one CUDA event that orders its steps; submit the frames of one
- * state in order from one host thread.  Engines that are part of a b2sd_share_stream_state pair refuse these calls. */
+ * lanes -- the frame program is cut into encoder body | last encoder conv + UNet + scheduler step | decoder, and only the
+ * middle stage is serialised per state, so the encoder of frame n+1 and the decoder of frame n-1 overlap the UNet of frame n.
+ * This is how one stateful stream (T > 1, where frame n+1 needs frame n's latent buffer) runs on several lanes: step one
+ * state on each in turn.  A state carries one CUDA event that orders its steps; submit the frames of one state in order from
+ * one host thread. */
 typedef struct b2sd_state* b2sd_state_handle;
 /* a zeroed state sized for h's batch and size (h prepared); allocated stream-ordered on `stream` */
 int b2sd_state_create(b2sd_handle h, b2sd_state_handle* out, void* stream);
@@ -473,10 +468,9 @@ int b2sd_step_state(b2sd_handle h, b2sd_state_handle state, const void* frame_in
  * b2sd_set_prompt_embeds / b2sd_set_timesteps) -- with one device-to-device copy when it holds something else; so lanes whose
  * states never override copy nothing.  b2sd_step_ex and the other calls without a state use the global values.
  * An override is immutable: an update makes a new one, and the one it replaces is freed after the last step that copies it.
- * The calls refuse what b2sd_step_state refuses (null handles, a state of another store / batch / size, an engine of a
- * b2sd_share_stream_state pair, an unprepared engine).  A state's bookkeeping is host state without a lock: calls that take
- * one state (b2sd_step_state and the three below) must not run concurrently, from whichever engine or thread; calls on
- * different states may.  The overrides of a weight store's states share a memory pool that keeps a few blocks' worth of
+ * The calls refuse what b2sd_step_state refuses (null handles, a state of another store / batch / size, an unprepared
+ * engine).  A state's bookkeeping is host state without a lock: calls that take one state (b2sd_step_state and the three
+ * below) must not run concurrently, from whichever engine or thread; calls on different states may.  The overrides of a weight store's states share a memory pool that keeps a few blocks' worth of
  * memory across synchronisations; it is released when the last engine of the store and the last override are gone. */
 /* Compute `state`'s prompt block from embeddings in DEVICE memory, fp16 [ctx_tokens][cross_attention_dim], on engine h (any
  * engine that may step the state), stream-ordered on `stream` after the frames queued there, without a host synchronisation.

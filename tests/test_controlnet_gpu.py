@@ -314,9 +314,9 @@ def test_zero_initialised_controlnet_is_bit_identical(cuda):
         assert torch.equal(plain.step_u8(f).cpu(), cnz.step_u8(f).cpu()), f"frame {i}"
 
 
-def test_controlnet_lanes_are_bit_identical(cuda):
-    """Two stage-pipelined lanes of one T=4 stream equal a single engine bit for bit; four independent T=1 lanes under the
-    throughput policy equal their parent processing the same frames one after another."""
+def test_controlnet_lanes_stepping_one_state_are_bit_identical(cuda):
+    """One T=4 stream state stepped alternately on two lanes (stage-pipelined) equals a single engine bit for bit; four
+    independent T=1 lanes under the throughput policy equal their parent processing the same frames one after another."""
     from oracle import controlnet as ocn
     from oracle import unet as ounet
     from oracle import weights as ow
@@ -326,11 +326,12 @@ def test_controlnet_lanes_are_bit_identical(cuda):
     # a lane runs the launch policy of two frames in flight: the single engine uses the same one (same summation order)
     single, *_ = _engine(True, tl, 128, cn16, concurrency=2, hed=hed)
     owner, *_ = _engine(True, tl, 128, cn16, concurrency=2, hed=hed)
-    lane = owner.add_lane(share_state=True)
+    lane = owner.add_lane()
+    state = owner.new_state()
     for i in range(6):
         f = ow.make_frame(128, 128, seed=60 + i).to(cuda)
         a = single.step_u8(f).cpu()
-        b = (owner if i % 2 == 0 else lane).step_u8(f).cpu()
+        b = (owner if i % 2 == 0 else lane).step_u8(f, state=state).cpu()
         assert torch.equal(a, b), f"stage-pipelined frame {i}"
     par, *_ = _engine(True, [32], 128, cn16, concurrency=4, hed=hed)
     lanes = [par.add_lane() for _ in range(3)]

@@ -236,7 +236,7 @@ class FakeEngine:
     def set_concurrency(self, n):
         pass
 
-    def add_lane(self, share_state=False):
+    def add_lane(self):
         self.lanes.append(FakeEngine(self.log, len(self.lanes) + 1, self.states))
         return self.lanes[-1]
 

@@ -35,8 +35,8 @@ class FakeOut:
 class FakeEngine:
     """Stands for host.stream.StreamDiffusion: lanes share one log and one state counter, as lanes share one weight store."""
 
-    def __init__(self, log, lane=0, share_state=False, states=None):
-        self.log, self.lane, self.share_state = log, lane, share_state
+    def __init__(self, log, lane=0, states=None):
+        self.log, self.lane = log, lane
         self.states = [] if states is None else states
         self.lanes, self.concurrency = [], None
         self.device = "cpu"
@@ -44,8 +44,8 @@ class FakeEngine:
     def set_concurrency(self, n):
         self.concurrency = n
 
-    def add_lane(self, share_state=False):
-        lane = FakeEngine(self.log, len(self.lanes) + 1, share_state, self.states)
+    def add_lane(self):   # as StreamDiffusion.add_lane: every lane is an independent engine
+        lane = FakeEngine(self.log, len(self.lanes) + 1, self.states)
         self.lanes.append(lane)
         return lane
 
@@ -120,7 +120,7 @@ def fake_pipeline(monkeypatch):
 
 def test_lanes_rotate_over_every_submission(fake_pipeline):
     pipe, log = fake_pipeline([18, 26, 35, 45], per_peer_streams=True, lanes=3)
-    assert pipe.lanes == 3 and not any(e.share_state for e in pipe.model.stream.lanes), "per-peer lanes are independent"
+    assert pipe.lanes == 3
     a, b = pipe.open_stream(), pipe.open_stream()
     for i, who in enumerate([a, b, pipe, b, a, a, b]):
         who.enqueue(("f", i))
@@ -147,19 +147,25 @@ def test_each_peer_steps_its_own_state(fake_pipeline):
     assert sb.closed
 
 
-def test_open_stream_is_refused_when_the_mode_is_off(fake_pipeline):
+def test_mode_off_refuses_open_stream_and_lanes_step_one_own_state(fake_pipeline):
     pipe, log = fake_pipeline([18, 26, 35, 45], lanes=5)
     assert not pipe.per_peer_streams
-    assert pipe.lanes == 2 and all(e.share_state for e in pipe.model.stream.lanes), "shared mode: two stage-pipelined lanes"
+    assert pipe.lanes == 2, "one stream: two stage-pipelined lanes"
     with pytest.raises(RuntimeError, match="per_peer_streams"):
         pipe.open_stream()
-    pipe.enqueue(("f", 0))
-    assert log[0][1] is None and pipe.model.stream.states == [], "shared mode steps the engines' own state"
+    for i in range(4):
+        pipe.enqueue(("f", i))
+    states = pipe.model.stream.states
+    assert len(states) == 1, "the pipeline's own stream is one state"
+    assert [(lane, state) for lane, state, _ in log] == [(0, states[0]), (1, states[0])] * 2, \
+        "independent lanes step that state in turn"
+    for tl, lanes in (([18, 26, 35, 45], 1), ([32], 8)):
+        assert fake_pipeline(tl, lanes=lanes)[0]._own_state is None, "one lane, or T = 1: the engines' own latent buffers"
 
 
-def test_lane_defaults(fake_pipeline):
+def test_lane_default_for_each_stream_batch(fake_pipeline):
     from ai_rtc_agent_b200.host import pipeline as P
-    assert fake_pipeline([18, 26, 35, 45], per_peer_streams=True)[0].lanes == P.DEFAULT_LANES_PER_PEER
+    assert fake_pipeline([18, 26, 35, 45], per_peer_streams=True)[0].lanes == P.DEFAULT_LANES_STATEFUL
     assert fake_pipeline([18, 26, 35, 45])[0].lanes == P.DEFAULT_LANES_STATEFUL
     assert fake_pipeline([32], per_peer_streams=True)[0].lanes == P.DEFAULT_LANES_ONE_STEP
     assert fake_pipeline([32])[0].lanes == P.DEFAULT_LANES_ONE_STEP

@@ -250,27 +250,29 @@ def test_global_updates_reach_every_peer_at_the_matching_point(cuda, monkeypatch
 
 
 def test_prepare_resets_every_state(cuda, monkeypatch):
-    pool, ded = _pipelines("tiny-sd15", T4, 128, [dict(per_peer_streams=True, lanes=2), dict(lanes=1, policy=2)], monkeypatch)
-    frames = _frames(2, {0: 6, 1: 6}, 128, 128, base=600)
-    a, b = pool.open_stream(), pool.open_stream()
-    for i in range(3):
-        a.enqueue(frames[0][i])
-        b.enqueue(frames[1][i])
-        pool.enqueue(frames[0][i])
-    _fresh(pool)                                      # StreamDiffusion.prepare under the pipeline: every live state restarts
-    got = {0: [a.enqueue(f) for f in frames[0][3:]], 1: [b.enqueue(f) for f in frames[1][3:]],
-           2: [pool.enqueue(f) for f in frames[0][3:]]}
-    got = {p: [t.result().cpu() for t in ts] for p, ts in got.items()}
-    want = _dedicated(ded, {0: frames[0][3:], 1: frames[1][3:]})
-    want[2] = want[0]
-    _assert_equal(got, want, "after prepare")
-    a.close()
-    b.close()
+    """prepare() restarts every live state: the peers' and the pipeline's own, which is a state on two lanes with per-peer
+    streams on and off."""
+    for per_peer in (True, False):
+        pool, ded = _pipelines("tiny-sd15", T4, 128, [dict(per_peer_streams=per_peer, lanes=2), dict(lanes=1, policy=2)],
+                               monkeypatch)
+        assert pool._own_state is not None
+        frames = _frames(2, {0: 6, 1: 6}, 128, 128, base=600)
+        frames[2] = frames[0]                         # the pipeline's own stream
+        targets = {0: pool.open_stream(), 1: pool.open_stream()} if per_peer else {}
+        targets[2] = pool
+        for i in range(3):
+            for p, target in targets.items():
+                target.enqueue(frames[p][i])
+        _fresh(pool)                                  # StreamDiffusion.prepare under the pipeline: every live state restarts
+        got = {p: [target.enqueue(f) for f in frames[p][3:]] for p, target in targets.items()}
+        got = {p: [t.result().cpu() for t in ts] for p, ts in got.items()}
+        _assert_equal(got, _dedicated(ded, {p: frames[p][3:] for p in targets}), f"after prepare, per_peer={per_peer}")
+        for p in targets.keys() - {2}:
+            targets[p].close()
 
 
-def test_refusals(cuda):
-    """A state runs only on engines of its weight store, batch and size; never on a b2sd_share_stream_state pair; and the
-    engine must be prepared."""
+def test_state_refusals(cuda):
+    """A state runs only on engines of its weight store, batch and size, and the engine must be prepared."""
     import ctypes as C
     from ai_rtc_agent_b200.host import arch as A
     from ai_rtc_agent_b200.host import capi
@@ -295,16 +297,6 @@ def test_refusals(cuda):
     for eng in (other_store, other_size, other_batch):
         with pytest.raises(capi.B2Error, match="another weight store, batch or size"):
             eng.step_u8(frame, state=state)
-    owner = mk()
-    owner.prepare("p", guidance_scale=0.0)
-    paired = owner.add_lane(share_state=True)
-    free = owner.add_lane()
-    free_state = free.new_state()
-    with pytest.raises(capi.B2Error, match="share_stream_state pair"):
-        owner.new_state()
-    for eng in (owner, paired):
-        with pytest.raises(capi.B2Error, match="share_stream_state pair"):
-            eng.step_u8(frame, state=free_state)
     lib = capi.lib()
     raw = mk()                                        # never prepared
     h = C.c_void_p()
@@ -320,8 +312,8 @@ def test_refusals(cuda):
     torch.cuda.synchronize()
 
 
-def test_engines_release_device_memory_without_the_garbage_collector(cuda, monkeypatch):
-    """Engines, their lanes (independent or stage-pipelined), their stream states and a per-peer pipeline form no reference
+def test_engines_lanes_and_states_release_device_memory_without_the_garbage_collector(cuda, monkeypatch):
+    """Engines, their lanes (stepping a state alternately or not), their stream states and a per-peer pipeline form no reference
     cycle: dropping the last reference returns their device memory at once.  Otherwise it stays allocated until the garbage
     collector happens to run, and a process that builds pipelines one after another can run out of HBM."""
     from ai_rtc_agent_b200.host import arch as A
@@ -347,14 +339,16 @@ def test_engines_release_device_memory_without_the_garbage_collector(cuda, monke
         lane.step_u8(frame, state=state)
         owner = StreamDiffusion(A.TINY_SD15, usd, vsd, T4, lambda p: emb, width=512, height=512)
         owner.prepare("p", guidance_scale=0.0)
-        paired = owner.add_lane(share_state=True)
-        paired.step_u8(frame)
+        paired = owner.add_lane()
+        shared = owner.new_state()
+        owner.step_u8(frame, state=shared)
+        paired.step_u8(frame, state=shared)
         pool, = _pipelines("tiny-sd15", T4, 512, [dict(per_peer_streams=True, lanes=2)], monkeypatch)
         with pool.open_stream() as peer:
             peer.enqueue(frame).result()
         pool.enqueue(frame).result()
         used = free0 - free()
-        del root, lane, state, owner, paired, pool, peer
+        del root, lane, state, owner, paired, shared, pool, peer
         left = free0 - free()
     finally:
         gc.enable()

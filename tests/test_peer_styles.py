@@ -76,7 +76,7 @@ class FakeEngine:
     def set_concurrency(self, n):
         pass
 
-    def add_lane(self, share_state=False):
+    def add_lane(self):
         self.lanes.append(FakeEngine(self.log, f"{self.name}.{len(self.lanes) + 1}", self.states))
         self.lanes[-1].lora = self.lora
         return self.lanes[-1]

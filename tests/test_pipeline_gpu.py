@@ -210,10 +210,10 @@ def test_two_lanes_equal_sequential_processing(cuda, monkeypatch):
 
 @pytest.mark.parametrize("model_id,tl", [("tiny-turbo", [20, 40]), ("tiny-sd15", [18, 26, 35, 45])])
 def test_stateful_stream_stage_pipelined_over_two_lanes(cuda, monkeypatch, model_id, tl):
-    """T > 1: frame n+1 needs frame n's x_t_latent_buffer, so the two lanes SHARE the stream-batch state and only overlap the
-    TAESD encoder / decoder stages with the other lane's UNet stage (b2sd_share_stream_state).  Frames submitted back to back
-    must equal the same pipeline driven one frame at a time, track the oracle (incl. the T-1 frame output lag), and leave the
-    shared latent buffer in the oracle's state."""
+    """T > 1: frame n+1 needs frame n's x_t_latent_buffer, so the two lanes step the pipeline's one stream state in turn and
+    only overlap the TAESD encoder / decoder stages with the other lane's UNet stage.  Frames submitted back to back must
+    equal the same pipeline driven one frame at a time, track the oracle (incl. the T-1 frame output lag), and leave the
+    latent buffer in the oracle's state."""
     from oracle import pipeline as opipe
     from oracle import weights as ow
     seq, orc = _pipeline(model_id, tl, 128, monkeypatch, lanes=2)

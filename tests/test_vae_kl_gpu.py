@@ -270,17 +270,19 @@ def test_kl_float_entries_match_u8(cuda):
         assert (got.int() - u8.int()).abs().max().item() <= 1, f"{t.dtype} entry"
 
 
-def test_kl_lanes_are_bit_identical(cuda):
-    """Two stage-pipelined lanes of one T=4 stream equal a single engine bit for bit; eight independent T=1 lanes under the
-    throughput policy equal their parent processing the same frames one after another."""
+def test_kl_lanes_stepping_one_state_are_bit_identical(cuda):
+    """One T=4 stream state stepped alternately on two lanes (stage-pipelined) equals a single engine bit for bit; eight
+    independent T=1 lanes under the throughput policy equal their parent processing the same frames one after another."""
     from oracle import weights as ow
     tl = [18, 26, 35, 45]
     single, *_ = _engine(True, tl, 128, concurrency=2)
     owner, *_ = _engine(True, tl, 128, concurrency=2)
-    lane = owner.add_lane(share_state=True)
+    lane = owner.add_lane()
+    state = owner.new_state()
     for i in range(6):
         f = ow.make_frame(128, 128, seed=160 + i).to(cuda)
-        assert torch.equal(single.step_u8(f).cpu(), (owner if i % 2 == 0 else lane).step_u8(f).cpu()), f"stage-pipelined frame {i}"
+        got = (owner if i % 2 == 0 else lane).step_u8(f, state=state).cpu()
+        assert torch.equal(single.step_u8(f).cpu(), got), f"stage-pipelined frame {i}"
     par, *_ = _engine(True, [32], 128, concurrency=8)
     lanes = [par.add_lane() for _ in range(7)]
     frames = [ow.make_frame(128, 128, seed=170 + i).to(cuda) for i in range(8)]

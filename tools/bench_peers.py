@@ -132,8 +132,8 @@ def run_model(model: str, tl, args, info) -> dict:
 
     lane_counts = args.lanes if T > 1 else [None]
     if args.conditioning:
-        from ai_rtc_agent_b200.host.pipeline import DEFAULT_LANES_PER_PEER
-        pool, pool_mb = build(model, tl, True, (DEFAULT_LANES_PER_PEER if DEFAULT_LANES_PER_PEER in lane_counts else lane_counts[0])
+        from ai_rtc_agent_b200.host.pipeline import DEFAULT_LANES_STATEFUL
+        pool, pool_mb = build(model, tl, True, (DEFAULT_LANES_STATEFUL if DEFAULT_LANES_STATEFUL in lane_counts else lane_counts[0])
                               if T > 1 else None)
         for p in (p for p in args.peers if p >= 2):
             for r in range(args.repeats):
@@ -156,8 +156,8 @@ def run_model(model: str, tl, args, info) -> dict:
     pools = {}
     for lanes in lane_counts:
         pools[lanes] = build(model, tl, True, lanes)
-    from ai_rtc_agent_b200.host.pipeline import DEFAULT_LANES_PER_PEER
-    default = pools.get(DEFAULT_LANES_PER_PEER if T > 1 else None, next(iter(pools.values())))[0]
+    from ai_rtc_agent_b200.host.pipeline import DEFAULT_LANES_STATEFUL
+    default = pools.get(DEFAULT_LANES_STATEFUL if T > 1 else None, next(iter(pools.values())))[0]
     # one peer: shared mode and per-peer mode (default lanes) alternately
     for r in range(args.repeats):
         emit(dict(mode="shared", peers=1, lanes=shared.lanes, repeat=r, pool_mb=round(shared_mb), **measure(shared, 0, frames, args.frames, args.warmup)))

@@ -41,8 +41,18 @@ struct AttnParams {
     float scale_log2;
 };
 
-template <int DA, int BKV>
-__global__ void __launch_bounds__(AT_THREADS, 1) attn_kernel(const __grid_constant__ AttnParams p) {
+// attn_kernel<.., IP = true>: the decoupled image segment of an IP-Adapter cross-attention (AttnDesc::n_ip)
+struct AttnIpParams : AttnParams {
+    CUtensorMap tmk_ip, tmv_ip;
+    const int* n_ip;
+};
+
+// With IP, one more key block follows the text blocks through the same K / V^T rings: the image keys, with a softmax of their
+// own.  Its numerators are scaled by l_txt / l_ip before they become the A operand, so that the epilogue's division by l_txt
+// turns them into softmax(Q Kip^T) and O needs no second accumulator (P * l_txt / l_ip <= l_txt <= skv fits fp16).  n_ip = 0
+// skips the block: the result is then bit-identical to the kernel without IP.
+template <int DA, int BKV, bool IP = false>
+__global__ void __launch_bounds__(AT_THREADS, 1) attn_kernel(const __grid_constant__ std::conditional_t<IP, AttnIpParams, AttnParams> p) {
     constexpr int DP = DA * 64;
     constexpr int NST = AT_STAGES;
     constexpr int KVA = BKV / 64;                       // kv atoms per block (V^T tiles)
@@ -86,6 +96,8 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_kernel(const __grid_consta
     __syncthreads();
     pdl_launch_dependents();   // the next kernel may start its own prologue now
     pdl_wait();                // ... and everything below reads the previous kernel's output
+    int n_ip = 0;
+    if constexpr (IP) n_ip = *p.n_ip;
 
     if (warp == AT_CONS / 32) {
         if (lane == 0) {
@@ -112,12 +124,34 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_kernel(const __grid_consta
                 for (int a = 0; a < KVA; ++a)
                     tma_load_2d(sv + a * (DP * 128), &p.tmv, &v_full[st], (int)(b * p.vt_bstride) + j * BKV + a * 64, h * DP);
             };
+            // the image block: ring slot of block nblk, 64 keys (K atoms of [64 rows][128 B], one V^T atom)
+            auto load_k_ip = [&]() {
+                if constexpr (IP) {
+                    const int st = nblk % NST;
+                    mbar_wait(&k_empty[st], ((nblk / NST) & 1) ^ 1);
+                    uint8_t* sk = sKV + st * STAGE_BYTES;
+                    mbar_expect_tx(&k_full[st], DA * ATTN_IP_KEYS * 128);
+#pragma unroll
+                    for (int a = 0; a < DA; ++a)
+                        tma_load_2d(sk + a * (ATTN_IP_KEYS * 128), &p.tmk_ip, &k_full[st], h * DP + a * 64, 0);
+                }
+            };
+            auto load_v_ip = [&]() {
+                if constexpr (IP) {
+                    const int st = nblk % NST;
+                    mbar_wait(&v_empty[st], ((nblk / NST) & 1) ^ 1);
+                    mbar_expect_tx(&v_full[st], DP * 128);
+                    tma_load_2d(sKV + st * STAGE_BYTES + K_BYTES, &p.tmv_ip, &v_full[st], 0, h * DP);
+                }
+            };
             // issue order = the order in which slots become free: K(j+1) [after QK(j+1-NST)] before V(j) [after PV(j-NST)]
             load_k(0);
             for (int j = 0; j < nblk; ++j) {
                 if (j + 1 < nblk) load_k(j + 1);
+                else if (n_ip > 0) load_k_ip();
                 load_v(j);
             }
+            if (n_ip > 0) load_v_ip();
         }
     } else {
         // ===== consumer warpgroup wg: query rows [64 wg, 64 wg + 64) of the tile; this thread: rows rq and rq + 8 =====
@@ -207,6 +241,78 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_kernel(const __grid_consta
             wgmma_wait<0>();
             wgmma_fence_regs(o);
             if (lane == 0) mbar_arrive(&v_empty[st]);
+        }
+        if (n_ip > 0) {
+            // image segment: S2 = Q Kip^T (64 keys), its own softmax over the first n_ip, O += P2 * (l_txt / l2) Vip
+            const int st = nblk % NST;
+            const uint32_t ph = (uint32_t)(nblk / NST) & 1u;
+            const uint32_t sk = skv_addr + st * STAGE_BYTES;
+            float s[ATTN_IP_KEYS / 2];
+#pragma unroll
+            for (int i = 0; i < ATTN_IP_KEYS / 2; ++i) s[i] = 0.f;
+            mbar_wait(&k_full[st], ph);
+            wgmma_fence_regs(s);
+            wgmma_fence();
+#pragma unroll
+            for (int a = 0; a < DA; ++a) {
+                const uint64_t dq = make_kmajor_sw128_desc(sq_addr + a * (AT_BQ * 128));
+                const uint64_t dk = make_kmajor_sw128_desc(sk + a * (ATTN_IP_KEYS * 128));
+#pragma unroll
+                for (int k = 0; k < 4; ++k) Wgmma<ATTN_IP_KEYS>::ss(s, dq + 2 * k, dk + 2 * k, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(s);
+            float m2[2], f2[2];
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+                float mx = -INFINITY;
+#pragma unroll
+                for (int jj = 0; jj < ATTN_IP_KEYS / 8; ++jj)
+#pragma unroll
+                    for (int u = 0; u < 2; ++u)
+                        if (8 * jj + q2 + u < n_ip) mx = fmaxf(mx, s[4 * jj + 2 * hr + u]);
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                m2[hr] = mx * p.scale_log2;
+            }
+            float p2[ATTN_IP_KEYS / 2];
+            float rs[2] = {0.f, 0.f};
+#pragma unroll
+            for (int jj = 0; jj < ATTN_IP_KEYS / 8; ++jj)
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+                    for (int u = 0; u < 2; ++u) {
+                        float e = ex2_approx(s[4 * jj + 2 * hr + u] * p.scale_log2 - m2[hr]);
+                        if (8 * jj + q2 + u >= n_ip) e = 0.f;
+                        p2[4 * jj + 2 * hr + u] = e;
+                        rs[hr] += e;
+                    }
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+                float l = l_run[hr], l2 = rs[hr];   // row sums over the 4 lanes of the row, as the epilogue forms l_txt
+                l += __shfl_xor_sync(0xffffffffu, l, 1);
+                l += __shfl_xor_sync(0xffffffffu, l, 2);
+                l2 += __shfl_xor_sync(0xffffffffu, l2, 1);
+                l2 += __shfl_xor_sync(0xffffffffu, l2, 2);
+                f2[hr] = l / l2;
+            }
+            uint32_t pa[ATTN_IP_KEYS / 16][4];
+#pragma unroll
+            for (int jj = 0; jj < ATTN_IP_KEYS / 8; ++jj)
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr)
+                    pa[jj >> 1][(jj & 1) * 2 + hr] = pack_half2(p2[4 * jj + 2 * hr] * f2[hr], p2[4 * jj + 2 * hr + 1] * f2[hr]);
+            const uint32_t sv = sk + K_BYTES;
+            mbar_wait(&v_full[st], ph);
+            wgmma_fence_regs(o);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < ATTN_IP_KEYS / 16; ++kk) Wgmma<DP>::rs(o, pa[kk], make_kmajor_sw128_desc(sv) + 2 * kk, 1u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(o);
         }
         // epilogue: O / l -> fp16 -> global
 #pragma unroll
@@ -485,9 +591,25 @@ int attn_plan(const AttnDesc& d, AttnPlan* plan) {
     if (encode_2d(&plan->tmq, d.q, (long)d.heads * d.dp, (long)d.nb * d.sq, d.ldq, 64, AT_BQ, "q")) return -1;
     if (encode_2d(&plan->tmk, d.k, (long)d.heads * d.dp, d.k_rows, d.ldk, 64, bkv, "k")) return -1;
     if (encode_2d(&plan->tmv, d.vt, d.vt_cols, (long)d.heads * d.dp, d.ldvt, 64, d.dp, "vt")) return -1;
+    if (d.n_ip || d.k_ip || d.vt_ip) {
+        const auto misaligned = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) != 0; };
+        if (!d.n_ip || !d.k_ip || !d.vt_ip || misaligned(d.k_ip) || misaligned(d.vt_ip)) {
+            b2_set_error("attn: the image segment needs k_ip, vt_ip (16-byte aligned) and n_ip together");
+            return -1;
+        }
+        // the whole padded 64-key block: k_ip [64][ldk], vt_ip [heads*dp][64]
+        if (encode_2d(&plan->tmk_ip, d.k_ip, (long)d.heads * d.dp, ATTN_IP_KEYS, d.ldk, 64, ATTN_IP_KEYS, "k_ip")) return -1;
+        if (encode_2d(&plan->tmv_ip, d.vt_ip, ATTN_IP_KEYS, (long)d.heads * d.dp, ATTN_IP_KEYS, 64, d.dp, "vt_ip")) return -1;
+    }
     plan->grid = dim3((d.sq + AT_BQ - 1) / AT_BQ, d.heads, d.nb);
     plan->smem = attn_smem_bytes(d.dp / 64, bkv);
     return 0;
+}
+
+// attn_kernel<DA, BKV, IP = true> for each padded head dim
+static const void* attn_ip_kernel(int dp) {
+    return dp == 64 ? (const void*)attn_kernel<1, 128, true>
+                    : dp == 128 ? (const void*)attn_kernel<2, 128, true> : (const void*)attn_kernel<3, 64, true>;
 }
 
 int attn_init() {
@@ -501,6 +623,11 @@ int attn_init() {
             b2_set_error("cudaFuncSetAttribute(attn) failed");
             return -1;
         }
+        for (int dp : {64, 128, 192})
+            if (cudaFuncSetAttribute(attn_ip_kernel(dp), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
+                b2_set_error("cudaFuncSetAttribute(attn, image segment) failed");
+                return -1;
+            }
         attr_set = true;
     }
     return 0;
@@ -529,7 +656,15 @@ int attn_launch(const AttnPlan& plan, cudaStream_t s) {
     p.k_bstride = d.k_bstride; p.vt_bstride = d.vt_bstride;
     p.scale_log2 = (float)(1.4426950408889634 / sqrt((double)d.d_real));
     cudaError_t e;
-    if (d.dp == 64) e = launch_k(attn_kernel<1, 128>, plan.grid, dim3(AT_THREADS), plan.smem, s, 1, p);
+    if (d.n_ip) {
+        AttnIpParams pi;
+        static_cast<AttnParams&>(pi) = p;
+        pi.tmk_ip = plan.tmk_ip; pi.tmv_ip = plan.tmv_ip;
+        pi.n_ip = d.n_ip;
+        if (d.dp == 64) e = launch_k(attn_kernel<1, 128, true>, plan.grid, dim3(AT_THREADS), plan.smem, s, 1, pi);
+        else if (d.dp == 128) e = launch_k(attn_kernel<2, 128, true>, plan.grid, dim3(AT_THREADS), plan.smem, s, 1, pi);
+        else e = launch_k(attn_kernel<3, 64, true>, plan.grid, dim3(AT_THREADS), plan.smem, s, 1, pi);
+    } else if (d.dp == 64) e = launch_k(attn_kernel<1, 128>, plan.grid, dim3(AT_THREADS), plan.smem, s, 1, p);
     else if (d.dp == 128) e = launch_k(attn_kernel<2, 128>, plan.grid, dim3(AT_THREADS), plan.smem, s, 1, p);
     else e = launch_k(attn_kernel<3, 64>, plan.grid, dim3(AT_THREADS), plan.smem, s, 1, p);
     if (e != cudaSuccess) {

@@ -25,10 +25,20 @@ struct AttnDesc {
     int nb, heads, sq, skv;
     int d_real;         // true head dim (softmax scale = d_real^-0.5)
     int dp;             // padded head dim: 64, 128 or 192 (zero-padded columns)
+    // Decoupled image segment (IP-Adapter), all null = none: out = softmax(Q K^T) V + softmax(Q Kip^T) Vip, the second
+    // softmax over the first *n_ip keys (device int, 0..64; 0 skips the segment).  Shared by every batch item.  The caller
+    // allocates full 64-key blocks with zeroed padding: k_ip [64][ldk] (head layout of k), vt_ip [heads*dp][64].  An image
+    // scale is folded into vt_ip.
+    const __half* k_ip;
+    const __half* vt_ip;
+    const int* n_ip;
 };
+
+constexpr int ATTN_IP_KEYS = 64;   // keys of the image segment's block (the most n_ip may be)
 
 struct AttnPlan {
     CUtensorMap tmq, tmk, tmv;
+    CUtensorMap tmk_ip, tmv_ip;   // the image segment's (AttnDesc::n_ip set)
     AttnDesc d;
     dim3 grid;
     size_t smem;

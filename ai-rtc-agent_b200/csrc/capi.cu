@@ -203,16 +203,27 @@ int b2sd_op_rgb_to_nv12(const void* rgb_nchw, void* y, int y_pitch, void* uv, in
 }
 int b2sd_codec_probe(void) { return codec_probe(); }
 
-int b2sd_op_attention(const b2sd_attn_desc* d, void* stream) {
+static int op_attention(const b2sd_attn_desc* d, const void* k_ip, const void* vt_ip, const int* n_ip, void* stream) {
     AttnDesc a{};
     a.q = reinterpret_cast<const __half*>(d->q); a.ldq = d->ldq;
     a.k = reinterpret_cast<const __half*>(d->k); a.ldk = d->ldk; a.k_bstride = d->k_bstride; a.k_rows = d->k_rows;
     a.vt = reinterpret_cast<const __half*>(d->vt); a.ldvt = d->ldvt; a.vt_bstride = d->vt_bstride; a.vt_cols = d->vt_cols;
     a.out = reinterpret_cast<__half*>(d->out); a.ldo = d->ldo;
     a.nb = d->nb; a.heads = d->heads; a.sq = d->sq; a.skv = d->skv; a.d_real = d->d_real; a.dp = d->dp;
+    a.k_ip = reinterpret_cast<const __half*>(k_ip); a.vt_ip = reinterpret_cast<const __half*>(vt_ip); a.n_ip = n_ip;
     AttnPlan plan;
     if (attn_plan(a, &plan)) return -1;
     return attn_launch(plan, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2sd_op_attention(const b2sd_attn_desc* d, void* stream) { return op_attention(d, nullptr, nullptr, nullptr, stream); }
+
+int b2sd_op_attention_ip(const b2sd_attn_desc* d, const void* k_ip, const void* vt_ip, const int* n_ip, void* stream) {
+    if (!k_ip || !vt_ip || !n_ip || d->dp == 512) {
+        b2_set_error("b2sd_op_attention_ip: k_ip, vt_ip and n_ip are required, and dp must be 64, 128 or 192");
+        return -1;
+    }
+    return op_attention(d, k_ip, vt_ip, n_ip, stream);
 }
 
 int b2sd_op_groupnorm(const void* xa, int ca, int lda, const void* xb, int cb, int ldb, const float* gamma,

@@ -371,6 +371,7 @@ struct CondPool {
 struct CondOverride {
     uint64_t id = 0;
     uint64_t store = 0;            // WeightStore::id of the parameters it was computed with
+    bool own_text = false;         // a prompt block from the state's own prompt embeddings (else from the global ones)
     void* buf = nullptr;
     size_t bytes = 0;
     cudaEvent_t ready = nullptr;   // recorded once buf holds the block
@@ -437,6 +438,15 @@ struct b2sd_engine {
 
     __half* ctx_global = nullptr;   // the global prompt embeddings and timesteps: ctx / tsteps again after a state's refresh
     float* tsteps_global = nullptr;
+    // IP-Adapter image prompt (cfg.ip_tokens > 0): the image tokens the image program reads, [ATTN_IP_KEYS][D] with zeroed rows
+    // past the prompt's tokens, and the global ones; the token count and scale of the global prompt.  The image program writes
+    // every UNet cross-attention's image K / V^T and the token count the attention kernel reads (ip_count) into the prompt block.
+    __half* ip_tok = nullptr;
+    __half* ip_tok_global = nullptr;
+    int ip_n_global = 0;
+    float ip_scale_global = 1.f;
+    float ip_scale = 1.f;   // the scale the image program's V^T launches apply when they run
+    int* ip_count = nullptr;
 
     // The conditioning the frame program reads, as two contiguous blocks: [COND_PROMPT] every cross-attention K / V^T cache
     // (UNet and ControlNet), [COND_TIME] every resnet's per-slot time bias.  A step first makes each block hold what its state
@@ -461,7 +471,7 @@ struct b2sd_engine {
 
     unsigned long long* ln_stats = nullptr;   // slab of per-row LayerNorm statistics [rows][2] (see IgEpilogue::rowstat_out)
     size_t ln_stats_cap = 0, ln_stats_used = 0;   // in 64-bit words
-    std::vector<Op> prog_frame, prog_prompt, prog_time;
+    std::vector<Op> prog_frame, prog_prompt, prog_time, prog_image;
     std::map<std::string, Act> taps;
     SmallConvArgs head{};   // encoder head (reads the caller's frame)
     SmallConvArgs cn_head{};   // ControlNet conditioning embedding conv_in (reads the caller's frame as the control image)
@@ -700,9 +710,19 @@ struct b2sd_engine {
 
     // choose N tile / split-K for a good grid (igemm_autotile), plan, and append the launch
     // append a planned contraction
-    void push_igemm(std::vector<Op>& dst, const IgemmDesc& d, const IgemmPlan& plan, const std::string& label, double flops) {
+    // scale_src: acc_scale is read from there when the launch runs (the image program's V^T: the scale of the image prompt
+    // being computed)
+    void push_igemm(std::vector<Op>& dst, const IgemmDesc& d, const IgemmPlan& plan, const std::string& label, double flops,
+                    const float* scale_src = nullptr) {
         if (&dst == &prog_frame) launches += 1;
-        dst.push_back(Op([plan](cudaStream_t s) { return igemm_launch(plan, s); }, label, flops));
+        if (scale_src)
+            dst.push_back(Op([plan, sp = scale_src](cudaStream_t s) {
+                IgemmPlan q = plan;
+                q.p.epi.acc_scale = *sp;
+                return igemm_launch(q, s);
+            }, label, flops));
+        else
+            dst.push_back(Op([plan](cudaStream_t s) { return igemm_launch(plan, s); }, label, flops));
         dst.back().rec.kind = B2SD_LAUNCH_IGEMM;
         igemm_record(d, &plan, &dst.back().rec.igemm, &dst.back().rec.plan);
     }
@@ -716,10 +736,11 @@ struct b2sd_engine {
         r.kind = B2SD_LAUNCH_ATTN;
         r.attn = b2sd_attn_desc{a.q, a.ldq, a.k, a.ldk, (int64_t)a.k_bstride, (int64_t)a.k_rows, a.vt, a.ldvt, (int64_t)a.vt_bstride,
                                 (int64_t)a.vt_cols, a.out, a.ldo, a.nb, a.heads, a.sq, a.skv, a.d_real, a.dp};
+        r.attn_k_ip = a.k_ip; r.attn_vt_ip = a.vt_ip; r.attn_n_ip = a.n_ip;
     }
 
     // choose N tile / split-K for a good grid (igemm_autotile), plan, and append the launch
-    int add_igemm(std::vector<Op>& dst, IgemmDesc d) {
+    int add_igemm(std::vector<Op>& dst, IgemmDesc d, const float* scale_src = nullptr) {
         const bool geglu = (d.epi.flags & IG_GEGLU) != 0;
         const int n_gemm = geglu ? 2 * d.epi.n_valid : d.epi.n_valid;
         const bool extras = d.epi.rowstat_out || d.epi.colsum || d.epi.out2;   // not implemented by the swapped-orientation epilogue
@@ -739,7 +760,7 @@ struct b2sd_engine {
         snprintf(label, sizeof(label), "igemm %s rows=%ld n=%d kb=%d bn=%d splits=%d grid=%u,%u,%u %s", cur.c_str(),
                  plan.rows_total, d.epi.n_valid, plan.p.total_kb, plan.p.BN, plan.splits, plan.grid.x, plan.grid.y,
                  plan.grid.z, plan.p.swap ? "swapped" : (plan.pair ? "pairs" : "taps"));
-        push_igemm(dst, d, plan, label, 2.0 * (double)plan.rows_total * n_gemm * plan.p.total_kb * IG_BK);
+        push_igemm(dst, d, plan, label, 2.0 * (double)plan.rows_total * n_gemm * plan.p.total_kb * IG_BK, scale_src);
         return 0;
     }
 
@@ -1106,6 +1127,27 @@ int b2sd_engine::build_transformer(const std::string& p, const Act& x, int heads
         TRY(add_igemm(prog_prompt, d));
         allow_swap = true;
     }
+    // ---- IP-Adapter: the image tokens' K [64][Cp] and scale * V^T [Cp][64] (UNet only: the ControlNet's stay text-only, as in
+    // diffusers).  Rows / columns past the prompt's tokens come from its zeroed token rows, so they are finite.
+    __half *kip = nullptr, *vipt = nullptr;
+    if (cfg.ip_tokens && p.compare(0, 11, "controlnet.") != 0) {
+        __half* wk = pack_rows(t + "attn2.k_ip", {{t + "attn2.to_k_ip.weight", head_perm(0)}}, D, s);
+        __half* wv = pack_rows(t + "attn2.v_ip", {{t + "attn2.to_v_ip.weight", head_perm(0)}}, D, s);
+        kip = static_cast<__half*>(cond[COND_PROMPT].take((size_t)ATTN_IP_KEYS * Cp * 2));
+        vipt = static_cast<__half*>(cond[COND_PROMPT].take((size_t)Cp * ATTN_IP_KEYS * 2));
+        if (!wk || !wv || !kip || !vipt) return -1;
+        allow_swap = false;
+        ActView tokv{ip_tok, 1, 1, ATTN_IP_KEYS, D, D};
+        TRY(add_linear(prog_image, tokv, wk, Cp, D, nullptr, kip, Cp, nullptr, 0));
+        ActView wvv{wv, 1, 1, Cp, D, D};
+        IgemmDesc d{};
+        d.nseg = 1; d.src[0] = wvv; d.ntap[0] = 1;
+        d.w = ip_tok; d.w_rows = ATTN_IP_KEYS; d.w_ld = D; d.stride = 1;
+        d.Nb = 1; d.Ho = 1; d.Wo = Cp;
+        d.epi.out = vipt; d.epi.ldc = ATTN_IP_KEYS; d.epi.acc_scale = 1.f; d.epi.res_scale = 1.f; d.epi.n_valid = ATTN_IP_KEYS;
+        TRY(add_igemm(prog_image, d, &ip_scale));
+        allow_swap = true;
+    }
     Act q2 = new_act(1, 1, (int)M, Cp);
     if (fold) {
         LnFold f;
@@ -1127,6 +1169,7 @@ int b2sd_engine::build_transformer(const std::string& p, const Act& x, int heads
         a.vt = vct; a.ldvt = Lpad; a.vt_bstride = 0; a.vt_cols = L;
         a.out = ao2.p; a.ldo = C;
         a.nb = B; a.heads = heads; a.sq = HW; a.skv = L; a.d_real = d_real; a.dp = dp;
+        if (kip) { a.k_ip = kip; a.vt_ip = vipt; a.n_ip = ip_count; }
         AttnPlan plan;
         TRY(attn_plan(a, &plan));
         push_attn(plan, "attn " + p);
@@ -1665,7 +1708,7 @@ int b2sd_engine::build_kl_decoder(const Act& x0, cudaStream_t s) {
 
 int b2sd_engine::build_program(cudaStream_t s) {
     prog.reset();
-    prog_frame.clear(); prog_prompt.clear(); prog_time.clear();
+    prog_frame.clear(); prog_prompt.clear(); prog_time.clear(); prog_image.clear();
     taps.clear();
     launches = 0;
     drop_graphs();
@@ -1704,8 +1747,12 @@ int b2sd_engine::build_program(cudaStream_t s) {
                 resnets += 2 * (1 + cn);
             }
             bytes[COND_PROMPT] += transformers * (r(L * Cp * 2) + r(Cp * Lpad * 2));
+            if (cfg.ip_tokens)   // the UNet's own (not the ControlNet's): image K [64][Cp] and V^T [Cp][64]
+                bytes[COND_PROMPT] += (transformers - cn * (cfg.down_attn[i] ? lpb : 0) - (i == nlev - 1 ? cn : 0)) *
+                                      2 * r((size_t)ATTN_IP_KEYS * Cp * 2);
             bytes[COND_TIME] += resnets * r((size_t)B * ch[i] * sizeof(float));
         }
+        if (cfg.ip_tokens) bytes[COND_PROMPT] += r(sizeof(int));   // ip_count
         for (int k = 0; k < 2; ++k) {
             CondBlock& b = cond[k];
             b.cap = bytes[k];
@@ -1717,6 +1764,7 @@ int b2sd_engine::build_program(cudaStream_t s) {
             CUDA_OK(cudaMemsetAsync(b.p, 0, b.cap, s));
             CUDA_OK(cudaMemsetAsync(b.global, 0, b.cap, s));
         }
+        ip_count = cfg.ip_tokens ? static_cast<int*>(cond[COND_PROMPT].take(sizeof(int))) : nullptr;
     }
 
     allow_swap = false;
@@ -1980,36 +2028,42 @@ static int keep_global(b2sd_engine* h, int k, cudaStream_t s) {
     return 0;
 }
 
+// Make block k hold override ov (nullptr: the lane's global values)
+static int bind_block(b2sd_engine* h, int k, CondOverride* ov, cudaStream_t s) {
+    auto& b = h->cond[k];
+    const uint64_t want = ov ? ov->id : COND_GLOBAL;
+    if (b.held == want) return 0;
+    b.held = COND_UNKNOWN;
+    if (ov) {
+        CUDA_OK(cudaStreamWaitEvent(s, ov->ready, 0));
+        CUDA_OK(cudaMemcpyAsync(b.p, ov->buf, b.used, cudaMemcpyDeviceToDevice, s));
+        cudaEvent_t* use = nullptr;
+        for (auto& u : ov->uses)
+            if (u.first == s) use = &u.second;
+        if (!use) {
+            ov->uses.emplace_back(s, nullptr);
+            use = &ov->uses.back().second;
+            CUDA_OK(cudaEventCreateWithFlags(use, cudaEventDisableTiming));
+        }
+        CUDA_OK(cudaEventRecord(*use, s));
+    } else {
+        CUDA_OK(cudaMemcpyAsync(b.p, b.global, b.used, cudaMemcpyDeviceToDevice, s));
+    }
+    b.held = want;
+    ++h->cond_binds;
+    return 0;
+}
+
 // Make the blocks hold what `st` is stepped with (nullptr: a step without a state), before the frame program reads them
 static int bind_conditioning(b2sd_engine* h, const b2sd_state* st, cudaStream_t s) {
     for (int k = 0; k < 2; ++k) {
-        auto& b = h->cond[k];
         CondOverride* ov = st ? st->cond[k].get() : nullptr;
-        const uint64_t want = ov ? ov->id : COND_GLOBAL;
-        if (b.held == want) continue;
         if (ov && ov->store != h->ws->id) {
             b2_set_error("the state's own %s was computed with another weight store's parameters (a style's or its parent's): "
                          "set it again on an engine of this store", k == COND_PROMPT ? "prompt" : "timesteps");
             return -1;
         }
-        b.held = COND_UNKNOWN;
-        if (ov) {
-            CUDA_OK(cudaStreamWaitEvent(s, ov->ready, 0));
-            CUDA_OK(cudaMemcpyAsync(b.p, ov->buf, b.used, cudaMemcpyDeviceToDevice, s));
-            cudaEvent_t* use = nullptr;
-            for (auto& u : ov->uses)
-                if (u.first == s) use = &u.second;
-            if (!use) {
-                ov->uses.emplace_back(s, nullptr);
-                use = &ov->uses.back().second;
-                CUDA_OK(cudaEventCreateWithFlags(use, cudaEventDisableTiming));
-            }
-            CUDA_OK(cudaEventRecord(*use, s));
-        } else {
-            CUDA_OK(cudaMemcpyAsync(b.p, b.global, b.used, cudaMemcpyDeviceToDevice, s));
-        }
-        b.held = want;
-        ++h->cond_binds;
+        TRY(bind_block(h, k, ov, s));
     }
     return 0;
 }
@@ -2043,7 +2097,7 @@ static std::shared_ptr<CondPool> cond_pool(b2sd_engine* h) {
 
 // The prompt / time program has just computed `st`'s values into h's block k on s: copy them into a new override of the state
 // (h's block holds it).  The override it replaces is freed after every copy out of it.
-static int publish_override(b2sd_engine* h, b2sd_state* st, int k, cudaStream_t s) {
+static int publish_override(b2sd_engine* h, b2sd_state* st, int k, cudaStream_t s, bool own_text = false) {
     static std::atomic<uint64_t> next_id{1};
     auto& b = h->cond[k];
     std::unique_ptr<CondOverride> ov(new CondOverride);
@@ -2051,6 +2105,7 @@ static int publish_override(b2sd_engine* h, b2sd_state* st, int k, cudaStream_t 
     if (!ov->pool) return -1;
     ov->id = next_id++;
     ov->store = h->ws->id;
+    ov->own_text = own_text;
     ov->bytes = b.used;
     cudaError_t e = cudaEventCreateWithFlags(&ov->ready, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaMallocFromPoolAsync(&ov->buf, ov->bytes, ov->pool->pool, s);
@@ -2087,6 +2142,7 @@ int b2sd_create_lane(b2sd_handle parent, const b2sd_config* cfg, b2sd_handle* ou
     c.control_processor = parent->cfg.control_processor;
     c.vae = parent->cfg.vae;
     c.vae_scaling_factor = parent->cfg.vae_scaling_factor;
+    c.ip_tokens = parent->cfg.ip_tokens;
     for (int i = 0; i < 4; ++i)
         if (c.block_out_channels[i] != parent->cfg.block_out_channels[i] || c.heads[i] != parent->cfg.heads[i] ||
             c.down_attn[i] != parent->cfg.down_attn[i]) {
@@ -2134,6 +2190,10 @@ static int create_engine(const b2sd_config* cfg, std::shared_ptr<WeightStore> st
         b2_set_error("b2sd_create: vae_scaling_factor must be >= 0 (0 = 0.18215)");
         return -1;
     }
+    if (cfg->ip_tokens < 0 || cfg->ip_tokens > ATTN_IP_KEYS) {
+        b2_set_error("b2sd_create: ip_tokens must be 0 (no image prompts) or 1..%d (got %d)", ATTN_IP_KEYS, cfg->ip_tokens);
+        return -1;
+    }
     int dev = 0;
     cudaDeviceProp prop;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess) {
@@ -2172,6 +2232,17 @@ static int create_engine(const b2sd_config* cfg, std::shared_ptr<WeightStore> st
     if (e->tile_counters) cudaMemset(e->tile_counters, 0, 65536 * sizeof(int));
     e->ctx_global = static_cast<__half*>(e->state.alloc((size_t)cfg->ctx_tokens * cfg->cross_attention_dim * 2));
     e->tsteps_global = static_cast<float*>(e->state.alloc(B * sizeof(float)));
+    if (cfg->ip_tokens) {
+        const size_t ip_bytes = (size_t)ATTN_IP_KEYS * cfg->cross_attention_dim * 2;
+        e->ip_tok = static_cast<__half*>(e->state.alloc(ip_bytes));
+        e->ip_tok_global = static_cast<__half*>(e->state.alloc(ip_bytes));
+        if (!e->ip_tok || !e->ip_tok_global || cudaMemset(e->ip_tok, 0, ip_bytes) != cudaSuccess ||
+            cudaMemset(e->ip_tok_global, 0, ip_bytes) != cudaSuccess) {
+            b2_set_error("b2sd_create: cudaMalloc failed");
+            delete e;
+            return -1;
+        }
+    }
     if (!e->x_in.p || !e->noise || !e->coef || !e->tsteps || !e->ctx || !e->temb || !e->gn_ws || !e->ctx_global || !e->tsteps_global ||
         (cfg->controlnet && (!e->cn_temb_h || !e->cn_temb))) {
         b2_set_error("b2sd_create: cudaMalloc failed");
@@ -2306,6 +2377,7 @@ static int refresh_time(b2sd_handle h, cudaStream_t s) {
 static bool lora_target(const std::string& key, const Raw& r) {
     for (const char* pre : {"vae.", "controlnet.", "hed."})
         if (key.compare(0, strlen(pre), pre) == 0) return false;
+    if (key.find("_ip.weight") != std::string::npos) return false;   // IP-Adapter's to_k_ip / to_v_ip: styles share them
     return !r.derived && r.shape.size() >= 2;
 }
 
@@ -2325,6 +2397,38 @@ static int make_live_base(b2sd_handle h) {
     }
     w.live_ready = true;
     return 0;
+}
+
+// *p = v as a 4-byte memset node on s (cuMemsetD32Async: the value travels with the command, nothing host-side to keep alive)
+static int set_int_async(int* p, int v, cudaStream_t s) {
+    using MemsetD32 = CUresult (*)(CUdeviceptr, unsigned int, size_t, CUstream);
+    static MemsetD32 fn = nullptr;
+    if (!fn) {
+        void* fp = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuMemsetD32Async", &fp, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess || !fp) {
+            b2_set_error("cudaGetDriverEntryPoint(cuMemsetD32Async) failed");
+            return -1;
+        }
+        fn = reinterpret_cast<MemsetD32>(fp);
+    }
+    const CUresult r = fn(reinterpret_cast<CUdeviceptr>(p), (unsigned int)v, 1, s);
+    if (r != CUDA_SUCCESS) {
+        b2_set_error("cuMemsetD32Async failed: %d", (int)r);
+        return -1;
+    }
+    return 0;
+}
+
+// The image program on ip_tok, whose first n rows hold an image prompt's tokens (n = 0: none): every UNet cross-attention's
+// image K / V^T (V^T times scale) and the token count the attention kernel reads, in the prompt block.  Nothing without
+// ip_tokens.
+static int run_image(b2sd_handle h, int n, float scale, cudaStream_t s) {
+    if (!h->cfg.ip_tokens) return 0;
+    h->ip_scale = scale;
+    TRY(h->run(h->prog_image, s));
+    return set_int_async(h->ip_count, n, s);
 }
 
 int b2sd_prepare(b2sd_handle h, const void* prompt_embeds, const float* timesteps, const float* coef,
@@ -2367,6 +2471,7 @@ int b2sd_prepare(b2sd_handle h, const void* prompt_embeds, const float* timestep
         return -1;
     }
     TRY(h->run(h->prog_prompt, s));
+    TRY(run_image(h, h->ip_n_global, h->ip_scale_global, s));
     TRY(refresh_time(h, s));
     CUDA_OK(cudaMemcpyAsync(h->ctx_global, h->ctx, (size_t)h->cfg.ctx_tokens * h->cfg.cross_attention_dim * 2,
                             cudaMemcpyDeviceToDevice, s));
@@ -2422,7 +2527,7 @@ int b2sd_export_packed(b2sd_handle h, const char* path) {
     }
     BlobWriter w{f};
     w.put("B2SDPACK", 8);
-    w.pod((uint32_t)3);   // 3: b2sd_config carries `vae` / `vae_scaling_factor` (2: up to `control_processor`; 1 and 2 still load)
+    w.pod((uint32_t)4);   // 4: b2sd_config carries `ip_tokens` (3: up to `vae_scaling_factor`, 2: up to `control_processor`; 1-3 still load)
     b2sd_config cfg = h->cfg;
     cfg.batch = 0; cfg.height = 0; cfg.width = 0; cfg.use_cuda_graph = 0; cfg.do_add_noise = 0;   // the blob is independent of these
     w.pod(cfg);
@@ -2485,12 +2590,19 @@ int b2sd_import_packed(b2sd_handle h, const char* path) {
     rd.get(magic, 8);
     const uint32_t version = rd.pod<uint32_t>();
     // version 1 blobs predate the ControlNet fields at the end of b2sd_config: they hold no ControlNet (both fields 0);
-    // version 2 blobs end b2sd_config before `vae`: they hold TAESD (vae = 0)
+    // version 2 blobs end b2sd_config before `vae`: they hold TAESD (vae = 0); version 3 blobs before `ip_tokens`: no IP-Adapter
     b2sd_config cfg{};
     if (version == 1) rd.get(&cfg, offsetof(b2sd_config, controlnet));
     else if (version == 2) rd.get(&cfg, offsetof(b2sd_config, vae));
+    else if (version == 3) rd.get(&cfg, offsetof(b2sd_config, ip_tokens));
     else cfg = rd.pod<b2sd_config>();
-    bool same = rd.ok && memcmp(magic, "B2SDPACK", 8) == 0 && version >= 1 && version <= 3 && cfg.cross_attention_dim == h->cfg.cross_attention_dim &&
+    if (rd.ok && version >= 1 && version <= 4 && (cfg.ip_tokens != 0) != (h->cfg.ip_tokens != 0)) {
+        fclose(f);
+        b2_set_error("b2sd_import_packed: %s was packed %s an IP-Adapter and this engine has %s", path,
+                     cfg.ip_tokens ? "with" : "without", h->cfg.ip_tokens ? "one" : "none");
+        return -1;
+    }
+    bool same = rd.ok && memcmp(magic, "B2SDPACK", 8) == 0 && version >= 1 && version <= 4 && cfg.cross_attention_dim == h->cfg.cross_attention_dim &&
                 cfg.layers_per_block == h->cfg.layers_per_block && cfg.norm_groups == h->cfg.norm_groups && cfg.ctx_tokens == h->cfg.ctx_tokens &&
                 cfg.controlnet == h->cfg.controlnet && cfg.control_processor == h->cfg.control_processor && cfg.vae == h->cfg.vae &&
                 (cfg.vae != B2SD_VAE_KL || cfg.vae_scaling_factor == h->cfg.vae_scaling_factor);
@@ -2558,6 +2670,7 @@ int b2sd_set_prompt_embeds(b2sd_handle h, const void* prompt_embeds, void* strea
     CUDA_OK(cudaMemcpyAsync(h->ctx, prompt_embeds, bytes, cudaMemcpyHostToDevice, s));
     CUDA_OK(cudaStreamSynchronize(s));
     CUDA_OK(cudaMemcpyAsync(h->ctx_global, h->ctx, bytes, cudaMemcpyDeviceToDevice, s));
+    if (h->cfg.ip_tokens) TRY(bind_block(h, COND_PROMPT, nullptr, s));   // keep the global image part of the block
     h->cond[COND_PROMPT].held = COND_UNKNOWN;
     TRY(h->run(h->prog_prompt, s));
     return keep_global(h, COND_PROMPT, s);
@@ -2737,6 +2850,7 @@ int b2sd_refresh_conditioning(b2sd_handle h, void* stream) {
     h->cond[COND_PROMPT].held = COND_UNKNOWN;
     h->cond[COND_TIME].held = COND_UNKNOWN;
     TRY(h->run(h->prog_prompt, s));
+    TRY(run_image(h, h->ip_n_global, h->ip_scale_global, s));
     TRY(refresh_time(h, s));
     TRY(keep_global(h, COND_PROMPT, s));
     return keep_global(h, COND_TIME, s);
@@ -2868,6 +2982,16 @@ static int check_state(const char* fn, b2sd_handle h, const b2sd_state* state) {
     return 0;
 }
 
+// The prompt block a refresh of `st`'s text (own_text = false) or image part (own_text = true) starts from: the state's override
+// if it was computed on h's store and, for an image refresh, from the state's own prompt embeddings; else nullptr, the lane's
+// global values.  An override whose text part came from the global prompt is not kept: the global block is recomputed by
+// every global refresh (a new prompt, a LoRA switch), the override's copy of it is not.  After a move to another store of the
+// family the state's own prompt and image prompt are set again.
+static CondOverride* prompt_base(b2sd_engine* h, b2sd_state* st, bool own_text) {
+    CondOverride* ov = st->cond[COND_PROMPT].get();
+    return ov && ov->store == h->ws->id && (ov->own_text || !own_text) ? ov : nullptr;
+}
+
 // Run h's prompt (k = COND_PROMPT) or time refresh on s with `input` (device) in place of the global embeddings / timesteps,
 // put the global ones back, and publish the block as the state's override.  Stream-ordered after the frames queued on s, and
 // no host synchronisation: the refresh writes only h's block, which no other stream reads.
@@ -2881,12 +3005,15 @@ static int state_refresh(const char* fn, b2sd_handle h, b2sd_state* state, int k
     const void* global = k == COND_PROMPT ? (const void*)h->ctx_global : (const void*)h->tsteps_global;
     const size_t bytes = k == COND_PROMPT ? (size_t)h->cfg.ctx_tokens * h->cfg.cross_attention_dim * 2
                                           : (size_t)h->cfg.batch * sizeof(float);
+    // with image prompts the prompt program leaves the image part of the block alone: start from the state's block, so that
+    // the state keeps its own image prompt
+    if (k == COND_PROMPT && h->cfg.ip_tokens) TRY(bind_block(h, k, prompt_base(h, state, false), s));
     h->cond[k].held = COND_UNKNOWN;
     CUDA_OK(cudaMemcpyAsync(dst, input, bytes, cudaMemcpyDeviceToDevice, s));
     const int rc = k == COND_PROMPT ? h->run(h->prog_prompt, s) : refresh_time(h, s);
     CUDA_OK(cudaMemcpyAsync(dst, global, bytes, cudaMemcpyDeviceToDevice, s));
     TRY(rc);
-    return publish_override(h, state, k, s);
+    return publish_override(h, state, k, s, k == COND_PROMPT);
 }
 
 int b2sd_state_set_prompt_embeds(b2sd_handle h, b2sd_state_handle state, const void* prompt_embeds, void* stream) {
@@ -2896,6 +3023,58 @@ int b2sd_state_set_prompt_embeds(b2sd_handle h, b2sd_state_handle state, const v
 
 int b2sd_state_set_timesteps(b2sd_handle h, b2sd_state_handle state, const float* timesteps, void* stream) {
     return state_refresh("b2sd_state_set_timesteps", h, state, COND_TIME, timesteps, reinterpret_cast<cudaStream_t>(stream));
+}
+
+// n rows of image tokens (nullptr: none) into h->ip_tok, the rest zeroed
+static int load_image_tokens(const char* fn, b2sd_handle h, const void* tokens, int n, float scale, cudaStream_t s) {
+    if (!h->cfg.ip_tokens) {
+        b2_set_error("%s: the engine was created without image prompts (b2sd_config.ip_tokens = 0)", fn);
+        return -1;
+    }
+    if (tokens && (n < 1 || n > h->cfg.ip_tokens || !isfinite(scale))) {
+        b2_set_error("%s: n_tok must be 1..%d and scale finite (got %d, %f)", fn, h->cfg.ip_tokens, n, (double)scale);
+        return -1;
+    }
+    const size_t row = (size_t)h->cfg.cross_attention_dim * 2;
+    if (!tokens) n = 0;
+    if (n) CUDA_OK(cudaMemcpyAsync(h->ip_tok, tokens, n * row, cudaMemcpyDefault, s));
+    CUDA_OK(cudaMemsetAsync(reinterpret_cast<char*>(h->ip_tok) + n * row, 0, (ATTN_IP_KEYS - n) * row, s));
+    return 0;
+}
+
+int b2sd_set_image_embeds(b2sd_handle h, const void* tokens_f16, int n_tok, float scale, void* stream) {
+    if (!h || !h->built) {
+        b2_set_error("b2sd_set_image_embeds: call b2sd_prepare first");
+        return -1;
+    }
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    TRY(load_image_tokens("b2sd_set_image_embeds", h, tokens_f16, n_tok, scale, s));
+    CUDA_OK(cudaStreamSynchronize(s));   // as b2sd_set_prompt_embeds: the caller's host buffer may go once this returns
+    h->ip_n_global = tokens_f16 ? n_tok : 0;
+    h->ip_scale_global = tokens_f16 ? scale : 1.f;
+    CUDA_OK(cudaMemcpyAsync(h->ip_tok_global, h->ip_tok, (size_t)ATTN_IP_KEYS * h->cfg.cross_attention_dim * 2,
+                            cudaMemcpyDeviceToDevice, s));
+    // the block holds the global text part before the image program overwrites the image part
+    TRY(bind_block(h, COND_PROMPT, nullptr, s));
+    h->cond[COND_PROMPT].held = COND_UNKNOWN;
+    TRY(run_image(h, h->ip_n_global, h->ip_scale_global, s));
+    return keep_global(h, COND_PROMPT, s);
+}
+
+int b2sd_state_set_image_embeds(b2sd_handle h, b2sd_state_handle state, const void* tokens_f16, int n_tok, float scale,
+                                void* stream) {
+    const char* fn = "b2sd_state_set_image_embeds";
+    TRY(check_state(fn, h, state));
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    TRY(load_image_tokens(fn, h, tokens_f16, n_tok, scale, s));
+    CondOverride* base = prompt_base(h, state, true);   // the state's text part: its own prompt's, or the global one
+    TRY(bind_block(h, COND_PROMPT, base, s));
+    h->cond[COND_PROMPT].held = COND_UNKNOWN;
+    const int rc = run_image(h, tokens_f16 ? n_tok : 0, scale, s);
+    CUDA_OK(cudaMemcpyAsync(h->ip_tok, h->ip_tok_global, (size_t)ATTN_IP_KEYS * h->cfg.cross_attention_dim * 2,
+                            cudaMemcpyDeviceToDevice, s));
+    TRY(rc);
+    return publish_override(h, state, COND_PROMPT, s, base != nullptr);
 }
 
 int b2sd_state_clear_conditioning(b2sd_state_handle state, int which) {

@@ -136,6 +136,7 @@ class LaunchRecord(C.Structure):
         ("smallconv", SmallConvArgs), ("upsample2x", Upsample2xArgs), ("maxpool2x2", MaxPool2x2Args),
         ("hed_project", HedProjectArgs), ("hed_fuse", HedFuseArgs), ("lcm_step", LcmStepArgs), ("post_u8", PostU8Args),
         ("small_linear", SmallLinearArgs), ("timestep_embedding", TimestepEmbeddingArgs),
+        ("attn_k_ip", C.c_void_p), ("attn_vt_ip", C.c_void_p), ("attn_n_ip", C.c_void_p),
     ]
 
 
@@ -148,7 +149,7 @@ class EngineConfig(C.Structure):
         ("cross_attention_dim", C.c_int), ("layers_per_block", C.c_int), ("norm_groups", C.c_int),
         ("ctx_tokens", C.c_int), ("batch", C.c_int), ("height", C.c_int), ("width", C.c_int),
         ("do_add_noise", C.c_int), ("use_cuda_graph", C.c_int), ("controlnet", C.c_int), ("control_processor", C.c_int),
-        ("vae", C.c_int), ("vae_scaling_factor", C.c_float),
+        ("vae", C.c_int), ("vae_scaling_factor", C.c_float), ("ip_tokens", C.c_int),
     ]
 
 
@@ -194,6 +195,7 @@ def lib() -> C.CDLL:
         _lib.b2sd_igemm_partial_floats.restype = C.c_uint64
         vp, ci, cf, i64 = C.c_void_p, C.c_int, C.c_float, C.c_int64
         _lib.b2sd_op_attention.argtypes = [C.POINTER(AttnDesc), vp]
+        _lib.b2sd_op_attention_ip.argtypes = [C.POINTER(AttnDesc), vp, vp, vp, vp]
         _lib.b2sd_op_groupnorm.argtypes = [vp, ci, ci, vp, ci, ci, vp, vp, vp, ci, ci, ci, ci, cf, ci, vp]
         _lib.b2sd_groupnorm_last_path.argtypes = []
         _lib.b2sd_groupnorm_last_path.restype = C.c_int
@@ -232,8 +234,10 @@ def lib() -> C.CDLL:
         _lib.b2sd_state_set_prompt_embeds.argtypes = [vp, vp, vp, vp]
         _lib.b2sd_state_set_timesteps.argtypes = [vp, vp, vp, vp]
         _lib.b2sd_state_clear_conditioning.argtypes = [vp, ci]
+        _lib.b2sd_set_image_embeds.argtypes = [vp, vp, ci, cf, vp]
+        _lib.b2sd_state_set_image_embeds.argtypes = [vp, vp, vp, ci, cf, vp]
         for name in ("state_create", "state_reset", "state_destroy", "step_state", "state_set_prompt_embeds", "state_set_timesteps",
-                     "state_clear_conditioning"):
+                     "state_clear_conditioning", "set_image_embeds", "state_set_image_embeds"):
             getattr(_lib, "b2sd_" + name).restype = C.c_int
         _lib.b2sd_set_live_params.argtypes = [vp, ci]
         _lib.b2sd_apply_lora.argtypes = [vp, ci, C.POINTER(LoraFactor), vp]
@@ -257,7 +261,7 @@ def lib() -> C.CDLL:
         for name in ("create", "create_lane", "destroy", "load_tensor", "prepare", "export_packed", "import_packed", "set_prompt_embeds", "set_timesteps", "step",
                      "step_ex", "get_tensor", "launches_per_step"):
             getattr(_lib, "b2sd_" + name).restype = C.c_int
-        for name in ("attention", "groupnorm", "layernorm", "upsample2x", "smallconv", "smallconv_ex", "maxpool2x2", "hed_project", "hed_fuse", "lcm_step", "post_u8", "post_f16", "nv12_to_rgb", "rgb_to_nv12"):
+        for name in ("attention", "attention_ip", "groupnorm", "layernorm", "upsample2x", "smallconv", "smallconv_ex", "maxpool2x2", "hed_project", "hed_fuse", "lcm_step", "post_u8", "post_f16", "nv12_to_rgb", "rgb_to_nv12"):
             getattr(_lib, "b2sd_op_" + name).restype = C.c_int
     return _lib
 

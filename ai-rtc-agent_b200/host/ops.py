@@ -121,6 +121,22 @@ def attention(q, k, vt, out, *, nb, heads, sq, skv, d_real, dp, k_bstride, vt_bs
     return out
 
 
+def attention_ip(q, k, vt, out, k_ip, vt_ip, n_ip, *, nb, heads, sq, skv, d_real, dp, k_bstride, vt_bstride):
+    """attention() plus IP-Adapter's decoupled image segment: k_ip [64, k.stride(0)] and vt_ip [heads*dp, 64] (fp16, keys past
+    n_ip zeroed), n_ip a device int32 tensor of one element (0..64)."""
+    d = capi.AttnDesc()
+    d.q, d.ldq = q.data_ptr(), q.stride(0)
+    d.k, d.ldk, d.k_bstride, d.k_rows = k.data_ptr(), k.stride(0), k_bstride, k.shape[0]
+    d.vt, d.ldvt, d.vt_bstride, d.vt_cols = vt.data_ptr(), vt.stride(0), vt_bstride, vt.shape[1]
+    d.out, d.ldo = out.data_ptr(), out.stride(0)
+    d.nb, d.heads, d.sq, d.skv, d.d_real, d.dp = nb, heads, sq, skv, d_real, dp
+    assert k_ip.shape[0] == 64 and k_ip.stride(0) == k.stride(0) and vt_ip.shape[1] == 64 and vt_ip.stride(0) == 64
+    assert n_ip.dtype == torch.int32 and n_ip.is_cuda
+    capi.check(capi.lib().b2sd_op_attention_ip(C.byref(d), k_ip.data_ptr(), vt_ip.data_ptr(), n_ip.data_ptr(), _sp()),
+               "b2sd_op_attention_ip")
+    return out
+
+
 GN_PATHS = {0: "cluster", 1: "fused", 2: "stats+apply"}
 
 

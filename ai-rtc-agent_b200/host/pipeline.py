@@ -106,7 +106,7 @@ class StreamDiffusionPipeline:
 
     def __init__(self, model_id: str, t_index_list: Optional[List[int]] = None, width: int = 512, height: int = 512,
                  prompt: str = DEFAULT_PROMPT, lanes: Optional[int] = None, per_peer_streams: Optional[bool] = None,
-                 live_lora: Optional[bool] = None):
+                 live_lora: Optional[bool] = None, ip_adapter: Optional[str] = None):
         """lanes: frames in flight for enqueue() ($B200SD_LANES overrides the default).  With a 1-step stream batch (SD-Turbo)
         consecutive frames are independent: DEFAULT_LANES_ONE_STEP lanes process frame n+1.. while frame n is still on the GPU.
         With T > 1 the stream batch carries state from frame to frame: the pipeline's stream is then a stream state that two lanes
@@ -120,7 +120,11 @@ class StreamDiffusionPipeline:
         reference: with T > 1 a frame's output then mixes in frames of the other callers.
 
         live_lora (None: $B200SD_LIVE_LORA, default off): update_lora() switches style LoRAs while the pipeline runs.  The base
-        weights stay on the device (more HBM, see README), and the packed-weight blob is neither read nor written."""
+        weights stay on the device (more HBM, see README), and the packed-weight blob is neither read nor written.
+
+        ip_adapter (None: $B200SD_IP_ADAPTER, default none): an IP-Adapter file (h94 ip-adapter_sd15.safetensors layout) or a
+        directory holding one and its image_encoder/; "synthetic" for seeded weights with a synthetic model.
+        update_image_prompt() then steers the video with an image, globally or per viewer (PeerStream.update_image_prompt)."""
         if per_peer_streams is None:
             per_peer_streams = env_flag(PER_PEER_STREAMS_ENV)
         self.per_peer_streams = bool(per_peer_streams)
@@ -133,6 +137,7 @@ class StreamDiffusionPipeline:
             live_lora = env_flag(LIVE_LORA_ENV)
         self.model = StreamDiffusionWrapper.__new__(StreamDiffusionWrapper)
         self.model.live_lora = bool(live_lora)
+        self.model.ip_adapter = ip_adapter
         self.model.__init__(
             model_id_or_path=model_id,
             device=self.device,
@@ -203,6 +208,19 @@ class StreamDiffusionPipeline:
         self.model.stream.update_prompt(prompt)
         self._release(cur)
 
+    def update_image_prompt(self, image, scale: float = 1.0):
+        """The global image prompt (IP-Adapter): `image` is a PIL image or an HWC uint8 array / tensor, never a path; None clears
+        it.  scale weighs the image attention against the text's.  Every stream's, including open peer streams with an image
+        prompt of their own (PeerStream.update_image_prompt); each keeps its own prompt.  The image is encoded before anything
+        changes; frames enqueued before the call use the old image prompt and frames enqueued after it the new one."""
+        sd = self.model.stream
+        tokens = None if image is None else sd.image_tokens(image)
+        cur = self._quiesce()
+        try:
+            sd.set_image_tokens(tokens, scale)
+        finally:
+            self._release(cur)
+
     def update_lora(self, lora_dict: Optional[Dict[str, float]]):
         """The style LoRAs ({safetensors path: scale}, the wrapper's lora_dict form; None or {}: none) of every stream: the
         pipeline's own and every open peer stream, each keeping its own prompt / t_index_list.  Frames enqueued before the
@@ -226,6 +244,8 @@ class StreamDiffusionPipeline:
         if peer._style is not None:
             peer._style.users -= 1
             peer._style, peer._lora = None, None
+            if peer._state is not None:
+                peer._state.home = self.model.stream
 
     def _set_peer_style(self, peer, lora_dict: Optional[Dict[str, float]]) -> None:
         """Move `peer` to the lane pool of lora_dict's style (the pipeline's own when it is the global one), building the style
@@ -255,7 +275,8 @@ class StreamDiffusionPipeline:
             self._styles[target.key] = self._styles.pop(target.key)   # most recently used
         # the viewer's own conditioning is computed again with the new weights, on the lane that takes its next frame
         pool = target or self
-        if state.own_prompt is not None or state.own_t_index_list is not None:
+        image = getattr(state, "own_image", None)
+        if state.own_prompt is not None or state.own_t_index_list is not None or image is not None:
             prompt, t_index_list = state.own_prompt, state.own_t_index_list
 
             def rebind(engine):
@@ -263,11 +284,14 @@ class StreamDiffusionPipeline:
                     state.set_prompt(prompt, engine=engine)
                 if t_index_list is not None:
                     state.set_t_index_list(t_index_list, engine=engine)
+                if image is not None:
+                    state.set_image_tokens(*image, engine=engine)
             self._update_state(rebind, pool)
         self._leave_style(peer)
         if target is not None:
             target.users += 1
             peer._style, peer._lora = target, dict(lora_dict or {})
+            state.home = target._engines[0]
         # back within the bound: unused styles, least recently used first, each freed after its last frames
         for k in [k for k, st in self._styles.items() if st.users == 0]:
             if len(self._styles) <= _max_styles():
@@ -533,6 +557,20 @@ class PeerStream:
         pipeline.update_prompt replaces it."""
         state = self._live_state()
         self._pipeline._update_state(lambda engine: state.set_prompt(prompt, engine=engine), self._style)
+
+    @property
+    def image_prompt(self):
+        """(tokens, scale) of this viewer's image prompt: its own (update_image_prompt) or the pipeline's global one (None: none)"""
+        own = self._live_state().own_image
+        return own if own is not None else self._pipeline.model.stream.image_prompt
+
+    def update_image_prompt(self, image, scale: float = 1.0) -> None:
+        """This viewer's own image prompt (IP-Adapter): a PIL image or an HWC uint8 array / tensor, never a path; None: the
+        pipeline's global one again.  update_prompt's ordering; the viewer keeps its own prompt.  A later global
+        pipeline.update_image_prompt replaces it."""
+        state = self._live_state()
+        tokens = None if image is None else self._pipeline.model.stream.image_tokens(image)
+        self._pipeline._update_state(lambda engine: state.set_image_tokens(tokens, scale, engine=engine), self._style)
 
     def update_t_index_list(self, t_index_list: List[int]) -> None:
         """This viewer's own t_index_list, with the semantics of the global update_t_index_list (only the time embedding's

@@ -11,7 +11,7 @@ import ctypes as C
 import math
 import os
 import weakref
-from typing import Callable, Dict, List, Optional
+from typing import Callable, Dict, List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -73,6 +73,7 @@ class ImageProcessor:
 class StreamDiffusion:
     styles = ()          # instances made by __init__ get a list (add_style)
     _is_style = False
+    image_prompt = None  # the global image prompt: (host tokens [n_tok][D], scale) (set_image_tokens)
 
     def __init__(self, arch: UNetArch, unet_sd: Dict[str, torch.Tensor], vae_sd: Dict[str, torch.Tensor],
                  t_index_list: List[int], prompt_encoder: Callable[[str], torch.Tensor],
@@ -82,7 +83,8 @@ class StreamDiffusion:
                  packed_blob: Optional[str] = None, parent: Optional["StreamDiffusion"] = None,
                  controlnet_sd: Optional[Dict[str, torch.Tensor]] = None,
                  hed_sd: Optional[Dict[str, torch.Tensor]] = None, use_tiny_vae: bool = True,
-                 vae_scaling_factor: float = 0.18215, live_lora: bool = False, style_of: Optional["StreamDiffusion"] = None):
+                 vae_scaling_factor: float = 0.18215, live_lora: bool = False, style_of: Optional["StreamDiffusion"] = None,
+                 ip_adapter=None):
         """vae_sd: TAESD (use_tiny_vae=True) or the model's own AutoencoderKL (use_tiny_vae=False: latents = vae_scaling_factor
         times the mean of the encoder's distribution, decoded from x0 / vae_scaling_factor).
         controlnet_sd: a diffusers ControlNetModel state dict (empty when the weights come from packed_blob); every
@@ -90,7 +92,9 @@ class StreamDiffusion:
         ControlNetHED.pth state dict, empty with packed_blob) its HED edge map.  Lanes inherit their parent's ControlNet.
         live_lora: keep the base UNet weights on the device so that apply_lora() can switch LoRAs at run time (not with
         packed_blob; lanes inherit it).
-        style_of: make a style of that live engine instead (add_style)."""
+        style_of: make a style of that live engine instead (add_style).
+        ip_adapter: an image_prompt.IPAdapter (load_adapter): image prompts through the UNet's cross-attentions
+        (set_image_tokens / update_image_prompt); lanes and styles inherit it."""
         if live_lora and packed_blob is not None:
             raise ValueError("live_lora needs the weights themselves: a packed blob does not carry the base weights")
         if hed_sd is not None and controlnet_sd is None:
@@ -142,6 +146,8 @@ class StreamDiffusion:
         cfg.control_processor = capi.CONTROL_HED if hed_sd is not None else capi.CONTROL_FRAME
         cfg.vae = capi.VAE_TINY if use_tiny_vae else capi.VAE_KL
         cfg.vae_scaling_factor = 0.0 if use_tiny_vae else float(vae_scaling_factor)
+        cfg.ip_tokens = ip_adapter.n_tok if ip_adapter is not None else 0
+        self.ip_adapter = ip_adapter   # with packed_blob its UNet weights come from the blob
         if not torch.cuda.is_available():
             raise capi.B2Error("no CUDA device: the H100 pipeline has no CPU fallback")
         if self.device.index is None:
@@ -150,7 +156,7 @@ class StreamDiffusion:
         self._ctor = dict(torch_dtype=torch_dtype, width=width, height=height, do_add_noise=do_add_noise,
                           use_denoising_batch=use_denoising_batch, frame_buffer_size=frame_buffer_size, cfg_type=cfg_type,
                           device=device, use_cuda_graph=use_cuda_graph, use_tiny_vae=use_tiny_vae,
-                          vae_scaling_factor=vae_scaling_factor, live_lora=live_lora)
+                          vae_scaling_factor=vae_scaling_factor, live_lora=live_lora, ip_adapter=ip_adapter)
         self.live_lora = bool(live_lora)
         # extra engines over this one's weights (add_lane).  A lane keeps no reference to its parent: an engine and its lanes then
         # form no reference cycle, so their device memory is released as soon as the last reference goes, not at the next
@@ -180,6 +186,8 @@ class StreamDiffusion:
             capi.check(self._lib.b2sd_import_packed(self._handle, os.fsencode(packed_blob)), f"b2sd_import_packed({packed_blob})")
         else:
             self._load("", unet_sd)
+            if ip_adapter is not None:
+                self._load("", ip_adapter.unet)
             self._load("vae.", vae_sd)
             self._load("controlnet.", controlnet_sd or {})
             self._load("hed.", hed_sd or {})
@@ -284,6 +292,11 @@ class StreamDiffusion:
             setattr(self, name, getattr(other, name))
         self.t_list = list(other.t_list)
         self._engine_prepare()
+        if other.image_prompt is not None:   # a new lane or style starts with the family's global image prompt
+            tokens, scale = other.image_prompt
+            capi.check(self._lib.b2sd_set_image_embeds(self._handle, tokens.data_ptr(), tokens.shape[0], scale, self._stream()),
+                       "b2sd_set_image_embeds")
+            self.image_prompt = other.image_prompt
 
     def add_lane(self) -> "StreamDiffusion":
         """Another engine over the same weights, prepared identically (same prompt embedding, schedule and seed-2 noise):
@@ -359,7 +372,32 @@ class StreamDiffusion:
         for eng in self._family():
             eng.prompt, eng.prompt_embeds = prompt, self.prompt_embeds
             capi.check(self._lib.b2sd_set_prompt_embeds(eng._handle, emb.data_ptr(), self._stream()), "b2sd_set_prompt_embeds")
-        self.clear_overrides(prompt=True, t_index_list=False)
+        self.clear_overrides(prompt=True, t_index_list=False, image_prompt=False)
+
+    def image_tokens(self, image) -> torch.Tensor:
+        """(1, n_tok, D) fp16 image-prompt tokens of `image` (a PIL image or HWC uint8 array / tensor): the adapter's image encoder
+        (set by the pipeline; a seeded synthetic one otherwise), then its projection"""
+        if self.ip_adapter is None:
+            raise RuntimeError("this engine was built without an IP-Adapter (ip_adapter=...)")
+        enc = getattr(self, "image_encoder", None)
+        if enc is None:
+            from .image_prompt import SyntheticImageEncoder
+            enc = self.image_encoder = SyntheticImageEncoder(self.ip_adapter.embed_dim)
+        return self.ip_adapter.tokens(enc(image))
+
+    @torch.no_grad()
+    def set_image_tokens(self, tokens: Optional[torch.Tensor], scale: float = 1.0) -> None:
+        """The global image prompt as (1, n_tok, D) fp16 tokens (image_tokens), None to clear: this engine's, its lanes' and its
+        styles' (b2sd_set_image_embeds), and every live state's (a state's own image prompt is dropped, its own prompt kept)."""
+        ptr, n = 0, 0
+        if tokens is not None:
+            tokens = tokens.reshape(-1, self.arch.cross_attention_dim).to(torch.float16).cpu().contiguous()
+            ptr, n = tokens.data_ptr(), tokens.shape[0]
+        for eng in self._family():
+            capi.check(self._lib.b2sd_set_image_embeds(eng._handle, ptr or None, n, float(scale), self._stream()),
+                       "b2sd_set_image_embeds")
+        self.image_prompt = None if tokens is None else (tokens, float(scale))
+        self.clear_overrides(prompt=False, t_index_list=False, image_prompt=True)
 
     def _timestep_tensor(self, sub_timesteps: List[int]) -> torch.Tensor:
         t = torch.tensor([float(v) for v in sub_timesteps], dtype=torch.float32)
@@ -378,11 +416,12 @@ class StreamDiffusion:
             capi.check(self._lib.b2sd_set_timesteps(eng._handle, t.data_ptr(), self._stream()), "b2sd_set_timesteps")
         self.clear_overrides(prompt=False, t_index_list=True)
 
-    def clear_overrides(self, prompt: bool = True, t_index_list: bool = True) -> None:
-        """Every live state of this engine's weights follows the global prompt and / or t_index_list again."""
+    def clear_overrides(self, prompt: bool = True, t_index_list: bool = True, image_prompt: Optional[bool] = None) -> None:
+        """Every live state of this engine's weights follows the global prompt, t_index_list and / or image prompt again
+        (image_prompt: default with the prompt)."""
         for state in list(self._states):
             if not state.closed:
-                state.clear_overrides(prompt=prompt, t_index_list=t_index_list)
+                state.clear_overrides(prompt=prompt, t_index_list=t_index_list, image_prompt=image_prompt)
 
     @torch.no_grad()
     def apply_lora(self, lora_dict: Optional[Dict[str, float]]) -> None:
@@ -421,6 +460,8 @@ class StreamDiffusion:
                 continue
             if state.own_prompt is not None:
                 state.set_prompt(state.own_prompt, engine=self)
+            if state.own_image is not None:
+                state.set_image_tokens(*state.own_image, engine=self)
             if state.own_t_index_list is not None:
                 state.set_t_index_list(state.own_t_index_list, engine=self)
 
@@ -648,6 +689,8 @@ class StreamState:
 
     own_prompt: Optional[str] = None               # None: the global prompt
     own_t_index_list: Optional[List[int]] = None   # None: the global t_index_list
+    own_image: Optional[Tuple[torch.Tensor, float]] = None   # (device tokens [n_tok][D], scale); None: the global image prompt
+    home: Optional[StreamDiffusion] = None   # where clear_overrides recomputes what it keeps (None: the creating engine)
 
     def __init__(self, engine: StreamDiffusion):
         self._engine = engine          # keeps the engine (and its stream / library) alive while the state exists
@@ -679,12 +722,41 @@ class StreamState:
                    "b2sd_state_set_timesteps")
         self.own_t_index_list = t_index_list
 
-    def clear_overrides(self, prompt: bool = True, t_index_list: bool = True) -> None:
-        """Follow the global prompt and / or t_index_list again from the next step on (no device work)."""
-        for on, which, attr in ((prompt, capi.COND_PROMPT, "own_prompt"), (t_index_list, capi.COND_TIME, "own_t_index_list")):
+    @torch.no_grad()
+    def set_image_tokens(self, tokens: Optional[torch.Tensor], scale: float = 1.0,
+                         engine: Optional[StreamDiffusion] = None) -> None:
+        """This stream's own image prompt as (1, n_tok, D) fp16 tokens (StreamDiffusion.image_tokens), None: the global one
+        again.  The state's own prompt, if any, is kept.  Same stream and synchronisation rules as set_prompt."""
+        eng = engine or self._engine
+        if tokens is None:
+            self.clear_overrides(prompt=False, t_index_list=False, image_prompt=True, engine=eng)
+            return
+        tokens = _on_device(tokens.reshape(-1, eng.arch.cross_attention_dim).to(torch.float16), eng.device)
+        capi.check(self._lib.b2sd_state_set_image_embeds(eng._handle, self.handle, tokens.data_ptr(), tokens.shape[0],
+                                                         float(scale), eng._stream()), "b2sd_state_set_image_embeds")
+        self.own_image = (tokens, float(scale))
+
+    def clear_overrides(self, prompt: bool = True, t_index_list: bool = True, image_prompt: Optional[bool] = None,
+                        engine: Optional[StreamDiffusion] = None) -> None:
+        """Follow the global prompt, t_index_list and / or image prompt (default: with the prompt) again from the next step on.
+        The prompt and the image prompt share one conditioning block: dropping one of them recomputes the block with the other
+        on `engine` (default self.home); otherwise there is no device work."""
+        engine = engine or self.home
+        if image_prompt is None:
+            image_prompt = prompt
+        keep_prompt = None if prompt else self.own_prompt
+        keep_image = None if image_prompt else self.own_image
+        for on, which in ((prompt or image_prompt, capi.COND_PROMPT), (t_index_list, capi.COND_TIME)):
             if on:
                 capi.check(self._lib.b2sd_state_clear_conditioning(self.handle, which), "b2sd_state_clear_conditioning")
-                setattr(self, attr, None)
+        if prompt or image_prompt:
+            self.own_prompt = self.own_image = None
+            if keep_prompt is not None:
+                self.set_prompt(keep_prompt, engine=engine)
+            if keep_image is not None:
+                self.set_image_tokens(*keep_image, engine=engine)
+        if t_index_list:
+            self.own_t_index_list = None
 
     @property
     def handle(self) -> C.c_void_p:

@@ -82,6 +82,12 @@ class VideoStreamTrack(_Base):
         if not self._stopped:
             self._target().update_lora(lora_dict)
 
+    def update_image_prompt(self, image, scale: float = 1.0) -> None:
+        """As update_prompt, for the IP-Adapter image prompt (a PIL image or an HWC uint8 array / tensor, never a path; None
+        clears it): this viewer's own with per-peer streams (PeerStream.update_image_prompt), else the pipeline's global one"""
+        if not self._stopped:
+            self._target().update_image_prompt(image, scale)
+
     async def _recv_source(self):
         try:
             return await self.track.recv()

@@ -247,13 +247,15 @@ def layout_variant(batch: int, height: int, width: int) -> str:
 
 def packed_blob_path(engine_dir, model_id_or_path: str, arch_name: str, use_lcm_lora: bool, lcm_lora_id: Optional[str],
                      lora_dict: Optional[Dict[str, float]], vae_id: Optional[str], synthetic: bool, variant: str = "",
-                     controlnet: Optional[str] = None, control_processor: Optional[str] = None, full_vae: bool = False) -> str:
+                     controlnet: Optional[str] = None, control_processor: Optional[str] = None, full_vae: bool = False,
+                  ip_adapter: Optional[str] = None) -> str:
     """Where the packed-weight blob of this model lives: `<engine_dir>/engines--<model>/b2sd-<arch>-<recipe hash>.b2pack`,
     the directory naming of the reference's TensorRT cache (lib/wrapper.py:593, `engines--` + model id with / -> --).
     The hash covers everything that changes the weight VALUES (LoRAs and their scales, LCM-LoRA, VAE, ControlNet, synthetic
     seed), not
     batch / resolution / prompt (the blob does not depend on them, unlike the reference's static-shape engines).
-    full_vae (use_tiny_vae=False) enters the recipe only when set, so the names of TAESD blobs do not change."""
+    full_vae (use_tiny_vae=False) enters the recipe only when set, so the names of TAESD blobs do not change; so does
+    ip_adapter (an adapter file or directory, or "synthetic"), with the adapter file's real path, size and mtime."""
     import hashlib
     import json
     recipe = {"lcm": bool(use_lcm_lora), "lcm_id": lcm_lora_id, "vae": vae_id, "synthetic": bool(synthetic), "layout": variant,
@@ -272,6 +274,13 @@ def packed_blob_path(engine_dir, model_id_or_path: str, arch_name: str, use_lcm_
             if name.endswith((".safetensors", ".json")):
                 st = os.stat(os.path.join(repo, name))
                 recipe.setdefault("controlnet_files", []).append((name, st.st_size, int(st.st_mtime)))
+    if ip_adapter is not None:
+        recipe["ip_adapter"] = ip_adapter
+        if os.path.exists(ip_adapter):   # a replaced adapter file must not hit the old blob
+            from .image_prompt import adapter_file
+            f = os.path.realpath(adapter_file(ip_adapter))
+            st = os.stat(f)
+            recipe["ip_adapter_file"] = (f, st.st_size, int(st.st_mtime))
     digest = hashlib.sha256(json.dumps(recipe, sort_keys=True).encode()).hexdigest()[:16]
     name = "engines--" + model_id_or_path.strip("/").replace("/", "--")
     return os.path.join(str(engine_dir), name, f"b2sd-{arch_name}-{digest}.b2pack")

@@ -57,6 +57,9 @@ class StreamDiffusionWrapper:
     # constructor keeps the reference's signature; StreamDiffusionPipeline(live_lora=...) sets it on the instance before
     # __init__ runs.
     live_lora: Optional[bool] = None
+    # IP-Adapter image prompts (update_image_prompt): an adapter file or directory, "synthetic" (seeded weights, with synthetic
+    # models only), or None for $B200SD_IP_ADAPTER (unset: none).  Set on the instance before __init__, as live_lora.
+    ip_adapter: Optional[str] = None
 
     def __init__(
         self,
@@ -143,10 +146,13 @@ class StreamDiffusionWrapper:
         self.cuda_stream = CudaStreamPtr(cuda_stream_handle) if cuda_stream_handle is not None else None
         self._ext_stream = (torch.cuda.ExternalStream(cuda_stream_handle) if cuda_stream_handle is not None else None)
 
+        self._image_encoder = None
         self.stream: StreamDiffusion = self._load_model(
             model_id_or_path=model_id_or_path, lora_dict=lora_dict, lcm_lora_id=lcm_lora_id, vae_id=vae_id,
             t_index_list=t_index_list, do_add_noise=do_add_noise, use_lcm_lora=use_lcm_lora, cfg_type=cfg_type,
             controlnet_id_or_path=controlnet_id_or_path, controlnet_processor_id=controlnet_processor_id)
+        if self._image_encoder is not None:
+            self.stream.image_encoder = self._image_encoder
 
     # -- model loading: replaces _load_trt_model/_load_model (lib/wrapper.py:409-944) --------------------
     def _load_model(self, model_id_or_path, lora_dict, lcm_lora_id, vae_id, t_index_list, do_add_noise,
@@ -173,6 +179,8 @@ class StreamDiffusionWrapper:
                   vae_scaling_factor=W.resolve_vae_scaling_factor(repo if have_ckpt else None))
         cn = controlnet_id_or_path is not None
         hed = cn and controlnet_processor_id == "hed"
+        adapter = self._load_ip_adapter(arch, synthetic_ok)
+        kw["ip_adapter"] = adapter
         blob = None
         # blobs are kept for real checkpoints; seeded synthetic weights (benchmarks, tests) only with B200SD_PACK_CACHE=synthetic
         mode = os.getenv("B200SD_PACK_CACHE", "1")
@@ -183,7 +191,8 @@ class StreamDiffusionWrapper:
                                       lora_dict, vae_id, synthetic=not have_ckpt,
                                       variant=W.layout_variant(self.batch_size, self.height, self.width),
                                       controlnet=controlnet_id_or_path, control_processor=controlnet_processor_id,
-                                      full_vae=not tiny_vae)
+                                      full_vae=not tiny_vae,
+                                      ip_adapter=None if adapter is None else adapter.path or "synthetic")
         encoder = make_prompt_encoder(repo if have_ckpt else None, arch.cross_attention_dim, self.device, allow_synthetic=synthetic_ok)
         if blob is not None and os.path.exists(blob) and (have_ckpt or synthetic_ok):
             try:
@@ -201,6 +210,23 @@ class StreamDiffusionWrapper:
         self._blob_to_write = blob
         return StreamDiffusion(arch, unet_sd, vae_sd, t_index_list, encoder, controlnet_sd=cn_sd, hed_sd=hed_sd,
                                live_lora=self.live_lora, **kw)
+
+    def _load_ip_adapter(self, arch, synthetic_ok: bool):
+        """The IP-Adapter of self.ip_adapter / $B200SD_IP_ADAPTER with its image encoder (the stream's image_encoder), or None"""
+        import os
+        from . import image_prompt as I
+        path = self.ip_adapter if self.ip_adapter is not None else os.getenv(I.IP_ADAPTER_ENV) or None
+        if path is None:
+            return None
+        if path == "synthetic":
+            if not synthetic_ok:
+                raise ValueError("ip_adapter='synthetic' (seeded adapter weights) is for synthetic models only")
+            adapter = I.adapter_from_state_dict(I.synthetic_adapter_state_dict(arch), arch)
+            self._image_encoder = I.SyntheticImageEncoder(adapter.embed_dim)
+        else:
+            adapter = I.load_adapter(path, arch)
+            self._image_encoder = I.make_image_encoder(path, adapter.embed_dim, self.device, allow_synthetic=synthetic_ok)
+        return adapter
 
     def _on_stream(self):
         return torch.cuda.stream(self._ext_stream) if self._ext_stream is not None else _NullCtx()

@@ -129,6 +129,12 @@ typedef struct {
     int nb, heads, sq, skv, d_real, dp;   /* dp: 64, 128, 192 (zero-padded heads) or 512 (d_real 512) */
 } b2sd_attn_desc;
 int b2sd_op_attention(const b2sd_attn_desc* d, void* stream);
+/* The same (dp 64 / 128 / 192) with IP-Adapter's decoupled image segment, shared by every batch item:
+ *   out = softmax(Q K^T / sqrt(d_real)) V + softmax(Q Kip^T / sqrt(d_real)) Vip
+ * over the first *n_ip image keys (device int, 0..64, read by the kernel; 0 = b2sd_op_attention's result, bit for bit).
+ * k_ip: [64][ldk] with k's head layout; vt_ip = Vip^T: [heads*dp][64]; both 16-byte aligned, whole 64-key blocks whose keys
+ * past n_ip must be finite (zeroed).  A scale on the image term is folded into vt_ip. */
+int b2sd_op_attention_ip(const b2sd_attn_desc* d, const void* k_ip, const void* vt_ip, const int* n_ip, void* stream);
 
 /* GroupNorm(+SiLU) over the channel concatenation [xa | xb] (xb may be NULL), NHWC fp16.  y must not overlap xa or xb
  * (the statistics are centred on a value of x that other CTAs read after some have written y): refused. */
@@ -209,6 +215,10 @@ typedef struct {
                                     as to_q / to_k / to_v / to_out.0 with q/k/v as [512][512]); the latent is scaling_factor times the
                                     mean of the encoder's distribution (not a sample).  Inherited by lanes. */
     float vae_scaling_factor;    /* with vae = B2SD_VAE_KL: vae/config.json scaling_factor; 0 = 0.18215 */
+    int ip_tokens;               /* IP-Adapter image prompts: 0 = off; else the most image tokens a prompt may have, 1..64.  The
+                                    UNet's cross-attentions (not the ControlNet's) then add a decoupled attention over the image
+                                    tokens' K / V (weights "...attn2.to_k_ip.weight" / "...attn2.to_v_ip.weight" beside to_k /
+                                    to_v), see b2sd_set_image_embeds.  Inherited by lanes and styles. */
 } b2sd_config;
 enum { B2SD_CONTROL_FRAME = 0, B2SD_CONTROL_HED = 1 };
 enum { B2SD_VAE_TINY = 0, B2SD_VAE_KL = 1 };
@@ -423,6 +433,10 @@ typedef struct {
     b2sd_post_u8_args post_u8;
     b2sd_small_linear_args small_linear;
     b2sd_timestep_embedding_args timestep_embedding;
+    /* _ATTN with IP-Adapter's image segment: b2sd_op_attention_ip's k_ip, vt_ip and n_ip (device memory); NULL otherwise */
+    const void* attn_k_ip;
+    const void* attn_vt_ip;
+    const int* attn_n_ip;
 } b2sd_launch_record;
 /* One b2sd_step with the frame program run eagerly (no CUDA graph) and `fn` called around every kernel launch: `stream` is
  * synchronised, fn(user, index, 0, rec) runs, the launch is enqueued, `stream` is synchronised, fn(user, index, 1, rec) runs.
@@ -479,6 +493,20 @@ int b2sd_state_set_prompt_embeds(b2sd_handle h, b2sd_state_handle state, const v
 /* The same for the time block from the state's per-slot timesteps in DEVICE memory, fp32 [batch]; as b2sd_set_timesteps, only
  * the time embedding changes (alpha / beta / c_skip / c_out keep their b2sd_prepare values). */
 int b2sd_state_set_timesteps(b2sd_handle h, b2sd_state_handle state, const float* timesteps, void* stream);
+/* IP-Adapter image prompt (an engine with ip_tokens > 0), shared by the frame's cross-attentions like the prompt:
+ * tokens_f16 fp16 [n_tok][cross_attention_dim] (host or device memory, 1 <= n_tok <= ip_tokens; NULL clears the image prompt),
+ * scale (finite) multiplies the image attention term (folded into the image V^T).  b2sd_set_image_embeds refreshes the engine's
+ * global prompt block, as b2sd_set_prompt_embeds does; b2sd_state_set_image_embeds computes the state's prompt block (its own
+ * prompt if it has one computed on h's weight store, else the engine's) with this image prompt, as
+ * b2sd_state_set_prompt_embeds does (tokens in DEVICE memory, stream-ordered, no host synchronisation), and
+ * b2sd_state_set_prompt_embeds keeps the state's image prompt likewise.  A state's image prompt without a prompt of its own
+ * takes the text part from the engine's global block at the call, so a global refresh (b2sd_set_prompt_embeds,
+ * b2sd_refresh_conditioning) is followed by setting the state's image prompt again, as its own prompt is.  After a move to another store of the family set the
+ * state's prompt, then its image prompt, again.  Clearing the state's prompt block (b2sd_state_clear_conditioning(state, 0))
+ * drops both.  Neither call recaptures a CUDA graph. */
+int b2sd_set_image_embeds(b2sd_handle h, const void* tokens_f16, int n_tok, float scale, void* stream);
+int b2sd_state_set_image_embeds(b2sd_handle h, b2sd_state_handle state, const void* tokens_f16, int n_tok, float scale,
+                                void* stream);
 /* Drop the state's override of the prompt (which = 0) or time (which = 1) block: later steps use the engines' global values.
  * No device work; the override is freed after the steps already submitted with it. */
 int b2sd_state_clear_conditioning(b2sd_state_handle state, int which);

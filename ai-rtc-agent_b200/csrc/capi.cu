@@ -56,6 +56,7 @@ static void to_igemm_desc(const b2sd_igemm_desc* d, IgemmDesc& g) {
     g.epi.out2 = reinterpret_cast<__half*>(d->out2);
     g.epi.ld2 = d->ld2;
     g.epi.col2 = d->col2;
+    g.epi.acc_scale_b = d->acc_scale_b;
 }
 
 static b2sd_act_view from_view(const ActView& a) {
@@ -118,6 +119,7 @@ void igemm_record(const IgemmDesc& g, const IgemmPlan* plan, b2sd_igemm_desc* d,
     d->out2 = g.epi.out2;
     d->ld2 = g.epi.ld2;
     d->col2 = g.epi.col2;
+    d->acc_scale_b = g.epi.acc_scale_b;
     if (plan) {
         d->bn = plan->p.BN;
         d->splits = plan->splits;

@@ -210,7 +210,7 @@ static int igemm_autotile_single(IgemmDesc d, bool allow_swap, IgemmPlan* plan_o
     const long rows_all = (long)d.Nb * d.Ho * d.Wo;
     // Swapped orientation by default only where it measured faster (tools/bench_op.py, cold weights): the 8x8 level,
     // where a 128-pixel M tile would be half empty.  B2_SWAP=1 forces it for every eligible UNet contraction.
-    const bool swap_here = allow_swap && !geglu && !pad0 && d.epi.n_valid >= 128 && (d.epi.n_valid & 7) == 0 &&
+    const bool swap_here = allow_swap && !geglu && !pad0 && !d.epi.acc_scale_b && d.epi.n_valid >= 128 && (d.epi.n_valid & 7) == 0 &&
                            (swap_on || (!swap_off && tuned && rows_all <= 64 && total_kb >= 90));
     if (swap_here) {
         d.swap = 1;
@@ -372,6 +372,8 @@ struct CondOverride {
     uint64_t id = 0;
     uint64_t store = 0;            // WeightStore::id of the parameters it was computed with
     bool own_text = false;         // a prompt block from the state's own prompt embeddings (else from the global ones)
+    bool own_time = false;         // a time block whose time biases are from the state's own timesteps (else the global ones)
+    bool own_control = false;      // ... and whose ControlNet scales are the state's own (else the global ones)
     void* buf = nullptr;
     size_t bytes = 0;
     cudaEvent_t ready = nullptr;   // recorded once buf holds the block
@@ -432,6 +434,9 @@ struct b2sd_engine {
     float* temb = nullptr;     // [B][4*C0]
     float* cn_temb_h = nullptr;   // ControlNet time_embedding (its own weights), [B][4*C0]
     float* cn_temb = nullptr;
+    // per-slot ControlNet conditioning scale [B] that the zero convs read (in the time block), and the engine's global values
+    float* cn_scale = nullptr;
+    float cn_scale_global[16] = {1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f};
     float* gn_ws = nullptr;    // GroupNorm chunk partials (shared: launches are stream-ordered)
     int* tile_counters = nullptr;
     float coef_host[4][64]{};
@@ -802,7 +807,7 @@ struct b2sd_engine {
     // conv3x3 (or 1x1) over one source with bias / relu / residual
     int add_conv(std::vector<Op>& dst, const Act& x, const std::string& wkey, const std::string& bkey, int taps,
                  int stride, const Act& y, int flags, const Act* res, cudaStream_t s, float acc_scale = 1.f,
-                 float res_scale = 1.f) {
+                 float res_scale = 1.f, const float* acc_scale_b = nullptr) {
         const Raw* w = get(wkey);
         if (!w) return -1;
         cur = wkey;
@@ -823,6 +828,7 @@ struct b2sd_engine {
         d.epi.colbias_bstride = 0;
         if (res) { d.epi.res = res->p; d.epi.ldr = res->ld; }
         d.epi.acc_scale = acc_scale; d.epi.res_scale = res_scale;
+        d.epi.acc_scale_b = acc_scale_b;
         d.epi.flags = flags;
         d.epi.n_valid = cout;
         // the TAESD body at 256x256 and above: persistent halo-tile kernel with resident weights (tconv.cu)
@@ -1346,7 +1352,8 @@ int b2sd_engine::build_hed(const uint8_t** control, cudaStream_t s) {
 // ControlNetModel body: conv_in(x) + cond (broadcast to every stream-batch slot), the UNet's down blocks and mid block under the
 // "controlnet." prefix with its own time embedding, then the zero convs: skips[k] <- skips[k] + controlnet_down_blocks.k(f_k),
 // *mid <- *mid + controlnet_mid_block(f_mid), each one 1x1 contraction with the UNet tensor as its epilogue residual, written
-// to a new buffer (conditioning scale 1.0).
+// to a new buffer.  Each slot's residual is scaled by its conditioning scale (cn_scale, read when the launch runs: diffusers
+// multiplies the zero conv's output, bias included, by controlnet_conditioning_scale).
 int b2sd_engine::build_controlnet(const Act& cond, std::vector<Act>& skips, Act* mid, cudaStream_t s) {
     const std::string P = "controlnet.";
     const int B = cfg.batch, nlev = 4;
@@ -1397,15 +1404,18 @@ int b2sd_engine::build_controlnet(const Act& cond, std::vector<Act>& skips, Act*
         return -1;
     }
     allow_swap = false;
+    cn_scale = static_cast<float*>(this->cond[COND_TIME].take((size_t)B * sizeof(float)));   // (`cond` is the embedding here)
+    if (!cn_scale) return -1;
     for (size_t k = 0; k < feats.size(); ++k) {
         const std::string w = P + "controlnet_down_blocks." + std::to_string(k);
         Act o = new_act(skips[k].n, skips[k].h, skips[k].w, skips[k].c);
-        TRY(add_conv(prog_frame, feats[k], w + ".weight", w + ".bias", 1, 1, o, 0, &skips[k], s));
+        TRY(add_conv(prog_frame, feats[k], w + ".weight", w + ".bias", 1, 1, o, 0, &skips[k], s, 1.f, 1.f, cn_scale));
         skips[k] = o;
         taps["cn.res." + std::to_string(k)] = o;
     }
     Act o = new_act(mid->n, mid->h, mid->w, mid->c);
-    TRY(add_conv(prog_frame, h, P + "controlnet_mid_block.weight", P + "controlnet_mid_block.bias", 1, 1, o, 0, mid, s));
+    TRY(add_conv(prog_frame, h, P + "controlnet_mid_block.weight", P + "controlnet_mid_block.bias", 1, 1, o, 0, mid, s, 1.f, 1.f,
+                 cn_scale));
     *mid = o;
     taps["cn.mid"] = o;
     allow_swap = true;
@@ -1752,6 +1762,7 @@ int b2sd_engine::build_program(cudaStream_t s) {
                                       2 * r((size_t)ATTN_IP_KEYS * Cp * 2);
             bytes[COND_TIME] += resnets * r((size_t)B * ch[i] * sizeof(float));
         }
+        if (cfg.controlnet) bytes[COND_TIME] += r((size_t)B * sizeof(float));   // the per-slot ControlNet scale
         if (cfg.ip_tokens) bytes[COND_PROMPT] += r(sizeof(int));   // ip_count
         for (int k = 0; k < 2; ++k) {
             CondBlock& b = cond[k];
@@ -2020,6 +2031,21 @@ static int state_reset(b2sd_state* st, cudaStream_t s) {
 }
 
 // ---- conditioning blocks ----------------------------------------------------------------------------
+// The engine's global ControlNet scales into the time block, as a kernel argument: stream-ordered, and no host buffer has to
+// outlive the call
+struct Scales16 { float v[16]; };
+__global__ void write_scales_kernel(float* dst, Scales16 v, int n) {
+    if ((int)threadIdx.x < n) dst[threadIdx.x] = v.v[threadIdx.x];
+}
+static int write_global_scales(b2sd_engine* h, cudaStream_t s) {
+    if (!h->cn_scale) return 0;
+    Scales16 v;
+    memcpy(v.v, h->cn_scale_global, sizeof(v.v));
+    write_scales_kernel<<<1, 32, 0, s>>>(h->cn_scale, v, h->cfg.batch);
+    CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
 // Block k now holds the lane's global values (after b2sd_prepare / b2sd_set_*, which computed them into it): keep a copy to rebind.
 static int keep_global(b2sd_engine* h, int k, cudaStream_t s) {
     auto& b = h->cond[k];
@@ -2473,6 +2499,7 @@ int b2sd_prepare(b2sd_handle h, const void* prompt_embeds, const float* timestep
     TRY(h->run(h->prog_prompt, s));
     TRY(run_image(h, h->ip_n_global, h->ip_scale_global, s));
     TRY(refresh_time(h, s));
+    TRY(write_global_scales(h, s));
     CUDA_OK(cudaMemcpyAsync(h->ctx_global, h->ctx, (size_t)h->cfg.ctx_tokens * h->cfg.cross_attention_dim * 2,
                             cudaMemcpyDeviceToDevice, s));
     CUDA_OK(cudaMemcpyAsync(h->tsteps_global, h->tsteps, B * sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -2685,8 +2712,31 @@ int b2sd_set_timesteps(b2sd_handle h, const float* timesteps, void* stream) {
     CUDA_OK(cudaMemcpyAsync(h->tsteps, timesteps, h->cfg.batch * sizeof(float), cudaMemcpyHostToDevice, s));
     CUDA_OK(cudaStreamSynchronize(s));
     CUDA_OK(cudaMemcpyAsync(h->tsteps_global, h->tsteps, h->cfg.batch * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    if (h->cn_scale) TRY(bind_block(h, COND_TIME, nullptr, s));   // keep the global ControlNet scales of the block
     h->cond[COND_TIME].held = COND_UNKNOWN;
     TRY(refresh_time(h, s));
+    return keep_global(h, COND_TIME, s);
+}
+
+int b2sd_set_control_scale(b2sd_handle h, const float* scale_per_slot, void* stream) {
+    if (!h || !h->built || !scale_per_slot) {
+        b2_set_error("b2sd_set_control_scale: null argument, or b2sd_prepare not called");
+        return -1;
+    }
+    if (!h->cn_scale) {
+        b2_set_error("b2sd_set_control_scale: the engine was created without a ControlNet (b2sd_config.controlnet = 0)");
+        return -1;
+    }
+    for (int k = 0; k < h->cfg.batch; ++k)
+        if (!isfinite(scale_per_slot[k])) {
+            b2_set_error("b2sd_set_control_scale: the scale of slot %d is not finite (%f)", k, (double)scale_per_slot[k]);
+            return -1;
+        }
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    memcpy(h->cn_scale_global, scale_per_slot, h->cfg.batch * sizeof(float));
+    TRY(bind_block(h, COND_TIME, nullptr, s));   // keep the global time biases of the block
+    h->cond[COND_TIME].held = COND_UNKNOWN;
+    TRY(write_global_scales(h, s));
     return keep_global(h, COND_TIME, s);
 }
 
@@ -2849,6 +2899,7 @@ int b2sd_refresh_conditioning(b2sd_handle h, void* stream) {
     CUDA_OK(cudaMemcpyAsync(h->tsteps, h->tsteps_global, h->cfg.batch * sizeof(float), cudaMemcpyDeviceToDevice, s));
     h->cond[COND_PROMPT].held = COND_UNKNOWN;
     h->cond[COND_TIME].held = COND_UNKNOWN;
+    TRY(write_global_scales(h, s));
     TRY(h->run(h->prog_prompt, s));
     TRY(run_image(h, h->ip_n_global, h->ip_scale_global, s));
     TRY(refresh_time(h, s));
@@ -2992,6 +3043,15 @@ static CondOverride* prompt_base(b2sd_engine* h, b2sd_state* st, bool own_text) 
     return ov && ov->store == h->ws->id && (ov->own_text || !own_text) ? ov : nullptr;
 }
 
+// The time block a refresh of `st`'s timesteps (control = false) or ControlNet scales (control = true) starts from, so that it
+// keeps the other part: the state's override if it was computed on h's store and holds that part of its own; else nullptr, the
+// lane's global values.  As for the prompt block, a part taken from the global values is not kept: the state's own
+// settings are set again after a global refresh.
+static CondOverride* time_base(b2sd_engine* h, b2sd_state* st, bool control) {
+    CondOverride* ov = st->cond[COND_TIME].get();
+    return ov && ov->store == h->ws->id && (control ? ov->own_time : ov->own_control) ? ov : nullptr;
+}
+
 // Run h's prompt (k = COND_PROMPT) or time refresh on s with `input` (device) in place of the global embeddings / timesteps,
 // put the global ones back, and publish the block as the state's override.  Stream-ordered after the frames queued on s, and
 // no host synchronisation: the refresh writes only h's block, which no other stream reads.
@@ -3008,12 +3068,21 @@ static int state_refresh(const char* fn, b2sd_handle h, b2sd_state* state, int k
     // with image prompts the prompt program leaves the image part of the block alone: start from the state's block, so that
     // the state keeps its own image prompt
     if (k == COND_PROMPT && h->cfg.ip_tokens) TRY(bind_block(h, k, prompt_base(h, state, false), s));
+    // with a ControlNet the time program leaves the ControlNet scales of the block alone: start from the state's block if it
+    // holds the state's own scales
+    CondOverride* tbase = k == COND_TIME && h->cn_scale ? time_base(h, state, false) : nullptr;
+    if (k == COND_TIME && h->cn_scale) TRY(bind_block(h, k, tbase, s));
     h->cond[k].held = COND_UNKNOWN;
     CUDA_OK(cudaMemcpyAsync(dst, input, bytes, cudaMemcpyDeviceToDevice, s));
     const int rc = k == COND_PROMPT ? h->run(h->prog_prompt, s) : refresh_time(h, s);
     CUDA_OK(cudaMemcpyAsync(dst, global, bytes, cudaMemcpyDeviceToDevice, s));
     TRY(rc);
-    return publish_override(h, state, k, s, k == COND_PROMPT);
+    TRY(publish_override(h, state, k, s, k == COND_PROMPT));
+    if (k == COND_TIME) {
+        state->cond[k]->own_time = true;
+        state->cond[k]->own_control = tbase != nullptr;
+    }
+    return 0;
 }
 
 int b2sd_state_set_prompt_embeds(b2sd_handle h, b2sd_state_handle state, const void* prompt_embeds, void* stream) {
@@ -3023,6 +3092,28 @@ int b2sd_state_set_prompt_embeds(b2sd_handle h, b2sd_state_handle state, const v
 
 int b2sd_state_set_timesteps(b2sd_handle h, b2sd_state_handle state, const float* timesteps, void* stream) {
     return state_refresh("b2sd_state_set_timesteps", h, state, COND_TIME, timesteps, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2sd_state_set_control_scale(b2sd_handle h, b2sd_state_handle state, const float* scale_per_slot, void* stream) {
+    const char* fn = "b2sd_state_set_control_scale";
+    TRY(check_state(fn, h, state));
+    if (!scale_per_slot) {
+        b2_set_error("%s: null argument", fn);
+        return -1;
+    }
+    if (!h->cn_scale) {
+        b2_set_error("%s: the engine was created without a ControlNet (b2sd_config.controlnet = 0)", fn);
+        return -1;
+    }
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    CondOverride* base = time_base(h, state, true);   // the state's time biases: its own timesteps', or the global ones
+    TRY(bind_block(h, COND_TIME, base, s));
+    h->cond[COND_TIME].held = COND_UNKNOWN;
+    CUDA_OK(cudaMemcpyAsync(h->cn_scale, scale_per_slot, h->cfg.batch * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    TRY(publish_override(h, state, COND_TIME, s));
+    state->cond[COND_TIME]->own_time = base != nullptr;
+    state->cond[COND_TIME]->own_control = true;
+    return 0;
 }
 
 // n rows of image tokens (nullptr: none) into h->ip_tok, the rest zeroed
@@ -3392,6 +3483,7 @@ int b2sd_audit_refresh(b2sd_handle h, b2sd_audit_fn fn, void* user, void* stream
     std::vector<Op> time_ops;
     TRY(time_embedding_ops(h, &time_ops));
     h->cond[COND_PROMPT].held = h->cond[COND_TIME].held = COND_UNKNOWN;
+    TRY(write_global_scales(h, au.s));
     TRY(au.program(h->prog_prompt));
     TRY(au.program(time_ops));
     TRY(au.program(h->prog_time));

@@ -48,7 +48,8 @@ __device__ __forceinline__ void rowstat_add(const IgEpilogue& e, long orow, floa
 // 16 accumulator columns [col0, col0+16) of output row `orow` (batch item b); the accumulators are
 // acc[OFF .. OFF+16) of a register array (compile-time indices only: nothing may spill to local memory).
 // SILU: compile the IG_SILU branch in (kernels that never see the flag leave it out: it costs registers in the wide tiles).
-template <int OFF, int N, typename T, bool SILU = false>
+// ASCALE: likewise the per-batch-item factor e.acc_scale_b.
+template <int OFF, int N, typename T, bool SILU = false, bool ASCALE = false>
 __device__ __forceinline__ void epi_store16(const IgEpilogue& e, const T (&acc)[N], int b, long orow, int col0, float mu = 0.f,
                                             float rstd = 1.f) {
     int nv = e.n_valid - col0;
@@ -83,6 +84,11 @@ __device__ __forceinline__ void epi_store16(const IgEpilogue& e, const T (&acc)[
     if (e.acc_scale != 1.0f) {
 #pragma unroll
         for (int i = 0; i < 16; ++i) v[i] *= e.acc_scale;
+    }
+    if (ASCALE && e.acc_scale_b) {
+        const float sb = e.acc_scale_b[b];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) v[i] *= sb;
     }
     if (e.res) {
         const __half* rp = e.res + orow * e.ldr + col0;
@@ -163,7 +169,7 @@ __device__ __forceinline__ void rowstat_quad(const IgEpilogue& e, const EpiRow& 
 //   ln_fma: LayerNorm-folded launch with vectorisable pitches: x = rstd * acc - rstd * mu * colsum + bias'
 //   GEGLU: tile columns [0, BN/2) are values, [BN/2, BN) gates; out = v * gelu_erf(g)
 //   otherwise: bias / scale / residual / ReLU, optional row statistics and transposed V block
-template <int BN, bool SILU = false>
+template <int BN, bool SILU = false, bool ASCALE = false>
 __device__ __forceinline__ void epi_frag(const IgEpilogue& e, const float (&acc)[BN / 2], const EpiRow (&rw)[2], int ntile,
                                          bool ln_fma, int lane) {
     const int q2 = 2 * (lane & 3);
@@ -233,6 +239,11 @@ __device__ __forceinline__ void epi_frag(const IgEpilogue& e, const float (&acc)
                 if (e.acc_scale != 1.0f) {
                     x[0] *= e.acc_scale;
                     x[1] *= e.acc_scale;
+                }
+                if (ASCALE && e.acc_scale_b) {
+                    const float sb = e.acc_scale_b[rw[h].b];
+                    x[0] *= sb;
+                    x[1] *= sb;
                 }
                 if (e.res) {
                     const __half* rp = e.res + rw[h].orow * e.ldr + col;

@@ -156,7 +156,7 @@ __device__ __forceinline__ void splitk_sum16(uint32_t stg_local, int cc, int row
 // with the same weight tile: each CTA loads its own 128 pixel rows and HALF of the weight rows, multicast into both CTAs'
 // shared memory, so each SM fetches half of the weight bytes from L2.  A ring slot is refilled only when the warps of BOTH
 // CTAs have released it (every consumer warp arrives on its own and on the peer's empty barrier).
-template <int BN, bool PAIR, bool SILU, bool PAD0 = false>
+template <int BN, bool PAIR, bool SILU, bool PAD0 = false, bool ASCALE = false>
 __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -340,7 +340,7 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
                     rw[h].b = n;
                     ln_row_stats(e, rw[h].orow, rw[h].ok, rw[h].mu, rw[h].rstd);
                 }
-                epi_frag<BN, SILU>(e, acc, rw, ntile, ln_fma, lane);
+                epi_frag<BN, SILU, ASCALE>(e, acc, rw, ntile, ln_fma, lane);
             }
             B2_TS(if (ts && it == 0 && threadIdx.x == 0) ts[5] = globaltimer_ns();)
         }
@@ -421,7 +421,7 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& p) {
                     const long orow = ((long)n * p.Ho + h) * p.Wo + w;
                     float mu, rstd;
                     ln_row_stats(p.epi, orow, true, mu, rstd);
-                    epi_store16<0, 16, float, SILU>(p.epi, acc, n, orow, ntile * BN + cc * 16, mu, rstd);
+                    epi_store16<0, 16, float, SILU, ASCALE>(p.epi, acc, n, orow, ntile * BN + cc * 16, mu, rstd);
                 }
             }
         }
@@ -440,6 +440,13 @@ __global__ void __launch_bounds__(IG_THREADS, 1) igemm_kernel(const __grid_const
 // Downsample2D(padding=0).  Its own instantiations (single CTAs, N tiles 64 / 128 / 256), so every other kernel is unchanged.
 template <int BN>
 __global__ void __launch_bounds__(IG_THREADS, 1) igemm_pad0_kernel(const __grid_constant__ IgemmParams p) { igemm_body<BN, false, false, true>(p); }
+// Per-batch-item accumulator factor (IgEpilogue::acc_scale_b: the ControlNet zero convs' per-slot conditioning scale).  Its own
+// instantiations, single CTAs and CTA pairs, at every N tile the frame program's policy picks for a contraction without
+// GEGLU / SiLU / tap origin 0 / swap (16 / 32 / 64 / 128 / 160 / 256), so every other kernel is unchanged.
+template <int BN, bool PAIR>
+__global__ void __launch_bounds__(IG_THREADS, 1) igemm_ascale_kernel(const __grid_constant__ IgemmParams p) {
+    igemm_body<BN, PAIR, false, false, true>(p);
+}
 
 using IgemmFn = void (*)(IgemmParams);
 // every N tile the planner can produce (multiples of 16 up to 256); CTA pairs need BN % 32 == 0.  At 168 registers the widest
@@ -457,7 +464,19 @@ static IgemmFn igemm_fn(int bn) {
 }
 // IG_SILU epilogues (the ControlNet conditioning embedding: N = 16 / 32 / 96 / 256, single CTAs, N tiles <= 128) are separate
 // instantiations, so the SiLU code costs the other kernels no registers (a 256-wide SiLU tile would spill)
-static IgemmFn igemm_select(int bn, bool pair, bool silu, bool pad0 = false) {
+static IgemmFn igemm_select(int bn, bool pair, bool silu, bool pad0 = false, bool ascale = false) {
+    if (ascale) {
+        if (silu || pad0) return nullptr;
+        switch (bn) {
+            case 16: return pair ? nullptr : igemm_ascale_kernel<16, false>;
+            case 32: return pair ? igemm_ascale_kernel<32, true> : igemm_ascale_kernel<32, false>;
+            case 64: return pair ? igemm_ascale_kernel<64, true> : igemm_ascale_kernel<64, false>;
+            case 128: return pair ? igemm_ascale_kernel<128, true> : igemm_ascale_kernel<128, false>;
+            case 160: return pair ? igemm_ascale_kernel<160, true> : igemm_ascale_kernel<160, false>;
+            case 256: return pair ? igemm_ascale_kernel<256, true> : igemm_ascale_kernel<256, false>;
+            default: return nullptr;
+        }
+    }
     if (pad0) {
         if (pair || silu) return nullptr;
         switch (bn) {
@@ -549,8 +568,10 @@ size_t igemm_partial_floats(int splits, long rows_total, int n_valid) {
 // Swapped orientation plan: output channels on the M side (128 per CTA), a tile of BN pixels on the N side.
 static int plan_swap(const IgemmDesc& d, IgemmPlan* plan) {
     IgemmParams& p = plan->p;
-    if ((d.epi.flags & (IG_GEGLU | IG_PAD0)) || d.nseg < 1 || d.nseg > IG_MAX_SRC || d.epi.rowstat_out || d.epi.colsum || d.epi.out2) {
-        b2_set_error("igemm(swap): unsupported (GEGLU / tap origin 0 / LayerNorm fold / row statistics / transposed V / nseg %d)", d.nseg);
+    if ((d.epi.flags & (IG_GEGLU | IG_PAD0)) || d.nseg < 1 || d.nseg > IG_MAX_SRC || d.epi.rowstat_out || d.epi.colsum || d.epi.out2 ||
+        d.epi.acc_scale_b) {
+        b2_set_error("igemm(swap): unsupported (GEGLU / tap origin 0 / LayerNorm fold / row statistics / transposed V / "
+                     "per-item scale / nseg %d)", d.nseg);
         return -1;
     }
     int BN = d.BN;
@@ -665,9 +686,9 @@ int b2_device_sms() {
 
 // CTAs of the kernel for this tile that one SM holds at once as far as registers and threads allow (the plan sizes the
 // shared memory).  Dry runs do not touch the device: they assume the one CTA per SM that 288 threads at 168 registers allow.
-static int igemm_ctas_per_sm(int bn, bool pair, bool silu, bool pad0) {
+static int igemm_ctas_per_sm(int bn, bool pair, bool silu, bool pad0, bool ascale) {
     if (g_plan_dry) return 1;
-    IgemmFn fn = igemm_select(bn, pair, silu, pad0);
+    IgemmFn fn = igemm_select(bn, pair, silu, pad0, ascale);
     int n = 0;
     if (fn && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, IG_THREADS, 0) == cudaSuccess && n > 0) return n;
     cudaGetLastError();
@@ -701,6 +722,11 @@ int igemm_plan(const IgemmDesc& d, IgemmPlan* plan) {
     const bool pair = d.pair != 0;
     if ((d.epi.flags & IG_SILU) && !igemm_select(BN, pair, true)) {
         b2_set_error("igemm: no SiLU-epilogue kernel for BN %d%s (16/32/64/128, single CTAs)", BN, pair ? " (CTA pair)" : "");
+        return -1;
+    }
+    if (d.epi.acc_scale_b && ((d.epi.flags & (IG_GEGLU | IG_SILU | IG_PAD0)) || d.epi.colsum || !igemm_select(BN, pair, false, false, true))) {
+        b2_set_error("igemm: no per-item-scale kernel for BN %d%s (16/32/64/128/160/256, pairs from 32; no GEGLU / SiLU / tap "
+                     "origin 0 / LayerNorm fold)", BN, pair ? " (CTA pair)" : "");
         return -1;
     }
     if ((d.epi.flags & IG_PAD0) && !igemm_select(BN, pair, (d.epi.flags & IG_SILU) != 0, true)) {
@@ -807,7 +833,7 @@ int igemm_plan(const IgemmDesc& d, IgemmPlan* plan) {
     // The mainloop is TMA-latency bound: throughput per SM = bytes in flight / latency.  When registers admit only one CTA per
     // SM (the case of this kernel: 288 threads at up to 168 registers) the ring takes (nearly) all the shared memory; only
     // when two could be resident AND the launch needs them is the ring halved so that they fit.
-    const int per_sm = igemm_ctas_per_sm(BN, pair, (d.epi.flags & IG_SILU) != 0, (d.epi.flags & IG_PAD0) != 0);
+    const int per_sm = igemm_ctas_per_sm(BN, pair, (d.epi.flags & IG_SILU) != 0, (d.epi.flags & IG_PAD0) != 0, d.epi.acc_scale_b != nullptr);
     const long resident = (long)per_sm * b2_device_sms();   // CTAs the GPU runs at once
     static const char* pc_env = getenv("B2_PERSIST_CTAS");   // tuning: CTAs of a persistent launch (default: one resident wave)
     const long persist_ctas = pc_env ? atoi(pc_env) : resident;
@@ -872,8 +898,9 @@ int igemm_init() {
     static bool attr_set = false;
     if (!attr_set) {
         for (int bn = 16; bn <= 256; bn += 16) {
-            for (int pair = 0; pair < 4; ++pair) {   // single CTAs, CTA pairs, single CTAs with the SiLU epilogue, tap origin 0
-                IgemmFn fn = igemm_select(bn, pair == 1, pair == 2, pair == 3);
+            // single CTAs, CTA pairs, single CTAs with the SiLU epilogue, tap origin 0, per-item scale (single CTAs, pairs)
+            for (int pair = 0; pair < 6; ++pair) {
+                IgemmFn fn = igemm_select(bn, pair == 1 || pair == 5, pair == 2, pair == 3, pair >= 4);
                 if (!fn) continue;
                 cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
                 if (e != cudaSuccess) {
@@ -891,10 +918,12 @@ int igemm_init() {
 int igemm_launch(const IgemmPlan& plan, cudaStream_t stream) {
     if (igemm_init()) return -1;
     const int cz = plan.splits > 1 ? plan.splits : 1;
-    IgemmFn fn = igemm_select(plan.p.BN, plan.pair, (plan.p.epi.flags & IG_SILU) != 0, (plan.p.epi.flags & IG_PAD0) != 0);
+    IgemmFn fn = igemm_select(plan.p.BN, plan.pair, (plan.p.epi.flags & IG_SILU) != 0, (plan.p.epi.flags & IG_PAD0) != 0,
+                              plan.p.epi.acc_scale_b != nullptr);
     if (!fn) {
-        b2_set_error("igemm launch: no kernel for BN %d%s%s%s", plan.p.BN, plan.pair ? " (CTA pair)" : "",
-                     (plan.p.epi.flags & IG_SILU) ? " with the SiLU epilogue" : "", (plan.p.epi.flags & IG_PAD0) ? " with tap origin 0" : "");
+        b2_set_error("igemm launch: no kernel for BN %d%s%s%s%s", plan.p.BN, plan.pair ? " (CTA pair)" : "",
+                     (plan.p.epi.flags & IG_SILU) ? " with the SiLU epilogue" : "", (plan.p.epi.flags & IG_PAD0) ? " with tap origin 0" : "",
+                     plan.p.epi.acc_scale_b ? " with a per-item scale" : "");
         return -1;
     }
     cudaError_t e = plan.pair ? launch_kc(fn, plan.grid, dim3(IG_THREADS), plan.smem, stream, 2, cz, plan.p)

@@ -56,6 +56,10 @@ struct IgEpilogue {
     // which is the K-major V^T operand the attention kernel's P.V MMA reads (was a separate swapped-operand GEMM launch)
     __half* out2;
     int ld2, col2;
+    // ---- per-batch-item factor of the contraction term, read when the launch runs (the ControlNet zero convs: the per-slot
+    // conditioning scale): out = acc_scale_b[b] * acc_scale * (acc + bias) + res_scale * res.  Null: 1.  Its own kernel
+    // instantiations (igemm_ascale_kernel); normal orientation, no GEGLU / SiLU / tap origin 0 / LayerNorm fold.
+    const float* acc_scale_b;
 };
 
 constexpr float IG_STAT_SCALE = 1048576.f;   // 2^20 fixed point of the row statistics

@@ -188,7 +188,7 @@ bool tconv_eligible(const IgemmDesc& d) {
     const IgEpilogue& e = d.epi;
     return d.nseg == 1 && d.ntap[0] == 9 && d.stride <= 1 && !d.swap && d.src[0].C == TC_C && e.n_valid == TC_C &&
            d.w_rows >= TC_C && d.w_ld == 9 * TC_C && d.src[0].H == d.Ho && d.src[0].W == d.Wo && d.src[0].N == d.Nb &&
-           !(e.flags & (IG_GEGLU | IG_SPLITK | IG_SILU)) && !e.colsum && !e.rowstat_out && !e.out2 && (e.ldc & 7) == 0 &&
+           !(e.flags & (IG_GEGLU | IG_SPLITK | IG_SILU)) && !e.colsum && !e.rowstat_out && !e.out2 && !e.acc_scale_b && (e.ldc & 7) == 0 &&
            (!e.res || (e.ldr & 7) == 0) && e.colbias_bstride == 0 &&
            (d.src[0].ld & 7) == 0 && !(reinterpret_cast<uintptr_t>(d.src[0].ptr) & 15) && !(reinterpret_cast<uintptr_t>(d.w) & 15) &&
            !(reinterpret_cast<uintptr_t>(e.out) & 15) && !(reinterpret_cast<uintptr_t>(e.res) & 15) &&
@@ -202,7 +202,7 @@ int tconv_plan(const IgemmDesc& d, TconvPlan* plan) {
     *plan = TconvPlan{};
     if (!tconv_eligible(d)) {
         b2_set_error("tconv: needs a stride-1 3x3 convolution with 64 input and 64 output channels, 16-byte-aligned pitches and an "
-                     "epilogue of a batch-shared bias / scale / residual / ReLU");
+                     "epilogue of a batch-shared bias / scale / residual / ReLU (no per-item scale)");
         return -1;
     }
     TconvParams& p = plan->p;

@@ -32,6 +32,7 @@ class IgemmDesc(C.Structure):
         ("flags", C.c_int), ("n_valid", C.c_int), ("swap", C.c_int),
         ("rowstat_out", C.c_void_p), ("rowstat_in", C.c_void_p), ("colsum", C.c_void_p), ("ln_c", C.c_int), ("ln_eps", C.c_float),
         ("out2", C.c_void_p), ("ld2", C.c_int), ("col2", C.c_int),
+        ("acc_scale_b", C.c_void_p),
     ]
 
 
@@ -233,11 +234,14 @@ def lib() -> C.CDLL:
         _lib.b2sd_step_state.argtypes = [vp, vp, vp, ci, ci, ci, vp, ci, vp]
         _lib.b2sd_state_set_prompt_embeds.argtypes = [vp, vp, vp, vp]
         _lib.b2sd_state_set_timesteps.argtypes = [vp, vp, vp, vp]
+        _lib.b2sd_set_control_scale.argtypes = [vp, vp, vp]
+        _lib.b2sd_state_set_control_scale.argtypes = [vp, vp, vp, vp]
         _lib.b2sd_state_clear_conditioning.argtypes = [vp, ci]
         _lib.b2sd_set_image_embeds.argtypes = [vp, vp, ci, cf, vp]
         _lib.b2sd_state_set_image_embeds.argtypes = [vp, vp, vp, ci, cf, vp]
         for name in ("state_create", "state_reset", "state_destroy", "step_state", "state_set_prompt_embeds", "state_set_timesteps",
-                     "state_clear_conditioning", "set_image_embeds", "state_set_image_embeds"):
+                     "state_clear_conditioning", "set_image_embeds", "state_set_image_embeds", "set_control_scale",
+                     "state_set_control_scale"):
             getattr(_lib, "b2sd_" + name).restype = C.c_int
         _lib.b2sd_set_live_params.argtypes = [vp, ci]
         _lib.b2sd_apply_lora.argtypes = [vp, ci, C.POINTER(LoraFactor), vp]

@@ -42,13 +42,15 @@ def igemm(srcs: Sequence[Tuple[torch.Tensor, int]], w: torch.Tensor, out: torch.
           tconv: bool = False, pair: bool = False, pad0: bool = False,
           rowstat_out: Optional[torch.Tensor] = None, rowstat_in: Optional[torch.Tensor] = None,
           colsum: Optional[torch.Tensor] = None, ln_c: int = 0, ln_eps: float = 1e-5,
-          out2: Optional[torch.Tensor] = None, col2: int = 0) -> torch.Tensor:
+          out2: Optional[torch.Tensor] = None, col2: int = 0, acc_scale_b: Optional[torch.Tensor] = None) -> torch.Tensor:
     """srcs: [(NHWC fp16 tensor, ntap)], w: packed fp16 [rows, K]; out: NHWC fp16 [nb,ho,wo,ldc>=n].  pad0: 3x3 taps read input
-    (stride*out + tap), the zero padding only after the last row / column (AutoencoderKL's Downsample2D)."""
+    (stride*out + tap), the zero padding only after the last row / column (AutoencoderKL's Downsample2D).  acc_scale_b: fp32
+    [nb] on the device, a factor of each batch item's contraction term (acc + bias)."""
     d = _igemm_desc(srcs, w, out, stride=stride, colbias=colbias, res=res, acc_scale=acc_scale, res_scale=res_scale, relu=relu,
                     geglu=geglu, silu=silu, bn=bn, splits=splits, n_valid=n_valid, timeline=timeline, swap=swap, tconv=tconv, pair=pair,
                     pad0=pad0,
-                    rowstat_out=rowstat_out, rowstat_in=rowstat_in, colsum=colsum, ln_c=ln_c, ln_eps=ln_eps, out2=out2, col2=col2)
+                    rowstat_out=rowstat_out, rowstat_in=rowstat_in, colsum=colsum, ln_c=ln_c, ln_eps=ln_eps, out2=out2, col2=col2,
+                    acc_scale_b=acc_scale_b)
     capi.check(capi.lib().b2sd_op_igemm(C.byref(d), capi.current_stream_ptr()), "b2sd_op_igemm")
     return out
 
@@ -65,7 +67,7 @@ def igemm_engine_plan(srcs, w, out, *, autotile: int = 1, allow_swap: bool = Tru
 
 def _igemm_desc(srcs, w, out, *, stride=1, colbias=None, res=None, acc_scale=1.0, res_scale=1.0, relu=False, geglu=False,
                 silu=False, bn=0, splits=1, n_valid=None, timeline=None, swap=False, tconv=False, pair=False, pad0=False, rowstat_out=None,
-                rowstat_in=None, colsum=None, ln_c=0, ln_eps=1e-5, out2=None, col2=0) -> capi.IgemmDesc:
+                rowstat_in=None, colsum=None, ln_c=0, ln_eps=1e-5, out2=None, col2=0, acc_scale_b=None) -> capi.IgemmDesc:
     d = capi.IgemmDesc()
     d.nseg = len(srcs)
     for i, (t, ntap) in enumerate(srcs):
@@ -91,6 +93,9 @@ def _igemm_desc(srcs, w, out, *, stride=1, colbias=None, res=None, acc_scale=1.0
         assert res.dtype == torch.float16
         d.res, d.ldr = res.data_ptr(), _pitch(res)
     d.acc_scale, d.res_scale = acc_scale, res_scale
+    if acc_scale_b is not None:
+        assert acc_scale_b.dtype == torch.float32 and acc_scale_b.is_cuda and acc_scale_b.numel() >= nb
+        d.acc_scale_b = acc_scale_b.data_ptr()
     d.flags = (capi.IG_RELU if relu else 0) | (capi.IG_GEGLU if geglu else 0) | (capi.IG_TCONV if tconv else 0) | (capi.IG_PAIR if pair else 0) \
         | (capi.IG_SILU if silu else 0) | (capi.IG_PAD0 if pad0 else 0)
     if rowstat_out is not None:

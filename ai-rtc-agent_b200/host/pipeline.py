@@ -21,6 +21,7 @@ from typing import Dict, List, Optional, Tuple
 import numpy as np
 import torch
 
+from .stream import check_control
 from .wrapper import LIVE_LORA_ENV, StreamDiffusionWrapper
 
 DEFAULT_PROMPT = "fireworks in the night sky"
@@ -33,6 +34,7 @@ DEFAULT_LANES_STATEFUL = 2    # T > 1: lanes stage-pipeline each stream state th
                               # 2 lanes 47.0 / 54.3 fps at 1 / 2+ peers, p50 42.5 / 36.8 ms; 3 lanes 47.1 / 56.1 fps at 1 / 4+
                               # peers but p50 63.7 / 53.4 ms and 3 GB more; 4 lanes no faster)
 PER_PEER_STREAMS_ENV = "B200SD_PER_PEER_STREAMS"
+CONTROLNET_ENV = "B200SD_CONTROLNET"
 MAX_STYLES_ENV = "B200SD_MAX_STYLES"
 DEFAULT_MAX_STYLES = 4        # viewers' own styles held at once (PeerStream.update_lora); each holds a UNet copy and its lanes
 STYLE_LANES = DEFAULT_LANES_STATEFUL   # lanes of each such style
@@ -106,7 +108,8 @@ class StreamDiffusionPipeline:
 
     def __init__(self, model_id: str, t_index_list: Optional[List[int]] = None, width: int = 512, height: int = 512,
                  prompt: str = DEFAULT_PROMPT, lanes: Optional[int] = None, per_peer_streams: Optional[bool] = None,
-                 live_lora: Optional[bool] = None, ip_adapter: Optional[str] = None):
+                 live_lora: Optional[bool] = None, ip_adapter: Optional[str] = None, controlnet: Optional[str] = None,
+                 controlnet_processor: Optional[str] = "hed"):
         """lanes: frames in flight for enqueue() ($B200SD_LANES overrides the default).  With a 1-step stream batch (SD-Turbo)
         consecutive frames are independent: DEFAULT_LANES_ONE_STEP lanes process frame n+1.. while frame n is still on the GPU.
         With T > 1 the stream batch carries state from frame to frame: the pipeline's stream is then a stream state that two lanes
@@ -124,7 +127,12 @@ class StreamDiffusionPipeline:
 
         ip_adapter (None: $B200SD_IP_ADAPTER, default none): an IP-Adapter file (h94 ip-adapter_sd15.safetensors layout) or a
         directory holding one and its image_encoder/; "synthetic" for seeded weights with a synthetic model.
-        update_image_prompt() then steers the video with an image, globally or per viewer (PeerStream.update_image_prompt)."""
+        update_image_prompt() then steers the video with an image, globally or per viewer (PeerStream.update_image_prompt).
+
+        controlnet (None: $B200SD_CONTROLNET, default none): a diffusers ControlNetModel (id or path; "synthetic" with a
+        synthetic model), conditioned on each frame's HED edge map (controlnet_processor="hed") or on the frame itself
+        (controlnet_processor=None).  update_controlnet_scale() then sets its strength and guidance window, globally or per
+        viewer (PeerStream.update_controlnet_scale)."""
         if per_peer_streams is None:
             per_peer_streams = env_flag(PER_PEER_STREAMS_ENV)
         self.per_peer_streams = bool(per_peer_streams)
@@ -138,6 +146,8 @@ class StreamDiffusionPipeline:
         self.model = StreamDiffusionWrapper.__new__(StreamDiffusionWrapper)
         self.model.live_lora = bool(live_lora)
         self.model.ip_adapter = ip_adapter
+        if controlnet is None:
+            controlnet = os.getenv(CONTROLNET_ENV) or None
         self.model.__init__(
             model_id_or_path=model_id,
             device=self.device,
@@ -153,6 +163,8 @@ class StreamDiffusionPipeline:
             use_tiny_vae=True,
             cfg_type="self",
             engine_dir=os.getenv("TRT_ENGINES_CACHE", "./models/engines"),
+            controlnet_id_or_path=controlnet,
+            controlnet_processor_id=controlnet_processor,
         )
         stateful = len(self.t_index_list) > 1     # x_t_latent_buffer chains frame n+1 to frame n
         if lanes is None:
@@ -239,6 +251,20 @@ class StreamDiffusionPipeline:
         finally:
             self._release(cur)
 
+    def update_controlnet_scale(self, scale: float, control_guidance_start: float = 0.0, control_guidance_end: float = 1.0):
+        """The global ControlNet settings (diffusers' controlnet_conditioning_scale, control_guidance_start / _end): every
+        stream's, including open peer streams with settings of their own (PeerStream.update_controlnet_scale); each keeps its
+        own t_index_list, which masks its slots.  Checked before anything changes; frames enqueued before the call use the old
+        settings and frames enqueued after it the new ones."""
+        if not self.model.stream.has_controlnet:
+            raise RuntimeError("update_controlnet_scale needs a pipeline with a ControlNet (controlnet=... or $B200SD_CONTROLNET)")
+        check_control(scale, control_guidance_start, control_guidance_end)
+        cur = self._quiesce()
+        try:
+            self.model.update_controlnet_scale(scale, control_guidance_start, control_guidance_end)
+        finally:
+            self._release(cur)
+
     # ---- viewers' own styles (PeerStream.update_lora) ------------------------------------------------------------------
     def _leave_style(self, peer) -> None:
         if peer._style is not None:
@@ -275,15 +301,17 @@ class StreamDiffusionPipeline:
             self._styles[target.key] = self._styles.pop(target.key)   # most recently used
         # the viewer's own conditioning is computed again with the new weights, on the lane that takes its next frame
         pool = target or self
-        image = getattr(state, "own_image", None)
-        if state.own_prompt is not None or state.own_t_index_list is not None or image is not None:
+        image, control = getattr(state, "own_image", None), getattr(state, "own_control", None)
+        if state.own_prompt is not None or state.own_t_index_list is not None or image is not None or control is not None:
             prompt, t_index_list = state.own_prompt, state.own_t_index_list
 
             def rebind(engine):
                 if prompt is not None:
                     state.set_prompt(prompt, engine=engine)
                 if t_index_list is not None:
-                    state.set_t_index_list(t_index_list, engine=engine)
+                    state.set_t_index_list(t_index_list, engine=engine)   # with the viewer's ControlNet settings
+                elif control is not None:
+                    state.set_control_scale(*control, engine=engine)
                 if image is not None:
                     state.set_image_tokens(*image, engine=engine)
             self._update_state(rebind, pool)
@@ -577,6 +605,23 @@ class PeerStream:
         timesteps change) and update_prompt's ordering."""
         state = self._live_state()
         self._pipeline._update_state(lambda engine: state.set_t_index_list(t_index_list, engine=engine), self._style)
+
+    @property
+    def controlnet_scale(self) -> Tuple[float, float, float]:
+        """This viewer's ControlNet (scale, start, end): its own (update_controlnet_scale) or the pipeline's global ones"""
+        own = self._live_state().own_control
+        return own if own is not None else self._pipeline.model.stream.control
+
+    def update_controlnet_scale(self, scale: float, control_guidance_start: float = 0.0,
+                                control_guidance_end: float = 1.0) -> None:
+        """This viewer's own ControlNet settings (the pipeline's update_controlnet_scale), masked with its own t_index_list if
+        it has one; update_prompt's ordering.  It keeps them through a global prompt / t_index_list / image prompt / LoRA
+        update and a style move; a later global pipeline.update_controlnet_scale replaces them."""
+        state = self._live_state()
+        if not self._pipeline.model.stream.has_controlnet:
+            raise RuntimeError("update_controlnet_scale needs a pipeline with a ControlNet (controlnet=... or $B200SD_CONTROLNET)")
+        control = check_control(scale, control_guidance_start, control_guidance_end)
+        self._pipeline._update_state(lambda engine: state.set_control_scale(*control, engine=engine), self._style)
 
     @property
     def lora(self) -> Dict[str, float]:

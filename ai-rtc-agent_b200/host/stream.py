@@ -48,6 +48,32 @@ def lcm_boundary_scalings(timestep: int):
     return LCM_SIGMA_DATA * LCM_SIGMA_DATA / denom, scaled / denom ** 0.5
 
 
+# ---- ControlNet conditioning scale and guidance window ----------------------------------------------------
+DEFAULT_CONTROL = (1.0, 0.0, 1.0)   # (controlnet_conditioning_scale, control_guidance_start, control_guidance_end)
+
+
+def check_control(scale: float, start: float = 0.0, end: float = 1.0) -> Tuple[float, float, float]:
+    """(scale, start, end) as floats, with diffusers' checks (StableDiffusionControlNetPipeline.check_inputs): a finite
+    scale (negative allowed), 0 <= start < end <= 1."""
+    scale, start, end = float(scale), float(start), float(end)
+    if not math.isfinite(scale):
+        raise ValueError(f"controlnet_conditioning_scale must be finite (got {scale})")
+    if start >= end:
+        raise ValueError(f"control guidance start: {start} cannot be larger or equal to control guidance end: {end}")
+    if start < 0.0:
+        raise ValueError(f"control guidance start: {start} can't be smaller than 0")
+    if end > 1.0:
+        raise ValueError(f"control guidance end: {end} can't be larger than 1.0")
+    return scale, start, end
+
+
+def control_scales(control: Tuple[float, float, float], t_index_list: List[int], n_steps: int) -> List[float]:
+    """The per-slot ControlNet scale of a stream batch: slot k stands for step t_index_list[k] of the n_steps-step timestep
+    table, and is kept as diffusers' pipeline keeps step i of an n_steps-step run (controlnet_keep), times the scale."""
+    scale, start, end = control
+    return [scale * (0.0 if (i / n_steps < start or (i + 1) / n_steps > end) else 1.0) for i in t_index_list]
+
+
 class ImageProcessor:
     """The part of diffusers' VaeImageProcessor the reference reaches (lib/wrapper.py:364)."""
 
@@ -74,6 +100,8 @@ class StreamDiffusion:
     styles = ()          # instances made by __init__ get a list (add_style)
     _is_style = False
     image_prompt = None  # the global image prompt: (host tokens [n_tok][D], scale) (set_image_tokens)
+    control = DEFAULT_CONTROL   # the global ControlNet (scale, start, end) (set_control_scale)
+    has_controlnet = False      # built with a ControlNet (inherited by lanes and styles)
 
     def __init__(self, arch: UNetArch, unet_sd: Dict[str, torch.Tensor], vae_sd: Dict[str, torch.Tensor],
                  t_index_list: List[int], prompt_encoder: Callable[[str], torch.Tensor],
@@ -143,6 +171,7 @@ class StreamDiffusion:
         cfg.do_add_noise = int(do_add_noise)
         cfg.use_cuda_graph = int(use_cuda_graph)
         cfg.controlnet = int(controlnet_sd is not None)
+        self.has_controlnet = controlnet_sd is not None or (parent or style_of or self).has_controlnet
         cfg.control_processor = capi.CONTROL_HED if hed_sd is not None else capi.CONTROL_FRAME
         cfg.vae = capi.VAE_TINY if use_tiny_vae else capi.VAE_KL
         cfg.vae_scaling_factor = 0.0 if use_tiny_vae else float(vae_scaling_factor)
@@ -285,12 +314,20 @@ class StreamDiffusion:
         noise = self.init_noise.cpu().contiguous()
         capi.check(self._lib.b2sd_prepare(self._handle, emb.data_ptr(), tsteps.data_ptr(), coef.data_ptr(),
                                           noise.data_ptr(), self._stream()), "b2sd_prepare")
+        self._push_control()
         self._prepared = True
+
+    def _push_control(self) -> None:
+        """This engine's global per-slot ControlNet scales from self.control and self.t_list (b2sd_set_control_scale)"""
+        if self.has_controlnet:
+            v = torch.tensor(control_scales(self.control, self.t_list, len(self.timesteps)), dtype=torch.float32)
+            capi.check(self._lib.b2sd_set_control_scale(self._handle, v.data_ptr(), self._stream()), "b2sd_set_control_scale")
 
     def _prepare_like(self, other: "StreamDiffusion") -> None:
         for name in self._SCHEDULE_ATTRS:
             setattr(self, name, getattr(other, name))
         self.t_list = list(other.t_list)
+        self.control = other.control
         self._engine_prepare()
         if other.image_prompt is not None:   # a new lane or style starts with the family's global image prompt
             tokens, scale = other.image_prompt
@@ -414,7 +451,25 @@ class StreamDiffusion:
         for eng in self._family():
             eng.t_list, eng.sub_timesteps, eng.sub_timesteps_tensor = self.t_list, self.sub_timesteps, self.sub_timesteps_tensor
             capi.check(self._lib.b2sd_set_timesteps(eng._handle, t.data_ptr(), self._stream()), "b2sd_set_timesteps")
+            eng._push_control()   # the slots are masked with the new list
         self.clear_overrides(prompt=False, t_index_list=True)
+
+    @torch.no_grad()
+    def set_control_scale(self, scale: float, start: float = 0.0, end: float = 1.0) -> None:
+        """The global ControlNet settings (diffusers' controlnet_conditioning_scale, control_guidance_start / _end): this
+        engine's, its lanes' and its styles' (b2sd_set_control_scale), and every live state's (a state's own settings are
+        dropped, its own t_index_list kept).  Slot k of the stream batch is conditioned with scale times diffusers'
+        controlnet_keep of step t_index_list[k] of the len(self.timesteps)-step table (control_scales).  The settings are
+        checked before anything changes; on the current CUDA stream, after the frames queued there."""
+        if not self.has_controlnet:
+            raise RuntimeError("this engine was built without a ControlNet")
+        control = check_control(scale, start, end)
+        for eng in self._family():
+            eng.control = control
+            eng._push_control()
+        for state in list(self._states):
+            if not state.closed:
+                state.clear_overrides(prompt=False, t_index_list=False, control=True)
 
     def clear_overrides(self, prompt: bool = True, t_index_list: bool = True, image_prompt: Optional[bool] = None) -> None:
         """Every live state of this engine's weights follows the global prompt, t_index_list and / or image prompt again
@@ -464,6 +519,8 @@ class StreamDiffusion:
                 state.set_image_tokens(*state.own_image, engine=self)
             if state.own_t_index_list is not None:
                 state.set_t_index_list(state.own_t_index_list, engine=self)
+            elif state.own_control is not None:
+                state.set_control_scale(*state.own_control, engine=self)
 
     def conditioning_binds(self) -> int:
         """How many conditioning block copies this engine's steps have issued (b2sd_conditioning_binds).  Test aid."""
@@ -685,11 +742,14 @@ class StreamState:
 
     A state may also have its own prompt and its own t_index_list (set_prompt / set_t_index_list): a device copy of the
     conditioning blocks the engines compute from them (cross-attention K / V^T, resnet time biases), which a lane copies in
-    before it steps the state.  Without them the state follows the engines' global prompt and t_index_list."""
+    before it steps the state.  Without them the state follows the engines' global prompt and t_index_list.  Likewise its own
+    ControlNet settings (set_control_scale), which live in the time block beside the time biases: the per-slot scales follow
+    the t_index_list the state is stepped with, its own or the global one."""
 
     own_prompt: Optional[str] = None               # None: the global prompt
     own_t_index_list: Optional[List[int]] = None   # None: the global t_index_list
     own_image: Optional[Tuple[torch.Tensor, float]] = None   # (device tokens [n_tok][D], scale); None: the global image prompt
+    own_control: Optional[Tuple[float, float, float]] = None  # ControlNet (scale, start, end); None: the global settings
     home: Optional[StreamDiffusion] = None   # where clear_overrides recomputes what it keeps (None: the creating engine)
 
     def __init__(self, engine: StreamDiffusion):
@@ -721,6 +781,30 @@ class StreamState:
         capi.check(self._lib.b2sd_state_set_timesteps(eng._handle, self.handle, t.data_ptr(), eng._stream()),
                    "b2sd_state_set_timesteps")
         self.own_t_index_list = t_index_list
+        if eng.has_controlnet:   # the slots are masked with the state's own list
+            self._push_control(eng)
+
+    @torch.no_grad()
+    def set_control_scale(self, scale: float, start: float = 0.0, end: float = 1.0,
+                          engine: Optional[StreamDiffusion] = None) -> None:
+        """This stream's own ControlNet settings (StreamDiffusion.set_control_scale's meaning), masked with the state's own
+        t_index_list if it has one, else the global one.  The state's own t_index_list is kept.  Checked before anything
+        changes; same stream and synchronisation rules as set_prompt."""
+        eng = engine or self._engine
+        if not eng.has_controlnet:
+            raise RuntimeError("this engine was built without a ControlNet")
+        control = check_control(scale, start, end)
+        self._push_control(eng, control)
+        self.own_control = control
+
+    def _push_control(self, eng: StreamDiffusion, control: Optional[Tuple[float, float, float]] = None) -> None:
+        """The state's per-slot ControlNet scales (b2sd_state_set_control_scale) from `control` (default its own settings, else
+        the global ones) and the t_index_list it is stepped with"""
+        control = control or self.own_control or eng.control
+        t_index_list = self.own_t_index_list if self.own_t_index_list is not None else eng.t_list
+        v = _on_device(torch.tensor(control_scales(control, t_index_list, len(eng.timesteps)), dtype=torch.float32), eng.device)
+        capi.check(self._lib.b2sd_state_set_control_scale(eng._handle, self.handle, v.data_ptr(), eng._stream()),
+                   "b2sd_state_set_control_scale")
 
     @torch.no_grad()
     def set_image_tokens(self, tokens: Optional[torch.Tensor], scale: float = 1.0,
@@ -737,26 +821,33 @@ class StreamState:
         self.own_image = (tokens, float(scale))
 
     def clear_overrides(self, prompt: bool = True, t_index_list: bool = True, image_prompt: Optional[bool] = None,
-                        engine: Optional[StreamDiffusion] = None) -> None:
-        """Follow the global prompt, t_index_list and / or image prompt (default: with the prompt) again from the next step on.
-        The prompt and the image prompt share one conditioning block: dropping one of them recomputes the block with the other
-        on `engine` (default self.home); otherwise there is no device work."""
+                        engine: Optional[StreamDiffusion] = None, control: bool = False) -> None:
+        """Follow the global prompt, t_index_list, image prompt (default: with the prompt) and / or ControlNet settings again
+        from the next step on.  The prompt and the image prompt share one conditioning block, and so do the t_index_list and
+        the ControlNet settings: dropping one of a pair recomputes the block with the other on `engine` (default self.home);
+        otherwise there is no device work."""
         engine = engine or self.home
         if image_prompt is None:
             image_prompt = prompt
         keep_prompt = None if prompt else self.own_prompt
         keep_image = None if image_prompt else self.own_image
-        for on, which in ((prompt or image_prompt, capi.COND_PROMPT), (t_index_list, capi.COND_TIME)):
-            if on:
-                capi.check(self._lib.b2sd_state_clear_conditioning(self.handle, which), "b2sd_state_clear_conditioning")
+        if prompt or image_prompt:
+            capi.check(self._lib.b2sd_state_clear_conditioning(self.handle, capi.COND_PROMPT), "b2sd_state_clear_conditioning")
         if prompt or image_prompt:
             self.own_prompt = self.own_image = None
             if keep_prompt is not None:
                 self.set_prompt(keep_prompt, engine=engine)
             if keep_image is not None:
                 self.set_image_tokens(*keep_image, engine=engine)
-        if t_index_list:
-            self.own_t_index_list = None
+        if t_index_list or control:
+            keep_t = None if t_index_list else self.own_t_index_list
+            keep_control = None if control else self.own_control
+            capi.check(self._lib.b2sd_state_clear_conditioning(self.handle, capi.COND_TIME), "b2sd_state_clear_conditioning")
+            self.own_t_index_list, self.own_control = None, keep_control
+            if keep_t is not None:
+                self.set_t_index_list(keep_t, engine=engine)   # with the settings kept
+            elif keep_control is not None:
+                self.set_control_scale(*keep_control, engine=engine)
 
     @property
     def handle(self) -> C.c_void_p:

@@ -299,6 +299,14 @@ class StreamDiffusionWrapper:
         with self._on_stream():
             self.stream.apply_lora(lora_dict)
 
+    def update_controlnet_scale(self, scale: float, control_guidance_start: float = 0.0,
+                                control_guidance_end: float = 1.0) -> None:
+        """The ControlNet's strength and guidance window, as diffusers' StableDiffusionControlNetPipeline takes them
+        (controlnet_conditioning_scale, control_guidance_start / _end): frames computed after the call use them.  Slot k of
+        the stream batch stands for step t_index_list[k] of the timestep table.  See StreamDiffusion.set_control_scale."""
+        with self._on_stream():
+            self.stream.set_control_scale(scale, control_guidance_start, control_guidance_end)
+
     def update_t_index_list(self, t_index_list: List[int]) -> None:
         """lib/wrapper.py:389-407: swaps the sub-timesteps only."""
         if t_index_list == self.stream.t_list:

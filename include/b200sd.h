@@ -51,7 +51,7 @@ enum {
 };
 
 /* conv3x3 / conv1x1 / Linear as one implicit GEMM:
- *   out[row][j] = acc_scale * (sum_seg sum_tap sum_c src[seg](row, tap, c) * w[j][k] + colbias[b][j])
+ *   out[row][j] = acc_scale_b[b] * acc_scale * (sum_seg sum_tap sum_c src[seg](row, tap, c) * w[j][k] + colbias[b][j])
  *                 + res_scale * res[row][j]        (then ReLU / SiLU / GEGLU per flags)
  * K order of the packed weight rows = segments in sequence, each [tap][c]. */
 typedef struct {
@@ -89,6 +89,11 @@ typedef struct {
     float ln_eps;
     void* out2;
     int ld2, col2;
+    /* acc_scale_b  optional fp32 [nb] in device memory, read when the kernel runs: a factor of batch item b's contraction term
+     *              (NULL = 1).  Normal orientation (swap = 0), bn 16 / 32 / 64 / 128 / 160 / 256 (CTA pairs from 32), split-K
+     *              (applied once, after the reduction); not with GEGLU, SiLU, tap origin 0, the LayerNorm fold or
+     *              B2SD_IG_TCONV (the halo-tile kernel refuses it). */
+    const float* acc_scale_b;
 } b2sd_igemm_desc;
 
 int b2sd_op_igemm(const b2sd_igemm_desc* d, void* stream);
@@ -507,6 +512,21 @@ int b2sd_state_set_timesteps(b2sd_handle h, b2sd_state_handle state, const float
 int b2sd_set_image_embeds(b2sd_handle h, const void* tokens_f16, int n_tok, float scale, void* stream);
 int b2sd_state_set_image_embeds(b2sd_handle h, b2sd_state_handle state, const void* tokens_f16, int n_tok, float scale,
                                 void* stream);
+/* ControlNet conditioning scale (an engine with controlnet = 1), per stream-batch slot: each slot's ControlNet residuals
+ * (every zero conv's output, bias included) are multiplied by its scale before they are added to the UNet's skips, as diffusers'
+ * controlnet_conditioning_scale does; a guidance window (control_guidance_start / _end) is a scale of 0 on the slots outside
+ * it.  The scales live in the time block beside the time biases, so a change is one small device write: no graph recapture, no
+ * parameter changes.  b2sd_set_control_scale sets the engine's global scales from host memory, fp32 [batch], finite (1 after
+ * b2sd_create), stream-ordered on `stream` without a host synchronisation; it keeps the global time biases, and
+ * b2sd_set_timesteps keeps the global scales.  b2sd_state_set_control_scale computes the state's time block with scales in
+ * DEVICE memory (which the caller checks: they are not read on the host), as b2sd_state_set_timesteps does: it keeps the state's
+ * own timesteps if it has some computed on h's weight store, and b2sd_state_set_timesteps keeps the state's own scales likewise.
+ * Scales or timesteps of a state without the other part of its own take that part from the engine's global block at the
+ * call, so a global refresh is followed by setting them again; after a move to another store of the family set the state's
+ * timesteps, then its scales, again.  Clearing the state's time block (b2sd_state_clear_conditioning(state, 1)) drops both.
+ * Both calls refuse an engine without a ControlNet. */
+int b2sd_set_control_scale(b2sd_handle h, const float* scale_per_slot, void* stream);
+int b2sd_state_set_control_scale(b2sd_handle h, b2sd_state_handle state, const float* scale_per_slot, void* stream);
 /* Drop the state's override of the prompt (which = 0) or time (which = 1) block: later steps use the engines' global values.
  * No device work; the override is freed after the steps already submitted with it. */
 int b2sd_state_clear_conditioning(b2sd_state_handle state, int which);

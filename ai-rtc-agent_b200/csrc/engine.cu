@@ -432,11 +432,12 @@ struct b2sd_engine {
     float* temb_sin = nullptr; // [B][C0]
     float* temb_h = nullptr;   // [B][4*C0]
     float* temb = nullptr;     // [B][4*C0]
-    float* cn_temb_h = nullptr;   // ControlNet time_embedding (its own weights), [B][4*C0]
-    float* cn_temb = nullptr;
-    // per-slot ControlNet conditioning scale [B] that the zero convs read (in the time block), and the engine's global values
+    float* cn_temb_h[B2SD_MAX_CONTROLNETS] = {};   // each ControlNet's time_embedding (its own weights), [B][4*C0]
+    float* cn_temb[B2SD_MAX_CONTROLNETS] = {};
+    // per-slot ControlNet conditioning scales [nets][B] that the zero convs read (net i row i, in the time block), and the
+    // engine's global values (1 after b2sd_create)
     float* cn_scale = nullptr;
-    float cn_scale_global[16] = {1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f};
+    float cn_scale_global[B2SD_MAX_CONTROLNETS][16];
     float* gn_ws = nullptr;    // GroupNorm chunk partials (shared: launches are stream-ordered)
     int* tile_counters = nullptr;
     float coef_host[4][64]{};
@@ -479,8 +480,10 @@ struct b2sd_engine {
     std::vector<Op> prog_frame, prog_prompt, prog_time, prog_image;
     std::map<std::string, Act> taps;
     SmallConvArgs head{};   // encoder head (reads the caller's frame)
-    SmallConvArgs cn_head{};   // ControlNet conditioning embedding conv_in (reads the caller's frame as the control image)
-    SmallConvArgs hed_head{};  // HED's first conv (reads the caller's frame) when the control image is its edge map
+    // each ControlNet's conditioning embedding conv_in (reads the caller's frame as the control image, with processor FRAME)
+    SmallConvArgs cn_head[B2SD_MAX_CONTROLNETS]{};
+    SmallConvArgs hed_head{};  // HED's first conv (reads the caller's frame) when a control image is its edge map
+    int control_processor(int net) const { return net == 0 ? cfg.control_processor : cfg.control_processor_more[net - 1]; }
     Act image;              // decoder output, fp16 NHWC (ld 8)
     bool built = false;
     int concurrency = 1;   // frames expected in flight on this GPU (b2sd_set_concurrency): > 1 selects the throughput launch policy
@@ -892,9 +895,9 @@ struct b2sd_engine {
     std::vector<float> host_copy(const std::string& key);
     int derive(const std::string& name, const std::vector<int64_t>& shape, const std::vector<float>& v);
     const float* const_vec(const std::string& name, const std::vector<float>& v);
-    int build_cond_embedding(Act* out, cudaStream_t s);
+    int build_cond_embedding(int net, const uint8_t** hed_control, Act* out, cudaStream_t s);
     int build_hed(const uint8_t** control, cudaStream_t s);
-    int build_controlnet(const Act& cond, std::vector<Act>& skips, Act* mid, cudaStream_t s);
+    int build_controlnet(int net, const Act& cond, std::vector<Act>& skips, Act* mid, cudaStream_t s);
     int build_transformer(const std::string& p, const Act& x, int heads, Act* out, cudaStream_t s);
     int build_taesd_block(const std::string& p, const Act& x, Act* out, cudaStream_t s);
     int build_program(cudaStream_t s);
@@ -1136,7 +1139,7 @@ int b2sd_engine::build_transformer(const std::string& p, const Act& x, int heads
     // ---- IP-Adapter: the image tokens' K [64][Cp] and scale * V^T [Cp][64] (UNet only: the ControlNet's stay text-only, as in
     // diffusers).  Rows / columns past the prompt's tokens come from its zeroed token rows, so they are finite.
     __half *kip = nullptr, *vipt = nullptr;
-    if (cfg.ip_tokens && p.compare(0, 11, "controlnet.") != 0) {
+    if (cfg.ip_tokens && p.compare(0, 10, "controlnet") != 0) {   // not under any net's "controlnet." / "controlnet<i>."
         __half* wk = pack_rows(t + "attn2.k_ip", {{t + "attn2.to_k_ip.weight", head_perm(0)}}, D, s);
         __half* wv = pack_rows(t + "attn2.v_ip", {{t + "attn2.to_v_ip.weight", head_perm(0)}}, D, s);
         kip = static_cast<__half*>(cond[COND_PROMPT].take((size_t)ATTN_IP_KEYS * Cp * 2));
@@ -1237,14 +1240,20 @@ int b2sd_engine::build_taesd_block(const std::string& p, const Act& x, Act* out,
     return add_conv(prog_frame, b, p + ".conv.4.weight", p + ".conv.4.bias", 9, 1, *out, IG_RELU, &x, s);
 }
 
+// The weight prefix of ControlNet `net`: "controlnet." for net 0, "controlnet<i>." for net i (never "controlnet.<i>.", so that
+// a key under "controlnet." always belongs to net 0)
+static std::string cn_prefix(int net) { return net == 0 ? std::string("controlnet.") : "controlnet" + std::to_string(net) + "."; }
+
 // ControlNetConditioningEmbedding (diffusers controlnet.py): conv_in 3->16 + SiLU, six 3x3 convs 16->16, 16->32/2, 32->32,
 // 32->96/2, 96->96, 96->256/2 each + SiLU, conv_out 256->C0.  conv_in reads the caller's frame (b2sd_step_ex launches cn_head
 // next to the encoder head); the rest is stage 1 of the frame program (it depends on the frame only).  The 16/32/96-channel
 // activations are stored 64/64/128 wide with zero padding columns, so the following layers run as 64/64/128-channel
 // tensor-core contractions (zero weights on the padding channels, pack_conv_weight_launch).  The epilogues write only the
-// valid columns: the padding is cleared once here, and stays finite (0 * NaN would be NaN).
-int b2sd_engine::build_cond_embedding(Act* out, cudaStream_t s) {
-    const std::string p = "controlnet.controlnet_cond_embedding.";
+// valid columns: the padding is cleared once here, and stays finite (0 * NaN would be NaN).  With several nets each has its
+// own; HED runs once, for the first net that reads its edge map (*hed_control, null until then), and later ones share it.
+int b2sd_engine::build_cond_embedding(int net, const uint8_t** hed_control, Act* out, cudaStream_t s) {
+    const std::string p = cn_prefix(net) + "controlnet_cond_embedding.";
+    SmallConvArgs& cn_head = this->cn_head[net];
     cur = p;
     allow_swap = false;
     auto padded = [&](int n, int hh, int ww, int c) {
@@ -1260,11 +1269,10 @@ int b2sd_engine::build_cond_embedding(Act* out, cudaStream_t s) {
     if (!cn_head.wt || !cn_head.bias) return -1;
     cn_head.y = a.p; cn_head.ldy = a.ld; cn_head.nb = 1; cn_head.h = a.h; cn_head.w_ = a.w; cn_head.cin = 3; cn_head.cout = 16;
     ++launches;
-    if (cfg.control_processor == B2SD_CONTROL_HED) {   // the control image is HED's edge map, computed in this stage
-        const uint8_t* control = nullptr;
-        TRY(build_hed(&control, s));
+    if (control_processor(net) == B2SD_CONTROL_HED) {   // the control image is HED's edge map, computed in this stage
+        if (!*hed_control) TRY(build_hed(hed_control, s));
         SmallConvArgs c = cn_head;
-        c.x = control; c.in_h = a.h; c.in_w = a.w; c.flags = SC_IN_U8 | SC_OUT_SILU;
+        c.x = *hed_control; c.in_h = a.h; c.in_w = a.w; c.flags = SC_IN_U8 | SC_OUT_SILU;
         prog_frame.push_back(Op([c](cudaStream_t st) { return smallconv_launch(c, st); }, "smallconv controlnet_cond_embedding.conv_in",
                                 smallconv_record(c)));
     }
@@ -1279,7 +1287,8 @@ int b2sd_engine::build_cond_embedding(Act* out, cudaStream_t s) {
     }
     *out = new_act(1, lh, lw, cfg.block_out_channels[0]);
     TRY(add_conv(prog_frame, a, p + "conv_out.weight", p + "conv_out.bias", 9, 1, *out, 0, nullptr, s));
-    taps["cn_cond"] = *out;
+    taps["cn" + std::to_string(net) + "_cond"] = *out;
+    if (net == 0) taps["cn_cond"] = *out;
     return 0;
 }
 
@@ -1353,11 +1362,15 @@ int b2sd_engine::build_hed(const uint8_t** control, cudaStream_t s) {
 // "controlnet." prefix with its own time embedding, then the zero convs: skips[k] <- skips[k] + controlnet_down_blocks.k(f_k),
 // *mid <- *mid + controlnet_mid_block(f_mid), each one 1x1 contraction with the UNet tensor as its epilogue residual, written
 // to a new buffer.  Each slot's residual is scaled by its conditioning scale (cn_scale, read when the launch runs: diffusers
-// multiplies the zero conv's output, bias included, by controlnet_conditioning_scale).
-int b2sd_engine::build_controlnet(const Act& cond, std::vector<Act>& skips, Act* mid, cudaStream_t s) {
-    const std::string P = "controlnet.";
+// multiplies the zero conv's output, bias included, by controlnet_conditioning_scale).  Net i > 0 reads its own prefix, time
+// embedding and row of scales, and its zero convs take the previous net's outputs as their residuals: the nets' residuals
+// are summed into the skips as ((skip + r_0) + r_1) + ...
+int b2sd_engine::build_controlnet(int net, const Act& cond, std::vector<Act>& skips, Act* mid, cudaStream_t s) {
+    const std::string P = cn_prefix(net);
+    const std::string tap = net == 0 ? "cn" : "cn" + std::to_string(net);
     const int B = cfg.batch, nlev = 4;
     const int* ch = cfg.block_out_channels;
+    float* cn_temb = this->cn_temb[net];
     cur = P + "conv_in";
     allow_swap = true;
     Act h = new_act(B, lh, lw, ch[0]);
@@ -1369,9 +1382,9 @@ int b2sd_engine::build_controlnet(const Act& cond, std::vector<Act>& skips, Act*
         a.x = x_in.p; a.y = h.p; a.ldy = h.ld; a.nb = B; a.h = lh; a.w_ = lw; a.cin = 4; a.cout = ch[0]; a.in_h = lh; a.in_w = lw;
         a.res = cond.p; a.ldr = cond.ld; a.res_bstride = 0;
         ++launches;
-        prog_frame.push_back(Op([a](cudaStream_t st) { return smallconv_launch(a, st); }, "smallconv controlnet.conv_in", smallconv_record(a)));
+        prog_frame.push_back(Op([a](cudaStream_t st) { return smallconv_launch(a, st); }, "smallconv " + P + "conv_in", smallconv_record(a)));
     }
-    taps["cn.conv_in"] = h;
+    taps[tap + ".conv_in"] = h;
     std::vector<Act> feats{h};
     for (int i = 0; i < nlev; ++i) {
         const std::string bp = P + "down_blocks." + std::to_string(i);
@@ -1404,20 +1417,27 @@ int b2sd_engine::build_controlnet(const Act& cond, std::vector<Act>& skips, Act*
         return -1;
     }
     allow_swap = false;
-    cn_scale = static_cast<float*>(this->cond[COND_TIME].take((size_t)B * sizeof(float)));   // (`cond` is the embedding here)
-    if (!cn_scale) return -1;
+    if (net == 0) {   // every net's row of scales, [nets][B]  (`cond` is the embedding here)
+        cn_scale = static_cast<float*>(this->cond[COND_TIME].take((size_t)cfg.controlnet * B * sizeof(float)));
+        if (!cn_scale) return -1;
+    }
+    float* scale = cn_scale + (size_t)net * B;
+    auto tap_both = [&](const std::string& name, const Act& a) {   // net 0 also keeps its single-net names
+        taps[tap + name] = a;
+        if (net == 0) taps["cn0" + name] = a;
+    };
     for (size_t k = 0; k < feats.size(); ++k) {
         const std::string w = P + "controlnet_down_blocks." + std::to_string(k);
         Act o = new_act(skips[k].n, skips[k].h, skips[k].w, skips[k].c);
-        TRY(add_conv(prog_frame, feats[k], w + ".weight", w + ".bias", 1, 1, o, 0, &skips[k], s, 1.f, 1.f, cn_scale));
+        TRY(add_conv(prog_frame, feats[k], w + ".weight", w + ".bias", 1, 1, o, 0, &skips[k], s, 1.f, 1.f, scale));
         skips[k] = o;
-        taps["cn.res." + std::to_string(k)] = o;
+        tap_both(".res." + std::to_string(k), o);
     }
     Act o = new_act(mid->n, mid->h, mid->w, mid->c);
     TRY(add_conv(prog_frame, h, P + "controlnet_mid_block.weight", P + "controlnet_mid_block.bias", 1, 1, o, 0, mid, s, 1.f, 1.f,
-                 cn_scale));
+                 scale));
     *mid = o;
-    taps["cn.mid"] = o;
+    tap_both(".mid", o);
     allow_swap = true;
     return 0;
 }
@@ -1732,7 +1752,7 @@ int b2sd_engine::build_program(cudaStream_t s) {
         for (int i = 0; i < nlev; ++i) {
             const long tokens_i = (long)B * (lh >> i) * (lw >> i);
             int blocks_i = (cfg.down_attn[i] ? cfg.layers_per_block + (cfg.layers_per_block + 1) : 0) + (i == nlev - 1 ? 1 : 0);
-            if (cfg.controlnet) blocks_i += (cfg.down_attn[i] ? cfg.layers_per_block : 0) + (i == nlev - 1 ? 1 : 0);
+            blocks_i += cfg.controlnet * ((cfg.down_attn[i] ? cfg.layers_per_block : 0) + (i == nlev - 1 ? 1 : 0));
             words += 3 * 2 * tokens_i * blocks_i;
         }
         ln_stats_cap = (size_t)words;
@@ -1743,7 +1763,7 @@ int b2sd_engine::build_program(cudaStream_t s) {
     {
         // the conditioning blocks, sized from the shapes build_transformer (K [L][Cp], V^T [Cp][Lpad] per block) and build_resnet
         // (time bias [B][cout] per resnet) take from them, and zeroed once (V^T's pad columns are never written)
-        const int L = cfg.ctx_tokens, Lpad = 128 * ((L + 127) / 128), lpb = cfg.layers_per_block, cn = cfg.controlnet ? 1 : 0;
+        const int L = cfg.ctx_tokens, Lpad = 128 * ((L + 127) / 128), lpb = cfg.layers_per_block, cn = cfg.controlnet;
         auto r = [](size_t b) { return (b + 1023) & ~size_t(1023); };
         size_t bytes[2] = {0, 0};
         for (int i = 0; i < nlev; ++i) {
@@ -1762,7 +1782,7 @@ int b2sd_engine::build_program(cudaStream_t s) {
                                       2 * r((size_t)ATTN_IP_KEYS * Cp * 2);
             bytes[COND_TIME] += resnets * r((size_t)B * ch[i] * sizeof(float));
         }
-        if (cfg.controlnet) bytes[COND_TIME] += r((size_t)B * sizeof(float));   // the per-slot ControlNet scale
+        if (cfg.controlnet) bytes[COND_TIME] += r((size_t)cfg.controlnet * B * sizeof(float));   // the per-slot ControlNet scales
         if (cfg.ip_tokens) bytes[COND_PROMPT] += r(sizeof(int));   // ip_count
         for (int k = 0; k < 2; ++k) {
             CondBlock& b = cond[k];
@@ -1815,8 +1835,10 @@ int b2sd_engine::build_program(cudaStream_t s) {
     }
     latent_conv = "vae.encoder.layers." + std::to_string(li);
     }
-    Act cond;   // ControlNet conditioning embedding of this frame's control image: batch 1, latent resolution, C0 channels
-    if (cfg.controlnet) TRY(build_cond_embedding(&cond, s));
+    // each ControlNet's conditioning embedding of this frame's control image: batch 1, latent resolution, C0 channels
+    Act cond[B2SD_MAX_CONTROLNETS];
+    const uint8_t* hed_control = nullptr;   // HED's edge map, once a net reads it
+    for (int i = 0; i < cfg.controlnet; ++i) TRY(build_cond_embedding(i, &hed_control, &cond[i], s));
     {
         // latent head + StreamDiffusion.encode_image add-noise: x_t = alpha0 * z + beta0 * init_noise[0]
         // (AutoencoderKL: z = scaling_factor * mean, the scale applied with alpha0 in the epilogue)
@@ -1877,7 +1899,7 @@ int b2sd_engine::build_program(cudaStream_t s) {
     }
     // ControlNet: its down path + mid block over the same x / timesteps / prompt; the zero convs add its 12 + 1 residuals to the
     // skips the up path concatenates and to the mid-block output (the UNet's own down path above used them unmodified)
-    if (cfg.controlnet) TRY(build_controlnet(cond, skips, &h, s));
+    for (int i = 0; i < cfg.controlnet; ++i) TRY(build_controlnet(i, cond[i], skips, &h, s));
     for (int i = 0; i < nlev; ++i) {
         const int co = ch[nlev - 1 - i];
         const int hd = cfg.heads[nlev - 1 - i];
@@ -2039,10 +2061,12 @@ __global__ void write_scales_kernel(float* dst, Scales16 v, int n) {
 }
 static int write_global_scales(b2sd_engine* h, cudaStream_t s) {
     if (!h->cn_scale) return 0;
-    Scales16 v;
-    memcpy(v.v, h->cn_scale_global, sizeof(v.v));
-    write_scales_kernel<<<1, 32, 0, s>>>(h->cn_scale, v, h->cfg.batch);
-    CUDA_OK(cudaGetLastError());
+    for (int i = 0; i < h->cfg.controlnet; ++i) {   // one net's row per launch
+        Scales16 v;
+        memcpy(v.v, h->cn_scale_global[i], sizeof(v.v));
+        write_scales_kernel<<<1, 32, 0, s>>>(h->cn_scale + (size_t)i * h->cfg.batch, v, h->cfg.batch);
+        CUDA_OK(cudaGetLastError());
+    }
     return 0;
 }
 
@@ -2166,6 +2190,7 @@ int b2sd_create_lane(b2sd_handle parent, const b2sd_config* cfg, b2sd_handle* ou
     b2sd_config c = cfg ? *cfg : parent->cfg;
     c.controlnet = parent->cfg.controlnet;   // a lane runs the parent's networks
     c.control_processor = parent->cfg.control_processor;
+    memcpy(c.control_processor_more, parent->cfg.control_processor_more, sizeof(c.control_processor_more));
     c.vae = parent->cfg.vae;
     c.vae_scaling_factor = parent->cfg.vae_scaling_factor;
     c.ip_tokens = parent->cfg.ip_tokens;
@@ -2200,13 +2225,21 @@ static int create_engine(const b2sd_config* cfg, std::shared_ptr<WeightStore> st
         b2_set_error("b2sd_create: cross_attention_dim must be a multiple of 64");
         return -1;
     }
-    if (cfg->controlnet != 0 && cfg->controlnet != 1) {
-        b2_set_error("b2sd_create: controlnet must be 0 or 1 (got %d)", cfg->controlnet);
+    if (cfg->controlnet < 0 || cfg->controlnet > B2SD_MAX_CONTROLNETS) {
+        b2_set_error("b2sd_create: controlnet must be 0..%d (got %d)", B2SD_MAX_CONTROLNETS, cfg->controlnet);
         return -1;
     }
     if (cfg->control_processor != B2SD_CONTROL_FRAME && (cfg->control_processor != B2SD_CONTROL_HED || !cfg->controlnet)) {
         b2_set_error("b2sd_create: control_processor must be 0 (the frame) or 1 (HED, with a ControlNet) (got %d)", cfg->control_processor);
         return -1;
+    }
+    for (int i = 1; i < B2SD_MAX_CONTROLNETS; ++i) {
+        const int p = cfg->control_processor_more[i - 1];
+        if (p != B2SD_CONTROL_FRAME && (p != B2SD_CONTROL_HED || i >= cfg->controlnet)) {
+            b2_set_error("b2sd_create: control_processor_more[%d] must be 0 (the frame) or 1 (HED, with a ControlNet %d) (got %d)",
+                         i - 1, i, p);
+            return -1;
+        }
     }
     if (cfg->vae != B2SD_VAE_TINY && cfg->vae != B2SD_VAE_KL) {
         b2_set_error("b2sd_create: vae must be 0 (TAESD) or 1 (AutoencoderKL) (got %d)", cfg->vae);
@@ -2249,10 +2282,13 @@ static int create_engine(const b2sd_config* cfg, std::shared_ptr<WeightStore> st
     e->temb_sin = static_cast<float*>(e->state.alloc((size_t)B * C0 * sizeof(float)));
     e->temb_h = static_cast<float*>(e->state.alloc((size_t)B * 4 * C0 * sizeof(float)));
     e->temb = static_cast<float*>(e->state.alloc((size_t)B * 4 * C0 * sizeof(float)));
-    if (cfg->controlnet) {
-        e->cn_temb_h = static_cast<float*>(e->state.alloc((size_t)B * 4 * C0 * sizeof(float)));
-        e->cn_temb = static_cast<float*>(e->state.alloc((size_t)B * 4 * C0 * sizeof(float)));
+    bool cn_ok = true;
+    for (int i = 0; i < cfg->controlnet; ++i) {
+        e->cn_temb_h[i] = static_cast<float*>(e->state.alloc((size_t)B * 4 * C0 * sizeof(float)));
+        e->cn_temb[i] = static_cast<float*>(e->state.alloc((size_t)B * 4 * C0 * sizeof(float)));
+        cn_ok = cn_ok && e->cn_temb_h[i] && e->cn_temb[i];
     }
+    for (auto& row : e->cn_scale_global) std::fill(row, row + 16, 1.f);
     e->gn_ws = static_cast<float*>(e->state.alloc(groupnorm_partial_floats(B, cfg->norm_groups) * sizeof(float)));
     e->tile_counters = static_cast<int*>(e->state.alloc(65536 * sizeof(int)));
     if (e->tile_counters) cudaMemset(e->tile_counters, 0, 65536 * sizeof(int));
@@ -2270,7 +2306,7 @@ static int create_engine(const b2sd_config* cfg, std::shared_ptr<WeightStore> st
         }
     }
     if (!e->x_in.p || !e->noise || !e->coef || !e->tsteps || !e->ctx || !e->temb || !e->gn_ws || !e->ctx_global || !e->tsteps_global ||
-        (cfg->controlnet && (!e->cn_temb_h || !e->cn_temb))) {
+        !cn_ok) {
         b2_set_error("b2sd_create: cudaMalloc failed");
         delete e;
         return -1;
@@ -2387,7 +2423,7 @@ static int time_embedding_ops(b2sd_handle h, std::vector<Op>* ops) {
         return 0;
     };
     TRY(embed("", h->temb_h, h->temb));
-    if (h->cfg.controlnet) TRY(embed("controlnet.", h->cn_temb_h, h->cn_temb));
+    for (int i = 0; i < h->cfg.controlnet; ++i) TRY(embed(cn_prefix(i), h->cn_temb_h[i], h->cn_temb[i]));
     return 0;
 }
 
@@ -2399,9 +2435,10 @@ static int refresh_time(b2sd_handle h, cudaStream_t s) {
     return h->run(h->prog_time, s);
 }
 
-// A UNet matrix a LoRA may re-fuse: a loaded (not derived) parameter without a sub-network prefix, 2-D or 4-D
+// A UNet matrix a LoRA may re-fuse: a loaded (not derived) parameter without a sub-network prefix ("controlnet" covers every
+// net's "controlnet." / "controlnet<i>."), 2-D or 4-D
 static bool lora_target(const std::string& key, const Raw& r) {
-    for (const char* pre : {"vae.", "controlnet.", "hed."})
+    for (const char* pre : {"vae.", "controlnet", "hed."})
         if (key.compare(0, strlen(pre), pre) == 0) return false;
     if (key.find("_ip.weight") != std::string::npos) return false;   // IP-Adapter's to_k_ip / to_v_ip: styles share them
     return !r.derived && r.shape.size() >= 2;
@@ -2554,7 +2591,9 @@ int b2sd_export_packed(b2sd_handle h, const char* path) {
     }
     BlobWriter w{f};
     w.put("B2SDPACK", 8);
-    w.pod((uint32_t)4);   // 4: b2sd_config carries `ip_tokens` (3: up to `vae_scaling_factor`, 2: up to `control_processor`; 1-3 still load)
+    // 5: b2sd_config carries `control_processor_more` (4: up to `ip_tokens`, 3: up to `vae_scaling_factor`, 2: up to
+    // `control_processor`; 1-4 still load)
+    w.pod((uint32_t)5);
     b2sd_config cfg = h->cfg;
     cfg.batch = 0; cfg.height = 0; cfg.width = 0; cfg.use_cuda_graph = 0; cfg.do_add_noise = 0;   // the blob is independent of these
     w.pod(cfg);
@@ -2617,21 +2656,25 @@ int b2sd_import_packed(b2sd_handle h, const char* path) {
     rd.get(magic, 8);
     const uint32_t version = rd.pod<uint32_t>();
     // version 1 blobs predate the ControlNet fields at the end of b2sd_config: they hold no ControlNet (both fields 0);
-    // version 2 blobs end b2sd_config before `vae`: they hold TAESD (vae = 0); version 3 blobs before `ip_tokens`: no IP-Adapter
+    // version 2 blobs end b2sd_config before `vae`: they hold TAESD (vae = 0); version 3 blobs before `ip_tokens`: no IP-Adapter;
+    // version 4 blobs before `control_processor_more`: at most one ControlNet
     b2sd_config cfg{};
     if (version == 1) rd.get(&cfg, offsetof(b2sd_config, controlnet));
     else if (version == 2) rd.get(&cfg, offsetof(b2sd_config, vae));
     else if (version == 3) rd.get(&cfg, offsetof(b2sd_config, ip_tokens));
+    else if (version == 4) rd.get(&cfg, offsetof(b2sd_config, control_processor_more));
     else cfg = rd.pod<b2sd_config>();
-    if (rd.ok && version >= 1 && version <= 4 && (cfg.ip_tokens != 0) != (h->cfg.ip_tokens != 0)) {
+    if (rd.ok && version >= 1 && version <= 5 && (cfg.ip_tokens != 0) != (h->cfg.ip_tokens != 0)) {
         fclose(f);
         b2_set_error("b2sd_import_packed: %s was packed %s an IP-Adapter and this engine has %s", path,
                      cfg.ip_tokens ? "with" : "without", h->cfg.ip_tokens ? "one" : "none");
         return -1;
     }
-    bool same = rd.ok && memcmp(magic, "B2SDPACK", 8) == 0 && version >= 1 && version <= 4 && cfg.cross_attention_dim == h->cfg.cross_attention_dim &&
+    bool same = rd.ok && memcmp(magic, "B2SDPACK", 8) == 0 && version >= 1 && version <= 5 && cfg.cross_attention_dim == h->cfg.cross_attention_dim &&
                 cfg.layers_per_block == h->cfg.layers_per_block && cfg.norm_groups == h->cfg.norm_groups && cfg.ctx_tokens == h->cfg.ctx_tokens &&
-                cfg.controlnet == h->cfg.controlnet && cfg.control_processor == h->cfg.control_processor && cfg.vae == h->cfg.vae &&
+                cfg.controlnet == h->cfg.controlnet && cfg.control_processor == h->cfg.control_processor &&
+                memcmp(cfg.control_processor_more, h->cfg.control_processor_more, sizeof(cfg.control_processor_more)) == 0 &&
+                cfg.vae == h->cfg.vae &&
                 (cfg.vae != B2SD_VAE_KL || cfg.vae_scaling_factor == h->cfg.vae_scaling_factor);
     for (int i = 0; i < 4 && same; ++i)
         same = cfg.block_out_channels[i] == h->cfg.block_out_channels[i] && cfg.heads[i] == h->cfg.heads[i] && cfg.down_attn[i] == h->cfg.down_attn[i];
@@ -2718,26 +2761,49 @@ int b2sd_set_timesteps(b2sd_handle h, const float* timesteps, void* stream) {
     return keep_global(h, COND_TIME, s);
 }
 
-int b2sd_set_control_scale(b2sd_handle h, const float* scale_per_slot, void* stream) {
-    if (!h || !h->built || !scale_per_slot) {
-        b2_set_error("b2sd_set_control_scale: null argument, or b2sd_prepare not called");
+// The single-net form of a control-scale call refuses an engine with several nets
+static int refuse_multi(const char* fn, b2sd_handle h) {
+    if (h && h->cfg.controlnet > 1) {
+        b2_set_error("%s: the engine has %d ControlNets; set their scales with %ss", fn, h->cfg.controlnet, fn);
+        return -1;
+    }
+    return 0;
+}
+
+static int set_control_scales(const char* fn, b2sd_handle h, const float* per_net_slot, void* stream) {
+    if (!h || !h->built || !per_net_slot) {
+        b2_set_error("%s: null argument, or b2sd_prepare not called", fn);
         return -1;
     }
     if (!h->cn_scale) {
-        b2_set_error("b2sd_set_control_scale: the engine was created without a ControlNet (b2sd_config.controlnet = 0)");
+        b2_set_error("%s: the engine was created without a ControlNet (b2sd_config.controlnet = 0)", fn);
         return -1;
     }
-    for (int k = 0; k < h->cfg.batch; ++k)
-        if (!isfinite(scale_per_slot[k])) {
-            b2_set_error("b2sd_set_control_scale: the scale of slot %d is not finite (%f)", k, (double)scale_per_slot[k]);
-            return -1;
-        }
+    const int B = h->cfg.batch;
+    for (int i = 0; i < h->cfg.controlnet; ++i)
+        for (int k = 0; k < B; ++k)
+            if (!isfinite(per_net_slot[i * B + k])) {
+                if (h->cfg.controlnet == 1)
+                    b2_set_error("%s: the scale of slot %d is not finite (%f)", fn, k, (double)per_net_slot[k]);
+                else
+                    b2_set_error("%s: the scale of net %d, slot %d is not finite (%f)", fn, i, k, (double)per_net_slot[i * B + k]);
+                return -1;
+            }
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    memcpy(h->cn_scale_global, scale_per_slot, h->cfg.batch * sizeof(float));
+    for (int i = 0; i < h->cfg.controlnet; ++i) memcpy(h->cn_scale_global[i], per_net_slot + i * B, B * sizeof(float));
     TRY(bind_block(h, COND_TIME, nullptr, s));   // keep the global time biases of the block
     h->cond[COND_TIME].held = COND_UNKNOWN;
     TRY(write_global_scales(h, s));
     return keep_global(h, COND_TIME, s);
+}
+
+int b2sd_set_control_scale(b2sd_handle h, const float* scale_per_slot, void* stream) {
+    TRY(refuse_multi("b2sd_set_control_scale", h));
+    return set_control_scales("b2sd_set_control_scale", h, scale_per_slot, stream);
+}
+
+int b2sd_set_control_scales(b2sd_handle h, const float* per_net_slot, void* stream) {
+    return set_control_scales("b2sd_set_control_scales", h, per_net_slot, stream);
 }
 
 // ---- live parameters ------------------------------------------------------------------------------------------------------
@@ -3094,8 +3160,7 @@ int b2sd_state_set_timesteps(b2sd_handle h, b2sd_state_handle state, const float
     return state_refresh("b2sd_state_set_timesteps", h, state, COND_TIME, timesteps, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int b2sd_state_set_control_scale(b2sd_handle h, b2sd_state_handle state, const float* scale_per_slot, void* stream) {
-    const char* fn = "b2sd_state_set_control_scale";
+static int state_set_control_scales(const char* fn, b2sd_handle h, b2sd_state* state, const float* scale_per_slot, void* stream) {
     TRY(check_state(fn, h, state));
     if (!scale_per_slot) {
         b2_set_error("%s: null argument", fn);
@@ -3109,11 +3174,21 @@ int b2sd_state_set_control_scale(b2sd_handle h, b2sd_state_handle state, const f
     CondOverride* base = time_base(h, state, true);   // the state's time biases: its own timesteps', or the global ones
     TRY(bind_block(h, COND_TIME, base, s));
     h->cond[COND_TIME].held = COND_UNKNOWN;
-    CUDA_OK(cudaMemcpyAsync(h->cn_scale, scale_per_slot, h->cfg.batch * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(h->cn_scale, scale_per_slot, (size_t)h->cfg.controlnet * h->cfg.batch * sizeof(float),
+                            cudaMemcpyDeviceToDevice, s));
     TRY(publish_override(h, state, COND_TIME, s));
     state->cond[COND_TIME]->own_time = base != nullptr;
     state->cond[COND_TIME]->own_control = true;
     return 0;
+}
+
+int b2sd_state_set_control_scale(b2sd_handle h, b2sd_state_handle state, const float* scale_per_slot, void* stream) {
+    TRY(refuse_multi("b2sd_state_set_control_scale", h));
+    return state_set_control_scales("b2sd_state_set_control_scale", h, state, scale_per_slot, stream);
+}
+
+int b2sd_state_set_control_scales(b2sd_handle h, b2sd_state_handle state, const float* per_net_slot, void* stream) {
+    return state_set_control_scales("b2sd_state_set_control_scales", h, state, per_net_slot, stream);
 }
 
 // n rows of image tokens (nullptr: none) into h->ip_tok, the rest zeroed
@@ -3185,10 +3260,11 @@ int b2sd_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* fra
 
 // The input heads of a frame, in launch order: the encoder head, and with a ControlNet the head that reads the frame as the
 // control image -- the frame itself in [0, 1] at the engine's size (same nearest resize), or HED's edge map, whose first conv
-// reads the frame here and whose remaining layers run in stage 1
+// reads the frame here and whose remaining layers run in stage 1.  With several nets: HED's head once, before the first net
+// that reads the edge map, and one head per net that reads the frame, in net order.
 struct InputHeads {
-    SmallConvArgs conv[2];
-    const char* label[2];
+    SmallConvArgs conv[1 + B2SD_MAX_CONTROLNETS];
+    const char* label[1 + B2SD_MAX_CONTROLNETS];
     int n = 0;
 };
 
@@ -3199,12 +3275,17 @@ static InputHeads input_heads(b2sd_handle h, const void* frame_in, int in_kind, 
     in.conv[0].flags = in_flags | (h->head.flags & SC_IN_OFFSET);   // AutoencoderKL: 2x - 1 as the offset input mode
     in.label[0] = "smallconv head";
     in.n = 1;
-    if (h->cfg.controlnet) {
-        const bool hed = h->cfg.control_processor == B2SD_CONTROL_HED;
-        in.conv[1] = hed ? h->hed_head : h->cn_head;
-        in.conv[1].flags = in_flags | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
-        in.label[1] = hed ? "smallconv hed head" : "smallconv controlnet head";
-        in.n = 2;
+    static const char* cn_label[B2SD_MAX_CONTROLNETS] = {"smallconv controlnet head", "smallconv controlnet1 head",
+                                                         "smallconv controlnet2 head", "smallconv controlnet3 head"};
+    bool hed_done = false;
+    for (int i = 0; i < h->cfg.controlnet; ++i) {
+        const bool hed = h->control_processor(i) == B2SD_CONTROL_HED;
+        if (hed && hed_done) continue;
+        hed_done = hed_done || hed;
+        in.conv[in.n] = hed ? h->hed_head : h->cn_head[i];
+        in.conv[in.n].flags = in_flags | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
+        in.label[in.n] = hed ? "smallconv hed head" : cn_label[i];
+        ++in.n;
     }
     for (int i = 0; i < in.n; ++i) {
         in.conv[i].x = frame_in; in.conv[i].in_h = in_h; in.conv[i].in_w = in_w;

@@ -144,6 +144,9 @@ class LaunchRecord(C.Structure):
 AUDIT_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_int, C.POINTER(LaunchRecord))
 
 
+MAX_CONTROLNETS = 4   # B2SD_MAX_CONTROLNETS
+
+
 class EngineConfig(C.Structure):
     _fields_ = [
         ("block_out_channels", C.c_int * 4), ("heads", C.c_int * 4), ("down_attn", C.c_int * 4),
@@ -151,6 +154,7 @@ class EngineConfig(C.Structure):
         ("ctx_tokens", C.c_int), ("batch", C.c_int), ("height", C.c_int), ("width", C.c_int),
         ("do_add_noise", C.c_int), ("use_cuda_graph", C.c_int), ("controlnet", C.c_int), ("control_processor", C.c_int),
         ("vae", C.c_int), ("vae_scaling_factor", C.c_float), ("ip_tokens", C.c_int),
+        ("control_processor_more", C.c_int * (MAX_CONTROLNETS - 1)),
     ]
 
 
@@ -236,12 +240,14 @@ def lib() -> C.CDLL:
         _lib.b2sd_state_set_timesteps.argtypes = [vp, vp, vp, vp]
         _lib.b2sd_set_control_scale.argtypes = [vp, vp, vp]
         _lib.b2sd_state_set_control_scale.argtypes = [vp, vp, vp, vp]
+        _lib.b2sd_set_control_scales.argtypes = [vp, vp, vp]
+        _lib.b2sd_state_set_control_scales.argtypes = [vp, vp, vp, vp]
         _lib.b2sd_state_clear_conditioning.argtypes = [vp, ci]
         _lib.b2sd_set_image_embeds.argtypes = [vp, vp, ci, cf, vp]
         _lib.b2sd_state_set_image_embeds.argtypes = [vp, vp, vp, ci, cf, vp]
         for name in ("state_create", "state_reset", "state_destroy", "step_state", "state_set_prompt_embeds", "state_set_timesteps",
                      "state_clear_conditioning", "set_image_embeds", "state_set_image_embeds", "set_control_scale",
-                     "state_set_control_scale"):
+                     "state_set_control_scale", "set_control_scales", "state_set_control_scales"):
             getattr(_lib, "b2sd_" + name).restype = C.c_int
         _lib.b2sd_set_live_params.argtypes = [vp, ci]
         _lib.b2sd_apply_lora.argtypes = [vp, ci, C.POINTER(LoraFactor), vp]

@@ -16,12 +16,12 @@ from __future__ import annotations
 import collections
 import os
 import weakref
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Tuple, Union
 
 import numpy as np
 import torch
 
-from .stream import check_control
+from .stream import check_controls
 from .wrapper import LIVE_LORA_ENV, StreamDiffusionWrapper
 
 DEFAULT_PROMPT = "fireworks in the night sky"
@@ -108,8 +108,9 @@ class StreamDiffusionPipeline:
 
     def __init__(self, model_id: str, t_index_list: Optional[List[int]] = None, width: int = 512, height: int = 512,
                  prompt: str = DEFAULT_PROMPT, lanes: Optional[int] = None, per_peer_streams: Optional[bool] = None,
-                 live_lora: Optional[bool] = None, ip_adapter: Optional[str] = None, controlnet: Optional[str] = None,
-                 controlnet_processor: Optional[str] = "hed"):
+                 live_lora: Optional[bool] = None, ip_adapter: Optional[str] = None,
+                 controlnet: Optional[Union[str, List[str]]] = None,
+                 controlnet_processor: Optional[Union[str, List[Optional[str]]]] = "hed"):
         """lanes: frames in flight for enqueue() ($B200SD_LANES overrides the default).  With a 1-step stream batch (SD-Turbo)
         consecutive frames are independent: DEFAULT_LANES_ONE_STEP lanes process frame n+1.. while frame n is still on the GPU.
         With T > 1 the stream batch carries state from frame to frame: the pipeline's stream is then a stream state that two lanes
@@ -132,7 +133,9 @@ class StreamDiffusionPipeline:
         controlnet (None: $B200SD_CONTROLNET, default none): a diffusers ControlNetModel (id or path; "synthetic" with a
         synthetic model), conditioned on each frame's HED edge map (controlnet_processor="hed") or on the frame itself
         (controlnet_processor=None).  update_controlnet_scale() then sets its strength and guidance window, globally or per
-        viewer (PeerStream.update_controlnet_scale)."""
+        viewer (PeerStream.update_controlnet_scale).  A list of ids runs several ControlNets (diffusers'
+        MultiControlNetModel), each with its own control image and settings; controlnet_processor is then one processor for
+        every net or a list with one per net ($B200SD_CONTROLNET stays a single id)."""
         if per_peer_streams is None:
             per_peer_streams = env_flag(PER_PEER_STREAMS_ENV)
         self.per_peer_streams = bool(per_peer_streams)
@@ -258,7 +261,7 @@ class StreamDiffusionPipeline:
         settings and frames enqueued after it the new ones."""
         if not self.model.stream.has_controlnet:
             raise RuntimeError("update_controlnet_scale needs a pipeline with a ControlNet (controlnet=... or $B200SD_CONTROLNET)")
-        check_control(scale, control_guidance_start, control_guidance_end)
+        check_controls(scale, control_guidance_start, control_guidance_end, self.model.stream.control_nets)
         cur = self._quiesce()
         try:
             self.model.update_controlnet_scale(scale, control_guidance_start, control_guidance_end)
@@ -607,10 +610,12 @@ class PeerStream:
         self._pipeline._update_state(lambda engine: state.set_t_index_list(t_index_list, engine=engine), self._style)
 
     @property
-    def controlnet_scale(self) -> Tuple[float, float, float]:
-        """This viewer's ControlNet (scale, start, end): its own (update_controlnet_scale) or the pipeline's global ones"""
+    def controlnet_scale(self) -> tuple:
+        """This viewer's ControlNet (scale, start, end): its own (update_controlnet_scale) or the pipeline's global ones.  With
+        several ControlNets each of the three is a list with one entry per net."""
         own = self._live_state().own_control
-        return own if own is not None else self._pipeline.model.stream.control
+        control = own if own is not None else self._pipeline.model.stream.control
+        return control if not isinstance(control[0], tuple) else tuple(list(v) for v in control)
 
     def update_controlnet_scale(self, scale: float, control_guidance_start: float = 0.0,
                                 control_guidance_end: float = 1.0) -> None:
@@ -620,7 +625,8 @@ class PeerStream:
         state = self._live_state()
         if not self._pipeline.model.stream.has_controlnet:
             raise RuntimeError("update_controlnet_scale needs a pipeline with a ControlNet (controlnet=... or $B200SD_CONTROLNET)")
-        control = check_control(scale, control_guidance_start, control_guidance_end)
+        control = check_controls(scale, control_guidance_start, control_guidance_end,
+                                 self._pipeline.model.stream.control_nets)
         self._pipeline._update_state(lambda engine: state.set_control_scale(*control, engine=engine), self._style)
 
     @property

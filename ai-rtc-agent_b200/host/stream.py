@@ -74,6 +74,52 @@ def control_scales(control: Tuple[float, float, float], t_index_list: List[int],
     return [scale * (0.0 if (i / n_steps < start or (i + 1) / n_steps > end) else 1.0) for i in t_index_list]
 
 
+def check_controls(scale, start=0.0, end=1.0, nets: int = 1):
+    """The settings of `nets` ControlNets, checked.  One net: check_control's (scale, start, end) floats.  Several: diffusers'
+    MultiControlNetModel semantics (StableDiffusionControlNetPipeline.__call__ / check_inputs): a float scale applies to every
+    net, a list has one per net; start / end may each be a float or a list, a float broadcast to the other's length (to
+    `nets` when both are floats); then each (scale, start, end) is checked as for one net.  Returned as three tuples of
+    length `nets`, (scales, starts, ends), so that set_control_scale(*settings) takes them back."""
+    if nets == 1:
+        return check_control(scale, start, end)
+    seq = (list, tuple)
+    if not isinstance(start, seq) and isinstance(end, seq):
+        start = len(end) * [start]
+    elif not isinstance(end, seq) and isinstance(start, seq):
+        end = len(start) * [end]
+    elif not isinstance(start, seq) and not isinstance(end, seq):
+        start, end = nets * [start], nets * [end]
+    if isinstance(scale, seq):
+        if any(isinstance(v, seq) for v in scale):
+            raise ValueError("A single batch of varying conditioning scale settings (e.g. [[1.0, 0.5], [0.2, 0.8]]) is not "
+                             "supported at the moment. The conditioning scale must be fixed across the batch.")
+        if len(scale) != nets:
+            raise ValueError("For multiple controlnets: When `controlnet_conditioning_scale` is specified as `list`, it must "
+                             "have the same length as the number of controlnets")
+    else:
+        scale = nets * [scale]
+    if len(start) != len(end):
+        raise ValueError(f"`control_guidance_start` has {len(start)} elements, but `control_guidance_end` has {len(end)} "
+                         "elements. Make sure to provide the same number of elements to each list.")
+    if len(start) != nets:
+        raise ValueError(f"`control_guidance_start`: {list(start)} has {len(start)} elements but there are {nets} controlnets "
+                         f"available. Make sure to provide {nets}.")
+    return tuple(zip(*[check_control(v, a, b) for v, a, b in zip(scale, start, end)]))
+
+
+def default_controls(nets: int):
+    """The settings of `nets` ControlNets before any update: scale 1 over the whole run for each"""
+    return DEFAULT_CONTROL if nets == 1 else tuple(nets * (v,) for v in DEFAULT_CONTROL)
+
+
+def control_vector(control, t_index_list: List[int], n_steps: int) -> List[float]:
+    """The per-slot scales of every net, [nets * batch], from settings as check_controls returns them: net i's row is
+    control_scales of its own (scale, start, end)"""
+    if isinstance(control[0], tuple):
+        return [v for c in zip(*control) for v in control_scales(c, t_index_list, n_steps)]
+    return control_scales(control, t_index_list, n_steps)
+
+
 class ImageProcessor:
     """The part of diffusers' VaeImageProcessor the reference reaches (lib/wrapper.py:364)."""
 
@@ -100,8 +146,9 @@ class StreamDiffusion:
     styles = ()          # instances made by __init__ get a list (add_style)
     _is_style = False
     image_prompt = None  # the global image prompt: (host tokens [n_tok][D], scale) (set_image_tokens)
-    control = DEFAULT_CONTROL   # the global ControlNet (scale, start, end) (set_control_scale)
+    control = DEFAULT_CONTROL   # the global ControlNet settings (check_controls; set_control_scale)
     has_controlnet = False      # built with a ControlNet (inherited by lanes and styles)
+    control_nets = 1            # with has_controlnet: how many ControlNets (inherited by lanes and styles)
 
     def __init__(self, arch: UNetArch, unet_sd: Dict[str, torch.Tensor], vae_sd: Dict[str, torch.Tensor],
                  t_index_list: List[int], prompt_encoder: Callable[[str], torch.Tensor],
@@ -112,12 +159,14 @@ class StreamDiffusion:
                  controlnet_sd: Optional[Dict[str, torch.Tensor]] = None,
                  hed_sd: Optional[Dict[str, torch.Tensor]] = None, use_tiny_vae: bool = True,
                  vae_scaling_factor: float = 0.18215, live_lora: bool = False, style_of: Optional["StreamDiffusion"] = None,
-                 ip_adapter=None):
+                 ip_adapter=None, control_processors: Optional[List[Optional[str]]] = None):
         """vae_sd: TAESD (use_tiny_vae=True) or the model's own AutoencoderKL (use_tiny_vae=False: latents = vae_scaling_factor
         times the mean of the encoder's distribution, decoded from x0 / vae_scaling_factor).
         controlnet_sd: a diffusers ControlNetModel state dict (empty when the weights come from packed_blob); every
         stream-batch slot is then conditioned on the current frame's control image: the frame itself, or with hed_sd (a
         ControlNetHED.pth state dict, empty with packed_blob) its HED edge map.  Lanes inherit their parent's ControlNet.
+        Several ControlNets (diffusers' MultiControlNetModel): controlnet_sd a list of 1..4 state dicts and control_processors
+        one processor per net, "hed" (needs hed_sd; the edge map is computed once per frame) or None (the frame itself).
         live_lora: keep the base UNet weights on the device so that apply_lora() can switch LoRAs at run time (not with
         packed_blob; lanes inherit it).
         style_of: make a style of that live engine instead (add_style).
@@ -127,6 +176,19 @@ class StreamDiffusion:
             raise ValueError("live_lora needs the weights themselves: a packed blob does not carry the base weights")
         if hed_sd is not None and controlnet_sd is None:
             raise ValueError("the HED processor needs a ControlNet")
+        nets_sd = controlnet_sd if isinstance(controlnet_sd, (list, tuple)) else None
+        if nets_sd is not None:
+            if not 1 <= len(nets_sd) <= capi.MAX_CONTROLNETS:
+                raise ValueError(f"1 to {capi.MAX_CONTROLNETS} ControlNets (got {len(nets_sd)})")
+            if control_processors is None or len(control_processors) != len(nets_sd):
+                raise ValueError("control_processors needs one processor per ControlNet")
+            for p in control_processors:
+                if p not in (None, "hed"):
+                    raise NotImplementedError(f"ControlNet processor {p!r} (only 'hed', or None: the frame itself)")
+            if ("hed" in control_processors) != (hed_sd is not None):
+                raise ValueError("hed_sd is needed exactly when a ControlNet's processor is 'hed'")
+        elif control_processors is not None:
+            raise ValueError("control_processors goes with a list of ControlNet state dicts")
         if frame_buffer_size != 1:
             raise NotImplementedError("frame_buffer_size > 1 is not on the reference's path (lib/pipeline.py:28)")
         if not use_denoising_batch:
@@ -170,9 +232,17 @@ class StreamDiffusion:
         cfg.height, cfg.width = height, width
         cfg.do_add_noise = int(do_add_noise)
         cfg.use_cuda_graph = int(use_cuda_graph)
-        cfg.controlnet = int(controlnet_sd is not None)
+        cfg.controlnet = len(nets_sd) if nets_sd is not None else int(controlnet_sd is not None)
         self.has_controlnet = controlnet_sd is not None or (parent or style_of or self).has_controlnet
-        cfg.control_processor = capi.CONTROL_HED if hed_sd is not None else capi.CONTROL_FRAME
+        self.control_nets = cfg.controlnet if controlnet_sd is not None else (parent or style_of or self).control_nets
+        self.control = default_controls(self.control_nets)
+        if nets_sd is None:
+            cfg.control_processor = capi.CONTROL_HED if hed_sd is not None else capi.CONTROL_FRAME
+        else:
+            procs = [capi.CONTROL_HED if p == "hed" else capi.CONTROL_FRAME for p in control_processors]
+            cfg.control_processor = procs[0]
+            for i, p in enumerate(procs[1:]):
+                cfg.control_processor_more[i] = p
         cfg.vae = capi.VAE_TINY if use_tiny_vae else capi.VAE_KL
         cfg.vae_scaling_factor = 0.0 if use_tiny_vae else float(vae_scaling_factor)
         cfg.ip_tokens = ip_adapter.n_tok if ip_adapter is not None else 0
@@ -218,7 +288,8 @@ class StreamDiffusion:
             if ip_adapter is not None:
                 self._load("", ip_adapter.unet)
             self._load("vae.", vae_sd)
-            self._load("controlnet.", controlnet_sd or {})
+            for i, sd in enumerate(nets_sd if nets_sd is not None else [controlnet_sd or {}]):
+                self._load("controlnet." if i == 0 else f"controlnet{i}.", sd)
             self._load("hed.", hed_sd or {})
 
     # the reference reaches the UNet and the VAE as `stream.unet` / `stream.vae`; both are this engine.  Properties, not attributes
@@ -318,10 +389,12 @@ class StreamDiffusion:
         self._prepared = True
 
     def _push_control(self) -> None:
-        """This engine's global per-slot ControlNet scales from self.control and self.t_list (b2sd_set_control_scale)"""
+        """This engine's global per-slot ControlNet scales from self.control and self.t_list (b2sd_set_control_scale, with
+        several nets b2sd_set_control_scales)"""
         if self.has_controlnet:
-            v = torch.tensor(control_scales(self.control, self.t_list, len(self.timesteps)), dtype=torch.float32)
-            capi.check(self._lib.b2sd_set_control_scale(self._handle, v.data_ptr(), self._stream()), "b2sd_set_control_scale")
+            v = torch.tensor(control_vector(self.control, self.t_list, len(self.timesteps)), dtype=torch.float32)
+            fn = "b2sd_set_control_scale" if self.control_nets == 1 else "b2sd_set_control_scales"
+            capi.check(getattr(self._lib, fn)(self._handle, v.data_ptr(), self._stream()), fn)
 
     def _prepare_like(self, other: "StreamDiffusion") -> None:
         for name in self._SCHEDULE_ATTRS:
@@ -459,11 +532,12 @@ class StreamDiffusion:
         """The global ControlNet settings (diffusers' controlnet_conditioning_scale, control_guidance_start / _end): this
         engine's, its lanes' and its styles' (b2sd_set_control_scale), and every live state's (a state's own settings are
         dropped, its own t_index_list kept).  Slot k of the stream batch is conditioned with scale times diffusers'
-        controlnet_keep of step t_index_list[k] of the len(self.timesteps)-step table (control_scales).  The settings are
-        checked before anything changes; on the current CUDA stream, after the frames queued there."""
+        controlnet_keep of step t_index_list[k] of the len(self.timesteps)-step table (control_scales).  With several
+        ControlNets each argument may be a float (every net) or a list (one per net), as check_controls takes them.  The
+        settings are checked before anything changes; on the current CUDA stream, after the frames queued there."""
         if not self.has_controlnet:
             raise RuntimeError("this engine was built without a ControlNet")
-        control = check_control(scale, start, end)
+        control = check_controls(scale, start, end, self.control_nets)
         for eng in self._family():
             eng.control = control
             eng._push_control()
@@ -749,7 +823,7 @@ class StreamState:
     own_prompt: Optional[str] = None               # None: the global prompt
     own_t_index_list: Optional[List[int]] = None   # None: the global t_index_list
     own_image: Optional[Tuple[torch.Tensor, float]] = None   # (device tokens [n_tok][D], scale); None: the global image prompt
-    own_control: Optional[Tuple[float, float, float]] = None  # ControlNet (scale, start, end); None: the global settings
+    own_control: Optional[tuple] = None   # ControlNet settings (check_controls); None: the global settings
     home: Optional[StreamDiffusion] = None   # where clear_overrides recomputes what it keeps (None: the creating engine)
 
     def __init__(self, engine: StreamDiffusion):
@@ -793,18 +867,18 @@ class StreamState:
         eng = engine or self._engine
         if not eng.has_controlnet:
             raise RuntimeError("this engine was built without a ControlNet")
-        control = check_control(scale, start, end)
+        control = check_controls(scale, start, end, eng.control_nets)
         self._push_control(eng, control)
         self.own_control = control
 
-    def _push_control(self, eng: StreamDiffusion, control: Optional[Tuple[float, float, float]] = None) -> None:
-        """The state's per-slot ControlNet scales (b2sd_state_set_control_scale) from `control` (default its own settings, else
-        the global ones) and the t_index_list it is stepped with"""
+    def _push_control(self, eng: StreamDiffusion, control: Optional[tuple] = None) -> None:
+        """The state's per-slot ControlNet scales (b2sd_state_set_control_scale, with several nets _scales) from `control`
+        (default its own settings, else the global ones) and the t_index_list it is stepped with"""
         control = control or self.own_control or eng.control
         t_index_list = self.own_t_index_list if self.own_t_index_list is not None else eng.t_list
-        v = _on_device(torch.tensor(control_scales(control, t_index_list, len(eng.timesteps)), dtype=torch.float32), eng.device)
-        capi.check(self._lib.b2sd_state_set_control_scale(eng._handle, self.handle, v.data_ptr(), eng._stream()),
-                   "b2sd_state_set_control_scale")
+        v = _on_device(torch.tensor(control_vector(control, t_index_list, len(eng.timesteps)), dtype=torch.float32), eng.device)
+        fn = "b2sd_state_set_control_scale" if eng.control_nets == 1 else "b2sd_state_set_control_scales"
+        capi.check(getattr(self._lib, fn)(eng._handle, self.handle, v.data_ptr(), eng._stream()), fn)
 
     @torch.no_grad()
     def set_image_tokens(self, tokens: Optional[torch.Tensor], scale: float = 1.0,

@@ -105,14 +105,16 @@ def synthetic_controlnet(arch: A.UNetArch, seed: int = 5678, zero_init: bool = F
     return sd
 
 
-def resolve_controlnet(controlnet_id_or_path: str, arch: A.UNetArch, synthetic_ok: bool) -> Dict[str, torch.Tensor]:
-    """A ControlNet on disk (directory or HF-cache id), else seeded synthetic weights when those are allowed, else an error."""
+def resolve_controlnet(controlnet_id_or_path: str, arch: A.UNetArch, synthetic_ok: bool, net: int = 0) -> Dict[str, torch.Tensor]:
+    """A ControlNet on disk (directory or HF-cache id), else seeded synthetic weights when those are allowed, else an error.
+    net: its position among several ControlNets; synthetic weights are seeded by it (net 0 with the single net's seed), so
+    that two synthetic nets differ."""
     repo = find_local_repo(controlnet_id_or_path)
     if repo is not None:
         return load_controlnet(repo, arch)
     if synthetic_ok:
         logger.warning("no ControlNet %s on disk: using seeded synthetic weights", controlnet_id_or_path)
-        return synthetic_controlnet(arch)
+        return synthetic_controlnet(arch, seed=5678 + net)
     raise FileNotFoundError(f"ControlNet '{controlnet_id_or_path}' not found on disk; set {ALLOW_SYNTHETIC_ENV}=1 to run with "
                             "seeded synthetic weights")
 
@@ -247,7 +249,7 @@ def layout_variant(batch: int, height: int, width: int) -> str:
 
 def packed_blob_path(engine_dir, model_id_or_path: str, arch_name: str, use_lcm_lora: bool, lcm_lora_id: Optional[str],
                      lora_dict: Optional[Dict[str, float]], vae_id: Optional[str], synthetic: bool, variant: str = "",
-                     controlnet: Optional[str] = None, control_processor: Optional[str] = None, full_vae: bool = False,
+                     controlnet=None, control_processor=None, full_vae: bool = False,
                   ip_adapter: Optional[str] = None) -> str:
     """Where the packed-weight blob of this model lives: `<engine_dir>/engines--<model>/b2sd-<arch>-<recipe hash>.b2pack`,
     the directory naming of the reference's TensorRT cache (lib/wrapper.py:593, `engines--` + model id with / -> --).
@@ -255,7 +257,8 @@ def packed_blob_path(engine_dir, model_id_or_path: str, arch_name: str, use_lcm_
     seed), not
     batch / resolution / prompt (the blob does not depend on them, unlike the reference's static-shape engines).
     full_vae (use_tiny_vae=False) enters the recipe only when set, so the names of TAESD blobs do not change; so does
-    ip_adapter (an adapter file or directory, or "synthetic"), with the adapter file's real path, size and mtime."""
+    ip_adapter (an adapter file or directory, or "synthetic"), with the adapter file's real path, size and mtime.
+    Several ControlNets: controlnet and control_processor are lists in net order, and the recipe holds them as lists."""
     import hashlib
     import json
     recipe = {"lcm": bool(use_lcm_lora), "lcm_id": lcm_lora_id, "vae": vae_id, "synthetic": bool(synthetic), "layout": variant,
@@ -269,11 +272,14 @@ def packed_blob_path(engine_dir, model_id_or_path: str, arch_name: str, use_lcm_
     if controlnet is not None:
         recipe["controlnet"] = controlnet
         recipe["control_processor"] = control_processor
-        repo = find_local_repo(controlnet)
-        for name in sorted(os.listdir(repo)) if repo else ():   # replaced ControlNet weights must not hit the old blob
-            if name.endswith((".safetensors", ".json")):
-                st = os.stat(os.path.join(repo, name))
-                recipe.setdefault("controlnet_files", []).append((name, st.st_size, int(st.st_mtime)))
+        for i, cn in enumerate(controlnet if isinstance(controlnet, (list, tuple)) else [controlnet]):
+            repo = find_local_repo(cn)
+            for name in sorted(os.listdir(repo)) if repo else ():   # replaced ControlNet weights must not hit the old blob
+                if name.endswith((".safetensors", ".json")):
+                    st = os.stat(os.path.join(repo, name))
+                    # net 0's entries as a single net's, later nets' tagged with their position
+                    entry = (name, st.st_size, int(st.st_mtime)) if i == 0 else (i, name, st.st_size, int(st.st_mtime))
+                    recipe.setdefault("controlnet_files", []).append(entry)
     if ip_adapter is not None:
         recipe["ip_adapter"] = ip_adapter
         if os.path.exists(ip_adapter):   # a replaced adapter file must not hit the old blob

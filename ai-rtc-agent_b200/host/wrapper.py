@@ -6,7 +6,8 @@ Not carried over (unreachable from lib/pipeline.py:23-42 and listed out-of-scope
 safety checker, similar-image filter, DataParallel, txt2img sampling, xformers/sfast/TensorRT acceleration switches, and
 ControlNet preprocessors other than HED.  Their keywords are accepted; asking for one of those features raises.  A ControlNet
 runs with controlnet_processor_id="hed" (the default: the frame's HED edge map is the control image) or None (the frame
-itself).  use_tiny_vae=False encodes and decodes with the model's own AutoencoderKL instead of TAESD (slower, the model's
+itself).  Several ControlNets (diffusers' MultiControlNetModel): controlnet_id_or_path a list of ids, controlnet_processor_id
+one processor for all or a list with one per net.  use_tiny_vae=False encodes and decodes with the model's own AutoencoderKL instead of TAESD (slower, the model's
 image quality); the latent is the mean of the encoder's distribution, not a sample of it."""
 from __future__ import annotations
 
@@ -50,6 +51,28 @@ def postprocess_image(image: torch.Tensor, output_type: str = "pil"):
 
 
 LIVE_LORA_ENV = "B200SD_LIVE_LORA"
+
+
+def control_args(controlnet_id_or_path, controlnet_processor_id):
+    """The ControlNet arguments with lists resolved: a list of one id (and of one processor) is the plain value, so it builds
+    the same engine as the string; with several ids the result is (ids, processors), a single processor repeated for every
+    net.  A processor list of another length than the ids is refused."""
+    seq = (list, tuple)
+    ids, procs = controlnet_id_or_path, controlnet_processor_id
+    if isinstance(ids, seq):
+        if not ids:
+            raise ValueError("controlnet_id_or_path: an empty list (None for no ControlNet)")
+        ids = list(ids)
+    if isinstance(procs, seq) and (len(procs) != (len(ids) if isinstance(ids, list) else 1)):
+        raise ValueError(f"controlnet_processor_id has {len(procs)} entries for "
+                         f"{len(ids) if isinstance(ids, list) else 1} ControlNet(s)")
+    if isinstance(ids, list) and len(ids) == 1:
+        ids = ids[0]
+    if isinstance(procs, seq) and len(procs) == 1:
+        procs = procs[0]
+    if isinstance(ids, list) and not isinstance(procs, seq):
+        procs = [procs] * len(ids)
+    return ids, list(procs) if isinstance(procs, seq) else procs
 
 
 class StreamDiffusionWrapper:
@@ -104,13 +127,15 @@ class StreamDiffusionWrapper:
         if mode == "img2img" and not use_denoising_batch:
             raise NotImplementedError("img2img mode must use denoising batch for now.")
 
+        controlnet_id_or_path, controlnet_processor_id = control_args(controlnet_id_or_path, controlnet_processor_id)
         unsupported = []
         if mode == "txt2img":
             unsupported.append("mode='txt2img'")
-        if controlnet_id_or_path is not None and controlnet_processor_id not in (None, "hed"):
-            # the reference prints "ControlNet conditioning not supported." for an unknown id and runs unconditioned; a caller
-            # who asked for a preprocessor should not silently get the raw frame instead
-            unsupported.append(f"controlnet_processor_id={controlnet_processor_id!r} (only 'hed', or None: the frame itself)")
+        for proc in controlnet_processor_id if isinstance(controlnet_processor_id, list) else [controlnet_processor_id]:
+            if controlnet_id_or_path is not None and proc not in (None, "hed"):
+                # the reference prints "ControlNet conditioning not supported." for an unknown id and runs unconditioned; a
+                # caller who asked for a preprocessor should not silently get the raw frame instead
+                unsupported.append(f"controlnet_processor_id={proc!r} (only 'hed', or None: the frame itself)")
         if use_safety_checker:
             unsupported.append("safety checker")
         if enable_similar_image_filter:
@@ -178,7 +203,10 @@ class StreamDiffusionWrapper:
                   device=self.device, use_tiny_vae=tiny_vae,
                   vae_scaling_factor=W.resolve_vae_scaling_factor(repo if have_ckpt else None))
         cn = controlnet_id_or_path is not None
-        hed = cn and controlnet_processor_id == "hed"
+        multi = isinstance(controlnet_id_or_path, list)
+        hed = cn and (("hed" in controlnet_processor_id) if multi else controlnet_processor_id == "hed")
+        if multi:
+            kw["control_processors"] = controlnet_processor_id
         adapter = self._load_ip_adapter(arch, synthetic_ok)
         kw["ip_adapter"] = adapter
         blob = None
@@ -197,7 +225,8 @@ class StreamDiffusionWrapper:
         if blob is not None and os.path.exists(blob) and (have_ckpt or synthetic_ok):
             try:
                 sd = StreamDiffusion(arch, {}, {}, t_index_list, encoder, packed_blob=blob,
-                                     controlnet_sd={} if cn else None, hed_sd={} if hed else None, **kw)
+                                     controlnet_sd=([{}] * len(controlnet_id_or_path) if multi else {}) if cn else None,
+                                     hed_sd={} if hed else None, **kw)
                 logger.info("loaded packed weights from %s", blob)
                 self.packed_blob = blob
                 return sd
@@ -205,7 +234,10 @@ class StreamDiffusionWrapper:
                 logger.warning("packed-weight blob %s unusable (%s); rebuilding from the checkpoint", blob, exc)
         arch, unet_sd, vae_sd, repo = resolve_weights(model_id_or_path, vae_id, lcm_lora_id, use_lcm_lora,
                                                       None if self.live_lora else lora_dict, self.sd_turbo, use_tiny_vae=tiny_vae)
-        cn_sd = W.resolve_controlnet(controlnet_id_or_path, arch, synthetic_ok) if cn else None
+        if multi:
+            cn_sd = [W.resolve_controlnet(c, arch, synthetic_ok, net=i) for i, c in enumerate(controlnet_id_or_path)]
+        else:
+            cn_sd = W.resolve_controlnet(controlnet_id_or_path, arch, synthetic_ok) if cn else None
         hed_sd = W.resolve_hed(synthetic_ok) if hed else None
         self._blob_to_write = blob
         return StreamDiffusion(arch, unet_sd, vae_sd, t_index_list, encoder, controlnet_sd=cn_sd, hed_sd=hed_sd,
@@ -303,7 +335,8 @@ class StreamDiffusionWrapper:
                                 control_guidance_end: float = 1.0) -> None:
         """The ControlNet's strength and guidance window, as diffusers' StableDiffusionControlNetPipeline takes them
         (controlnet_conditioning_scale, control_guidance_start / _end): frames computed after the call use them.  Slot k of
-        the stream batch stands for step t_index_list[k] of the timestep table.  See StreamDiffusion.set_control_scale."""
+        the stream batch stands for step t_index_list[k] of the timestep table.  With several ControlNets each argument is a float
+        for every net or a list with one per net (diffusers' MultiControlNetModel).  See StreamDiffusion.set_control_scale."""
         with self._on_stream():
             self.stream.set_control_scale(scale, control_guidance_start, control_guidance_end)
 

@@ -193,6 +193,7 @@ int b2sd_op_post_f16(const void* y_nhwc, int ldy, void* out_nchw_f16, int nb, in
  * cfg_type="self" with guidance_scale <= 1 (the only configuration lib/pipeline.py:23-42 builds).
  * ---------------------------------------------------------------------------------------------- */
 typedef struct b2sd_engine* b2sd_handle;
+#define B2SD_MAX_CONTROLNETS 4
 
 typedef struct {
     int block_out_channels[4];   /* (320,640,1280,1280) */
@@ -209,7 +210,8 @@ typedef struct {
     int controlnet;              /* 1: a ControlNet (weights under "controlnet." + diffusers ControlNetModel keys) conditions
                                     every stream-batch slot on the current frame (control image = frame / 255 at the engine's
                                     size); its 12 + 1 residuals are added to the UNet's skips and mid-block output.  0: none.
-                                    A lane inherits its parent's value. */
+                                    2..B2SD_MAX_CONTROLNETS: that many nets (control_processor_more).  A lane inherits its
+                                    parent's value. */
     int control_processor;       /* with controlnet = 1: B2SD_CONTROL_FRAME (0) or B2SD_CONTROL_HED (1): the control image is the
                                     HED edge map of the frame (controlnet_aux HEDdetector at the engine's size; weights under
                                     "hed." + ControlNetHED.pth keys, e.g. "hed.block1.convs.0.weight", "hed.norm").  Inherited
@@ -224,6 +226,14 @@ typedef struct {
                                     UNet's cross-attentions (not the ControlNet's) then add a decoupled attention over the image
                                     tokens' K / V (weights "...attn2.to_k_ip.weight" / "...attn2.to_v_ip.weight" beside to_k /
                                     to_v), see b2sd_set_image_embeds.  Inherited by lanes and styles. */
+    int control_processor_more[B2SD_MAX_CONTROLNETS - 1];
+                                 /* multi-ControlNet: controlnet = N (1..B2SD_MAX_CONTROLNETS) nets, net 0 with the weights and
+                                    processor above, net i >= 1 with weights under "controlnet<i>." (e.g.
+                                    "controlnet1.controlnet_mid_block.weight") and processor control_processor_more[i - 1]
+                                    (0 for the entries past the last net).  The HED edge map is computed once per frame however
+                                    many nets read it.  Each net's residuals are scaled by its own per-slot scales
+                                    (b2sd_set_control_scales) and summed into the UNet's skips in net order,
+                                    ((skip + r_0) + r_1) + ...  Inherited by lanes and styles. */
 } b2sd_config;
 enum { B2SD_CONTROL_FRAME = 0, B2SD_CONTROL_HED = 1 };
 enum { B2SD_VAE_TINY = 0, B2SD_VAE_KL = 1 };
@@ -524,9 +534,13 @@ int b2sd_state_set_image_embeds(b2sd_handle h, b2sd_state_handle state, const vo
  * Scales or timesteps of a state without the other part of its own take that part from the engine's global block at the
  * call, so a global refresh is followed by setting them again; after a move to another store of the family set the state's
  * timesteps, then its scales, again.  Clearing the state's time block (b2sd_state_clear_conditioning(state, 1)) drops both.
- * Both calls refuse an engine without a ControlNet. */
+ * Both calls refuse an engine without a ControlNet, and one with several (use b2sd_set_control_scales). */
 int b2sd_set_control_scale(b2sd_handle h, const float* scale_per_slot, void* stream);
 int b2sd_state_set_control_scale(b2sd_handle h, b2sd_state_handle state, const float* scale_per_slot, void* stream);
+/* The same for an engine with any number of ControlNets: per_net_slot is fp32 [controlnet][batch], row i net i's per-slot
+ * scales.  Same memory, ordering and keeping rules as the single-net calls above, which these equal with one net. */
+int b2sd_set_control_scales(b2sd_handle h, const float* per_net_slot, void* stream);
+int b2sd_state_set_control_scales(b2sd_handle h, b2sd_state_handle state, const float* per_net_slot, void* stream);
 /* Drop the state's override of the prompt (which = 0) or time (which = 1) block: later steps use the engines' global values.
  * No device work; the override is freed after the steps already submitted with it. */
 int b2sd_state_clear_conditioning(b2sd_state_handle state, int which);

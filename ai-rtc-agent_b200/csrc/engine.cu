@@ -22,6 +22,7 @@
 
 #include "../../include/b200sd.h"
 #include "attention.cuh"
+#include "canny.cuh"
 #include "elementwise.cuh"
 #include "igemm.cuh"
 #include "tconv.cuh"
@@ -402,6 +403,10 @@ struct b2sd_state {
     __half* buf = nullptr;
     cudaEvent_t done = nullptr;   // recorded after each step's copy-out; the next step of this stream waits on it
     std::unique_ptr<CondOverride> cond[2];   // the state's own prompt / time block; none: the stepping engine's global values
+    // the state's own Canny thresholds (b2sd_state_set_canny_thresholds): host values any engine passes to canny_head
+    bool canny = false;   // the family's engines run Canny
+    bool canny_own = false;
+    double canny_low = 100, canny_high = 200;
 };
 
 struct b2sd_engine {
@@ -483,7 +488,20 @@ struct b2sd_engine {
     // each ControlNet's conditioning embedding conv_in (reads the caller's frame as the control image, with processor FRAME)
     SmallConvArgs cn_head[B2SD_MAX_CONTROLNETS]{};
     SmallConvArgs hed_head{};  // HED's first conv (reads the caller's frame) when a control image is its edge map
+    // Canny (a net with processor B2SD_CONTROL_CANNY): canny_head (reads the caller's frame) writes canny.cls, stage 1 of the
+    // frame program runs the hysteresis launches on it.  The thresholds are host values passed to canny_head when a step
+    // launches it: the stepped state's own, else the engine's global ones (b2sd_set_canny_thresholds).
+    uint8_t* canny_cls = nullptr;
+    CannyCclArgs canny{};
+    double canny_low = 100, canny_high = 200;
+    struct U8Tap { const uint8_t* p; int h, w, c; };
+    std::map<std::string, U8Tap> u8_taps;   // dense u8 [1][h][w][c] buffers, read back as fp16 by b2sd_get_tensor
     int control_processor(int net) const { return net == 0 ? cfg.control_processor : cfg.control_processor_more[net - 1]; }
+    bool reads_canny() const {
+        for (int i = 0; i < cfg.controlnet; ++i)
+            if (control_processor(i) == B2SD_CONTROL_CANNY) return true;
+        return false;
+    }
     Act image;              // decoder output, fp16 NHWC (ld 8)
     bool built = false;
     int concurrency = 1;   // frames expected in flight on this GPU (b2sd_set_concurrency): > 1 selects the throughput launch policy
@@ -895,8 +913,9 @@ struct b2sd_engine {
     std::vector<float> host_copy(const std::string& key);
     int derive(const std::string& name, const std::vector<int64_t>& shape, const std::vector<float>& v);
     const float* const_vec(const std::string& name, const std::vector<float>& v);
-    int build_cond_embedding(int net, const uint8_t** hed_control, Act* out, cudaStream_t s);
+    int build_cond_embedding(int net, const uint8_t** shared_control, Act* out, cudaStream_t s);
     int build_hed(const uint8_t** control, cudaStream_t s);
+    int build_canny(const uint8_t** control, cudaStream_t s);
     int build_controlnet(int net, const Act& cond, std::vector<Act>& skips, Act* mid, cudaStream_t s);
     int build_transformer(const std::string& p, const Act& x, int heads, Act* out, cudaStream_t s);
     int build_taesd_block(const std::string& p, const Act& x, Act* out, cudaStream_t s);
@@ -1250,8 +1269,9 @@ static std::string cn_prefix(int net) { return net == 0 ? std::string("controlne
 // activations are stored 64/64/128 wide with zero padding columns, so the following layers run as 64/64/128-channel
 // tensor-core contractions (zero weights on the padding channels, pack_conv_weight_launch).  The epilogues write only the
 // valid columns: the padding is cleared once here, and stays finite (0 * NaN would be NaN).  With several nets each has its
-// own; HED runs once, for the first net that reads its edge map (*hed_control, null until then), and later ones share it.
-int b2sd_engine::build_cond_embedding(int net, const uint8_t** hed_control, Act* out, cudaStream_t s) {
+// own; HED and Canny each run once, for the first net that reads their edge map (shared_control[processor], null until then),
+// and later ones share it.
+int b2sd_engine::build_cond_embedding(int net, const uint8_t** shared_control, Act* out, cudaStream_t s) {
     const std::string p = cn_prefix(net) + "controlnet_cond_embedding.";
     SmallConvArgs& cn_head = this->cn_head[net];
     cur = p;
@@ -1269,10 +1289,12 @@ int b2sd_engine::build_cond_embedding(int net, const uint8_t** hed_control, Act*
     if (!cn_head.wt || !cn_head.bias) return -1;
     cn_head.y = a.p; cn_head.ldy = a.ld; cn_head.nb = 1; cn_head.h = a.h; cn_head.w_ = a.w; cn_head.cin = 3; cn_head.cout = 16;
     ++launches;
-    if (control_processor(net) == B2SD_CONTROL_HED) {   // the control image is HED's edge map, computed in this stage
-        if (!*hed_control) TRY(build_hed(hed_control, s));
+    const int proc = control_processor(net);
+    if (proc != B2SD_CONTROL_FRAME) {   // the control image is HED's or Canny's edge map, computed in this stage
+        const uint8_t** edge = &shared_control[proc];
+        if (!*edge) TRY(proc == B2SD_CONTROL_HED ? build_hed(edge, s) : build_canny(edge, s));
         SmallConvArgs c = cn_head;
-        c.x = *hed_control; c.in_h = a.h; c.in_w = a.w; c.flags = SC_IN_U8 | SC_OUT_SILU;
+        c.x = *edge; c.in_h = a.h; c.in_w = a.w; c.flags = SC_IN_U8 | SC_OUT_SILU;
         prog_frame.push_back(Op([c](cudaStream_t st) { return smallconv_launch(c, st); }, "smallconv controlnet_cond_embedding.conv_in",
                                 smallconv_record(c)));
     }
@@ -1355,6 +1377,41 @@ int b2sd_engine::build_hed(const uint8_t** control, cudaStream_t s) {
     prog_frame.push_back(Op([f](cudaStream_t st) { return hed_fuse_launch(f, st); }, "hed_fuse", r));
     taps["control"] = edge;
     *control = f.out;
+    return 0;
+}
+
+b2sd_launch_record canny_ccl_record(const CannyCclArgs& a, int stage) {
+    b2sd_launch_record r{};
+    r.kind = B2SD_LAUNCH_CANNY_CCL;
+    r.canny_ccl = b2sd_canny_ccl_args{a.cls, a.parent, a.flag, a.out, a.h, a.w, stage};
+    return r;
+}
+
+// controlnet_aux's CannyDetector (cv2.Canny, aperture 3, L1 gradient) at the engine's resolution: canny_head (launched by the
+// step, outside the graph) classifies every pixel of the frame; here the four hysteresis launches turn the class map into
+// the u8 edge image (3 channels).  A fixed launch count, no grid-wide barrier: each launch waits for the previous one.
+int b2sd_engine::build_canny(const uint8_t** control, cudaStream_t) {
+    const int H = cfg.height, W = cfg.width;
+    canny = CannyCclArgs{};
+    canny.h = H; canny.w = W;
+    canny.cls = canny_cls = static_cast<uint8_t*>(prog.alloc((size_t)H * W));
+    canny.parent = static_cast<int*>(prog.alloc((size_t)H * W * sizeof(int)));
+    canny.flag = static_cast<uint8_t*>(prog.alloc((size_t)H * W));
+    canny.out = static_cast<uint8_t*>(prog.alloc((size_t)H * W * 3));
+    if (!canny.cls || !canny.parent || !canny.flag || !canny.out) {
+        b2_set_error("canny: buffer allocation failed");
+        return -1;
+    }
+    ++launches;   // canny_head
+    static const char* label[CANNY_CCL_STAGES] = {"canny_ccl local", "canny_ccl merge", "canny_ccl flag", "canny_ccl out"};
+    for (int st = 0; st < CANNY_CCL_STAGES; ++st) {
+        const CannyCclArgs a = canny;
+        ++launches;
+        prog_frame.push_back(Op([a, st](cudaStream_t q) { return canny_ccl_launch(a, st, q); }, label[st], canny_ccl_record(a, st)));
+    }
+    u8_taps["canny_class"] = U8Tap{canny.cls, H, W, 1};
+    u8_taps["canny"] = U8Tap{canny.out, H, W, 3};
+    *control = canny.out;
     return 0;
 }
 
@@ -1740,6 +1797,7 @@ int b2sd_engine::build_program(cudaStream_t s) {
     prog.reset();
     prog_frame.clear(); prog_prompt.clear(); prog_time.clear(); prog_image.clear();
     taps.clear();
+    u8_taps.clear();
     launches = 0;
     drop_graphs();
     const int B = cfg.batch, H = cfg.height, W = cfg.width;
@@ -1837,8 +1895,8 @@ int b2sd_engine::build_program(cudaStream_t s) {
     }
     // each ControlNet's conditioning embedding of this frame's control image: batch 1, latent resolution, C0 channels
     Act cond[B2SD_MAX_CONTROLNETS];
-    const uint8_t* hed_control = nullptr;   // HED's edge map, once a net reads it
-    for (int i = 0; i < cfg.controlnet; ++i) TRY(build_cond_embedding(i, &hed_control, &cond[i], s));
+    const uint8_t* shared_control[3] = {};   // per processor: HED's / Canny's edge map, once a net reads it
+    for (int i = 0; i < cfg.controlnet; ++i) TRY(build_cond_embedding(i, shared_control, &cond[i], s));
     {
         // latent head + StreamDiffusion.encode_image add-noise: x_t = alpha0 * z + beta0 * init_noise[0]
         // (AutoencoderKL: z = scaling_factor * mean, the scale applied with alpha0 in the epilogue)
@@ -2015,6 +2073,7 @@ static int state_new(const b2sd_engine* h, cudaStream_t s, b2sd_state** out) {
     st->family = h->ws->family;
     st->batch = h->cfg.batch; st->height = h->cfg.height; st->width = h->cfg.width;
     st->bytes = state_bytes(h);
+    st->canny = h->reads_canny();
     cudaError_t e = cudaEventCreateWithFlags(&st->done, cudaEventDisableTiming);
     if (e == cudaSuccess && st->bytes) e = cudaMallocAsync(reinterpret_cast<void**>(&st->buf), st->bytes, s);
     if (e == cudaSuccess && st->bytes) e = cudaMemsetAsync(st->buf, 0, st->bytes, s);
@@ -2229,15 +2288,17 @@ static int create_engine(const b2sd_config* cfg, std::shared_ptr<WeightStore> st
         b2_set_error("b2sd_create: controlnet must be 0..%d (got %d)", B2SD_MAX_CONTROLNETS, cfg->controlnet);
         return -1;
     }
-    if (cfg->control_processor != B2SD_CONTROL_FRAME && (cfg->control_processor != B2SD_CONTROL_HED || !cfg->controlnet)) {
-        b2_set_error("b2sd_create: control_processor must be 0 (the frame) or 1 (HED, with a ControlNet) (got %d)", cfg->control_processor);
+    const auto edge_processor = [](int p) { return p == B2SD_CONTROL_HED || p == B2SD_CONTROL_CANNY; };
+    if (cfg->control_processor != B2SD_CONTROL_FRAME && (!edge_processor(cfg->control_processor) || !cfg->controlnet)) {
+        b2_set_error("b2sd_create: control_processor must be 0 (the frame), 1 (HED) or 2 (Canny), the last two with a ControlNet "
+                     "(got %d)", cfg->control_processor);
         return -1;
     }
     for (int i = 1; i < B2SD_MAX_CONTROLNETS; ++i) {
         const int p = cfg->control_processor_more[i - 1];
-        if (p != B2SD_CONTROL_FRAME && (p != B2SD_CONTROL_HED || i >= cfg->controlnet)) {
-            b2_set_error("b2sd_create: control_processor_more[%d] must be 0 (the frame) or 1 (HED, with a ControlNet %d) (got %d)",
-                         i - 1, i, p);
+        if (p != B2SD_CONTROL_FRAME && (!edge_processor(p) || i >= cfg->controlnet)) {
+            b2_set_error("b2sd_create: control_processor_more[%d] must be 0 (the frame), 1 (HED) or 2 (Canny), the last two with a "
+                         "ControlNet %d (got %d)", i - 1, i, p);
             return -1;
         }
     }
@@ -3254,48 +3315,125 @@ int b2sd_state_clear_conditioning(b2sd_state_handle state, int which) {
 
 int64_t b2sd_conditioning_binds(b2sd_handle h) { return h ? h->cond_binds : -1; }
 
+// ---- Canny thresholds: host values, passed to canny_head by the steps submitted after the call -----------------------------
+static int check_canny_thresholds(const char* fn, bool canny, double low, double high) {
+    if (!canny) {
+        b2_set_error("%s: the engine has no ControlNet with the Canny processor", fn);
+        return -1;
+    }
+    if (!isfinite(low) || !isfinite(high)) {
+        b2_set_error("%s: the thresholds must be finite (got %f, %f)", fn, low, high);
+        return -1;
+    }
+    return 0;
+}
+
+int b2sd_set_canny_thresholds(b2sd_handle h, double low, double high) {
+    if (!h) {
+        b2_set_error("b2sd_set_canny_thresholds: null handle");
+        return -1;
+    }
+    TRY(check_canny_thresholds("b2sd_set_canny_thresholds", h->reads_canny(), low, high));
+    h->canny_low = low;
+    h->canny_high = high;
+    return 0;
+}
+
+int b2sd_state_set_canny_thresholds(b2sd_state_handle state, double low, double high) {
+    if (!state) {
+        b2_set_error("b2sd_state_set_canny_thresholds: null state");
+        return -1;
+    }
+    TRY(check_canny_thresholds("b2sd_state_set_canny_thresholds", state->canny, low, high));
+    state->canny_own = true;
+    state->canny_low = low;
+    state->canny_high = high;
+    return 0;
+}
+
+int b2sd_state_clear_canny_thresholds(b2sd_state_handle state) {
+    if (!state) {
+        b2_set_error("b2sd_state_clear_canny_thresholds: null state");
+        return -1;
+    }
+    TRY(check_canny_thresholds("b2sd_state_clear_canny_thresholds", state->canny, 0, 0));
+    state->canny_own = false;
+    return 0;
+}
+
 int b2sd_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* frame_out, void* stream) {
     return b2sd_step_ex(h, frame_in, B2SD_IN_U8_NHWC, in_h, in_w, frame_out, B2SD_OUT_U8_NCHW, stream);
 }
 
 // The input heads of a frame, in launch order: the encoder head, and with a ControlNet the head that reads the frame as the
 // control image -- the frame itself in [0, 1] at the engine's size (same nearest resize), or HED's edge map, whose first conv
-// reads the frame here and whose remaining layers run in stage 1.  With several nets: HED's head once, before the first net
-// that reads the edge map, and one head per net that reads the frame, in net order.
+// reads the frame here and whose remaining layers run in stage 1, or Canny's classification of the frame's pixels, whose
+// hysteresis runs in stage 1.  With several nets: HED's head and Canny's head once each, before the first net that reads
+// their edge map, and one head per net that reads the frame, in net order.
+struct InputHead {
+    bool canny = false;   // canny_head with `edge`, else smallconv with `conv`
+    SmallConvArgs conv{};
+    CannyHeadArgs edge{};
+    const char* label = nullptr;
+    b2sd_launch_record record() const {
+        if (!canny) return smallconv_record(conv);
+        b2sd_launch_record r{};
+        r.kind = B2SD_LAUNCH_CANNY_HEAD;
+        r.canny_head = b2sd_canny_head_args{edge.x, edge.in_flags, edge.in_h, edge.in_w, edge.h, edge.w, edge.low, edge.high, edge.cls};
+        return r;
+    }
+    int launch(cudaStream_t s) const { return canny ? canny_head_launch(edge, s) : smallconv_launch(conv, s); }
+};
 struct InputHeads {
-    SmallConvArgs conv[1 + B2SD_MAX_CONTROLNETS];
-    const char* label[1 + B2SD_MAX_CONTROLNETS];
+    InputHead head[1 + B2SD_MAX_CONTROLNETS];
     int n = 0;
 };
 
-static InputHeads input_heads(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int in_w) {
+// `state`: the stepped state (its own Canny thresholds, if it has some), or nullptr
+static InputHeads input_heads(b2sd_handle h, const b2sd_state* state, const void* frame_in, int in_kind, int in_h, int in_w) {
     const int in_flags = in_kind == B2SD_IN_U8_NHWC ? SC_IN_U8 : (in_kind == B2SD_IN_F32_NCHW ? SC_IN_F32_NCHW : SC_IN_F16_NCHW);
     InputHeads in;
-    in.conv[0] = h->head;
-    in.conv[0].flags = in_flags | (h->head.flags & SC_IN_OFFSET);   // AutoencoderKL: 2x - 1 as the offset input mode
-    in.label[0] = "smallconv head";
+    in.head[0].conv = h->head;
+    in.head[0].conv.flags = in_flags | (h->head.flags & SC_IN_OFFSET);   // AutoencoderKL: 2x - 1 as the offset input mode
+    in.head[0].label = "smallconv head";
     in.n = 1;
     static const char* cn_label[B2SD_MAX_CONTROLNETS] = {"smallconv controlnet head", "smallconv controlnet1 head",
                                                          "smallconv controlnet2 head", "smallconv controlnet3 head"};
-    bool hed_done = false;
+    bool hed_done = false, canny_done = false;
     for (int i = 0; i < h->cfg.controlnet; ++i) {
-        const bool hed = h->control_processor(i) == B2SD_CONTROL_HED;
+        const int proc = h->control_processor(i);
+        InputHead& e = in.head[in.n];
+        if (proc == B2SD_CONTROL_CANNY) {
+            if (canny_done) continue;
+            canny_done = true;
+            const bool own = state && state->canny_own;
+            e.canny = true;
+            e.edge = CannyHeadArgs{frame_in, in_flags, in_h, in_w, h->cfg.height, h->cfg.width, 0, 0, h->canny_cls};
+            canny_thresholds(own ? state->canny_low : h->canny_low, own ? state->canny_high : h->canny_high, &e.edge.low,
+                             &e.edge.high);
+            e.label = "canny_head";
+            ++in.n;
+            continue;
+        }
+        const bool hed = proc == B2SD_CONTROL_HED;
         if (hed && hed_done) continue;
         hed_done = hed_done || hed;
-        in.conv[in.n] = hed ? h->hed_head : h->cn_head[i];
-        in.conv[in.n].flags = in_flags | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
-        in.label[in.n] = hed ? "smallconv hed head" : cn_label[i];
+        e.conv = hed ? h->hed_head : h->cn_head[i];
+        e.conv.flags = in_flags | (hed ? SC_IN_OFFSET | SC_OUT_RELU : SC_OUT_SILU);
+        e.label = hed ? "smallconv hed head" : cn_label[i];
         ++in.n;
     }
     for (int i = 0; i < in.n; ++i) {
-        in.conv[i].x = frame_in; in.conv[i].in_h = in_h; in.conv[i].in_w = in_w;
+        SmallConvArgs& c = in.head[i].conv;
+        c.x = frame_in; c.in_h = in_h; c.in_w = in_w;
     }
     return in;
 }
 
-static int step_heads(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int in_w, cudaStream_t s) {
-    const InputHeads in = input_heads(h, frame_in, in_kind, in_h, in_w);
-    for (int i = 0; i < in.n; ++i) TRY(smallconv_launch(in.conv[i], s));
+static int step_heads(b2sd_handle h, const b2sd_state* state, const void* frame_in, int in_kind, int in_h, int in_w,
+                      cudaStream_t s) {
+    const InputHeads in = input_heads(h, state, frame_in, in_kind, in_h, in_w);
+    for (int i = 0; i < in.n; ++i) TRY(in.head[i].launch(s));
     return 0;
 }
 
@@ -3369,7 +3507,7 @@ static int step_whole(b2sd_handle h, const b2sd_state* cond, const void* frame_i
         return -1;
     }
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    TRY(step_heads(h, frame_in, in_kind, in_h, in_w, s));
+    TRY(step_heads(h, cond, frame_in, in_kind, in_h, in_w, s));
     TRY(bind_conditioning(h, cond, s));
     TRY(run_frame(h, b2sd_engine::GRAPH_WHOLE, 0, h->prog_frame.size(), s));
     return step_tail(h, frame_out, out_kind, s);
@@ -3409,7 +3547,7 @@ int b2sd_step_state(b2sd_handle h, b2sd_state_handle state, const void* frame_in
         return -1;
     }
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    TRY(step_heads(h, frame_in, in_kind, in_h, in_w, s));
+    TRY(step_heads(h, state, frame_in, in_kind, in_h, in_w, s));
     TRY(step_stages(h, state, s));
     return step_tail(h, frame_out, out_kind, s);
 }
@@ -3418,6 +3556,24 @@ int b2sd_get_tensor(b2sd_handle h, const char* name, void* dst, int64_t capacity
     if (!h || !h->built || !name) {
         b2_set_error("b2sd_get_tensor: engine not prepared");
         return -1;
+    }
+    auto u8 = h->u8_taps.find(name);
+    if (u8 != h->u8_taps.end()) {
+        const b2sd_engine::U8Tap& t = u8->second;
+        const int64_t n = (int64_t)t.h * t.w * t.c;
+        if (count) *count = n;
+        if (dims4) { dims4[0] = 1; dims4[1] = t.h; dims4[2] = t.w; dims4[3] = t.c; }
+        if (!dst) return 0;
+        if (capacity < n) {
+            b2_set_error("b2sd_get_tensor: capacity %lld < %lld", (long long)capacity, (long long)n);
+            return -1;
+        }
+        CUDA_OK(cudaStreamSynchronize(reinterpret_cast<cudaStream_t>(stream)));
+        std::vector<uint8_t> host((size_t)n);
+        CUDA_OK(cudaMemcpy(host.data(), t.p, (size_t)n, cudaMemcpyDeviceToHost));
+        __half* d = static_cast<__half*>(dst);
+        for (int64_t i = 0; i < n; ++i) d[i] = __float2half((float)host[i]);   // 0..255: exact in fp16
+        return 0;
     }
     auto it = h->taps.find(name);
     if (it == h->taps.end()) {
@@ -3455,7 +3611,7 @@ int b2sd_profile(b2sd_handle h, const void* frame_in, int in_h, int in_w, void* 
     std::vector<double> acc(nops, 0.0);
     for (int it = 0; it < iters + 1; ++it) {  // first iteration is a warm-up
         CUDA_OK(cudaEventRecord(ev[0], s));
-        TRY(step_heads(h, frame_in, B2SD_IN_U8_NHWC, in_h, in_w, s));
+        TRY(step_heads(h, nullptr, frame_in, B2SD_IN_U8_NHWC, in_h, in_w, s));
         CUDA_OK(cudaEventRecord(ev[1], s));
         size_t i = 1;
         for (auto& op : h->prog_frame) {
@@ -3538,10 +3694,10 @@ int b2sd_audit_step(b2sd_handle h, const void* frame_in, int in_h, int in_w, voi
     TRY(bind_conditioning(h, nullptr, s));   // the engine's own stream: its global conditioning
     Audited au{"b2sd_audit_step", fn, user, s};
     // the input heads and the tail as b2sd_step_ex launches them for a u8 frame, with the caller's frame and size
-    const InputHeads in = input_heads(h, frame_in, B2SD_IN_U8_NHWC, in_h, in_w);
+    const InputHeads in = input_heads(h, nullptr, frame_in, B2SD_IN_U8_NHWC, in_h, in_w);
     for (int i = 0; i < in.n; ++i) {
-        const SmallConvArgs& a = in.conv[i];
-        TRY(au.launch(smallconv_record(a), in.label[i], [&] { return smallconv_launch(a, s); }));
+        const InputHead& e = in.head[i];
+        TRY(au.launch(e.record(), e.label, [&] { return e.launch(s); }));
     }
     TRY(au.program(h->prog_frame));
     uint8_t* out = static_cast<uint8_t*>(frame_out);

@@ -118,14 +118,25 @@ class TimestepEmbeddingArgs(C.Structure):
     _fields_ = [("t", C.c_void_p), ("out", C.c_void_p), ("nb", C.c_int), ("dim", C.c_int)]
 
 
+class CannyHeadArgs(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("in_flags", C.c_int), ("in_h", C.c_int), ("in_w", C.c_int), ("h", C.c_int), ("w", C.c_int),
+                ("low", C.c_int), ("high", C.c_int), ("cls", C.c_void_p)]
+
+
+class CannyCclArgs(C.Structure):
+    _fields_ = [("cls", C.c_void_p), ("parent", C.c_void_p), ("flag", C.c_void_p), ("out", C.c_void_p), ("h", C.c_int),
+                ("w", C.c_int), ("stage", C.c_int)]
+
+
 (LAUNCH_OTHER, LAUNCH_IGEMM, LAUNCH_TCONV, LAUNCH_ATTN, LAUNCH_GROUPNORM, LAUNCH_LAYERNORM, LAUNCH_SMALLCONV, LAUNCH_UPSAMPLE2X,
  LAUNCH_MAXPOOL2X2, LAUNCH_HED_PROJECT, LAUNCH_HED_FUSE, LAUNCH_LCM_STEP, LAUNCH_POST_U8, LAUNCH_SMALL_LINEAR,
- LAUNCH_TIMESTEP_EMBEDDING) = range(15)
+ LAUNCH_TIMESTEP_EMBEDDING, LAUNCH_CANNY_HEAD, LAUNCH_CANNY_CCL) = range(17)
 LAUNCH_KINDS = {LAUNCH_OTHER: "other", LAUNCH_IGEMM: "igemm", LAUNCH_TCONV: "tconv", LAUNCH_ATTN: "attn",
                 LAUNCH_GROUPNORM: "groupnorm", LAUNCH_LAYERNORM: "layernorm", LAUNCH_SMALLCONV: "smallconv",
                 LAUNCH_UPSAMPLE2X: "upsample2x", LAUNCH_MAXPOOL2X2: "maxpool2x2", LAUNCH_HED_PROJECT: "hed_project",
                 LAUNCH_HED_FUSE: "hed_fuse", LAUNCH_LCM_STEP: "lcm_step", LAUNCH_POST_U8: "post_u8",
-                LAUNCH_SMALL_LINEAR: "small_linear", LAUNCH_TIMESTEP_EMBEDDING: "timestep_embedding"}
+                LAUNCH_SMALL_LINEAR: "small_linear", LAUNCH_TIMESTEP_EMBEDDING: "timestep_embedding",
+                LAUNCH_CANNY_HEAD: "canny_head", LAUNCH_CANNY_CCL: "canny_ccl"}
 
 
 class LaunchRecord(C.Structure):
@@ -138,6 +149,7 @@ class LaunchRecord(C.Structure):
         ("hed_project", HedProjectArgs), ("hed_fuse", HedFuseArgs), ("lcm_step", LcmStepArgs), ("post_u8", PostU8Args),
         ("small_linear", SmallLinearArgs), ("timestep_embedding", TimestepEmbeddingArgs),
         ("attn_k_ip", C.c_void_p), ("attn_vt_ip", C.c_void_p), ("attn_n_ip", C.c_void_p),
+        ("canny_head", CannyHeadArgs), ("canny_ccl", CannyCclArgs),
     ]
 
 
@@ -171,7 +183,8 @@ IG_GEGLU = 2
 IG_SILU = 8
 IG_PAD0 = 16
 SC_IN_U8, SC_IN_TANH3, SC_OUT_RELU, SC_OUT_SILU, SC_IN_OFFSET = 1, 2, 4, 32, 64
-CONTROL_FRAME, CONTROL_HED = 0, 1
+CONTROL_FRAME, CONTROL_HED, CONTROL_CANNY = 0, 1, 2
+CONTROL_PROCESSORS = {None: CONTROL_FRAME, "hed": CONTROL_HED, "canny": CONTROL_CANNY}   # controlnet_processor_id -> value
 COND_PROMPT, COND_TIME = 0, 1      # b2sd_state_clear_conditioning
 VAE_TINY, VAE_KL = 0, 1
 IG_TCONV = 64
@@ -245,7 +258,10 @@ def lib() -> C.CDLL:
         _lib.b2sd_state_clear_conditioning.argtypes = [vp, ci]
         _lib.b2sd_set_image_embeds.argtypes = [vp, vp, ci, cf, vp]
         _lib.b2sd_state_set_image_embeds.argtypes = [vp, vp, vp, ci, cf, vp]
-        for name in ("state_create", "state_reset", "state_destroy", "step_state", "state_set_prompt_embeds", "state_set_timesteps",
+        _lib.b2sd_set_canny_thresholds.argtypes = [vp, C.c_double, C.c_double]
+        _lib.b2sd_state_set_canny_thresholds.argtypes = [vp, C.c_double, C.c_double]
+        _lib.b2sd_state_clear_canny_thresholds.argtypes = [vp]
+        for name in ("set_canny_thresholds", "state_set_canny_thresholds", "state_clear_canny_thresholds", "state_create", "state_reset", "state_destroy", "step_state", "state_set_prompt_embeds", "state_set_timesteps",
                      "state_clear_conditioning", "set_image_embeds", "state_set_image_embeds", "set_control_scale",
                      "state_set_control_scale", "set_control_scales", "state_set_control_scales"):
             getattr(_lib, "b2sd_" + name).restype = C.c_int

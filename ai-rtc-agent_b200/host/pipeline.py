@@ -131,8 +131,8 @@ class StreamDiffusionPipeline:
         update_image_prompt() then steers the video with an image, globally or per viewer (PeerStream.update_image_prompt).
 
         controlnet (None: $B200SD_CONTROLNET, default none): a diffusers ControlNetModel (id or path; "synthetic" with a
-        synthetic model), conditioned on each frame's HED edge map (controlnet_processor="hed") or on the frame itself
-        (controlnet_processor=None).  update_controlnet_scale() then sets its strength and guidance window, globally or per
+        synthetic model), conditioned on each frame's HED edge map (controlnet_processor="hed"), its Canny edge map
+        (controlnet_processor="canny", thresholds update_canny_thresholds) or on the frame itself (controlnet_processor=None).  update_controlnet_scale() then sets its strength and guidance window, globally or per
         viewer (PeerStream.update_controlnet_scale).  A list of ids runs several ControlNets (diffusers'
         MultiControlNetModel), each with its own control image and settings; controlnet_processor is then one processor for
         every net or a list with one per net ($B200SD_CONTROLNET stays a single id)."""
@@ -149,6 +149,7 @@ class StreamDiffusionPipeline:
         self.model = StreamDiffusionWrapper.__new__(StreamDiffusionWrapper)
         self.model.live_lora = bool(live_lora)
         self.model.ip_adapter = ip_adapter
+        self.model.canny_processor = True
         if controlnet is None:
             controlnet = os.getenv(CONTROLNET_ENV) or None
         self.model.__init__(
@@ -267,6 +268,16 @@ class StreamDiffusionPipeline:
             self.model.update_controlnet_scale(scale, control_guidance_start, control_guidance_end)
         finally:
             self._release(cur)
+
+    def update_canny_thresholds(self, low: float = 100.0, high: float = 200.0):
+        """The global Canny thresholds (controlnet_aux CannyDetector's low_threshold / high_threshold): every stream's,
+        including open peer streams with thresholds of their own (PeerStream.update_canny_thresholds).  Host values passed to
+        the Canny kernel when a frame is enqueued: frames enqueued before the call use the old ones, frames enqueued after it
+        the new ones, with no device work and no wait."""
+        if not self.model.stream.has_canny:
+            raise RuntimeError("update_canny_thresholds needs a pipeline with a ControlNet whose processor is 'canny' "
+                               "(controlnet_processor='canny')")
+        self.model.update_canny_thresholds(low, high)
 
     # ---- viewers' own styles (PeerStream.update_lora) ------------------------------------------------------------------
     def _leave_style(self, peer) -> None:
@@ -628,6 +639,23 @@ class PeerStream:
         control = check_controls(scale, control_guidance_start, control_guidance_end,
                                  self._pipeline.model.stream.control_nets)
         self._pipeline._update_state(lambda engine: state.set_control_scale(*control, engine=engine), self._style)
+
+    @property
+    def canny_thresholds(self) -> tuple:
+        """This viewer's Canny (low, high): its own (update_canny_thresholds) or the pipeline's global ones"""
+        own = self._live_state().own_canny
+        return own if own is not None else self._pipeline.model.stream.canny_thresholds
+
+    def update_canny_thresholds(self, low: float = 100.0, high: float = 200.0) -> None:
+        """This viewer's own Canny thresholds: its frames enqueued after the call use them, whichever lane or style runs them;
+        frames already queued, and every other viewer's frames, are unaffected.  No device work, no wait.  It keeps them
+        through prompt, t_index_list, image-prompt, ControlNet-scale and LoRA updates and style moves; a later global
+        pipeline.update_canny_thresholds replaces them."""
+        state = self._live_state()
+        if not self._pipeline.model.stream.has_canny:
+            raise RuntimeError("update_canny_thresholds needs a pipeline with a ControlNet whose processor is 'canny' "
+                               "(controlnet_processor='canny')")
+        state.set_canny_thresholds(low, high)
 
     @property
     def lora(self) -> Dict[str, float]:

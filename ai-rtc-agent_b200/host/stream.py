@@ -107,6 +107,17 @@ def check_controls(scale, start=0.0, end=1.0, nets: int = 1):
     return tuple(zip(*[check_control(v, a, b) for v, a, b in zip(scale, start, end)]))
 
 
+DEFAULT_CANNY_THRESHOLDS = (100.0, 200.0)   # controlnet_aux CannyDetector's low_threshold / high_threshold
+
+
+def check_canny_thresholds(low: float, high: float) -> Tuple[float, float]:
+    """(low, high) as floats, finite (cv2.Canny swaps a reversed pair and floors both; so does the engine)"""
+    low, high = float(low), float(high)
+    if not (math.isfinite(low) and math.isfinite(high)):
+        raise ValueError(f"Canny thresholds must be finite (got {low}, {high})")
+    return low, high
+
+
 def default_controls(nets: int):
     """The settings of `nets` ControlNets before any update: scale 1 over the whole run for each"""
     return DEFAULT_CONTROL if nets == 1 else tuple(nets * (v,) for v in DEFAULT_CONTROL)
@@ -149,6 +160,8 @@ class StreamDiffusion:
     control = DEFAULT_CONTROL   # the global ControlNet settings (check_controls; set_control_scale)
     has_controlnet = False      # built with a ControlNet (inherited by lanes and styles)
     control_nets = 1            # with has_controlnet: how many ControlNets (inherited by lanes and styles)
+    has_canny = False           # a ControlNet's processor is "canny" (inherited by lanes and styles)
+    canny_thresholds = DEFAULT_CANNY_THRESHOLDS   # the global Canny thresholds (set_canny_thresholds)
 
     def __init__(self, arch: UNetArch, unet_sd: Dict[str, torch.Tensor], vae_sd: Dict[str, torch.Tensor],
                  t_index_list: List[int], prompt_encoder: Callable[[str], torch.Tensor],
@@ -166,7 +179,9 @@ class StreamDiffusion:
         stream-batch slot is then conditioned on the current frame's control image: the frame itself, or with hed_sd (a
         ControlNetHED.pth state dict, empty with packed_blob) its HED edge map.  Lanes inherit their parent's ControlNet.
         Several ControlNets (diffusers' MultiControlNetModel): controlnet_sd a list of 1..4 state dicts and control_processors
-        one processor per net, "hed" (needs hed_sd; the edge map is computed once per frame) or None (the frame itself).
+        one processor per net, "hed" (needs hed_sd; the edge map is computed once per frame), "canny" (cv2.Canny's edge map,
+        computed once per frame; thresholds set_canny_thresholds) or None (the frame itself).  One state dict may take a
+        control_processors list of one.
         live_lora: keep the base UNet weights on the device so that apply_lora() can switch LoRAs at run time (not with
         packed_blob; lanes inherit it).
         style_of: make a style of that live engine instead (add_style).
@@ -177,14 +192,15 @@ class StreamDiffusion:
         if hed_sd is not None and controlnet_sd is None:
             raise ValueError("the HED processor needs a ControlNet")
         nets_sd = controlnet_sd if isinstance(controlnet_sd, (list, tuple)) else None
-        if nets_sd is not None:
-            if not 1 <= len(nets_sd) <= capi.MAX_CONTROLNETS:
-                raise ValueError(f"1 to {capi.MAX_CONTROLNETS} ControlNets (got {len(nets_sd)})")
-            if control_processors is None or len(control_processors) != len(nets_sd):
+        if nets_sd is not None or (controlnet_sd is not None and control_processors is not None):
+            n = len(nets_sd) if nets_sd is not None else 1
+            if not 1 <= n <= capi.MAX_CONTROLNETS:
+                raise ValueError(f"1 to {capi.MAX_CONTROLNETS} ControlNets (got {n})")
+            if control_processors is None or len(control_processors) != n:
                 raise ValueError("control_processors needs one processor per ControlNet")
             for p in control_processors:
-                if p not in (None, "hed"):
-                    raise NotImplementedError(f"ControlNet processor {p!r} (only 'hed', or None: the frame itself)")
+                if p not in capi.CONTROL_PROCESSORS:
+                    raise NotImplementedError(f"ControlNet processor {p!r} (only 'hed', 'canny', or None: the frame itself)")
             if ("hed" in control_processors) != (hed_sd is not None):
                 raise ValueError("hed_sd is needed exactly when a ControlNet's processor is 'hed'")
         elif control_processors is not None:
@@ -236,10 +252,11 @@ class StreamDiffusion:
         self.has_controlnet = controlnet_sd is not None or (parent or style_of or self).has_controlnet
         self.control_nets = cfg.controlnet if controlnet_sd is not None else (parent or style_of or self).control_nets
         self.control = default_controls(self.control_nets)
-        if nets_sd is None:
+        self.has_canny = "canny" in (control_processors or ()) or (parent or style_of or self).has_canny
+        if control_processors is None:
             cfg.control_processor = capi.CONTROL_HED if hed_sd is not None else capi.CONTROL_FRAME
         else:
-            procs = [capi.CONTROL_HED if p == "hed" else capi.CONTROL_FRAME for p in control_processors]
+            procs = [capi.CONTROL_PROCESSORS[p] for p in control_processors]
             cfg.control_processor = procs[0]
             for i, p in enumerate(procs[1:]):
                 cfg.control_processor_more[i] = p
@@ -402,6 +419,9 @@ class StreamDiffusion:
         self.t_list = list(other.t_list)
         self.control = other.control
         self._engine_prepare()
+        if self.has_canny:   # a new lane or style starts with the family's global thresholds
+            self.canny_thresholds = other.canny_thresholds
+            capi.check(self._lib.b2sd_set_canny_thresholds(self._handle, *self.canny_thresholds), "b2sd_set_canny_thresholds")
         if other.image_prompt is not None:   # a new lane or style starts with the family's global image prompt
             tokens, scale = other.image_prompt
             capi.check(self._lib.b2sd_set_image_embeds(self._handle, tokens.data_ptr(), tokens.shape[0], scale, self._stream()),
@@ -544,6 +564,20 @@ class StreamDiffusion:
         for state in list(self._states):
             if not state.closed:
                 state.clear_overrides(prompt=False, t_index_list=False, control=True)
+
+    def set_canny_thresholds(self, low: float = 100.0, high: float = 200.0) -> None:
+        """The global Canny thresholds (cv2.Canny's threshold1 / threshold2): this engine's, its lanes' and its styles'
+        (b2sd_set_canny_thresholds), and every live state's (a state's own thresholds are dropped).  Host values that the next
+        steps pass to the Canny kernel: frames submitted before the call keep the old ones; no device work, no synchronisation."""
+        if not self.has_canny:
+            raise RuntimeError("this engine has no ControlNet with the 'canny' processor")
+        low, high = check_canny_thresholds(low, high)
+        for eng in self._family():
+            capi.check(self._lib.b2sd_set_canny_thresholds(eng._handle, low, high), "b2sd_set_canny_thresholds")
+            eng.canny_thresholds = (low, high)
+        for state in list(self._states):
+            if not state.closed:
+                state.clear_canny_thresholds()
 
     def clear_overrides(self, prompt: bool = True, t_index_list: bool = True, image_prompt: Optional[bool] = None) -> None:
         """Every live state of this engine's weights follows the global prompt, t_index_list and / or image prompt again
@@ -824,6 +858,7 @@ class StreamState:
     own_t_index_list: Optional[List[int]] = None   # None: the global t_index_list
     own_image: Optional[Tuple[torch.Tensor, float]] = None   # (device tokens [n_tok][D], scale); None: the global image prompt
     own_control: Optional[tuple] = None   # ControlNet settings (check_controls); None: the global settings
+    own_canny: Optional[Tuple[float, float]] = None   # Canny thresholds; None: those of the engine that steps the state
     home: Optional[StreamDiffusion] = None   # where clear_overrides recomputes what it keeps (None: the creating engine)
 
     def __init__(self, engine: StreamDiffusion):
@@ -879,6 +914,21 @@ class StreamState:
         v = _on_device(torch.tensor(control_vector(control, t_index_list, len(eng.timesteps)), dtype=torch.float32), eng.device)
         fn = "b2sd_state_set_control_scale" if eng.control_nets == 1 else "b2sd_state_set_control_scales"
         capi.check(getattr(self._lib, fn)(eng._handle, self.handle, v.data_ptr(), eng._stream()), fn)
+
+    def set_canny_thresholds(self, low: float = 100.0, high: float = 200.0) -> None:
+        """This stream's own Canny thresholds (b2sd_state_set_canny_thresholds): host values that every engine stepping the
+        state passes to the Canny kernel, from the next step on.  Nothing else about the state (prompt, t_index_list,
+        ControlNet settings, image prompt, the engine or style that steps it) changes them; a global set_canny_thresholds
+        drops them."""
+        low, high = check_canny_thresholds(low, high)
+        capi.check(self._lib.b2sd_state_set_canny_thresholds(self.handle, low, high), "b2sd_state_set_canny_thresholds")
+        self.own_canny = (low, high)
+
+    def clear_canny_thresholds(self) -> None:
+        """Follow the stepping engine's global Canny thresholds again (no-op for an engine without Canny)"""
+        if self._engine.has_canny:
+            capi.check(self._lib.b2sd_state_clear_canny_thresholds(self.handle), "b2sd_state_clear_canny_thresholds")
+        self.own_canny = None
 
     @torch.no_grad()
     def set_image_tokens(self, tokens: Optional[torch.Tensor], scale: float = 1.0,

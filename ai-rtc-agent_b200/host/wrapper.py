@@ -4,9 +4,10 @@ with the TensorRT/diffusers model behind it replaced by the sm_90a engine (host/
 
 Not carried over (unreachable from lib/pipeline.py:23-42 and listed out-of-scope in SURVEY.md section 8):
 safety checker, similar-image filter, DataParallel, txt2img sampling, xformers/sfast/TensorRT acceleration switches, and
-ControlNet preprocessors other than HED.  Their keywords are accepted; asking for one of those features raises.  A ControlNet
-runs with controlnet_processor_id="hed" (the default: the frame's HED edge map is the control image) or None (the frame
-itself).  Several ControlNets (diffusers' MultiControlNetModel): controlnet_id_or_path a list of ids, controlnet_processor_id
+ControlNet preprocessors other than HED and Canny.  Their keywords are accepted; asking for one of those features raises.  A
+ControlNet runs with controlnet_processor_id="hed" (the default: the frame's HED edge map is the control image), "canny"
+(cv2.Canny's edge map, update_canny_thresholds; enabled by the canny_processor attribute, which StreamDiffusionPipeline sets)
+or None (the frame itself).  Several ControlNets (diffusers' MultiControlNetModel): controlnet_id_or_path a list of ids, controlnet_processor_id
 one processor for all or a list with one per net.  use_tiny_vae=False encodes and decodes with the model's own AutoencoderKL instead of TAESD (slower, the model's
 image quality); the latent is the mean of the encoder's distribution, not a sample of it."""
 from __future__ import annotations
@@ -83,6 +84,10 @@ class StreamDiffusionWrapper:
     # IP-Adapter image prompts (update_image_prompt): an adapter file or directory, "synthetic" (seeded weights, with synthetic
     # models only), or None for $B200SD_IP_ADAPTER (unset: none).  Set on the instance before __init__, as live_lora.
     ip_adapter: Optional[str] = None
+    # The Canny edge processor (controlnet_processor_id="canny", DESIGN.md §4.14).  The reference's constructor runs "hed" only and
+    # refuses every other processor id, and so does this one unless canny_processor is set on the instance before __init__, as
+    # live_lora is; StreamDiffusionPipeline and pack.py set it.
+    canny_processor: bool = False
 
     def __init__(
         self,
@@ -131,11 +136,14 @@ class StreamDiffusionWrapper:
         unsupported = []
         if mode == "txt2img":
             unsupported.append("mode='txt2img'")
+        processors = (None, "hed", "canny") if self.canny_processor else (None, "hed")
         for proc in controlnet_processor_id if isinstance(controlnet_processor_id, list) else [controlnet_processor_id]:
-            if controlnet_id_or_path is not None and proc not in (None, "hed"):
+            if controlnet_id_or_path is not None and proc not in processors:
                 # the reference prints "ControlNet conditioning not supported." for an unknown id and runs unconditioned; a
                 # caller who asked for a preprocessor should not silently get the raw frame instead
-                unsupported.append(f"controlnet_processor_id={proc!r} (only 'hed', or None: the frame itself)")
+                unsupported.append(f"controlnet_processor_id={proc!r} (only " +
+                                   ("'hed', 'canny'" if self.canny_processor else "'hed' ('canny' with canny_processor set)") +
+                                   ", or None: the frame itself)")
         if use_safety_checker:
             unsupported.append("safety checker")
         if enable_similar_image_filter:
@@ -207,6 +215,8 @@ class StreamDiffusionWrapper:
         hed = cn and (("hed" in controlnet_processor_id) if multi else controlnet_processor_id == "hed")
         if multi:
             kw["control_processors"] = controlnet_processor_id
+        elif cn and controlnet_processor_id == "canny":
+            kw["control_processors"] = ["canny"]
         adapter = self._load_ip_adapter(arch, synthetic_ok)
         kw["ip_adapter"] = adapter
         blob = None
@@ -339,6 +349,12 @@ class StreamDiffusionWrapper:
         for every net or a list with one per net (diffusers' MultiControlNetModel).  See StreamDiffusion.set_control_scale."""
         with self._on_stream():
             self.stream.set_control_scale(scale, control_guidance_start, control_guidance_end)
+
+    def update_canny_thresholds(self, low: float = 100.0, high: float = 200.0) -> None:
+        """The Canny processor's thresholds (controlnet_aux CannyDetector's low_threshold / high_threshold, cv2.Canny's
+        threshold1 / threshold2): frames submitted after the call use them.  One pair for every Canny ControlNet.  See
+        StreamDiffusion.set_canny_thresholds."""
+        self.stream.set_canny_thresholds(low, high)
 
     def update_t_index_list(self, t_index_list: List[int]) -> None:
         """lib/wrapper.py:389-407: swaps the sub-timesteps only."""

@@ -41,7 +41,7 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--full-vae", action="store_true", help="pack the model's own AutoencoderKL instead of TAESD (use_tiny_vae=False)")
     ap.add_argument("--controlnet-id", default=None, help="diffusers ControlNetModel (HF id or local directory) packed with the UNet")
     ap.add_argument("--controlnet-processor-id", default="hed", type=lambda v: None if v.lower() == "none" else v,
-                    help="control-image preprocessor: hed (default, the reference's) or none (the frame itself)")
+                    help="control-image preprocessor: hed (default, the reference's), canny or none (the frame itself)")
     ap.add_argument("--engine-dir", default=os.getenv("TRT_ENGINES_CACHE", "./models/engines"), help="cache root (lib/pipeline.py:35)")
     ap.add_argument("--width", type=int, default=512)
     ap.add_argument("--height", type=int, default=512)
@@ -73,11 +73,13 @@ def main(argv=None) -> int:
     if args.force and os.path.exists(blob):
         os.remove(blob)
     t0 = time.time()
-    w = StreamDiffusionWrapper(model_id_or_path=args.model_id, t_index_list=t_index_list, lora_dict=loras or None,
-                               lcm_lora_id=args.lcm_lora_id, vae_id=None if args.full_vae else args.vae_id,
-                               use_lcm_lora=not args.no_lcm_lora, use_tiny_vae=not args.full_vae,
-                               controlnet_id_or_path=args.controlnet_id, controlnet_processor_id=args.controlnet_processor_id,
-                               width=args.width, height=args.height, output_type="pt", mode="img2img", engine_dir=args.engine_dir)
+    w = StreamDiffusionWrapper.__new__(StreamDiffusionWrapper)
+    w.canny_processor = True   # pack blobs for every processor the library builds
+    w.__init__(model_id_or_path=args.model_id, t_index_list=t_index_list, lora_dict=loras or None,
+               lcm_lora_id=args.lcm_lora_id, vae_id=None if args.full_vae else args.vae_id,
+               use_lcm_lora=not args.no_lcm_lora, use_tiny_vae=not args.full_vae,
+               controlnet_id_or_path=args.controlnet_id, controlnet_processor_id=args.controlnet_processor_id,
+               width=args.width, height=args.height, output_type="pt", mode="img2img", engine_dir=args.engine_dir)
     reused = w.packed_blob is not None
     w.prepare(prompt="", num_inference_steps=50, guidance_scale=0.0)
     if w.packed_blob is None:

@@ -212,10 +212,12 @@ typedef struct {
                                     size); its 12 + 1 residuals are added to the UNet's skips and mid-block output.  0: none.
                                     2..B2SD_MAX_CONTROLNETS: that many nets (control_processor_more).  A lane inherits its
                                     parent's value. */
-    int control_processor;       /* with controlnet = 1: B2SD_CONTROL_FRAME (0) or B2SD_CONTROL_HED (1): the control image is the
+    int control_processor;       /* with controlnet = 1: B2SD_CONTROL_FRAME (0), B2SD_CONTROL_HED (1): the control image is the
                                     HED edge map of the frame (controlnet_aux HEDdetector at the engine's size; weights under
-                                    "hed." + ControlNetHED.pth keys, e.g. "hed.block1.convs.0.weight", "hed.norm").  Inherited
-                                    by lanes. */
+                                    "hed." + ControlNetHED.pth keys, e.g. "hed.block1.convs.0.weight", "hed.norm"), or
+                                    B2SD_CONTROL_CANNY (2): the Canny edge map of the frame (controlnet_aux CannyDetector,
+                                    cv2.Canny with aperture 3 and the L1 gradient, at the engine's size; no weights; thresholds
+                                    b2sd_set_canny_thresholds).  Inherited by lanes. */
     int vae;                     /* B2SD_VAE_TINY (0): TAESD (weights "vae." + AutoencoderTiny keys).  B2SD_VAE_KL (1): the model's
                                     own AutoencoderKL (weights "vae." + diffusers AutoencoderKL keys, e.g.
                                     "vae.encoder.down_blocks.0.resnets.0.conv1.weight", "vae.quant_conv.weight"; mid-block attention
@@ -230,12 +232,12 @@ typedef struct {
                                  /* multi-ControlNet: controlnet = N (1..B2SD_MAX_CONTROLNETS) nets, net 0 with the weights and
                                     processor above, net i >= 1 with weights under "controlnet<i>." (e.g.
                                     "controlnet1.controlnet_mid_block.weight") and processor control_processor_more[i - 1]
-                                    (0 for the entries past the last net).  The HED edge map is computed once per frame however
-                                    many nets read it.  Each net's residuals are scaled by its own per-slot scales
+                                    (0 for the entries past the last net).  The HED and Canny edge maps are each computed once
+                                    per frame however many nets read them.  Each net's residuals are scaled by its own per-slot scales
                                     (b2sd_set_control_scales) and summed into the UNet's skips in net order,
                                     ((skip + r_0) + r_1) + ...  Inherited by lanes and styles. */
 } b2sd_config;
-enum { B2SD_CONTROL_FRAME = 0, B2SD_CONTROL_HED = 1 };
+enum { B2SD_CONTROL_FRAME = 0, B2SD_CONTROL_HED = 1, B2SD_CONTROL_CANNY = 2 };
 enum { B2SD_VAE_TINY = 0, B2SD_VAE_KL = 1 };
 
 int b2sd_create(const b2sd_config* cfg, b2sd_handle* out);
@@ -347,7 +349,8 @@ int b2sd_step_ex(b2sd_handle h, const void* frame_in, int in_kind, int in_h, int
  * "vae.enc.down.I", "vae.enc.mid", "vae.dec.mid", "vae.dec.up.I" (block outputs); with a ControlNet also "cn_cond"
  * (conditioning embedding, batch 1), "cn.conv_in" (its conv_in(x) + cn_cond), "cn.res.K" (UNet skip K, in push order 0..11,
  * plus ControlNet residual K: what the up path reads) and "cn.mid" ("mid" plus the mid-block residual); with HED also
- * "control" (the u8 edge value as fp16, [1][h][w][1]).
+ * "control" (the u8 edge value as fp16, [1][h][w][1]); with Canny also "canny" (the u8 edge image, [1][h][w][3], 0 / 255) and
+ * "canny_class" (canny_head's class map, [1][h][w][1]: 0 none, 1 candidate, 2 strong), both as fp16.
  * Returns the element count via *count (pass dst = NULL to query).  Synchronises `stream`. */
 int b2sd_get_tensor(b2sd_handle h, const char* name, void* dst, int64_t capacity, int64_t* count, int* dims4,
                     void* stream);
@@ -375,7 +378,8 @@ int b2sd_launches_per_step(b2sd_handle h);
 enum { B2SD_LAUNCH_OTHER = 0, B2SD_LAUNCH_IGEMM = 1, B2SD_LAUNCH_TCONV = 2, B2SD_LAUNCH_ATTN = 3, B2SD_LAUNCH_GROUPNORM = 4,
        B2SD_LAUNCH_LAYERNORM = 5, B2SD_LAUNCH_SMALLCONV = 6, B2SD_LAUNCH_UPSAMPLE2X = 7, B2SD_LAUNCH_MAXPOOL2X2 = 8,
        B2SD_LAUNCH_HED_PROJECT = 9, B2SD_LAUNCH_HED_FUSE = 10, B2SD_LAUNCH_LCM_STEP = 11, B2SD_LAUNCH_POST_U8 = 12,
-       B2SD_LAUNCH_SMALL_LINEAR = 13, B2SD_LAUNCH_TIMESTEP_EMBEDDING = 14 };
+       B2SD_LAUNCH_SMALL_LINEAR = 13, B2SD_LAUNCH_TIMESTEP_EMBEDDING = 14, B2SD_LAUNCH_CANNY_HEAD = 15,
+       B2SD_LAUNCH_CANNY_CCL = 16 };
 typedef struct {
     const void* xa; int ca, lda;
     const void* xb; int cb, ldb;   /* xb NULL: no second source */
@@ -431,6 +435,13 @@ typedef struct {
 } b2sd_small_linear_args;
 /* out[b] = [cos | sin](t[b] * exp(-ln(10000) * j / (dim/2))), j < dim/2: fp32 [nb][dim] */
 typedef struct { const float* t; float* out; int nb, dim; } b2sd_timestep_embedding_args;
+/* Canny's input head: the frame x (in_flags 1 u8 NHWC, 8 fp32 NCHW, 16 fp16 NCHW, nearest-resized from in_h x in_w to h x w,
+ * floats as rint(clamp(v, 0, 1) * 255)) classified per pixel into cls u8 [h][w] (0 none, 1 candidate, 2 strong) with the
+ * integer thresholds low / high (swapped when reversed, floored, clamped to [-1, 2041]) */
+typedef struct b2sd_canny_head_args { const void* x; int in_flags, in_h, in_w, h, w, low, high; void* cls; } b2sd_canny_head_args;
+/* Canny's hysteresis, stage 0..3 (local labels, border merges, root flags, output): cls [h][w] -> out u8 [h][w][3], with the
+ * scratch parent int [h][w] and flag u8 [h][w] */
+typedef struct b2sd_canny_ccl_args { const void* cls; void* parent; void* flag; void* out; int h, w, stage; } b2sd_canny_ccl_args;
 typedef struct {
     int kind;
     const char* label;
@@ -452,6 +463,8 @@ typedef struct {
     const void* attn_k_ip;
     const void* attn_vt_ip;
     const int* attn_n_ip;
+    b2sd_canny_head_args canny_head;
+    b2sd_canny_ccl_args canny_ccl;
 } b2sd_launch_record;
 /* One b2sd_step with the frame program run eagerly (no CUDA graph) and `fn` called around every kernel launch: `stream` is
  * synchronised, fn(user, index, 0, rec) runs, the launch is enqueued, `stream` is synchronised, fn(user, index, 1, rec) runs.
@@ -544,6 +557,17 @@ int b2sd_state_set_control_scales(b2sd_handle h, b2sd_state_handle state, const 
 /* Drop the state's override of the prompt (which = 0) or time (which = 1) block: later steps use the engines' global values.
  * No device work; the override is freed after the steps already submitted with it. */
 int b2sd_state_clear_conditioning(b2sd_state_handle state, int which);
+/* Canny thresholds (an engine with a ControlNet whose processor is B2SD_CONTROL_CANNY; others are refused): cv2.Canny's
+ * threshold1 / threshold2, finite, swapped when low > high and floored; a pixel is a candidate when its L1 gradient magnitude
+ * is > low and strong when > high (100 / 200 after b2sd_create, controlnet_aux's defaults).  One pair per frame, shared by
+ * every Canny net.  They are host values that canny_head takes as kernel arguments when a step launches it, so a change needs
+ * no device work, no graph recapture and no synchronisation: steps submitted before the call keep the old values.
+ * b2sd_set_canny_thresholds sets the engine's global pair; b2sd_state_set_canny_thresholds the state's own pair, used by any
+ * engine that steps the state (lanes and styles alike, and nothing else about the state changes it);
+ * b2sd_state_clear_canny_thresholds makes the state follow the stepping engine's global pair again. */
+int b2sd_set_canny_thresholds(b2sd_handle h, double low, double high);
+int b2sd_state_set_canny_thresholds(b2sd_state_handle state, double low, double high);
+int b2sd_state_clear_canny_thresholds(b2sd_state_handle state);
 /* Test aid: how many block copies the steps of engine h have issued to bind a state's (or the global) conditioning */
 int64_t b2sd_conditioning_binds(b2sd_handle h);
 /* How many frames will be in flight on this GPU (lanes / independent streams).  1 (default): launch policy tuned for the
